@@ -46,7 +46,7 @@ def measured_peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def source_hash():
@@ -59,9 +59,9 @@ def source_hash():
 
 
 def ncu_traffic(kernel_name):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel_name` from the committed
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel_name` from
     `ncu --set full` captures (profiles/traffic.json, written by profiles/ncu_traffic.py), or None
-    when there is no capture of THIS build of the sources (source hash mismatch)."""
+    when there is no capture of THIS build of the sources (file absent or source hash mismatch)."""
     try:
         with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
             t = json.load(f)
@@ -342,13 +342,32 @@ def config2_description():
     return {"workload": "config2: Morlet(6) CWT, synthetic chirp N=2^20, 256 scales "
                         "(s0=2, dj=1/16, J=255), fp64, one signal per GPU",
             "n": c["n"], "scales": c["J"] + 1, "wavelet": "morlet(6)",
-            "l2": "no explicit flush: each step writes 4.29 GB of coefficients (>> 126 MB L2) "
+            "l2": "no explicit flush: each step writes 4.29 GB of coefficients (>> the 50 MB L2 of an H100) "
                   "and re-reads only the 16 MiB spectrum it just produced"}
 
 
 # ---------------------------------------------------------------------------------------------
 # config 2 (headline)
 # ---------------------------------------------------------------------------------------------
+DUMP_COLUMNS = 8192      # of the N = 2^20 columns of W: 256 rows x 8192 x 16 B = 32 MiB written
+
+
+def dump_config2_outputs(out_dir, eng, S, n):
+    """W of the last timed step (still resident on the device) as float64 .npy files: every row at a
+    fixed, seeded sample of columns, real and imaginary parts apart, and the sampled column indices."""
+    os.makedirs(out_dir, exist_ok=True)
+    cols = np.sort(np.random.RandomState(2).choice(n, min(n, DUMP_COLUMNS), replace=False))
+    re = np.empty((S, cols.size))
+    im = np.empty((S, cols.size))
+    row = np.empty(n, dtype=np.complex128)
+    for j in range(S):
+        eng._check(eng.lib.cwtb_get_w(eng.h, row.ctypes.data, 1, j, 1))
+        re[j], im[j] = row.real[cols], row.imag[cols]
+    np.save(os.path.join(out_dir, "W_real.npy"), re)
+    np.save(os.path.join(out_dir, "W_imag.npy"), im)
+    np.save(os.path.join(out_dir, "W_columns.npy"), cols.astype(np.float64))
+
+
 def run_config2(args, D, eng, pycwt, _engine):
     c = wl.C2
     sj = wl.config2_scales()
@@ -371,6 +390,8 @@ def run_config2(args, D, eng, pycwt, _engine):
     eng.sync()
     D.barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and D.rank == 0:
+        dump_config2_outputs(args.dump_outputs, eng, S, c["n"])
     ms_max = D.max(ms)
     value = D.world * pts / (ms_max * 1e-3)
     prof = eng.profile_last()    # per-kernel-type event times of one more (untimed, serialised) step
@@ -451,7 +472,7 @@ def run_config3(args, D, eng, pycwt, _engine):
     x = wl.config3_signal()
     out = {"workload": "config3: Paul(4) and DOG(2) CWT, chirp N=2^18 (float32), 128 scales, fp32 engine",
            "dtype": "f32", "metric": METRIC, "unit": UNIT}
-    steps = max(args.steps, 20)
+    steps = args.steps
     mod, kind = reference_module()
     os.environ["CWTB_PRECISION"] = "fp32"
     try:
@@ -599,13 +620,13 @@ def run_config5(args, D, eng, pycwt, _engine, comm=None):
     eng.cwt_batch_dev(dX, chunk, c["n"], c["dt"], sj, _engine.MORLET, c["f0"], _engine.F32)
     eng.bench_last(2)
     D.barrier()
-    ms = D.max(eng.bench_last(5))
+    ms = D.max(eng.bench_last(args.steps))
     launches = eng.last_launch_count()
     prof = eng.profile_last()
     eng.dev_free(dX)
     pts_chunk = chunk * S * c["n"]
-    out.update({"value": D.world * pts_chunk / (ms * 1e-3), "ms_per_step": ms, "steps": 5,
-                "step": "one 256-channel chunk (4 per GPU share)", "gpu_launches": launches * 5,
+    out.update({"value": D.world * pts_chunk / (ms * 1e-3), "ms_per_step": ms, "steps": args.steps,
+                "step": "one 256-channel chunk (4 per GPU share)", "gpu_launches": launches * args.steps,
                 "roofline": roofline_block(prof, c["n"] * 8, pts_chunk * 8 + chunk * c["n"] * 4, ms)})
     # end to end: host float32 channels in, per-channel spectra out, gathered over the ranks
     from pycwt_b200 import distributed as Dm
@@ -717,6 +738,9 @@ def main():
                     help="BASELINE.json configurations to measure (2 is always the headline)")
     ap.add_argument("--kernels-only", action="store_true",
                     help="profiling aid: time the resident-input kernels of config 2 only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of config 2, write what its last step computed (W at a "
+                         "fixed, seeded sample of columns) as DIR/<name>.npy, for comparing two builds")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

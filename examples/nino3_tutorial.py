@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The NINO3 sea-surface-temperature analysis of Torrence & Compo (1998) with the B200
+"""The NINO3 sea-surface-temperature analysis of Torrence & Compo (1998) with the H100
 engine: the call sequence a pycwt user writes (cf. docs/tutorial of the reference), minus the
 plotting.  Needs a CUDA device.
 
@@ -54,7 +54,7 @@ print("2-8 yr scale-averaged variance: max %.3f degC^2, 95%% level %.3f" % (std 
 eng = wavelet.default_engine()
 print("engine: %s, kernels of the cwt call above: %d launches" % (eng.version(), eng.last_launch_count()))
 
-# The same products without moving the coefficient array to the host (B200 extension):
+# The same products without moving the coefficient array to the host (an extension of this engine):
 r = wavelet.cwt_resident(dat_norm, dt, dj, s0, J, mother)
 assert np.allclose(r.global_power(), glbl_power, rtol=1e-12)
 assert np.allclose(r.scale_avg_power(2, 8), scale_avg, rtol=1e-12)

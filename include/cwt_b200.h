@@ -1,5 +1,5 @@
 /*
- * cwt_b200.h -- C ABI of the B200-native continuous-wavelet-transform engine.
+ * cwt_b200.h -- C ABI of the H100-native continuous-wavelet-transform engine.
  *
  * Drop-in boundary for the hot path of regeirk/pycwt.  The reference has no FFI
  * layer (it is pure Python); its "interface" for this path is the array math
@@ -61,7 +61,7 @@ const char *cwtb_version(void);
 /* Relative cut-off below which the analytic frequency response is treated as
  * zero when the per-scale band is pruned (default 1e-16: at the level of the fp64
  * rounding of the transform itself -- parity against the reference fixtures is the
- * same 5e-16 as with 1e-20, profiles/r1/eps_parity_r1.txt).  eps = 0 keeps every bin whose response
+ * same 5e-16 as with 1e-20).  eps = 0 keeps every bin whose response
  * is representable (the reference's own underflow-to-zero set). */
 int cwtb_set_band_eps(cwtb_ctx *ctx, double eps);
 /* Tolerance of the band-limited expansion path (replaces the per-scale inverse FFT of

@@ -1,8 +1,8 @@
 // Micro-benchmark: fp64 tensor-core MMA (mma.sync.m8n8k4.f64, SASS DMMA) against the fp64 FMA
-// pipe on B200: (1) DFMA only, (2) DMMA only, (3) both interleaved.  If time(3) ~ max(1, 2) the two
+// pipe on H100: (1) DFMA only, (2) DMMA only, (3) both interleaved.  If time(3) ~ max(1, 2) the two
 // run on different pipes and the tap sums of the expansion kernel (2 x taps of its ~38 fp64
 // instructions per point) can move to the tensor pipe.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o dmma_vs_dfma dmma_vs_dfma.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o dmma_vs_dfma dmma_vs_dfma.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void dmma(double &c0, double &c1, double a, double b) {
@@ -36,10 +36,10 @@ __global__ void __launch_bounds__(128) k(int mode, int iters, double *out) {
 }
 int main() {
   double *out;
-  cudaMalloc(&out, sizeof(double) * 148 * 16 * 128);
+  cudaMalloc(&out, sizeof(double) * 132 * 16 * 128);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  const int iters = 4000, ctas = 148 * 4;
+  const int iters = 4000, ctas = 132 * 4;
   for (int mode = 1; mode <= 3; ++mode) {
     k<<<ctas, 128>>>(mode, 10, out);
     cudaDeviceSynchronize();

@@ -1,8 +1,8 @@
-// Micro-benchmark: streaming bandwidth of the B200 memory system as a function of the working
+// Micro-benchmark: streaming bandwidth of the H100 memory system as a function of the working
 // set (L2-resident vs DRAM), for the access mixes of the two-kernel transform path:
 //   read-only, write-only, copy (read + write), and "read a small L2-resident buffer while
 //   streaming writes to a large one" (the second kernel with its intermediate kept in L2).
-// Build:  nvcc -O3 -gencode arch=compute_100a,code=sm_100a l2_bw.cu -o l2_bw
+// Build:  nvcc -O3 -gencode arch=compute_90a,code=sm_90a l2_bw.cu -o l2_bw
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -56,7 +56,7 @@ int main() {
   double2 *A, *B, *sink;
   CK(cudaMalloc(&A, big)); CK(cudaMalloc(&B, big)); CK(cudaMalloc(&sink, 64));
   CK(cudaMemset(A, 1, big)); CK(cudaMemset(B, 1, big));
-  const int grid = 148 * 8, block = 256;
+  const int grid = 132 * 8, block = 256;
   const size_t sizes_mb[] = {4, 8, 16, 24, 32, 48, 64, 96, 128, 256, 1024};
   printf("working set MB | read GB/s | write GB/s | write.cs GB/s | copy(r+w) GB/s | copy.cs GB/s\n");
   for (size_t mb : sizes_mb) {

@@ -1,4 +1,4 @@
-// Micro-benchmark: do warp shuffles and shared-memory accesses share one pipe on B200?
+// Micro-benchmark: do warp shuffles and shared-memory accesses share one pipe on H100?
 // (a) LDS.128+STS.128 only, (b) SHFL only, (c) both interleaved.  If time(c) ~ max(a, b) the
 // paths are independent and an FFT exchange can be split between them.
 #include <cstdio>
@@ -30,14 +30,14 @@ __global__ void k(int mode, int iters, double2 *out) {
 }
 int main() {
   double2 *out;
-  cudaMalloc(&out, sizeof(double2) * 148 * 8 * 256);
+  cudaMalloc(&out, sizeof(double2) * 132 * 8 * 256);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   for (int mode = 1; mode <= 3; ++mode) {
-    k<<<148 * 4, 256, 1024 * 16>>>(mode, 10, out);
+    k<<<132 * 4, 256, 1024 * 16>>>(mode, 10, out);
     cudaDeviceSynchronize();
     cudaEventRecord(e0);
-    k<<<148 * 4, 256, 1024 * 16>>>(mode, 2000, out);
+    k<<<132 * 4, 256, 1024 * 16>>>(mode, 2000, out);
     cudaEventRecord(e1);
     cudaEventSynchronize(e1);
     float ms;

@@ -1,5 +1,5 @@
 """Per-kernel device times of the paths bench.py's headline does not cover: wct / xwt / Monte-Carlo
-pair (config 4 geometry), resident reductions (config 2), fp32 configs.  One B200."""
+pair (config 4 geometry), resident reductions (config 2), fp32 configs.  One H100."""
 import os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -122,7 +122,7 @@ class Engine(object):
     def __init__(self, device=0, lib_path=None):
         self.lib = load_library(lib_path)
         if self.lib.cwtb_device_count() <= 0:
-            raise EngineError("no CUDA device visible: the B200 engine has no CPU fallback")
+            raise EngineError("no CUDA device visible: the CUDA engine has no CPU fallback")
         h = _P()
         rc = self.lib.cwtb_create(int(device), ctypes.byref(h))
         if rc != 0:

@@ -1,4 +1,4 @@
-"""Builds the CUDA engine (sm_100a) in-tree: pycwt_b200/libcwtb200.so.
+"""Builds the CUDA engine (sm_90a, H100) in-tree: pycwt_b200/libcwtb200.so.
 
 nvcc cross-compiles without a GPU.  The library is a plain C-ABI shared object
 (include/cwt_b200.h); no PyTorch involved.
@@ -16,7 +16,7 @@ DEPS = [os.path.join(HERE, "csrc", f) for f in
 LIB = os.path.join(HERE, "libcwtb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-std=c++17", "-O3", "-lineinfo",
-         "-gencode", "arch=compute_100a,code=sm_100a",
+         "-gencode", "arch=compute_90a,code=sm_90a",
          "-Xcompiler", "-fPIC", "-shared"]
 
 

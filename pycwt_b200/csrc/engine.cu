@@ -1,7 +1,7 @@
-// B200-native CWT engine: host planning, kernel launches and the C ABI of
+// H100-native CWT engine: host planning, kernel launches and the C ABI of
 // include/cwt_b200.h.  Device code is in kernels.cuh / fft_tile.cuh / cplx.cuh.
 //
-// Build (sm_100a):   nvcc -std=c++17 -O3 -lineinfo -gencode arch=compute_100a,code=sm_100a
+// Build (sm_90a):    nvcc -std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a
 //                         -Xcompiler -fPIC -shared engine.cu -o libcwtb200.so
 // Build (CPU emulation of the kernels, TESTS ONLY, never shipped/loaded by the package):
 //                    nvcc -std=c++17 -O2 -DCWTB_HOST_EMU ... -o libcwtb200_emu.so
@@ -175,7 +175,7 @@ struct cwtb_ctx {
   double expand_eps32 = 2e-7;    // fp32 engine
   int expand_mma = 1;            // fp64 expansion kernels with DMMA tap sums (CWTB_EXPAND_MMA=0: scalar kernel)
   int dense_margin = 2;          // pruned lengths within this many octaves of Np run as dense scales
-                                 // (CWTB_DENSE_MARGIN; config 2: 1.710 -> 1.686 ms, profiles/r2/sweep_e.txt)
+                                 // (CWTB_DENSE_MARGIN)
   int expand_min_log2R = 3;      // expansion needs Np / Nc >= 8 (CWTB_EXPAND_MIN_R: log2)
   Buf *ztmp = nullptr;           // intermediate of two_kernel_rows (set per stream; default Z)
   void *comm = nullptr;          // ncclComm_t of cwtb_comm_init (one rank per context)
@@ -184,17 +184,17 @@ struct cwtb_ctx {
   int group = 0;   // rows per two-kernel chunk; 0 = as many as fit in group_bytes of Z (CWTB_GROUP)
   size_t group_bytes = (size_t)512 << 20;
   size_t rows_chunk_bytes = (size_t)256 << 20;  // CWTB_ROWS_CHUNK_MB: launches of >= 8 waves beat keeping the
-                                                // intermediate in L2 (measured: wct 5.7 ms at 64 MiB, 4.8 ms at 256 MiB)
+                                                // intermediate in L2 (50 MB on H100)
   int l2_persist = 0;
   int direct_max_log2 = 13;
   int fused = 0;     // experimental: two-kernel scales through one persistent kernel (CWTB_FUSED=1)
   int ring = 3;      // Z ring slots of the fused kernel
   int pipe_ahead = 2;   // CWTB_FUSED=2: scales the first kernel runs in front of the second (CWTB_AHEAD)
-  int num_sms = 148;
-  int pf_dist = 148;   // PassB: L2 prefetch distance in tiles (CWTB_PF_DIST)
+  int num_sms = 132;
+  int pf_dist = 132;   // PassB: L2 prefetch distance in tiles, one per SM of an H100 (CWTB_PF_DIST)
   int gauss_rec = 1;   // dense Morlet scales: Gaussian by recurrence (CWTB_GAUSS_REC=0: exp per bin)
-  int pf_rows_a = 32, pf_rows_b = 32;   // the same for the batched row transforms (CWTB_PF_ROWS_A / _B; wct 4.35 -> 4.25 ms)
-  int pf_dist_a = 148;  // PassA (band): L2 prefetch distance in tiles (CWTB_PF_DIST_A)
+  int pf_rows_a = 32, pf_rows_b = 32;   // the same for the batched row transforms (CWTB_PF_ROWS_A / _B)
+  int pf_dist_a = 132;  // PassA (band): L2 prefetch distance in tiles (CWTB_PF_DIST_A)
   int k2_512_max_log2 = 16;  // largest K' that uses the 512-point second pass (CWTB_K2_512_MAX)
   int passb_rev = 1;    // second kernel walks the rows of a launch last-to-first (CWTB_PASSB_REV)
   int k2_band_log2 = 9; // second-pass length of the pruned two-kernel scales: 2^9 or 2^10 (CWTB_K2_BAND)
@@ -700,9 +700,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
       lmin = std::max(lmin, job.log2N - 14);          // weight tables of at most 2^14 phases
       double best = 1e300;
       // smallest expansion factor: 8.  Both kernels also run R = 4 (CWTB_EXPAND_MIN_R=2), but the coarse
-      // transform of Np/4 points is a two-kernel one itself: measured no gain (config 2 1.480 -> 1.496 ms,
-      // xwt 1.00 -> 1.18 ms; with the coarse transforms fanned out over streams 1.477 -> 1.466 ms, xwt
-      // unchanged, wct +0.7 %: profiles/r2/sweep_t_r4.txt)
+      // transform of Np/4 points is a two-kernel one itself, which eats what the shorter grid saves
       const int min_log2R = c->expand_min_log2R;
       for (int l = lmin; l <= lmin + 2 && job.log2N - l >= min_log2R; ++l) {
         double xi_b = 0;
@@ -713,7 +711,6 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
         if (xi_b > 0.25 && expand_gain(fam, s, klo, khi, kc, l, w, M_PI * w * (1.0 - xi_b)) > 64.0) continue;
         // cost model (us at Np = 2^20): the expansion kernel + the coarse transform.  Scalar kernel: its
         // fp64 work; tensor-core kernel: the W store until the DMMA steps of four taps exceed it
-        // (measured, profiles/r2/sweep_r.txt: 2.72 us with three DMMA steps of four taps, 3.33 with four, 4.1 with five)
         const int ksteps = job.log2N - l == 2 ? (w + 4) / 4 : (w + 3) / 4;   // R = 4 needs one more tap column
         const double xcost = mma ? std::max(2.72, 0.83 * ksteps) : 0.06 * (2 * w + 8);
         const double cost = xcost + (mma ? 18.0 : 12.0) * (double)(1ll << l) / (double)N;
@@ -1812,7 +1809,7 @@ const char *cwtb_version(void) {
 #ifdef CWTB_HOST_EMU
   return "cwt_b200 0.1 (host emulation build - tests only)";
 #else
-  return "cwt_b200 0.1 (sm_100a)";
+  return "cwt_b200 0.1 (sm_90a)";
 #endif
 }
 

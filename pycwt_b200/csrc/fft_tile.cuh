@@ -211,9 +211,9 @@ struct TileBarrier {
 
 // Ampere-style asynchronous copy global -> shared of one element (8 or 16 bytes) that bypasses the
 // register file: a thread can have its whole share of a tile in flight at once instead of
-// compiler-sized batches of loads followed by stores.  Measured on B200 for the first kernel of the
-// band scales (profiles/r2/split_b.txt): SLOWER than batches of four LDG.128 + STS.128 (13.6 -> 14.8 us
-// per row; the element-wise LDGSTS scatter costs more than the extra loads in flight gain): off.  cp_async_wait() makes the thread's own
+// compiler-sized batches of loads followed by stores.  Off by default for the first kernel of the band
+// scales: the element-wise LDGSTS scatter costs more than the extra loads in flight gain, against
+// batches of four LDG.128 + STS.128 (CWTB_PASSA_ASYNC=1 builds it in).  cp_async_wait() makes the thread's own
 // copies visible to itself; the CTA barrier that follows publishes them.  Host emulation: plain copy.
 #ifndef CWTB_PASSA_ASYNC
 #define CWTB_PASSA_ASYNC 0

@@ -66,8 +66,8 @@ HD double amp_eval(const Fam &fp, double s, int k) {
 
 // the same in the engine's arithmetic: the fp32 engine forms f = s*w in double (w spans 2^18 bins)
 // and evaluates the power and the exponential in float (the caller keeps orders above 8 in double:
-// their powers overflow float).  fp64 instructions run at half the fp32 rate on B200: one double exp per band product made
-// the band-product launches and the generating first kernel fp64-pipe bound in the fp32 engine.
+// their powers overflow float).  fp64 instructions run at half the fp32 rate on H100: one double exp per band product
+// would make the band-product launches and the generating first kernel fp64-pipe bound in the fp32 engine.
 template <typename T> HD T amp_eval_t(const Fam &fp, double s, int k) {
   if constexpr (sizeof(T) == 8) {
     return amp_eval(fp, s, k);
@@ -486,9 +486,8 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
 };
 
 // ---- Body: first kernel of the two-kernel path: K1-point transforms over r1 --------
-// (Measured and dropped, profiles/r2/sweep_k.txt: band scales that evaluate x^ * conj(psi^) * norm while the
-// tile is filled instead of reading the band buffer -- the first kernel of Np/K' = 2 scales got 55 % slower,
-// more than the band-product launch it saves: config 5 7.83 -> 7.92 ms, config 3 Paul 0.283 -> 0.321 ms.)
+// (Band scales read the band buffer rather than evaluate x^ * conj(psi^) * norm while the tile is filled:
+// the evaluation slows the first kernel of Np/K' = 2 scales by more than the band-product launch it saves.)
 enum { MODE_DENSE = 0, MODE_BAND = 1, MODE_REAL = 2, MODE_CPLX = 3 };
 
 template <typename T> struct PassAArgs {
@@ -787,9 +786,8 @@ template <typename T> struct ExpandArgs {
 // coarse samples in registers and walks its run (fully unrolled: window slots are compile-time
 // registers): one new sample (shared-memory read, the same address for the lanes of a run) and one
 // 16-byte store per output; lanes run over rho, so a warp stores min(R, 32) consecutive points
-// per run.  Measured on B200 (profiles/r2): the kernel is bound by the fp64 pipe (2 taps + ~12
-// other fp64 instructions per point at 64 lanes per SM and clock); 8 accumulator chains and 4 CTAs
-// per SM keep that pipe 63 % busy, longer runs or fewer chains were slower.
+// per run.  The kernel is bound by the fp64 pipe (2 taps + ~12 other fp64 instructions per point);
+// 8 accumulator chains and 4 CTAs per SM give that pipe the parallelism it needs.
 template <typename T, int TAPS, int EPI = EPI_STORE> struct ExpandBody {
   static constexpr int NTB = TileCfg<T>::NT;
   static constexpr int NT = NTB;
@@ -883,22 +881,20 @@ template <typename T, int TAPS, int EPI = EPI_STORE> struct ExpandBody {
 // The tap sum  acc[m][rho] = sum_t c[m + t - (taps/2 - 1)] * h[t][rho]  is a Toeplitz product: for 8
 // consecutive coarse positions m and 8 consecutive phases rho it is an (8 x taps) x (taps x 8) real
 // matrix product per component, i.e. taps/4 `mma.sync.m8n8k4.f64` (SASS DMMA.8x8x4) for the real and
-// as many for the imaginary part.  DMMA shares the fp64 pipe with DFMA on B200 (profiles/r2/
-// dmma_vs_dfma.txt: times add) but moves 20 % more FMAs through it, and the accumulation happens
-// inside the instruction: the scalar kernel's 2 x taps DFMA + 6 DADD per point (of ~38 fp64
-// instructions, the pipe that bounds it) become taps/2 DMMA per 64 points.
+// as many for the imaginary part.  On H100 the fp64 tensor-core rate is twice the DFMA rate, and the
+// accumulation happens inside the instruction: the scalar kernel's 2 x taps DFMA + 6 DADD per point
+// (of ~38 fp64 instructions, the pipe that bounds it) become taps/2 DMMA per 64 points.
 //   A fragment (8 x 4, row m, column t):  lane holds c[m0 + lane/4 + 4 ks + lane%4]   (shared memory)
 //   B fragment (4 x 8, row t, column rho): lane holds h[4 ks + lane%4][rho0 + lane/4] (registers)
 //   C fragment (8 x 8): lane holds acc[m0 + lane/4][rho0 + 2 (lane%4) + {0, 1}]: two adjacent outputs,
-//                       stored as one 32-byte access when the row is 32-byte aligned.
+//                       stored as two 16-byte streaming stores (sm_90 has no 32-byte store).
 // A warp owns 8 phases and a run of L coarse positions; a CTA (4 warps) covers min(R, 32) phases
 // x 4 L / (min(R, 32) / 8) coarse positions = 32 L outputs.  Tap counts 10 and 14 are padded to 12 / 16
 // with zero weights.  Not part of the host-emulation build (warp-collective instruction): the
 // emulated tests run the scalar ExpandBody, which stays the fp32 engine's kernel and the fallback.
 // (An fp32 counterpart on 3xTF32 -- x = x_hi + x_lo, three mma.sync.m16n8k8.tf32 per component and eight
-// taps -- gives the same 5e-7 parity but runs SLOWER than the scalar fp32 kernel, 3.54 vs 2.74 ms on
-// config 5: the legacy HMMA path of sm_100a issues ~15 cycles per MMA and SM here, no faster than FFMA.
-// Measured and dropped: profiles/r2/sweep_x_tf32x3_expansion_dropped.txt.)
+// taps -- gives the same 5e-7 parity but needs three MMAs and the hi/lo splits per tap pair; the fp32
+// engine keeps the scalar kernel.)
 __device__ __forceinline__ void dmma884(double &c0, double &c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
@@ -971,7 +967,6 @@ template <int TAPS, int EPI = EPI_STORE> struct ExpandMmaBody {
       const V stepb = nroot(a.nt, (kc * (unsigned)MB) << log2R);
       const V *run = sm + j * Lr + (R4 ? 2 * g : g) + q;
       V *rowp = a.W + (size_t)d.row * a.n0;
-      const bool wide = (((size_t)d.row * (size_t)a.n0) & 1) == 0;   // 32-byte aligned pairs
 #pragma unroll 4
       for (int mb = 0; mb < Lr / MB; ++mb) {
         if (ms + MB * mb >= Nc) break;                // warp-uniform: short coarse grids end inside the run
@@ -996,9 +991,6 @@ template <int TAPS, int EPI = EPI_STORE> struct ExpandMmaBody {
             if (two) x1 = cmul(p[1], cconj(x1));
             p[0] = x0;
             if (two) p[1] = x1;
-          } else if (wide && two) {
-            asm volatile("st.global.cs.v4.f64 [%0], {%1,%2,%3,%4};" ::"l"(p), "d"(x0.x), "d"(x0.y), "d"(x1.x), "d"(x1.y)
-                         : "memory");
           } else {
             st_stream(p, x0);
             if (two) st_stream(p + 1, x1);

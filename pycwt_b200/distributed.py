@@ -252,8 +252,8 @@ def scale_rows(n_scales, rank, world, layout='cyclic'):
 def cwt_scale_sharded(signal, dt, scales, family, param, precision, engine, comm=None, device=None,
                       fetch=False, layout='cyclic'):
     """One long signal, scales partitioned over the ranks (SURVEY 8e row 2).  Every rank
-    holds the signal and runs its own forward transform (0.05 ms at N = 2^20 -- cheaper than
-    broadcasting the 16 MiB spectrum), then transforms only its scales (`scale_rows`), which stay
+    holds the signal and runs its own forward transform (cheaper than broadcasting the 16 MiB
+    spectrum), then transforms only its scales (`scale_rows`), which stay
     resident in that GPU's HBM.  No collective on the data path; the per-scale global power
     (mean_n |W|^2, [S]) is all-gathered so that every rank sees the whole spectrum.
 

@@ -1,7 +1,7 @@
 """Device-resident transform and its derived products (SURVEY 8f rank 2).
 
 `pycwt.cwt` has to hand the caller a complex128 array of S x N coefficients; at the north-star
-size that is 4.3 GB over PCIe for 2.3 ms of GPU work.  What the reference's sample scripts
+size that is 4.3 GB over PCIe for a few ms of GPU work.  What the reference's sample scripts
 then do with W (pycwt/sample/simple_sample.py:64-96) are reductions of |W|^2:
 
     power        = |W|^2                      (optionally rectified: / s_j, Liu et al. 2007,

@@ -1,5 +1,5 @@
 """Continuous wavelet transform API with the signatures of pycwt/wavelet.py, executed by
-the B200 CUDA engine (pycwt_b200/csrc, C ABI in include/cwt_b200.h).
+the H100 CUDA engine (pycwt_b200/csrc, C ABI in include/cwt_b200.h).
 
 Division of labour (SURVEY 8a):
   * O(S) scalar work -- scale resolution, cone of influence, chi-square significance,

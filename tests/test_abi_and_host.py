@@ -32,7 +32,7 @@ def test_library_exports_every_declared_symbol(lib):
         assert hasattr(lib, s), "symbol %s declared in include/cwt_b200.h is not exported" % s
     # and the ctypes binding declares a prototype for each of them
     assert set(syms) == set(_engine._SIGNATURES), set(syms) ^ set(_engine._SIGNATURES)
-    assert b"sm_100a" in lib.cwtb_version()
+    assert b"sm_90a" in lib.cwtb_version()
 
 
 def test_no_cpu_fallback_without_device(lib):

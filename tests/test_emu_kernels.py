@@ -2,9 +2,9 @@
 
 tests/_emu/libcwtb200_emu.so is the SAME kernel source compiled with -DCWTB_HOST_EMU, where
 every CTA runs as a plain C++ loop over (phase, thread).  It exists so that index maths,
-plans, pruning and epilogues can be checked where no GPU is present (the build container).
+plans, pruning and epilogues can be checked where no GPU is present.
 It is test infrastructure only: the package never loads it (pycwt_b200._engine.LIB_PATH is the
-sm_100a library) and these tests patch the loader path only for their own duration."""
+sm_90a library) and these tests patch the loader path only for their own duration."""
 import numpy as np
 import pytest
 
