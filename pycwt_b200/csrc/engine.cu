@@ -89,6 +89,13 @@ __global__ void __launch_bounds__(BodyNT<Body>::value, BodyMinB<Body>::value) k_
   extern __shared__ __align__(16) unsigned char smraw[];
   run_phases<Body, 0>(a, smraw);
 }
+// persistent kernel of a body with run_tiles(): `total` work items of which `gm` per row
+template <class Body>
+__global__ void __launch_bounds__(Body::NTB, Body::MINB) k_persist(const __grid_constant__ typename Body::Args a,
+                                                                   unsigned gm, unsigned total) {
+  extern __shared__ __align__(16) unsigned char smraw[];
+  Body::run_tiles(a, gm, total, (typename Body::V *)smraw);
+}
 #endif
 
 // ======================================================================================
@@ -176,7 +183,7 @@ struct cwtb_ctx {
   int expand_mma = 1;            // fp64 expansion kernels with DMMA tap sums (CWTB_EXPAND_MMA=0: scalar kernel)
   int dense_margin = 2;          // pruned lengths within this many octaves of Np run as dense scales
                                  // (CWTB_DENSE_MARGIN)
-  int expand_min_log2R = 3;      // expansion needs Np / Nc >= 8 (CWTB_EXPAND_MIN_R: log2)
+  int expand_min_log2R = 0;      // log2 of the smallest Np / Nc (CWTB_EXPAND_MIN_R); 0: by kernel, see build_job
   Buf *ztmp = nullptr;           // intermediate of two_kernel_rows (set per stream; default Z)
   void *comm = nullptr;          // ncclComm_t of cwtb_comm_init (one rank per context)
   int comm_world = 1, comm_rank = 0;
@@ -699,9 +706,11 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
       int lmin = std::max(6, ilog2((unsigned long long)std::max<long long>(need, 1)));
       lmin = std::max(lmin, job.log2N - 14);          // weight tables of at most 2^14 phases
       double best = 1e300;
-      // smallest expansion factor: 8.  Both kernels also run R = 4 (CWTB_EXPAND_MIN_R=2), but the coarse
-      // transform of Np/4 points is a two-kernel one itself, which eats what the shorter grid saves
-      const int min_log2R = c->expand_min_log2R;
+      // smallest expansion factor: 4 for the tensor-core kernel, 8 for the scalar one.  With R = 4 config 2
+      // expands 16 more rows (an exact dense row costs more than an expansion row plus its two-kernel
+      // coarse transform of Np/4 points): 2.866 against 2.925 ms per step on H100 at 400 W, spread 0.012 ms.
+      // The scalar kernel's trade-off at R = 4 has not been measured on H100.
+      const int min_log2R = c->expand_min_log2R ? c->expand_min_log2R : (mma ? 2 : 3);
       for (int l = lmin; l <= lmin + 2 && job.log2N - l >= min_log2R; ++l) {
         double xi_b = 0;
         int w = expand_taps((double)hw / (double)(1ll << l), xeps, precision != CWTB_F64, max_taps, &xi_b);
@@ -1382,6 +1391,42 @@ static size_t band_chunk_elems(const cwtb_ctx *c, const Job &job, int G) {
   return bchunk;
 }
 
+#ifndef CWTB_HOST_EMU
+// one CTA per resident slot (occupancy x SMs), each looping over the rows x gm tiles of the launch
+template <class Body>
+static int launch_persistent(cwtb_ctx *c, unsigned gm, unsigned rows, const typename Body::Args &a) {
+  if (gm == 0 || rows == 0) return 0;
+  auto kern = k_persist<Body>;
+  const void *fn = (const void *)kern;
+  if (!c->configured.count(fn)) {
+    RT(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Body::SMEM));
+    c->configured.insert(fn);
+  }
+  int occ = 0;
+  RT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, Body::NTB, Body::SMEM));
+  if (occ < 1) return fail(c, CWTB_ERR_CUDA, "persistent kernel does not fit on an SM");
+  const unsigned long long total = (unsigned long long)gm * rows;
+  if (total > 0xffffffffull) return fail(c, CWTB_ERR_ARG, "too many tiles in one launch");
+  const unsigned grid = (unsigned)std::min<unsigned long long>(total, (unsigned long long)occ * c->num_sms);
+  int ev = -1;
+  if (c->profiling) {
+    ev = (int)c->prof.size() * 2;
+    while ((int)c->prof_events.size() < ev + 2) {
+      cudaEvent_t e;
+      RT(cudaEventCreate(&e));
+      c->prof_events.push_back(e);
+    }
+    c->prof.push_back({std::string(c->prof_tag) + body_name(__PRETTY_FUNCTION__), grid, rows, ev});
+    RT(cudaEventRecord(c->prof_events[ev], c->cur));
+  }
+  kern<<<grid, Body::NTB, Body::SMEM, c->cur>>>(a, gm, (unsigned)total);
+  RT(cudaGetLastError());
+  if (ev >= 0) RT(cudaEventRecord(c->prof_events[ev + 1], c->cur));
+  c->launches++;
+  return 0;
+}
+#endif
+
 template <typename T, int TAPS>
 static int launch_expand_t(cwtb_ctx *c, const ExpandArgs<T> &a, int rows, int min_log2Nc) {
   using B = ExpandBody<T, TAPS>;
@@ -1397,8 +1442,8 @@ static int launch_expand_t(cwtb_ctx *c, const ExpandArgs<T> &a, int rows, int mi
       // tiles per row: N / (32 L); a row whose coarse grid is shorter than one run (Nc < L, R > 32) needs
       // one tile per 32 phases instead
       const unsigned gm = a.N / (32u * std::min<unsigned>(ExpandMmaBody<TAPS>::L, 1u << min_log2Nc));
-      if (a.epi == EPI_MULCONJ) return launch<ExpandMmaBody<TAPS, EPI_MULCONJ>>(c, gm, rows, a);
-      return launch<ExpandMmaBody<TAPS>>(c, gm, rows, a);
+      if (a.epi == EPI_MULCONJ) return launch_persistent<ExpandMmaBody<TAPS, EPI_MULCONJ>>(c, gm, rows, a);
+      return launch_persistent<ExpandMmaBody<TAPS>>(c, gm, rows, a);
     }
   }
 #endif

@@ -887,7 +887,8 @@ template <typename T, int TAPS, int EPI = EPI_STORE> struct ExpandBody {
 //   A fragment (8 x 4, row m, column t):  lane holds c[m0 + lane/4 + 4 ks + lane%4]   (shared memory)
 //   B fragment (4 x 8, row t, column rho): lane holds h[4 ks + lane%4][rho0 + lane/4] (registers)
 //   C fragment (8 x 8): lane holds acc[m0 + lane/4][rho0 + 2 (lane%4) + {0, 1}]: two adjacent outputs,
-//                       stored as two 16-byte streaming stores (sm_90 has no 32-byte store).
+//                       stored as two 16-byte streaming stores (sm_90 has no 32-byte store) after an
+//                       exchange with the neighbour lane, so that each store instruction fills whole sectors.
 // A warp owns 8 phases and a run of L coarse positions; a CTA (4 warps) covers min(R, 32) phases
 // x 4 L / (min(R, 32) / 8) coarse positions = 32 L outputs.  Tap counts 10 and 14 are padded to 12 / 16
 // with zero weights.  Not part of the host-emulation build (warp-collective instruction): the
@@ -910,40 +911,80 @@ template <int TAPS, int EPI = EPI_STORE> struct ExpandMmaBody {
 #endif
   static constexpr int L = CWTB_MMA_L;              // coarse positions per warp run (8 L outputs per warp)
   static constexpr int KS = (TAPS + 3) / 4;         // k-steps of four taps
-  static constexpr int KS4 = (TAPS + 4) / 4;        // R = 4: one more tap column (see body<.., true>)
+  static constexpr int KS4 = (TAPS + 4) / 4;        // R = 4: one more tap column (see compute<true>)
   static constexpr int OUT_PER_CTA = 32 * L;
   static constexpr int STAGE = 8 * L + 4 * KS4;     // staged coarse samples incl. halo (R = 4: 4 runs of 2 L)
-  static constexpr int NPHASE = 2;
-  static constexpr size_t SMEM = (size_t)STAGE * sizeof(V);
-  template <int PH> __device__ static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
-    const ScaleDesc &d = a.descs[a.first + by];
-    if (a.log2N - d.ip_log2Nc == 2) body<PH, true>(a, d, bx, tid, (V *)smraw);
-    else body<PH, false>(a, d, bx, tid, (V *)smraw);
+  // two stages: the next tile's coarse samples arrive while this one computes and stores
+  static constexpr size_t SMEM = 2 * (size_t)STAGE * sizeof(V);
+  // work item w of a launch over `gm` tiles per row: row w / gm, tile w % gm
+  struct Tile {
+    const ScaleDesc *d;
+    int log2R, Nc, wpb, MT, m0, rb;
+    bool r4, live;
+  };
+  __device__ static Tile tile(const Args &a, unsigned w, unsigned gm) {
+    Tile t;
+    const int bx = (int)(w % gm);
+    t.d = &a.descs[a.first + (int)(w / gm)];
+    t.log2R = a.log2N - t.d->ip_log2Nc;
+    t.r4 = t.log2R == 2;
+    const int R = 1 << t.log2R;
+    t.Nc = 1 << t.d->ip_log2Nc;
+    t.wpb = t.r4 ? 1 : ((R < 32 ? R : 32) >> 3);   // warps side by side in rho: 1, 2 or 4
+    t.MT = (4 / t.wpb) * (t.r4 ? 2 * L : L);        // coarse positions per tile: 4 / wpb warp runs
+    const int mtiles = (t.Nc + t.MT - 1) / t.MT;
+    t.rb = bx / mtiles;
+    t.m0 = (bx % mtiles) * t.MT;
+    t.live = !(t.rb * 32 >= R && t.rb > 0);         // short rows use the first tiles of a row only
+    return t;
+  }
+  // the tile's coarse samples incl. halo, periodic on the coarse grid: one 16-byte cp.async each
+  __device__ static void load(const Args &a, const Tile &t, V *sm) {
+    if (!t.live) return;
+    const V *c = a.C + t.d->ip_coff;
+    const int n = t.MT + 4 * (t.r4 ? KS4 : KS);
+    for (int i = (int)threadIdx.x; i < n; i += NT) cp_async(&sm[i], &c[(t.m0 - (TAPS / 2 - 1) + i) & (t.Nc - 1)]);
+  }
+  // Persistent: CTA b works on items b, b + gridDim.x, ... of the launch's rows x gm tiles.  Each tile
+  // reads ~1 K coarse samples and writes 4096 outputs; prefetching the next tile's samples keeps the
+  // store stream going where a fresh CTA would first wait for its loads.
+  __device__ static void run_tiles(const Args &a, unsigned gm, unsigned total, V *sm) {
+    unsigned w = blockIdx.x;
+    Tile cur = tile(a, w, gm);
+    load(a, cur, sm);
+    for (int st = 0; w < total; w += gridDim.x, st ^= 1) {
+      cp_async_wait();
+      __syncthreads();   // this tile's samples are in, and every warp is done with the other stage
+      const unsigned wn = w + gridDim.x;
+      Tile nxt = cur;
+      if (wn < total) {
+        nxt = tile(a, wn, gm);
+        load(a, nxt, sm + (st ^ 1) * STAGE);
+      }
+      if (cur.live) {
+        if (cur.r4) compute<true>(a, cur, sm + st * STAGE);
+        else compute<false>(a, cur, sm + st * STAGE);
+      }
+      cur = nxt;
+    }
   }
   // R4 = false (R >= 8): MMA rows = 8 consecutive coarse positions, columns = 8 consecutive phases.
   // R4 = true  (R == 4): the 8 columns are 2 coarse positions x 4 phases, the rows step by two coarse
   //   positions: acc[m0 + 2 i + dm][rho] = sum_t' c[m0 + 2 i + t' - (taps/2 - 1)] * h[t' - dm][rho],
   //   t' < taps + 1 (B holds the weights shifted by dm, zero outside).  A warp then covers 16 coarse
   //   positions per MMA block and runs over 2 L of them: the same 8 L outputs per warp.
-  template <int PH, bool R4>
-  __device__ static void body(const Args &a, const ScaleDesc &d, int bx, int tid, V *sm) {
+  template <bool R4>
+  __device__ static void compute(const Args &a, const Tile &tl, const V *sm) {
     constexpr int KSr = R4 ? KS4 : KS;
     constexpr int Lr = R4 ? 2 * L : L;              // coarse positions per warp run
     constexpr int MB = R4 ? 16 : 8;                 // coarse positions per MMA block
-    const int log2R = a.log2N - d.ip_log2Nc;
+    const ScaleDesc &d = *tl.d;
+    const int log2R = tl.log2R;
     const int R = 1 << log2R;
-    const int Nc = 1 << d.ip_log2Nc;
-    const int wpb = R4 ? 1 : ((R < 32 ? R : 32) >> 3);   // warps side by side in rho: 1, 2 or 4
-    const int nrun = 4 / wpb;                       // runs per CTA
-    const int MT = nrun * Lr;
-    const int mtiles = (Nc + MT - 1) / MT;
-    const int mt = bx % mtiles, rb = bx / mtiles;
-    if (rb * 32 >= R && rb > 0) return;             // short rows use the first tiles of the launch only
-    const int m0 = mt * MT;
-    if constexpr (PH == 0) {
-      const V *c = a.C + d.ip_coff;
-      for (int i = tid; i < MT + 4 * KSr; i += NT) sm[i] = ldg(&c[(m0 - (TAPS / 2 - 1) + i) & (Nc - 1)]);
-    } else {
+    const int Nc = tl.Nc;
+    const int wpb = tl.wpb, rb = tl.rb, m0 = tl.m0;
+    {
+      const int tid = (int)threadIdx.x;
       const int wid = tid >> 5, lane = tid & 31;
       const int g = lane >> 2, q = lane & 3;
       const int pb = wid % wpb, j = wid / wpb;
@@ -979,21 +1020,29 @@ template <int TAPS, int EPI = EPI_STORE> struct ExpandMmaBody {
         }
         const int m = ms + MB * mb + mlane;
         const long long n = ((long long)m << log2R) + rlane;
-        V x0 = cmul(make_double2(cr0, ci0), tw0);
-        V x1 = cmul(make_double2(cr1, ci1), tw1);
+        const V x0 = cmul(make_double2(cr0, ci0), tw0);
+        const V x1 = cmul(make_double2(cr1, ci1), tw1);
         tw0 = cmul(tw0, stepb);
         tw1 = cmul(tw1, stepb);
-        if (m < Nc && n < a.n0) {
-          V *p = rowp + n;
-          const bool two = n + 1 < a.n0;
+        // Lanes q and q^1 hold outputs n .. n+3 (same m).  Stored as they sit, each 16-byte store
+        // instruction fills every 32-byte sector half (measured: half the write rate).  The pair swaps
+        // one value so that each instruction writes whole sectors: the even lane stores n, n+2, the odd
+        // lane n+1, n+3.
+        const bool odd = q & 1;
+        const V snd = odd ? x0 : x1;
+        const V rcv = make_double2(__shfl_xor_sync(0xffffffffu, snd.x, 1), __shfl_xor_sync(0xffffffffu, snd.y, 1));
+        const long long na = odd ? n - 1 : n;
+        V ya = odd ? rcv : x0;                      // output na
+        V yb = odd ? x1 : rcv;                      // output na + 2
+        if (m < Nc) {
+          V *p = rowp + na;
+          const bool sa = na < a.n0, sb = na + 2 < a.n0;
           if (EPI == EPI_MULCONJ) {
-            x0 = cmul(p[0], cconj(x0));
-            if (two) x1 = cmul(p[1], cconj(x1));
-            p[0] = x0;
-            if (two) p[1] = x1;
+            if (sa) p[0] = cmul(p[0], cconj(ya));
+            if (sb) p[2] = cmul(p[2], cconj(yb));
           } else {
-            st_stream(p, x0);
-            if (two) st_stream(p + 1, x1);
+            if (sa) st_stream(p, ya);
+            if (sb) st_stream(p + 2, yb);
           }
         }
       }
