@@ -79,6 +79,19 @@ int cwtb_set_expand_eps(cwtb_ctx *ctx, double eps_fp64, double eps_fp32);
  * the smoothing filter of wct / smooth / wct_mc then is circular at the rows' own length, as in
  * the reference.  Power-of-two lengths are unaffected. */
 int cwtb_set_padding(cwtb_ctx *ctx, int pad_to_pow2);
+/* Arithmetic of cwtb_xwt, cwtb_wct, cwtb_wct_mc and cwtb_wct_mc_seeded: CWTB_F64 (what a new
+ * context starts with) or CWTB_F32.  In fp32 the two transforms run in the fp32 engine (its band
+ * and expansion tolerances, relative error <= 1e-5 each) and the coherence products, the time
+ * smoothing and the scale boxcar are computed in float; the device holds half the bytes per
+ * scale-point.  Host inputs stay double: the series and host surrogates are rounded to float on
+ * the device, and device-drawn surrogates are drawn in double and rounded.  Outputs keep their
+ * types: W12 complex128 (after an fp32 cwtb_xwt the resident job is an fp32 one; cwtb_get_w widens
+ * it on the device), WCT and aWCT double, histogram counts int64, binned from the coherence as
+ * double.  WCT differs from fp64 by at most 2.5e-4 (DESIGN.md section 6).  Un-padded transforms
+ * (cwtb_set_padding(ctx, 0) with n0 not a power of two) have no fp32 path: the calls then return
+ * CWTB_ERR_UNSUPPORTED.  cwtb_smooth always runs in fp64.  Returns CWTB_ERR_ARG for any other
+ * value. */
+int cwtb_set_coherence_precision(cwtb_ctx *ctx, int precision);
 /* Time-smoothing filter of cwtb_smooth / cwtb_wct / cwtb_wct_mc.  Default (table == NULL): the
  * Gaussian exp(-0.5 (s/dt)^2 k^2) of Morlet.smooth (pycwt/mothers.py:83-91).  With a table
  * [n_rows][n] of real frequency responses (n = the transform length of the rows: next power of

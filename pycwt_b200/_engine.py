@@ -32,6 +32,7 @@ _SIGNATURES = {
     "cwtb_set_band_eps": (_I, [_P, _D]),
     "cwtb_set_expand_eps": (_I, [_P, _D, _D]),
     "cwtb_set_padding": (_I, [_P, _I]),
+    "cwtb_set_coherence_precision": (_I, [_P, _I]),
     "cwtb_set_smooth_filter": (_I, [_P, _P, _I, _I64]),
     "cwtb_host_alloc": (_I, [_P, ctypes.c_size_t, ctypes.POINTER(_P)]),
     "cwtb_host_free": (_I, [_P, _P]),
@@ -459,7 +460,8 @@ class Engine(object):
 
     # ---- cross wavelet / coherence ------------------------------------------------------
     @_locked
-    def xwt(self, y1, y2, dt, scales, family, param):
+    def xwt(self, y1, y2, dt, scales, family, param, precision=F64):
+        """W12 = W1 conj(W2) (complex128 whatever `precision`, the arithmetic of the call)."""
         y1 = np.ascontiguousarray(y1, dtype=np.float64)
         y2 = np.ascontiguousarray(y2, dtype=np.float64)
         if y1.shape != y2.shape or y1.ndim != 1:
@@ -467,6 +469,7 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         out = self.result_array((sj.size, y1.size), np.complex128)
         with self.lock:
+            self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_xwt(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), _ptr(sj),
                                           sj.size, int(family), float(param), _ptr(out)))
             self._resident_n0 = y1.size
@@ -474,7 +477,7 @@ class Engine(object):
         return out
 
     @_locked
-    def wct(self, y1, y2, dt, dj, scales, family, param, boxcar_len, want_angle=True):
+    def wct(self, y1, y2, dt, dj, scales, family, param, boxcar_len, want_angle=True, precision=F64):
         y1 = np.ascontiguousarray(y1, dtype=np.float64)
         y2 = np.ascontiguousarray(y2, dtype=np.float64)
         if y1.shape != y2.shape or y1.ndim != 1:
@@ -483,6 +486,7 @@ class Engine(object):
         WCT = self.result_array((sj.size, y1.size), np.float64)
         aWCT = self.result_array((sj.size, y1.size), np.float64) if want_angle else None
         with self.lock:
+            self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_wct(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
                                           _ptr(sj), sj.size, int(family), float(param),
                                           int(boxcar_len), _ptr(WCT),
@@ -508,7 +512,7 @@ class Engine(object):
 
     @_locked
     def wct_mc(self, noise, dt, dj, scales, family, param, boxcar_len, mask, maxscale, nbins,
-               hist):
+               hist, precision=F64):
         noise = np.ascontiguousarray(noise, dtype=np.float64)
         assert noise.ndim == 3 and noise.shape[1] == 2
         sj = np.ascontiguousarray(scales, dtype=np.float64)
@@ -516,6 +520,7 @@ class Engine(object):
         assert mask.shape == (sj.size, noise.shape[2])
         assert hist.dtype == np.int64 and hist.flags.c_contiguous and hist.shape == (sj.size, nbins)
         with self.lock:
+            self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_wct_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2],
                                              float(dt), float(dj), _ptr(sj), sj.size, int(family),
                                              float(param), int(boxcar_len), _ptr(mask),
@@ -525,13 +530,14 @@ class Engine(object):
 
     @_locked
     def wct_mc_seeded(self, seed, first_pair, n_pairs, n0, dt, scales, family, param, boxcar_len, mask,
-                      maxscale, nbins, hist):
+                      maxscale, nbins, hist, precision=F64):
         """Monte-Carlo coherence histograms of `n_pairs` surrogate pairs drawn on the device
         (Philox stream keyed by (seed, pair number)); accumulated into `hist`."""
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         assert mask.shape == (sj.size, int(n0))
         assert hist.dtype == np.int64 and hist.flags.c_contiguous and hist.shape == (sj.size, nbins)
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_pair), int(n_pairs),
                                                 int(n0), float(dt), _ptr(sj), sj.size, int(family),
                                                 float(param), int(boxcar_len), _ptr(mask), int(maxscale),

@@ -167,6 +167,8 @@ struct cwtb_ctx {
   int pad_pow2 = 1;              // 1: transform length = next power of two (reference default,
                                  // helpers.py:27-30); 0: the signal's own length (pyfftw policy,
                                  // helpers.py:15-19) -- cwtb_set_padding
+  int coh_precision = 0;         // arithmetic of xwt / wct / wct_mc: CWTB_F64 or CWTB_F32
+                                 // (cwtb_set_coherence_precision)
   std::map<unsigned, BluePlan> blue;
   long long serial = 0;          // counts transforms: identifies what is resident (cwtb_job_serial)
   int two_streams = 1;           // CWTB_STREAMS=1 disables the overlap
@@ -2311,59 +2313,67 @@ static int upload_window(cwtb_ctx *c, int K) {
   return upload_doubles(c, c->win, w);
 }
 
-// Morlet.smooth, time part (mothers.py:83-93), in place on X[S][n0] (complex128, device):
+extern "C++" {   // templates of the coherence pipeline, one instantiation per engine type
+// Morlet.smooth, time part (mothers.py:83-93), in place on X[S][n0] (complex, engine type T, device):
 // forward transform of the zero-padded rows with the Gaussian folded into its output pass,
 // inverse transform trimmed to n0.
-static int smooth_time(cwtb_ctx *c, double2 *X, int S, long long n0, unsigned N, const double *d_g) {
-  int e = ensure(c, c->F, (size_t)S * N * sizeof(double2));
+template <typename T>
+static int smooth_time(cwtb_ctx *c, cx<T> *X, int S, long long n0, unsigned N, const double *d_g) {
+  int e = ensure(c, c->F, (size_t)S * N * sizeof(cx<T>));
   if (e) return e;
-  double2 *F = (double2 *)c->F.p;
+  cx<T> *F = (cx<T> *)c->F.p;
   if (N < 2) return 0;  // single sample: filter is exp(0) = 1
   const bool table = c->filt_rows > 0;     // caller-supplied responses instead of Morlet's Gaussian
   if (table && (c->filt_rows != S || c->filt_n != (long long)N))
     return fail(c, CWTB_ERR_STATE, "smoothing filter table does not match the rows / transform length of this call");
   if ((N & (N - 1)) != 0) {
     // un-padded mode: circular filter at the rows' own length (N == n0), Bluestein transforms
-    if ((e = blue_rows(c, X, 0, n0, F, N, N, S, -1, 1.0, N))) return e;
-    if (table) {
-      FilterMulArgs fa{F, (const double *)c->filt.p, (long long)N, N, 1.0 / (double)N};
-      if ((e = launch<FilterMulBody>(c, (N + NT - 1) / NT, S, fa))) return e;
+    if constexpr (sizeof(T) == 8) {
+      if ((e = blue_rows(c, X, 0, n0, F, N, N, S, -1, 1.0, N))) return e;
+      if (table) {
+        FilterMulArgs<T> fa{F, (const double *)c->filt.p, (long long)N, N, 1.0 / (double)N};
+        if ((e = launch<FilterMulBody<T>>(c, (N + NT - 1) / NT, S, fa))) return e;
+      } else {
+        BlueGaussArgs ga{F, d_g, (long long)N, N, 1.0 / (double)N};
+        if ((e = launch<BlueGaussBody>(c, (N + NT - 1) / NT, S, ga))) return e;
+      }
+      return blue_rows(c, F, 0, N, X, n0, N, S, +1, 1.0, n0);
     } else {
-      BlueGaussArgs ga{F, d_g, (long long)N, N, 1.0 / (double)N};
-      if ((e = launch<BlueGaussBody>(c, (N + NT - 1) / NT, S, ga))) return e;
+      return fail(c, CWTB_ERR_UNSUPPORTED, "un-padded transforms run in fp64");
     }
-    return blue_rows(c, F, 0, N, X, n0, N, S, +1, 1.0, n0);
   }
   if (table) {
-    if ((e = fft_rows<double, -1>(c, X, 0, n0, n0, F, N, N, S, N))) return e;
-    FilterMulArgs fa{F, (const double *)c->filt.p, (long long)N, N, 1.0 / (double)N};
-    if ((e = launch<FilterMulBody>(c, (N + NT - 1) / NT, S, fa))) return e;
-  } else if ((e = fft_rows<double, -1>(c, X, 0, n0, n0, F, N, N, S, N, d_g, 1.0 / (double)N))) {
+    if ((e = fft_rows<T, -1>(c, X, 0, n0, n0, F, N, N, S, N))) return e;
+    FilterMulArgs<T> fa{F, (const double *)c->filt.p, (long long)N, N, 1.0 / (double)N};
+    if ((e = launch<FilterMulBody<T>>(c, (N + NT - 1) / NT, S, fa))) return e;
+  } else if ((e = fft_rows<T, -1>(c, X, 0, n0, n0, F, N, N, S, N, d_g, 1.0 / (double)N))) {
     return e;
   }
-  return fft_rows<double, +1>(c, F, 0, N, N, X, n0, N, S, n0);
+  return fft_rows<T, +1>(c, F, 0, N, N, X, n0, N, S, n0);
 }
 
-// two transforms + coherence pipeline; outputs are device pointers (any may be null)
-static int wct_core(cwtb_ctx *c, const Job &job, const double *dsig1, const double *dsig2, int K,
+// two transforms + coherence pipeline in the engine type T; outputs are device pointers (any may
+// be null) and double for every T
+template <typename T>
+static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2, int K,
                     double *dWCT, double *daWCT, const unsigned char *dmask, int maxscale, int nbins,
                     unsigned long long *dhist) {
+  using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
   const size_t cnt = (size_t)S * n0;
   int e;
-  if ((e = ensure(c, c->W, cnt * sizeof(double2)))) return e;
-  if ((e = ensure(c, c->W2, cnt * sizeof(double2)))) return e;
-  if ((e = ensure(c, c->C, cnt * sizeof(double2)))) return e;
-  if ((e = ensure(c, c->A12, cnt * sizeof(double2)))) return e;
-  if ((e = run_job<double>(c, job, dsig1, (double2 *)c->W.p, EPI_STORE))) return e;
-  if ((e = run_job<double>(c, job, dsig2, (double2 *)c->W2.p, EPI_STORE))) return e;
+  if ((e = ensure(c, c->W, cnt * sizeof(V)))) return e;
+  if ((e = ensure(c, c->W2, cnt * sizeof(V)))) return e;
+  if ((e = ensure(c, c->C, cnt * sizeof(V)))) return e;
+  if ((e = ensure(c, c->A12, cnt * sizeof(V)))) return e;
+  if ((e = run_job<T>(c, job, dsig1, (V *)c->W.p, EPI_STORE))) return e;
+  if ((e = run_job<T>(c, job, dsig2, (V *)c->W2.p, EPI_STORE))) return e;
   const double *d_scale = (const double *)c->rowd.p;      // [S] scales, then [S] g
   const double *d_g = d_scale + S;
-  WctPrepArgs pa{(const double2 *)c->W.p, (const double2 *)c->W2.p, d_scale, (double2 *)c->C.p,
-                 (double2 *)c->A12.p, daWCT, n0};
+  WctPrepArgs<T> pa{(const V *)c->W.p, (const V *)c->W2.p, d_scale, (V *)c->C.p, (V *)c->A12.p, daWCT, n0};
   const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
-  if ((e = launch<WctPrepBody>(c, gx, S, pa))) return e;
+  if ((e = launch<WctPrepBody<T>>(c, gx, S, pa))) return e;
 #ifndef CWTB_HOST_EMU
   if (c->angle_host && daWCT) {   // the angle is final here: its 8 B per point cross PCIe under the smoothing
     RT(cudaEventRecord(c->ev_angle, c->stream));
@@ -2371,17 +2381,38 @@ static int wct_core(cwtb_ctx *c, const Job &job, const double *dsig1, const doub
     RT(cudaMemcpyAsync(c->angle_host, daWCT, cnt * sizeof(double), cudaMemcpyDeviceToHost, c->copy_streams[0]));
   }
 #endif
-  if ((e = smooth_time(c, (double2 *)c->C.p, S, n0, job.N, d_g))) return e;
-  if ((e = smooth_time(c, (double2 *)c->A12.p, S, n0, job.N, d_g))) return e;
-  WctFinalArgs fa{(const double2 *)c->C.p, (const double2 *)c->A12.p, (const double *)c->win.p, dWCT,
-                  dmask, dhist, n0, S, K, maxscale, nbins};
+  if ((e = smooth_time<T>(c, (V *)c->C.p, S, n0, job.N, d_g))) return e;
+  if ((e = smooth_time<T>(c, (V *)c->A12.p, S, n0, job.N, d_g))) return e;
+  WctFinalArgs<T> fa{(const V *)c->C.p, (const V *)c->A12.p, (const double *)c->win.p, dWCT,
+                     dmask, dhist, n0, S, K, maxscale, nbins};
   if (K > 64) return fail(c, CWTB_ERR_UNSUPPORTED, "scale boxcar longer than 64 taps");
   const int rows_out = dWCT ? S : maxscale;
   if (rows_out <= 0) return 0;
-  using F16 = WctFinalBody<16>;
+  using F16 = WctFinalBody<T, 16>;
   const unsigned fx = (unsigned)((n0 + F16::CW - 1) / F16::CW), fy = (unsigned)((rows_out + F16::RS - 1) / F16::RS);
-  return K <= 16 ? launch<F16>(c, fx, fy, fa) : launch<WctFinalBody<64>>(c, fx, fy, fa);
+  return K <= 16 ? launch<F16>(c, fx, fy, fa) : launch<WctFinalBody<T, 64>>(c, fx, fy, fa);
 }
+
+// the engine precision of T, and host series (double) as device series of type T: the fp32
+// coherence converts on the device, so that its inputs are the fp64 inputs rounded
+template <typename T> constexpr int prec_of() { return sizeof(T) == 8 ? CWTB_F64 : CWTB_F32; }
+
+static int to_f32(cwtb_ctx *c, const double *in, float *out, long long n) {
+  CvtArgs<double, float> a{in, out, n};
+  return launch<CvtBody<double, float>>(c, (unsigned)((n + NT - 1) / NT), 1, a);
+}
+
+template <typename T> static int upload_series(cwtb_ctx *c, Buf &b, const double *y, long long n0) {
+  if constexpr (sizeof(T) == 8) {
+    return upload_signal_f64(c, b, y, n0);
+  } else {
+    int e = upload_signal_f64(c, c->scratch, y, n0);
+    if (e) return e;
+    if ((e = ensure(c, b, (size_t)n0 * sizeof(float)))) return e;
+    return to_f32(c, (const double *)c->scratch.p, (float *)b.p, n0);
+  }
+}
+}  // extern "C++"
 
 static int upload_row_tables(cwtb_ctx *c, const Job &job) {
   std::vector<double> v(2 * (size_t)job.S);
@@ -2600,35 +2631,45 @@ int cwtb_scale_avg_power(cwtb_ctx *c, const double *weights, double *out) {
   return 0;
 }
 
-int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, const double *scales,
-             int n_scales, int family, double param, void *W12_out) {
-  if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
-  int e = prepare(c, n0, dt, scales, n_scales, family, param, CWTB_F64, nullptr);
+// the resident job is a job of type T afterwards: cwtb_get_w widens an fp32 W12 on the device
+extern "C++" {
+template <typename T>
+static int xwt_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, const double *scales,
+                   int n_scales, int family, double param, void *W12_out) {
+  int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
-  if ((e = upload_signal_f64(c, c->sig, y1, n0))) return e;
-  if ((e = upload_signal_f64(c, c->sig2, y2, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig, y1, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig2, y2, n0))) return e;
   c->launches = 0;
   if ((e = time_begin(c))) return e;
-  if ((e = run_job<double>(c, c->job, (const double *)c->sig.p, nullptr, EPI_STORE))) return e;
-  if ((e = run_job<double>(c, c->job, (const double *)c->sig2.p, nullptr, EPI_MULCONJ))) return e;
+  if ((e = run_job<T>(c, c->job, (const T *)c->sig.p, nullptr, EPI_STORE))) return e;
+  if ((e = run_job<T>(c, c->job, (const T *)c->sig2.p, nullptr, EPI_MULCONJ))) return e;
   if ((e = time_end(c))) return e;
   c->job_dsig = nullptr;
   if (W12_out) return cwtb_get_w(c, W12_out, 1, 0, n_scales);
   RT(rt_sync(c->stream));
   return 0;
 }
+}  // extern "C++"
 
-int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, double dj,
-             const double *scales, int n_scales, int family, double param, int boxcar_len,
-             double *WCT_out, double *aWCT_out) {
-  (void)dj;
+int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, const double *scales,
+             int n_scales, int family, double param, void *W12_out) {
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct needs an analytic wavelet family");
-  int e = prepare(c, n0, dt, scales, n_scales, family, param, CWTB_F64, nullptr);
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
+  return c->coh_precision == CWTB_F32
+             ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out)
+             : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out);
+}
+
+extern "C++" {
+template <typename T>
+static int wct_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt,
+                   const double *scales, int n_scales, int family, double param, int boxcar_len,
+                   double *WCT_out, double *aWCT_out) {
+  int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
-  if ((e = upload_signal_f64(c, c->sig, y1, n0))) return e;
-  if ((e = upload_signal_f64(c, c->sig2, y2, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig, y1, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig2, y2, n0))) return e;
   if ((e = upload_window(c, boxcar_len))) return e;
   if ((e = upload_row_tables(c, c->job))) return e;
   const size_t cnt = (size_t)n_scales * n0;
@@ -2641,8 +2682,8 @@ int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
   c->angle_host = aWCT_out;
   early_angle = aWCT_out != nullptr;
 #endif
-  e = wct_core(c, c->job, (const double *)c->sig.p, (const double *)c->sig2.p, boxcar_len, dW,
-               aWCT_out ? dA : nullptr, nullptr, 0, 0, nullptr);
+  e = wct_core<T>(c, c->job, (const T *)c->sig.p, (const T *)c->sig2.p, boxcar_len, dW,
+                  aWCT_out ? dA : nullptr, nullptr, 0, 0, nullptr);
   c->angle_host = nullptr;
   if (e) return e;
   if ((e = time_end(c))) return e;
@@ -2653,6 +2694,25 @@ int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
 #ifndef CWTB_HOST_EMU
   if (early_angle) RT(rt_sync(c->copy_streams[0]));
 #endif
+  return 0;
+}
+}  // extern "C++"
+
+int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, double dj,
+             const double *scales, int n_scales, int family, double param, int boxcar_len,
+             double *WCT_out, double *aWCT_out) {
+  (void)dj;
+  if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct needs an analytic wavelet family");
+  return c->coh_precision == CWTB_F32
+             ? wct_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, WCT_out, aWCT_out)
+             : wct_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, WCT_out, aWCT_out);
+}
+
+int cwtb_set_coherence_precision(cwtb_ctx *c, int precision) {
+  if (!c) return CWTB_ERR_ARG;
+  if (precision != CWTB_F64 && precision != CWTB_F32) return fail(c, CWTB_ERR_ARG, "bad precision");
+  c->coh_precision = precision;
   return 0;
 }
 
@@ -2709,7 +2769,7 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
     R2CArgs ra{(const double *)Y, X, (long long)cnt};
     if ((e = launch<R2CBody>(c, (unsigned)((cnt + NT - 1) / NT), 1, ra))) return e;
   }
-  if ((e = smooth_time(c, X, S, n, N, (const double *)c->rowd.p + S))) return e;
+  if ((e = smooth_time<double>(c, X, S, n, N, (const double *)c->rowd.p + S))) return e;
   BoxcarArgs ba{X, Y, (const double *)c->win.p, n, S, boxcar_len};
   if ((e = launch<BoxcarBody>(c, (unsigned)((n + NT - 1) / NT), S, ba))) return e;
   if (is_complex) {
@@ -2726,14 +2786,13 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
 }
 
 // common part of the two Monte-Carlo entry points: `noise` host surrogates [n_pairs][2][n0], or
-// null -> drawn on the device from (seed, pair0 + i)
-static int wct_mc_core(cwtb_ctx *c, const double *noise, unsigned long long seed, long long pair0, int n_pairs,
-                       int64_t n0, double dt, const double *scales, int n_scales, int family, double param,
-                       int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
-  if (!c || !mask || !hist || n_pairs < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
-    return fail(c, CWTB_ERR_ARG, "wct_mc: bad argument");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc needs an analytic wavelet family");
-  int e = prepare(c, n0, dt, scales, n_scales, family, param, CWTB_F64, nullptr);
+// null -> drawn on the device from (seed, pair0 + i); coherence in the engine type T
+extern "C++" {
+template <typename T>
+static int wct_mc_run(cwtb_ctx *c, const double *noise, unsigned long long seed, long long pair0, int n_pairs,
+                      int64_t n0, double dt, const double *scales, int n_scales, int family, double param,
+                      int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
+  int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_window(c, boxcar_len))) return e;
   if ((e = upload_row_tables(c, c->job))) return e;
@@ -2744,22 +2803,33 @@ static int wct_mc_core(cwtb_ctx *c, const double *noise, unsigned long long seed
   if ((e = ensure(c, c->hist, hb))) return e;
   RT(rt_memset(c->hist.p, 0, hb, c->stream));
   // surrogates of at most `batch` pairs are resident at a time
+  // (host surrogates stay double on the device; an fp32 run rounds one pair at a time into sig)
   const int batch = noise ? n_pairs : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_pairs, ((size_t)256 << 20) / ((size_t)2 * n0 * sizeof(double))));
-  if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * 2 * n0 * sizeof(double)))) return e;
+  const size_t nsz = noise ? sizeof(double) : sizeof(T);
+  if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * 2 * n0 * nsz))) return e;
   if (noise) RT(rt_h2d(c->noise.p, noise, (size_t)n_pairs * 2 * n0 * sizeof(double), c->stream));
+  if (noise && sizeof(T) != 8 && (e = ensure(c, c->sig, (size_t)2 * n0 * sizeof(T)))) return e;
   RT(rt_sync(c->stream));
   c->launches = 0;
   if ((e = time_begin(c))) return e;
   for (int i0 = 0; i0 < n_pairs; i0 += batch) {
     const int nb = std::min(batch, n_pairs - i0);
     if (!noise) {
-      NoiseArgs na{(double *)c->noise.p, seed, pair0 + i0, (long long)n0, nb};
-      if ((e = launch<NoiseBody>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * nb), na))) return e;
+      NoiseArgs<T> na{(T *)c->noise.p, seed, pair0 + i0, (long long)n0, nb};
+      if ((e = launch<NoiseBody<T>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * nb), na))) return e;
     }
     for (int i = 0; i < nb; ++i) {
-      const double *a = (const double *)c->noise.p + (size_t)i * 2 * n0;
-      if ((e = wct_core(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, (const unsigned char *)c->mask.p,
-                        maxscale, nbins, (unsigned long long *)c->hist.p)))
+      const T *a;
+      if constexpr (sizeof(T) == 8) {
+        a = (const T *)c->noise.p + (size_t)i * 2 * n0;
+      } else if (noise) {
+        if ((e = to_f32(c, (const double *)c->noise.p + (size_t)i * 2 * n0, (float *)c->sig.p, 2 * n0))) return e;
+        a = (const T *)c->sig.p;
+      } else {
+        a = (const T *)c->noise.p + (size_t)i * 2 * n0;
+      }
+      if ((e = wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, (const unsigned char *)c->mask.p,
+                           maxscale, nbins, (unsigned long long *)c->hist.p)))
         return e;
     }
   }
@@ -2770,6 +2840,20 @@ static int wct_mc_core(cwtb_ctx *c, const double *noise, unsigned long long seed
   RT(rt_sync(c->stream));
   for (size_t i = 0; i < h.size(); ++i) hist[i] += (int64_t)h[i];
   return 0;
+}
+}  // extern "C++"
+
+static int wct_mc_core(cwtb_ctx *c, const double *noise, unsigned long long seed, long long pair0, int n_pairs,
+                       int64_t n0, double dt, const double *scales, int n_scales, int family, double param,
+                       int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
+  if (!c || !mask || !hist || n_pairs < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
+    return fail(c, CWTB_ERR_ARG, "wct_mc: bad argument");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc needs an analytic wavelet family");
+  return c->coh_precision == CWTB_F32
+             ? wct_mc_run<float>(c, noise, seed, pair0, n_pairs, n0, dt, scales, n_scales, family, param,
+                                 boxcar_len, mask, maxscale, nbins, hist)
+             : wct_mc_run<double>(c, noise, seed, pair0, n_pairs, n0, dt, scales, n_scales, family, param,
+                                  boxcar_len, mask, maxscale, nbins, hist);
 }
 
 int cwtb_wct_mc(cwtb_ctx *c, const double *noise, int n_pairs, int64_t n0, double dt, double dj,
@@ -2793,8 +2877,8 @@ int cwtb_mc_surrogates(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pai
   if (!c || !out || n_pairs < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, "mc_surrogates: bad argument");
   int e = ensure(c, c->noise, (size_t)n_pairs * 2 * n0 * sizeof(double));
   if (e) return e;
-  NoiseArgs na{(double *)c->noise.p, seed, first_pair, (long long)n0, n_pairs};
-  if ((e = launch<NoiseBody>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * n_pairs), na))) return e;
+  NoiseArgs<double> na{(double *)c->noise.p, seed, first_pair, (long long)n0, n_pairs};
+  if ((e = launch<NoiseBody<double>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * n_pairs), na))) return e;
   RT(rt_d2h(out, c->noise.p, (size_t)n_pairs * 2 * n0 * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;

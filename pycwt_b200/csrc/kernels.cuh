@@ -129,8 +129,15 @@ template <typename T> struct Epilogue {
     if (mode == EPI_GAUSS) {
       const long long qs = n < nfreq / 2 ? n : n - nfreq;   // numpy fftfreq ordering
       const double k = 6.283185307179586 * ((double)qs * invn);
-      const T f = (T)(exp(g * (k * k)) * post);
-      return cscale(x, f);
+      if constexpr (sizeof(T) == 8) {
+        const T f = (T)(exp(g * (k * k)) * post);
+        return cscale(x, f);
+      } else {
+        // argument in double (k spans the whole transform), exponential in float: one double
+        // transcendental per element would make the fp32 smoothing transforms fp64-pipe bound
+        const T f = expf((float)(g * (k * k))) * (float)post;
+        return cscale(x, f);
+      }
     }
     return x;
   }
@@ -1278,27 +1285,31 @@ template <typename T> struct IcwtBody {
 //   C   = (|W1|^2 + i |W2|^2) / s   (two real fields packed into one complex field: the
 //         smoothing filter is real, so one complex transform smooths both)
 //   A12 = W1 conj(W2) / s,   aWCT = angle(W1 conj(W2))
-struct WctPrepArgs {
-  const double2 *W1, *W2;
+// in the engine type T; the angle is written as double whatever T is
+template <typename T> struct WctPrepArgs {
+  const cx<T> *W1, *W2;
   const double *scale;   // per row
-  double2 *C, *A12;
+  cx<T> *C, *A12;
   double *aWCT;          // may be null
   long long n;
 };
-struct WctPrepBody {
-  using Args = WctPrepArgs;
+template <typename T> struct WctPrepBody {
+  using Args = WctPrepArgs<T>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
     const long long n = (long long)bx * NT + tid;
     if (n >= a.n) return;
     const size_t i = (size_t)by * a.n + n;
-    const double2 w1 = a.W1[i], w2 = a.W2[i];
-    const double s = a.scale[by];
-    const double2 w12 = cmul(w1, cconj(w2));
-    a.C[i] = make_double2((w1.x * w1.x + w1.y * w1.y) / s, (w2.x * w2.x + w2.y * w2.y) / s);
-    a.A12[i] = make_double2(w12.x / s, w12.y / s);
-    if (a.aWCT) a.aWCT[i] = atan2(w12.y, w12.x);
+    const cx<T> w1 = a.W1[i], w2 = a.W2[i];
+    const T s = (T)a.scale[by];
+    const cx<T> w12 = cmul(w1, cconj(w2));
+    a.C[i] = mk<T>((w1.x * w1.x + w1.y * w1.y) / s, (w2.x * w2.x + w2.y * w2.y) / s);
+    a.A12[i] = mk<T>(w12.x / s, w12.y / s);
+    if (a.aWCT) {
+      if constexpr (sizeof(T) == 8) a.aWCT[i] = atan2(w12.y, w12.x);
+      else a.aWCT[i] = (double)atan2f(w12.y, w12.x);
+    }
   }
 };
 
@@ -1308,9 +1319,10 @@ struct WctPrepBody {
 // geometry, of the rank that draws it and of how the pairs are batched.  Two 53-bit uniforms ->
 // two standard normals (Box-Muller).  The reference's surrogates are white noise as well
 // (helpers.py:146-173 filters a length-1 axis, SURVEY 8a row 10); this mode reproduces their
-// distribution, not numpy's bit stream (the host-RNG mode does that).
-struct NoiseArgs {
-  double *out;              // [n_pairs][2][n]
+// distribution, not numpy's bit stream (the host-RNG mode does that).  The draw is in double for
+// every T: the fp32 surrogates are the fp64 ones rounded.
+template <typename T> struct NoiseArgs {
+  T *out;                   // [n_pairs][2][n]
   unsigned long long seed;
   long long pair0;          // global index of the first pair
   long long n;
@@ -1328,8 +1340,8 @@ HD void philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsign
   }
   o[0] = c0; o[1] = c1; o[2] = c2; o[3] = c3;
 }
-struct NoiseBody {
-  using Args = NoiseArgs;
+template <typename T> struct NoiseBody {
+  using Args = NoiseArgs<T>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
@@ -1347,9 +1359,9 @@ struct NoiseBody {
     const double r = sqrt(-2.0 * log(u1));
     double sn, cs;
     sincospi_hd(2.0 * u2, &sn, &cs);
-    double *dst = a.out + (size_t)by * a.n + 2 * j;
-    dst[0] = r * cs;
-    if (2 * j + 1 < a.n) dst[1] = r * sn;
+    T *dst = a.out + (size_t)by * a.n + 2 * j;
+    dst[0] = (T)(r * cs);
+    if (2 * j + 1 < a.n) dst[1] = (T)(r * sn);
   }
 };
 
@@ -1387,8 +1399,9 @@ struct BoxcarBody {
 
 // ---- Body: coherence  WCT = |S12|^2 / (S1 S2)  after the scale boxcar; optional histogram
 // of floor(WCT * nbins) over masked points (wavelet.py:513, 624-630) ---------------------
-struct WctFinalArgs {
-  const double2 *C, *A12;   // time-smoothed fields
+// Fields, staging and sums in the engine type T; WCT is written (and binned) as double.
+template <typename T> struct WctFinalArgs {
+  const cx<T> *C, *A12;     // time-smoothed fields
   const double *win;
   double *WCT;              // may be null (Monte-Carlo mode)
   const unsigned char *mask;   // [rows][n], may be null
@@ -1400,17 +1413,18 @@ struct WctFinalArgs {
 // time-smoothed fields for these columns in shared memory (each input element is read from global
 // memory (RS + K - 1) / RS times instead of K times); in phase 1 a thread produces 4 consecutive
 // rows of one column, so every staged value feeds up to four accumulators.
-template <int KMAX_> struct WctFinalBody {
-  using Args = WctFinalArgs;
+template <typename T, int KMAX_> struct WctFinalBody {
+  using Args = WctFinalArgs<T>;
+  using V = cx<T>;
   static constexpr int NPHASE = 2;
   static constexpr int RS = 32, CW = 32, KMAX = KMAX_, RG = 4;   // KMAX sizes the shared memory
-  static constexpr size_t SMEM = (size_t)2 * (RS + KMAX - 1) * CW * sizeof(double2) + KMAX * sizeof(double);
+  static constexpr size_t SMEM = (size_t)2 * (RS + KMAX - 1) * CW * sizeof(V) + KMAX * sizeof(T);
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
     const int K = a.K, off = (K - 1) / 2;
     const int nrow = RS + K - 1;
-    double2 *sc = (double2 *)smraw;                   // [nrow][CW] of C
-    double2 *sx = sc + (size_t)(RS + KMAX - 1) * CW;  // [nrow][CW] of A12
-    double *sw = (double *)(sx + (size_t)(RS + KMAX - 1) * CW);
+    V *sc = (V *)smraw;                               // [nrow][CW] of C
+    V *sx = sc + (size_t)(RS + KMAX - 1) * CW;        // [nrow][CW] of A12
+    T *sw = (T *)(sx + (size_t)(RS + KMAX - 1) * CW);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
     const int rows_out = a.WCT ? a.rows : a.maxscale;  // Monte-Carlo mode: rows below maxscale only
@@ -1421,7 +1435,7 @@ template <int KMAX_> struct WctFinalBody {
         const int r = idx / CW, col = idx % CW;
         const int q = qlo + r;
         const long long n = n0 + col;
-        double2 c = make_double2(0.0, 0.0), x = c;
+        V c = mk<T>(0, 0), x = c;
         if (q >= 0 && q < a.rows && n < a.n) {
           c = a.C[(size_t)q * a.n + n];
           x = a.A12[(size_t)q * a.n + n];
@@ -1429,22 +1443,22 @@ template <int KMAX_> struct WctFinalBody {
         sc[idx] = c;
         sx[idx] = x;
       }
-      for (int t = tid; t < K; t += NT) sw[t] = a.win[t];
+      for (int t = tid; t < K; t += NT) sw[t] = (T)a.win[t];
     } else {
       for (int task = tid; task < (RS / RG) * CW; task += NT) {
         const int col = task % CW, g = task / CW;
         const long long n = n0 + col;
         if (n >= a.n) continue;
-        double cr[RG] = {0, 0, 0, 0}, ci[RG] = {0, 0, 0, 0}, xr[RG] = {0, 0, 0, 0}, xi[RG] = {0, 0, 0, 0};
+        T cr[RG] = {0, 0, 0, 0}, ci[RG] = {0, 0, 0, 0}, xr[RG] = {0, 0, 0, 0}, xi[RG] = {0, 0, 0, 0};
         // staged row u feeds output row i0 + RG g + e with tap t = e + K - 1 - (u - RG g)
         for (int du = 0; du < K + RG - 1; ++du) {
           const int u = RG * g + du;
-          const double2 c = sc[u * CW + col], x = sx[u * CW + col];
+          const V c = sc[u * CW + col], x = sx[u * CW + col];
 #pragma unroll
           for (int e = 0; e < RG; ++e) {
             const int t = e + K - 1 - du;
             if (t >= 0 && t < K) {
-              const double w = sw[t];
+              const T w = sw[t];
               cr[e] += w * c.x; ci[e] += w * c.y;
               xr[e] += w * x.x; xi[e] += w * x.y;
             }
@@ -1454,7 +1468,7 @@ template <int KMAX_> struct WctFinalBody {
         for (int e = 0; e < RG; ++e) {
           const int i = i0 + RG * g + e;
           if (i >= rows_out) break;
-          const double r2 = (xr[e] * xr[e] + xi[e] * xi[e]) / (cr[e] * ci[e]);
+          const double r2 = (double)((xr[e] * xr[e] + xi[e] * xi[e]) / (cr[e] * ci[e]));
           const size_t o = (size_t)i * a.n + n;
           if (a.WCT) a.WCT[o] = r2;
           if (a.hist && i < a.maxscale && a.mask[o] && r2 == r2) {
@@ -1720,17 +1734,18 @@ struct BlueMulBody {
 };
 
 // F[r][k] *= filt[r][k] * post: a caller-supplied real frequency response per row (time smoothing
-// with a filter other than Morlet's Gaussian: cwtb_set_smooth_filter)
-struct FilterMulArgs { double2 *f; const double *filt; long long pitch; unsigned n; double post; };
-struct FilterMulBody {
-  using Args = FilterMulArgs;
+// with a filter other than Morlet's Gaussian: cwtb_set_smooth_filter); the table is double for
+// every engine type T
+template <typename T> struct FilterMulArgs { cx<T> *f; const double *filt; long long pitch; unsigned n; double post; };
+template <typename T> struct FilterMulBody {
+  using Args = FilterMulArgs<T>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
     const unsigned k = (unsigned)bx * NT + tid;
     if (k >= a.n) return;
-    const double m = a.filt[(size_t)by * a.n + k] * a.post;
-    double2 *p = a.f + (size_t)by * a.pitch + k;
+    const T m = (T)(a.filt[(size_t)by * a.n + k] * a.post);
+    cx<T> *p = a.f + (size_t)by * a.pitch + k;
     p->x *= m; p->y *= m;
   }
 };

@@ -217,12 +217,15 @@ def surrogate_pair(seed, index, N, al1, al2):
 
 
 def wct_significance_sharded(al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet='morlet',
-                             mc_count=300, seed=0, engine=None, comm=None, device=None, device_rng=False):
+                             mc_count=300, seed=0, engine=None, comm=None, device=None, device_rng=False,
+                             precision='fp64'):
     """Monte-Carlo coherence significance (reference wavelet.py:531-647) with the surrogate
     pairs block-partitioned over the ranks (SURVEY 8e): every rank accumulates the [S, 1000]
     int64 histograms of its pairs on its GPU, ONE all-reduce (sum, ~1 MB) combines them and
-    every rank evaluates the percentiles.  The result is independent of the world size."""
+    every rank evaluates the percentiles.  The result is independent of the world size.
+    `precision`: 'fp64' (default) or 'fp32', as in wavelet.wct_significance."""
     from . import wavelet as wv
+    prec = wv._coherence_precision(precision)
     comm = _as_comm(comm)
     mother = wv._check_parameter_wavelet(wavelet)
     rank, world = _rank_world(comm)
@@ -230,11 +233,12 @@ def wct_significance_sharded(al1, al2, dt, dj, s0, J, significance_level=0.95, w
     lo, hi = shard_range(mc_count, rank, world)
     if device_rng:
         # surrogates drawn on each rank's GPU from the Philox stream keyed by (seed, pair number)
-        hist = wv._mc_histogram_seeded(prob, dt, dj, mother, seed, lo, hi - lo, engine=engine)
+        hist = wv._mc_histogram_seeded(prob, dt, dj, mother, seed, lo, hi - lo, engine=engine,
+                                       precision=prec)
     else:
         hist = wv._mc_histogram(prob, dt, dj, mother,
                                 lambda i: surrogate_pair(seed, i, prob['N'], al1, al2),
-                                range(lo, hi), progress=False, engine=engine)
+                                range(lo, hi), progress=False, engine=engine, precision=prec)
     hist = sum_over_ranks(hist, comm, device)
     return wv._mc_levels(prob, hist, significance_level)
 
@@ -292,7 +296,7 @@ def wct_halo(boxcar_len):
 
 
 def wct_scale_sharded(y1, y2, dt, dj=1 / 12, s0=-1, J=-1, wavelet='morlet', normalize=True,
-                      engine=None, comm=None, device=None):
+                      engine=None, comm=None, device=None, precision='fp64'):
     """Deterministic part of the wavelet coherence (reference wavelet.py:422-516) with the SCALES
     block-partitioned over the ranks (SURVEY 8e row 4).  The transforms and the time smoothing are
     per scale; only the scale boxcar couples neighbouring rows, so every rank computes its block
@@ -302,9 +306,12 @@ def wct_scale_sharded(y1, y2, dt, dj=1 / 12, s0=-1, J=-1, wavelet='morlet', norm
     single-GPU one row for row.  No collective on the data path: the coherence slabs stay with
     their rank; the per-scale mean coherence [S] is all-gathered.
 
+    `precision`: 'fp64' (default) or 'fp32', as in wavelet.wct.
+
     Returns (lo, hi, WCT[lo:hi], aWCT[lo:hi], mean_wct[S], freq[S])."""
     from . import wavelet as wv
     from . import _engine
+    prec = wv._coherence_precision(precision)
     comm = _as_comm(comm)
     rank, world = _rank_world(comm)
     mother = wv._check_parameter_wavelet(wavelet)
@@ -330,9 +337,11 @@ def wct_scale_sharded(y1, y2, dt, dj=1 / 12, s0=-1, J=-1, wavelet='morlet', norm
     eng = engine or _engine.default_engine()
     if hi > lo:
         with eng.lock:
-            wv._sync_padding(eng, n0)
+            if wv._sync_padding(eng, n0):
+                prec = _engine.F64      # un-padded transforms run in fp64
             with wv._smoothing_filter(eng, mother, sj[a:b], dt, n0):
-                WCT, aWCT = eng.wct(y1n, y2n, dt, dj, sj[a:b], *wv._family_of(mother), boxcar_len=klen)
+                WCT, aWCT = eng.wct(y1n, y2n, dt, dj, sj[a:b], *wv._family_of(mother), boxcar_len=klen,
+                                    precision=prec)
         WCT, aWCT = WCT[lo - a:hi - a], aWCT[lo - a:hi - a]
         local = WCT.mean(axis=1)
     else:

@@ -33,6 +33,16 @@ def _precision():
     return _PRECISIONS[os.environ.get('CWTB_PRECISION', 'fp64').lower()]
 
 
+def _coherence_precision(precision):
+    """Engine precision of the coherence paths from a spelling of `_PRECISIONS`
+    (CWTB_PRECISION governs cwt only)."""
+    try:
+        return _PRECISIONS[str(precision).lower()]
+    except KeyError:
+        raise ValueError("precision must be one of %s, got %r"
+                         % (", ".join(sorted(_PRECISIONS)), precision))
+
+
 def _resolve_scales(n0, dt, dj, s0, J, wavelet, freqs):
     """Scale vector exactly as the reference builds it (wavelet.py:75-88)."""
     if freqs is None:
@@ -279,11 +289,14 @@ def _standardise(y, normalize):
 
 
 def xwt(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
-        wavelet='morlet', normalize=True):
+        wavelet='morlet', normalize=True, precision='fp64'):
     """Cross wavelet transform W1 * conj(W2) (reference wavelet.py:316-419).
 
     Both transforms and the conjugate product (fused into the second transform's output
-    pass) run on the GPU.  Returns (W12, coi, freq, signif)."""
+    pass) run on the GPU.  Returns (W12, coi, freq, signif).  `precision` (an extension of
+    the reference signature): 'fp64' (default) or 'fp32', the arithmetic of the transforms;
+    W12 is complex128 either way.  Un-padded transforms run in fp64 whatever is asked."""
+    prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     y1, y1n, std1 = _standardise(y1, normalize)
     y2, y2n, std2 = _standardise(y2, normalize)
@@ -296,8 +309,9 @@ def xwt(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
     sj, freq = sj[keep], freq[keep]
     eng = _engine.default_engine()
     with eng.lock:
-        _sync_padding(eng, n0)
-        W12 = eng.xwt(y1n, y2n, dt, sj, *_family_of(wavelet))
+        if _sync_padding(eng, n0):
+            prec = _engine.F64      # un-padded transforms run in fp64
+        W12 = eng.xwt(y1n, y2n, dt, sj, *_family_of(wavelet), precision=prec)
     coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
     coi = wavelet.flambda() * wavelet.coi() * dt * coi
 
@@ -349,12 +363,17 @@ def _boxcar_len(wavelet, dj):
 
 
 def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
-        significance_level=0.95, wavelet='morlet', normalize=True, **kwargs):
+        significance_level=0.95, wavelet='morlet', normalize=True, precision='fp64',
+        **kwargs):
     """Wavelet coherence (reference wavelet.py:422-528).
 
     Returns (WCT, aWCT, coi, freq, sig).  The two transforms, the |W|^2/s and W12/s
     products, the Gaussian time smoothing, the scale boxcar and the coherence ratio run
-    on the GPU; `sig` comes from wct_significance (GPU Monte-Carlo) when sig=True."""
+    on the GPU; `sig` comes from wct_significance (GPU Monte-Carlo) when sig=True.
+    `precision` (an extension of the reference signature): 'fp64' (default) or 'fp32', the
+    arithmetic of the device pipeline, also that of the significance test; WCT and aWCT are
+    float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6)."""
+    prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     if not hasattr(wavelet, 'smooth'):
         # same failure mode as the reference for Paul / DOG (no smoothing operator)
@@ -373,17 +392,19 @@ def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
     if klen < 1:
         raise ValueError('smoothing window undefined for this wavelet (deltaj0 = -1)')
     with eng.lock:
-        _sync_padding(eng, len(y1n))
+        if _sync_padding(eng, len(y1n)):
+            prec = _engine.F64      # un-padded transforms run in fp64
         with _smoothing_filter(eng, wavelet, sj, dt, len(y1n)):
-            WCT, aWCT = eng.wct(y1n, y2n, dt, dj, sj, *_family_of(wavelet), boxcar_len=klen)
+            WCT, aWCT = eng.wct(y1n, y2n, dt, dj, sj, *_family_of(wavelet), boxcar_len=klen,
+                                precision=prec)
     coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
     coi = wavelet.flambda() * wavelet.coi() * dt * coi
     if sig:
         a1, b1, c1 = ar1(y1)
         a2, b2, c2 = ar1(y2)
-        sig = wct_significance(a1, a2, dt=dt, dj=dj, s0=s0, J=J,
+        sig = _wct_significance(a1, a2, dt=dt, dj=dj, s0=s0, J=J,
                                significance_level=significance_level,
-                               wavelet=wavelet, **kwargs)
+                               wavelet=wavelet, precision=precision, **kwargs)
     else:
         sig = np.asarray([0])
     return WCT, aWCT, coi, freq, sig
@@ -407,9 +428,11 @@ def _mc_problem(dt, dj, s0, J, wavelet):
                 mask=np.ascontiguousarray(outsidecoi, dtype=np.uint8))
 
 
-def _mc_histogram(prob, dt, dj, wavelet, draw, indices, progress=False, engine=None):
+def _mc_histogram(prob, dt, dj, wavelet, draw, indices, progress=False, engine=None,
+                  precision=_engine.F64):
     """1000-bin histograms of the coherence of the surrogate pairs draw(i), i in `indices`
-    (reference wavelet.py:609-630), accumulated on the GPU: int64 [S, nbins]."""
+    (reference wavelet.py:609-630), accumulated on the GPU: int64 [S, nbins].  `precision`:
+    engine precision of the coherence."""
     N, sj, nbins = prob['N'], prob['sj'], prob['nbins']
     hist = np.zeros((sj.size, nbins), dtype=np.int64)
     eng = engine or _engine.default_engine()
@@ -423,10 +446,10 @@ def _mc_histogram(prob, dt, dj, wavelet, draw, indices, progress=False, engine=N
         for k, i in enumerate(idx):
             noise[k, 0], noise[k, 1] = draw(i)
         with eng.lock:
-            _sync_padding(eng, N)
+            prec = _engine.F64 if _sync_padding(eng, N) else precision
             with _smoothing_filter(eng, wavelet, sj, dt, N):
                 eng.wct_mc(noise, dt, dj, sj, fam[0], fam[1], _boxcar_len(wavelet, dj), prob['mask'],
-                           prob['maxscale'], nbins, hist)
+                           prob['maxscale'], nbins, hist, precision=prec)
         bar.update(len(idx))
     bar.close()
     return hist
@@ -445,7 +468,8 @@ def _mc_levels(prob, hist, significance_level):
     return sig95
 
 
-def _mc_histogram_seeded(prob, dt, dj, wavelet, seed, first, count, engine=None):
+def _mc_histogram_seeded(prob, dt, dj, wavelet, seed, first, count, engine=None,
+                         precision=_engine.F64):
     """The same histograms with the surrogates drawn on the device (Philox stream keyed by
     (seed, pair number)): no host RNG, no noise H2D."""
     sj, nbins = prob['sj'], prob['nbins']
@@ -453,10 +477,10 @@ def _mc_histogram_seeded(prob, dt, dj, wavelet, seed, first, count, engine=None)
     eng = engine or _engine.default_engine()
     fam = _family_of(wavelet)
     with eng.lock:
-        _sync_padding(eng, prob['N'])
+        prec = _engine.F64 if _sync_padding(eng, prob['N']) else precision
         with _smoothing_filter(eng, wavelet, sj, dt, prob['N']):
             eng.wct_mc_seeded(seed, first, count, prob['N'], dt, sj, fam[0], fam[1], _boxcar_len(wavelet, dj),
-                              prob['mask'], prob['maxscale'], nbins, hist)
+                              prob['mask'], prob['maxscale'], nbins, hist, precision=prec)
     return hist
 
 
@@ -473,7 +497,19 @@ def wct_significance(al1, al2, dt, dj, s0, J, significance_level=0.95,
     the reference signature) the surrogates are drawn on the device from a counter-based
     Philox stream: statistically equivalent white noise, no host RNG or upload, about twice
     as fast; the result then depends on `seed` only, not on numpy's global state.  The
-    on-disk cache keeps the reference's key and format (~/.cache/pycwt/<key>.gz)."""
+    on-disk cache keeps the reference's key and format (~/.cache/pycwt/<key>.gz).
+    The parameter list stays the reference's (plus `seed`): the fp32 coherence of the surrogates
+    is reached through `wct(..., sig=True, precision='fp32')`."""
+    return _wct_significance(al1, al2, dt, dj, s0, J, significance_level, wavelet, mc_count,
+                             progress, cache, seed)
+
+
+def _wct_significance(al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet='morlet',
+                      mc_count=300, progress=True, cache=True, seed=None, precision='fp64'):
+    """wct_significance with `precision`: 'fp64' (default) or 'fp32', the arithmetic of the
+    device coherence.  The surrogates, ar1 and the levels stay float64 on the host; the fp32
+    levels agree with fp64 within a histogram bin, so the cache key does not include it."""
+    prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     if cache:
         aa = np.round(np.arctanh(np.array([al1, al2]) * 4))
@@ -497,9 +533,9 @@ def wct_significance(al1, al2, dt, dj, s0, J, significance_level=0.95,
         def draw(i):
             return rednoise(N, al1, 1), rednoise(N, al2, 1)
 
-        hist = _mc_histogram(prob, dt, dj, wavelet, draw, range(mc_count), progress)
+        hist = _mc_histogram(prob, dt, dj, wavelet, draw, range(mc_count), progress, precision=prec)
     else:
-        hist = _mc_histogram_seeded(prob, dt, dj, wavelet, seed, 0, mc_count)
+        hist = _mc_histogram_seeded(prob, dt, dj, wavelet, seed, 0, mc_count, precision=prec)
     sig95 = _mc_levels(prob, hist, significance_level)
 
     if cache:
