@@ -196,6 +196,34 @@ int cwtb_xwt(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,
 int cwtb_wct(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,
              double dt, double dj, const double *scales, int n_scales, int family,
              double param, int boxcar_len, double *WCT_out, double *aWCT_out);
+/* ---- resident coherence ---------------------------------------------------------------------
+ * cwtb_wct_resident computes what cwtb_wct computes (same arguments, same precision:
+ * cwtb_set_coherence_precision) but keeps WCT and aWCT (n_scales x n0 doubles each) in a device
+ * buffer of their own.  Only cwtb_wct_resident writes that buffer: it stays valid across later
+ * cwt / xwt / wct / Monte-Carlo calls, until the next cwtb_wct_resident or cwtb_coherence_release
+ * (which frees it; so does cwtb_destroy).  cwtb_coherence_serial changes at both, and is bumped
+ * before the buffer is written, so a cwtb_wct_resident that fails part-way changes it too.  The
+ * reading calls return CWTB_ERR_STATE when nothing is resident and CWTB_ERR_ARG for bad ranges. */
+int cwtb_wct_resident(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,
+                      double dt, double dj, const double *scales, int n_scales, int family,
+                      double param, int boxcar_len);
+int64_t cwtb_coherence_serial(cwtb_ctx *ctx);
+int cwtb_coherence_release(cwtb_ctx *ctx);
+/* Strided sub-grid of either field (outputs may be NULL), nrows x ncols doubles:
+ * out[r][c] = field[row0 + r*row_step][col0 + c*col_step], steps >= 1, every index inside the
+ * field.  Whole rows with unit steps are plain device-to-host copies. */
+int cwtb_coherence_window(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0,
+                          int64_t ncols, int64_t col_step, double *WCT_out, double *aWCT_out);
+/* Per row j, over the columns [lo[j], hi[j]) (lo / hi NULL: the whole row) where thr is NULL or
+ * WCT > thr[j] (false for a NaN threshold): out[j] = [count, sum WCT, sum cos aWCT, sum sin aWCT]
+ * (S x 4 doubles).  aWCT is not read when want_phase == 0 (its sums are 0).  Deterministic: fixed
+ * partition and summation order, repeated calls are bit-identical. */
+int cwtb_coherence_row_stats(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, const double *thr,
+                             int want_phase, double *out);
+/* out[3][n0]: sum_j weights[j]*WCT[j,n], sum_j weights[j]*cos aWCT[j,n], sum_j weights[j]*sin
+ * aWCT[j,n].  Rows with weight 0 are not read.  Deterministic. */
+int cwtb_coherence_scale_avg(cwtb_ctx *ctx, const double *weights, double *out);
+
 /* Morlet.smooth on a caller-supplied host array (mothers.py:61-104).
  * in: n_scales x n (complex128 if is_complex else float64); out same type. */
 int cwtb_smooth(cwtb_ctx *ctx, const void *in, int is_complex, int n_scales,

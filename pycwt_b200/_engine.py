@@ -66,6 +66,12 @@ _SIGNATURES = {
     "cwtb_scale_avg_power": (_I, [_P, _P, _P]),
     "cwtb_xwt": (_I, [_P, _P, _P, _I64, _D, _P, _I, _I, _D, _P]),
     "cwtb_wct": (_I, [_P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _P]),
+    "cwtb_wct_resident": (_I, [_P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I]),
+    "cwtb_coherence_serial": (_I64, [_P]),
+    "cwtb_coherence_release": (_I, [_P]),
+    "cwtb_coherence_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P, _P]),
+    "cwtb_coherence_row_stats": (_I, [_P, _P, _P, _P, _I, _P]),
+    "cwtb_coherence_scale_avg": (_I, [_P, _P, _P]),
     "cwtb_smooth": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _P]),
     "cwtb_wct_mc": (_I, [_P, _P, _I, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
     "cwtb_wct_mc_seeded": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
@@ -493,6 +499,84 @@ class Engine(object):
                                           _ptr(aWCT) if want_angle else None))
             self._resident = None                   # several intermediates, no single transform
         return WCT, aWCT
+
+    # ---- resident coherence (its own device buffer, see include/cwt_b200.h) ------------------
+    _coherence = None        # (rows, n0) of the resident coherence
+
+    @_locked
+    def wct_resident(self, y1, y2, dt, dj, scales, family, param, boxcar_len, precision=F64):
+        """`wct` with WCT and aWCT kept on the device; returns the coherence serial that
+        identifies them."""
+        y1 = np.ascontiguousarray(y1, dtype=np.float64)
+        y2 = np.ascontiguousarray(y2, dtype=np.float64)
+        if y1.shape != y2.shape or y1.ndim != 1:
+            raise ValueError("wct_resident: the two series must be 1-D and of equal length")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        self._coherence = None
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
+                                               _ptr(sj), sj.size, int(family), float(param),
+                                               int(boxcar_len)))
+        self._coherence = (sj.size, y1.size)
+        return self.coherence_serial()
+
+    @_locked
+    def coherence_serial(self):
+        return int(self.lib.cwtb_coherence_serial(self.h))
+
+    @_locked
+    def coherence_release(self):
+        self._coherence = None
+        self._check(self.lib.cwtb_coherence_release(self.h))
+
+    def _coherence_shape(self):
+        if self._coherence is None:
+            raise EngineError("no coherence resident")
+        return self._coherence
+
+    @_locked
+    def coherence_window(self, row0, nrows, row_step, col0, ncols, col_step, want_wct=True,
+                         want_angle=True):
+        """(WCT, aWCT)[row0::row_step][:nrows, col0::col_step][:, :ncols] of the resident
+        coherence; a field not asked for is None."""
+        self._coherence_shape()
+        WCT = self.result_array((nrows, ncols), np.float64) if want_wct else None
+        aWCT = self.result_array((nrows, ncols), np.float64) if want_angle else None
+        self._check(self.lib.cwtb_coherence_window(
+            self.h, int(row0), int(nrows), int(row_step), int(col0), int(ncols), int(col_step),
+            _ptr(WCT) if want_wct else None, _ptr(aWCT) if want_angle else None))
+        return WCT, aWCT
+
+    @_locked
+    def coherence_row_stats(self, lo, hi, thr=None, want_phase=False):
+        """[rows, 4]: count, sum WCT, sum cos aWCT, sum sin aWCT over the columns [lo[j], hi[j])
+        where thr is None or WCT > thr[j]."""
+        rows, _ = self._coherence_shape()
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        if lo.shape != (rows,) or hi.shape != (rows,):
+            raise ValueError("coherence_row_stats: one column range per row expected")
+        if thr is not None:
+            thr = np.ascontiguousarray(thr, dtype=np.float64)
+            if thr.shape != (rows,):
+                raise ValueError("coherence_row_stats: one threshold per row expected")
+        out = np.empty((rows, 4), dtype=np.float64)
+        self._check(self.lib.cwtb_coherence_row_stats(self.h, _ptr(lo), _ptr(hi),
+                                                      None if thr is None else _ptr(thr),
+                                                      1 if want_phase else 0, _ptr(out)))
+        return out
+
+    @_locked
+    def coherence_scale_avg(self, weights):
+        """[3, n0]: sum_j w_j WCT[j], sum_j w_j cos aWCT[j], sum_j w_j sin aWCT[j]."""
+        rows, n0 = self._coherence_shape()
+        w = np.ascontiguousarray(weights, dtype=np.float64)
+        if w.shape != (rows,):
+            raise ValueError("coherence_scale_avg: one weight per row expected")
+        out = self.result_array((3, n0), np.float64)
+        self._check(self.lib.cwtb_coherence_scale_avg(self.h, _ptr(w), _ptr(out)))
+        return out
 
     @_locked
     def smooth(self, W, dt, scales, boxcar_len):

@@ -49,6 +49,15 @@ HD void sincospi_hd(double x, double *s, double *c) {
 #endif
 }
 
+// sin(x), cos(x) in double
+HD void sincos_hd(double x, double *s, double *c) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  sincos(x, s, c);
+#else
+  ::sincos(x, s, c);
+#endif
+}
+
 // ---- DFT_R in registers: x[c] <- sum_i x[i] e^{SIGN 2 pi i * i*c/R}, natural order ----
 template <int SIGN, typename V> HD void dft2(V &a, V &b) {
   V t = csub(a, b);

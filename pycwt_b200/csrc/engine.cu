@@ -246,6 +246,13 @@ struct cwtb_ctx {
   int batch_pipeline = 1;        // CWTB_BATCH_PIPELINE=0: one synchronous chunk after the other
   double *angle_host = nullptr;  // cwtb_wct: host destination of the phase angle, copied on a copy stream
                                  // as soon as it exists (before the smoothing transforms), not after them
+  // resident coherence (cwtb_wct_resident): WCT [S][n0], aWCT at coh_angle_offset(S*n0).  Only
+  // cwtb_wct_resident writes this buffer, so it outlives any other call; cwtb_coherence_release
+  // frees it.  coh_serial is bumped before every write and on release (cwtb_coherence_serial).
+  Buf coh;
+  int coh_S = 0;                 // rows resident (0: none)
+  long long coh_n0 = 0;
+  long long coh_serial = 0;
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
   double last_ms = 0;
   int launches = 0;
@@ -1951,7 +1958,7 @@ void cwtb_destroy(cwtb_ctx *c) {
 #endif
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->Zxs[0], &c->Zxs[1], &c->Zxs[2], &c->Zxs[3], &c->Zxs[4], &c->Zxs[5], &c->Zxs[6], &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cin, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2661,11 +2668,18 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
              : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out);
 }
 
+// WCT and aWCT of a coherence share one device buffer; aWCT starts on a 256-byte boundary, so that
+// a flat index has the same alignment in both fields (the 16-byte loads of CohRowStatsBody)
+static size_t coh_angle_offset(size_t cnt) { return (cnt + 31) & ~(size_t)31; }
+
+// Coherence of two series in the engine type T into the device buffer `dst` (WCT, then aWCT at
+// coh_angle_offset), grown as needed.  `angle_host`: host destination of an early angle copy (see
+// wct_core), or null.
 extern "C++" {
 template <typename T>
 static int wct_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt,
                    const double *scales, int n_scales, int family, double param, int boxcar_len,
-                   double *WCT_out, double *aWCT_out) {
+                   Buf &dst, bool want_angle, double *angle_host) {
   int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_series<T>(c, c->sig, y1, n0))) return e;
@@ -2673,21 +2687,44 @@ static int wct_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, 
   if ((e = upload_window(c, boxcar_len))) return e;
   if ((e = upload_row_tables(c, c->job))) return e;
   const size_t cnt = (size_t)n_scales * n0;
-  if ((e = ensure(c, c->aux, 2 * cnt * sizeof(double)))) return e;
-  double *dW = (double *)c->aux.p, *dA = dW + cnt;
+  if ((e = ensure(c, dst, (coh_angle_offset(cnt) + cnt) * sizeof(double)))) return e;
+  double *dW = (double *)dst.p, *dA = dW + coh_angle_offset(cnt);
   c->launches = 0;
   if ((e = time_begin(c))) return e;
-  bool early_angle = false;
-#ifndef CWTB_HOST_EMU
-  c->angle_host = aWCT_out;
-  early_angle = aWCT_out != nullptr;
-#endif
+  c->angle_host = angle_host;
   e = wct_core<T>(c, c->job, (const T *)c->sig.p, (const T *)c->sig2.p, boxcar_len, dW,
-                  aWCT_out ? dA : nullptr, nullptr, 0, 0, nullptr);
+                  want_angle ? dA : nullptr, nullptr, 0, 0, nullptr);
   c->angle_host = nullptr;
   if (e) return e;
   if ((e = time_end(c))) return e;
   c->job_dsig = nullptr;
+  return 0;
+}
+}  // extern "C++"
+
+static int wct_dispatch(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt,
+                        const double *scales, int n_scales, int family, double param, int boxcar_len,
+                        Buf &dst, bool want_angle, double *angle_host) {
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct needs an analytic wavelet family");
+  return c->coh_precision == CWTB_F32
+             ? wct_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, dst, want_angle, angle_host)
+             : wct_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, dst, want_angle, angle_host);
+}
+
+int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, double dj,
+             const double *scales, int n_scales, int family, double param, int boxcar_len,
+             double *WCT_out, double *aWCT_out) {
+  (void)dj;
+  if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
+  bool early_angle = false;
+#ifndef CWTB_HOST_EMU
+  early_angle = aWCT_out != nullptr;
+#endif
+  int e = wct_dispatch(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, c->aux,
+                       aWCT_out != nullptr, early_angle ? aWCT_out : nullptr);
+  if (e) return e;
+  const size_t cnt = (size_t)n_scales * n0;
+  const double *dW = (const double *)c->aux.p, *dA = dW + coh_angle_offset(cnt);
   if (WCT_out) RT(rt_d2h(WCT_out, dW, cnt * sizeof(double), c->stream));
   if (aWCT_out && !early_angle) RT(rt_d2h(aWCT_out, dA, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
@@ -2696,17 +2733,142 @@ static int wct_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, 
 #endif
   return 0;
 }
-}  // extern "C++"
 
-int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, double dj,
-             const double *scales, int n_scales, int family, double param, int boxcar_len,
-             double *WCT_out, double *aWCT_out) {
+// ---- resident coherence ---------------------------------------------------------------------
+int cwtb_wct_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, double dj,
+                      const double *scales, int n_scales, int family, double param, int boxcar_len) {
   (void)dj;
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct needs an analytic wavelet family");
-  return c->coh_precision == CWTB_F32
-             ? wct_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, WCT_out, aWCT_out)
-             : wct_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, WCT_out, aWCT_out);
+  ++c->coh_serial;   // before the buffer is written: a call that fails part-way invalidates it too
+  c->coh_S = 0;
+  c->coh_n0 = 0;
+  int e = wct_dispatch(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, c->coh, true, nullptr);
+  if (e) return e;
+  RT(rt_sync(c->stream));
+  c->coh_S = n_scales;
+  c->coh_n0 = n0;
+  return 0;
+}
+
+int64_t cwtb_coherence_serial(cwtb_ctx *c) { return c ? c->coh_serial : -1; }
+
+int cwtb_coherence_release(cwtb_ctx *c) {
+  if (!c) return CWTB_ERR_ARG;
+  ++c->coh_serial;
+  c->coh_S = 0;
+  c->coh_n0 = 0;
+  if (c->coh.p) {
+#ifndef CWTB_HOST_EMU
+    RT(cudaSetDevice(c->device));
+#endif
+    RT(rt_sync(c->stream));
+    rt_free(c->coh.p);
+    c->coh.p = nullptr;
+    c->coh.bytes = 0;
+  }
+  return 0;
+}
+
+static int coh_ready(cwtb_ctx *c) {
+  if (!c) return CWTB_ERR_ARG;
+  if (c->coh_S <= 0 || !c->coh.p) return fail(c, CWTB_ERR_STATE, "no coherence resident");
+#ifndef CWTB_HOST_EMU
+  RT(cudaSetDevice(c->device));
+#endif
+  return 0;
+}
+
+int cwtb_coherence_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                          int64_t col_step, double *WCT_out, double *aWCT_out) {
+  int e = coh_ready(c);
+  if (e) return e;
+  const int S = c->coh_S;
+  const long long n0 = c->coh_n0;
+  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
+    return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
+  if (nrows == 0 || ncols == 0 || (!WCT_out && !aWCT_out)) return 0;
+  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
+      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
+    return fail(c, CWTB_ERR_ARG, "window outside the resident coherence");
+  const size_t cnt = (size_t)S * n0;
+  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
+  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
+    const size_t off = (size_t)row0 * n0, bytes = (size_t)nrows * n0 * sizeof(double);
+    if (WCT_out) RT(rt_d2h(WCT_out, dW + off, bytes, c->stream));
+    if (aWCT_out) RT(rt_d2h(aWCT_out, dA + off, bytes, c->stream));
+    RT(rt_sync(c->stream));
+    return 0;
+  }
+  const size_t m = (size_t)nrows * ncols;
+  if ((e = ensure(c, c->aux, 2 * m * sizeof(double)))) return e;
+  double *oW = (double *)c->aux.p, *oA = oW + m;
+  CohWindowArgs a{dW, dA, WCT_out ? oW : nullptr, aWCT_out ? oA : nullptr, n0, row0, row_step, col0, col_step, ncols};
+  if ((e = launch<CohWindowBody>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a))) return e;
+  if (WCT_out) RT(rt_d2h(WCT_out, oW, m * sizeof(double), c->stream));
+  if (aWCT_out) RT(rt_d2h(aWCT_out, oA, m * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+int cwtb_coherence_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, const double *thr,
+                             int want_phase, double *out) {
+  int e = coh_ready(c);
+  if (e) return e;
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = c->coh_S;
+  const long long n0 = c->coh_n0;
+  using B = CohRowStatsBody;
+  const int nchunk = (int)((n0 + B::CHUNK - 1) / B::CHUNK);
+  // aux: [lo S][hi S][thr S][partials S*nchunk*4][sums S*4], 8 bytes each
+  std::vector<long long> h(3 * (size_t)S);
+  for (int j = 0; j < S; ++j) {
+    h[j] = lo ? lo[j] : 0;
+    h[S + j] = hi ? hi[j] : n0;
+    if (h[j] < 0 || h[S + j] > n0 || h[j] > h[S + j])
+      return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
+  }
+  if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
+  const size_t npart = (size_t)S * nchunk * 4;
+  if ((e = ensure(c, c->aux, (3 * (size_t)S + npart + 4 * (size_t)S) * sizeof(double)))) return e;
+  long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
+  double *dthr = (double *)(dhi + S), *dpart = dthr + S, *dsum = dpart + npart;
+  RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
+  const size_t cnt = (size_t)S * n0;
+  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
+  CohRowStatsArgs a{dW, dA, dlo, dhi, thr ? dthr : nullptr, dpart, n0, nchunk, want_phase != 0};
+  if ((e = launch<B>(c, (unsigned)nchunk, (unsigned)S, a))) return e;
+  CohRowSumArgs r{dpart, dsum, S, nchunk};
+  if ((e = launch<CohRowSumBody>(c, (unsigned)((4 * S + NT - 1) / NT), 1, r))) return e;
+  RT(rt_d2h(out, dsum, (size_t)S * 4 * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+int cwtb_coherence_scale_avg(cwtb_ctx *c, const double *weights, double *out) {
+  int e = coh_ready(c);
+  if (e) return e;
+  if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = c->coh_S;
+  const long long n0 = c->coh_n0;
+  // aux: [weights S doubles][selected rows S ints][out 3*n0]: rows with a zero weight are not read
+  std::vector<double> w(weights, weights + S);
+  std::vector<int> sel;
+  for (int j = 0; j < S; ++j)
+    if (w[j] != 0.0) sel.push_back(j);
+  const int nsel = (int)sel.size();
+  const size_t head = (size_t)S + ((size_t)S + 1) / 2;
+  w.resize(head);
+  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
+  if ((e = ensure(c, c->aux, (head + 3 * (size_t)n0) * sizeof(double)))) return e;
+  double *dw = (double *)c->aux.p, *dout = dw + head;
+  RT(rt_h2d(dw, w.data(), head * sizeof(double), c->stream));
+  const size_t cnt = (size_t)S * n0;
+  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
+  CohScaleAvgArgs a{dW, dA, dw, (const int *)(dw + S), nsel, dout, n0};
+  if ((e = launch<CohScaleAvgBody>(c, (unsigned)((n0 + NT - 1) / NT), 1, a))) return e;
+  RT(rt_d2h(out, dout, 3 * (size_t)n0 * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
 }
 
 int cwtb_set_coherence_precision(cwtb_ctx *c, int precision) {

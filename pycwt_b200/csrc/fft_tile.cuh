@@ -244,6 +244,15 @@ template <typename V> HD V ldg(const V *p) {
 #endif
 }
 
+// streaming (evict-first) load for data a kernel reads once
+template <typename V> HD V ld_stream(const V *p) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  return __ldcs(p);
+#else
+  return *p;
+#endif
+}
+
 // streaming (evict-first) store for results that are never re-read by the engine
 template <typename V> HD void st_stream(V *p, V v) {
 #if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)

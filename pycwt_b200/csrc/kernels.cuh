@@ -1593,6 +1593,185 @@ template <typename T> struct ScaleAvgBody {
   }
 };
 
+// ---- Bodies: reductions of the resident coherence (cwtb_wct_resident) ----------------------
+// WCT and aWCT are two [rows][n] double fields whose flat indices have the same alignment.
+
+// Per-row sums over the columns [lo_j, hi_j) where thr is null or WCT > thr_j (false for a NaN
+// threshold): [count, sum WCT, sum cos aWCT, sum sin aWCT].  CTA (bx, j) covers the fixed chunk
+// [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j's range with 16-byte streaming loads, reduces
+// its threads' sums in a fixed order and writes its partial; CohRowSumBody adds the partials of a
+// row in chunk order.  No atomics: repeated calls are bit-identical.
+struct CohRowStatsArgs {
+  const double *WCT, *aWCT;
+  const long long *lo, *hi;   // per row
+  const double *thr;          // per row, or null
+  double *part;               // [rows][nchunk][4]
+  long long n;
+  int nchunk, want_phase;     // aWCT is not read when want_phase == 0
+};
+struct CohRowStatsBody {
+  using Args = CohRowStatsArgs;
+  static constexpr int NTB = 256, NPHASE = 3;
+  static constexpr int U = 4;                                  // 16-byte loads in flight per field
+  static constexpr long long CHUNK = 2LL * 16 * NTB;           // 16 pairs of columns per thread
+  static constexpr size_t SMEM = (size_t)4 * (NTB + 32) * sizeof(double);
+  HD static void add(double (&s)[4], double w, double ang, const Args &a, bool has_thr, double t) {
+    if (has_thr && !(w > t)) return;
+    s[0] += 1.0;
+    s[1] += w;
+    if (a.want_phase) {
+      double sn, cs;
+      sincos_hd(ang, &sn, &cs);
+      s[2] += cs;
+      s[3] += sn;
+    }
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double *sm = (double *)smraw;          // [4][NTB] thread sums, then [4][32] lane sums
+    if constexpr (PH == 0) {
+      double s[4] = {0, 0, 0, 0};
+      const long long lo = a.lo[by], hi = a.hi[by];
+      const long long c0 = lo + (long long)bx * CHUNK;
+      if (c0 < hi) {
+        const long long c1 = c0 + CHUNK < hi ? c0 + CHUNK : hi;
+        const bool has_thr = a.thr != nullptr;
+        const double t = has_thr ? a.thr[by] : 0.0;
+        const size_t p0 = (size_t)by * a.n + c0, p1 = (size_t)by * a.n + c1;
+        const size_t v0 = p0 + (p0 & 1), v1 = p1 - (p1 & 1);   // [v0, v1): whole 16-byte pairs
+        if (tid == 0 && (p0 & 1)) add(s, a.WCT[p0], a.want_phase ? a.aWCT[p0] : 0.0, a, has_thr, t);
+        if (tid == 1 && (p1 & 1) && p1 - 1 >= v0)
+          add(s, a.WCT[p1 - 1], a.want_phase ? a.aWCT[p1 - 1] : 0.0, a, has_thr, t);
+        for (size_t q0 = v0 + 2 * (size_t)tid; q0 < v1; q0 += (size_t)2 * NTB * U) {
+          double2 w[U], g[U];
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const size_t q = q0 + (size_t)2 * NTB * u;
+            w[u] = make_double2(0, 0);
+            g[u] = w[u];
+            if (q < v1) {
+              w[u] = ld_stream((const double2 *)(a.WCT + q));
+              if (a.want_phase) g[u] = ld_stream((const double2 *)(a.aWCT + q));
+            }
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            if (q0 + (size_t)2 * NTB * u < v1) {
+              add(s, w[u].x, g[u].x, a, has_thr, t);
+              add(s, w[u].y, g[u].y, a, has_thr, t);
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) sm[k * NTB + tid] = s[k];
+    } else if constexpr (PH == 1) {
+      if (tid < 4 * 32) {
+        const int k = tid >> 5, l = tid & 31;
+        double v = 0;
+        for (int i = l; i < NTB; i += 32) v += sm[k * NTB + i];
+        sm[4 * NTB + tid] = v;
+      }
+    } else {
+      if (tid < 4) {
+        double v = 0;
+        for (int l = 0; l < 32; ++l) v += sm[4 * NTB + tid * 32 + l];
+        a.part[((size_t)by * a.nchunk + bx) * 4 + tid] = v;
+      }
+    }
+  }
+};
+
+// out[j][k] = sum over chunks b (in order) of part[j][b][k]
+struct CohRowSumArgs { const double *part; double *out; int rows, nchunk; };
+struct CohRowSumBody {
+  using Args = CohRowSumArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const int i = bx * NT + tid;
+    if (i >= 4 * a.rows) return;
+    const double *p = a.part + (size_t)(i >> 2) * a.nchunk * 4 + (i & 3);
+    double v = 0;
+    for (int b = 0; b < a.nchunk; ++b) v += p[(size_t)b * 4];
+    a.out[i] = v;
+  }
+};
+
+// Scale average of the two fields over the selected rows (the selected-rows pattern of
+// ScaleAvgBody): out[0][n] = sum_j w_j WCT[j,n], out[1][n] = sum_j w_j cos aWCT[j,n],
+// out[2][n] = sum_j w_j sin aWCT[j,n].  One thread per column adds the rows in order: no atomics.
+struct CohScaleAvgArgs {
+  const double *WCT, *aWCT;
+  const double *w;     // per row
+  const int *sel;      // rows with a non-zero weight, ascending (device)
+  int nsel;
+  double *out;         // [3][n]
+  long long n;
+};
+struct CohScaleAvgBody {
+  using Args = CohScaleAvgArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const long long n = (long long)bx * NT + tid;
+    if (n >= a.n) return;
+    double sw = 0, sc = 0, ss = 0;
+    int i = 0;
+    for (; i + 4 <= a.nsel; i += 4) {
+      double wv[4], av[4], wj[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int j = a.sel[i + u];
+        wj[u] = a.w[j];
+        wv[u] = ld_stream(&a.WCT[(size_t)j * a.n + n]);
+        av[u] = ld_stream(&a.aWCT[(size_t)j * a.n + n]);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        double sn, cs;
+        sincos_hd(av[u], &sn, &cs);
+        sw += wj[u] * wv[u];
+        sc += wj[u] * cs;
+        ss += wj[u] * sn;
+      }
+    }
+    for (; i < a.nsel; ++i) {
+      const int j = a.sel[i];
+      double sn, cs;
+      sincos_hd(ld_stream(&a.aWCT[(size_t)j * a.n + n]), &sn, &cs);
+      sw += a.w[j] * ld_stream(&a.WCT[(size_t)j * a.n + n]);
+      sc += a.w[j] * cs;
+      ss += a.w[j] * sn;
+    }
+    st_stream(&a.out[n], sw);
+    st_stream(&a.out[a.n + n], sc);
+    st_stream(&a.out[2 * a.n + n], ss);
+  }
+};
+
+// Strided sub-grid: out[r][c] = field[row0 + r row_step][col0 + c col_step] of either field
+// (outputs may be null).  Grid: (ceil(ncols / NT), nrows).
+struct CohWindowArgs {
+  const double *WCT, *aWCT;
+  double *oW, *oA;     // [nrows][ncols], or null
+  long long n;
+  int row0, row_step;
+  long long col0, col_step, ncols;
+};
+struct CohWindowBody {
+  using Args = CohWindowArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long c = (long long)bx * NT + tid;
+    if (c >= a.ncols) return;
+    const size_t src = (size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + c * a.col_step;
+    const size_t dst = (size_t)by * a.ncols + c;
+    if (a.oW) a.oW[dst] = a.WCT[src];
+    if (a.oA) a.oA[dst] = a.aWCT[src];
+  }
+};
+
 // ---- Body: real -> complex widening / complex -> real part ---------------------------------
 struct R2CArgs { const double *in; double2 *out; long long count; };
 struct R2CBody {

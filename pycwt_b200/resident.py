@@ -13,15 +13,35 @@ then do with W (pycwt/sample/simple_sample.py:64-96) are reductions of |W|^2:
 `cwt_resident` runs the same transform as `cwt` but keeps W in HBM and returns a handle whose
 methods evaluate those products on the device, so only O(S) or O(N) numbers cross the bus.
 The handle is valid until the next transform on the same engine.
+
+`wct_resident` does the same for the wavelet coherence (see the second half of this module).
 """
+import collections
+
 import numpy as np
 
 from . import _engine
-from .helpers import fft, fft_kwargs
-from .wavelet import (_check_parameter_wavelet, _nan_rows, _precision, _resolve_scales,
-                      _sync_padding)
+from .helpers import ar1, fft, fft_kwargs
+from .wavelet import (_check_parameter_wavelet, _coi, _nan_rows, _precision, _resolve_scales,
+                      _sync_padding, _wct_on_device, _wct_problem, _wct_significance)
 
-__all__ = ['cwt_resident', 'ResidentTransform']
+__all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence']
+
+
+def _coi_ranges(wavelet, dt, n0, period):
+    """Columns inside the cone of influence, per scale: period_j <= coi[n] holds on one centred
+    range [lo_j, hi_j)."""
+    c = wavelet.flambda() * wavelet.coi() * dt
+    # coi[n] = c * (n0/2 - |n - (n0-1)/2|) >= period  <=>  |n - (n0-1)/2| <= n0/2 - period/c
+    half = n0 / 2 - period / c
+    mid = (n0 - 1) / 2
+    lo = np.ceil(mid - half - 1e-12).astype(np.int64)
+    hi = np.floor(mid + half + 1e-12).astype(np.int64) + 1
+    empty = half < 0
+    lo = np.clip(lo, 0, n0)
+    hi = np.clip(hi, 0, n0)
+    hi[empty] = lo[empty]
+    return lo, hi
 
 
 def _live(method):
@@ -108,20 +128,8 @@ class ResidentTransform(object):
         return self.engine.power(len(self.scales), self.n0, rs)
 
     def coi_ranges(self):
-        """Columns inside the cone of influence, per scale: period_j <= coi[n] holds on one
-        centred range [lo_j, hi_j)."""
-        n0 = self.n0
-        c = self.wavelet.flambda() * self.wavelet.coi() * self.dt
-        # coi[n] = c * (n0/2 - |n - (n0-1)/2|) >= period  <=>  |n - (n0-1)/2| <= n0/2 - period/c
-        half = n0 / 2 - self.period / c
-        mid = (n0 - 1) / 2
-        lo = np.ceil(mid - half - 1e-12).astype(np.int64)
-        hi = np.floor(mid + half + 1e-12).astype(np.int64) + 1
-        empty = half < 0
-        lo = np.clip(lo, 0, n0)
-        hi = np.clip(hi, 0, n0)
-        hi[empty] = lo[empty]
-        return lo, hi
+        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
+        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
 
     @_live
     def global_power(self, inside_coi=False):
@@ -192,3 +200,203 @@ def cwt_resident(signal, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', freqs=None,
         eng.cwt(sig, dt, sj, family, param, precision, fetch=False)
         serial = eng.job_serial()
     return ResidentTransform(eng, wavelet, n0, dt, dj, sj, freqs, precision, serial)
+
+
+# ---- resident coherence ------------------------------------------------------------------------
+# `wct` hands the caller two float64 [S, n0] fields; at config 4 that is 600 MB over PCIe for a few
+# ms of GPU work.  What the reference's sample script (pycwt/sample/sample_xwt.py) and Grinsted et
+# al. (2004) then do with them are contours of WCT / sig95, phase arrows on a sub-grid and
+# reductions over regions of the (scale, time) plane.  `wct_resident` runs the same pipeline as
+# `wct(sig=False)` and keeps WCT and aWCT on the device, in a buffer of their own: the handle stays
+# valid across later cwt / xwt / wct / Monte-Carlo calls, until the next `wct_resident` on the same
+# engine or `release()`.
+
+MeanPhase = collections.namedtuple('MeanPhase', 'angle strength count')
+
+
+def _slice_range(s, n, name):
+    """(start, count, step) of a slice with step >= 1 over range(n)."""
+    if not isinstance(s, slice):
+        raise ValueError("%s must be a slice, got %r" % (name, s))
+    if s.step is not None and (not isinstance(s.step, (int, np.integer)) or isinstance(s.step, bool)
+                               or s.step < 1):
+        raise ValueError("%s: the step must be an integer >= 1, got %r" % (name, s.step))
+    try:
+        start, stop, step = s.indices(n)
+    except TypeError as exc:
+        raise ValueError("%s: %s" % (name, exc))
+    return start, len(range(start, stop, step)), step
+
+
+def _ratio(num, den):
+    """num / den, NaN where den == 0."""
+    num = np.asarray(num, dtype=float)
+    den = np.asarray(den, dtype=float)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        return np.where(den > 0, num / np.where(den > 0, den, 1.0), np.nan)
+
+
+class ResidentCoherence(object):
+    """WCT and aWCT [S, n0] of one `wct_resident` call, resident on the device."""
+
+    def __init__(self, engine, problem, precision, serial):
+        p = problem
+        self.engine = engine
+        self.wavelet = p.wavelet
+        self.n0 = int(p.n0)
+        self.dt = float(p.dt)
+        self.dj = p.dj
+        self.s0 = p.s0
+        self.J = p.J
+        self.scales = p.sj
+        self.freq = p.freq
+        self.precision = precision
+        self._y = (np.array(p.y1, copy=True), np.array(p.y2, copy=True))   # raw series, for ar1
+        self._serial = serial
+        self._coi = None
+
+    @property
+    def coi(self):
+        if self._coi is None:
+            self._coi = _coi(self.wavelet, self.dt, self.n0)
+        return self._coi
+
+    @property
+    def shape(self):
+        return (len(self.scales), self.n0)
+
+    @property
+    def period(self):
+        return 1.0 / np.asarray(self.freq)
+
+    def coi_ranges(self):
+        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
+        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
+
+    # -- bookkeeping ---------------------------------------------------------------------
+    def _check_live(self):
+        if self.engine.coherence_serial() != self._serial:
+            raise _engine.EngineError("this coherence is no longer resident: it was released or "
+                                      "another wct_resident has run on the same engine")
+
+    def release(self):
+        """Free the device buffer (16 bytes per scale and time point).  The handle is invalid
+        afterwards; releasing an invalid handle does nothing."""
+        with self.engine.lock:
+            if self.engine.coherence_serial() == self._serial:
+                self.engine.coherence_release()
+
+    def _ranges(self, inside_coi):
+        if inside_coi:
+            return self.coi_ranges()
+        S = len(self.scales)
+        return np.zeros(S, dtype=np.int64), np.full(S, self.n0, dtype=np.int64)
+
+    def _threshold(self, sig95):
+        if sig95 is None:
+            return None
+        thr = np.asarray(sig95, dtype=float)
+        if thr.shape != (len(self.scales),):
+            raise ValueError("sig95 must have one entry per scale (%d), got shape %s"
+                             % (len(self.scales), thr.shape))
+        return thr
+
+    # -- the products --------------------------------------------------------------------
+    @_live
+    def coherence(self):
+        """WCT (float64, S x n0), as returned by `wct(..., sig=False)`: the expensive fetch."""
+        S, n0 = self.shape
+        return self.engine.coherence_window(0, S, 1, 0, n0, 1, want_angle=False)[0]
+
+    @_live
+    def phase(self):
+        """aWCT (float64, S x n0), as returned by `wct(..., sig=False)`."""
+        S, n0 = self.shape
+        return self.engine.coherence_window(0, S, 1, 0, n0, 1, want_wct=False)[1]
+
+    @_live
+    def window(self, rows=slice(None), cols=slice(None)):
+        """(WCT[rows, cols], aWCT[rows, cols]) for two slices with steps >= 1, gathered on the
+        device: only the sub-grid crosses the bus (contour and phase-arrow plots)."""
+        S, n0 = self.shape
+        r0, nr, rs = _slice_range(rows, S, 'rows')
+        c0, nc, cs = _slice_range(cols, n0, 'cols')
+        if nr == 0 or nc == 0:
+            return np.empty((nr, nc)), np.empty((nr, nc))
+        return self.engine.coherence_window(r0, nr, rs, c0, nc, cs)
+
+    @_live
+    def significance(self, significance_level=0.95, mc_count=300, progress=True, cache=True,
+                     seed=None):
+        """Monte-Carlo significance level per scale, as `wct(..., sig=True)` computes it (lag-1
+        autocorrelations of the raw series, this coherence's dt, dj, s0, J, wavelet and
+        precision).  The coherence stays resident."""
+        a1, _, _ = ar1(self._y[0])
+        a2, _, _ = ar1(self._y[1])
+        return _wct_significance(a1, a2, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
+                                 significance_level=significance_level, wavelet=self.wavelet,
+                                 mc_count=mc_count, progress=progress, cache=cache, seed=seed,
+                                 precision=self.precision)
+
+    @_live
+    def global_coherence(self, inside_coi=False, sig95=None):
+        """Mean WCT per scale over the selected points: inside the cone of influence
+        (period_j <= coi[n]) if `inside_coi`, where WCT[j, n] > sig95[j] if `sig95` is given
+        (false where sig95[j] is NaN).  NaN for a scale without points."""
+        lo, hi = self._ranges(inside_coi)
+        st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95))
+        return _ratio(st[:, 1], st[:, 0])
+
+    @_live
+    def significant_fraction(self, sig95):
+        """Per scale, the fraction of the points inside the cone of influence where
+        WCT > sig95[j]; NaN for a scale without such points."""
+        lo, hi = self.coi_ranges()
+        st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95))
+        return _ratio(st[:, 0], hi - lo)
+
+    @_live
+    def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, sig95=None,
+                   per_scale=False):
+        """Circular mean of aWCT over the points of the scales with period_min <= period <
+        period_max, inside the cone of influence if `inside_coi`, where WCT > sig95 if given
+        (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
+        |sum e^{i aWCT}| / count, count), for the whole band or, with `per_scale`, per scale
+        (arrays; NaN angle and strength where the count is 0)."""
+        per = self.period
+        sel = (per >= period_min) & (per < period_max)
+        lo, hi = self._ranges(inside_coi)
+        lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
+        st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95), want_phase=True)
+        cnt, c, s = st[:, 0], st[:, 2], st[:, 3]
+        if not per_scale:
+            cnt, c, s = cnt.sum(), c.sum(), s.sum()
+        angle = np.where(cnt > 0, np.arctan2(s, c), np.nan)
+        strength = _ratio(np.hypot(c, s), cnt)
+        if per_scale:
+            return MeanPhase(angle, strength, cnt.astype(np.int64))
+        return MeanPhase(float(angle), float(strength), int(cnt))
+
+    @_live
+    def scale_avg(self, period_min, period_max):
+        """Two length-n0 series over the scales with period_min <= period < period_max: the mean
+        WCT and the circular mean phase atan2(sum sin aWCT, sum cos aWCT)."""
+        per = self.period
+        sel = (per >= period_min) & (per < period_max)
+        if not sel.any():
+            raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
+        out = self.engine.coherence_scale_avg(sel.astype(float))
+        return out[0] / float(sel.sum()), np.arctan2(out[2], out[1])
+
+
+def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
+                 precision='fp64', engine=None):
+    """Same coherence as `wct(y1, y2, dt, dj, s0, J, sig=False, wavelet=wavelet,
+    normalize=normalize, precision=precision)`, WCT and aWCT kept on the device.
+
+    Returns a `ResidentCoherence`.  Scales, boxcar, un-padded fallback to fp64 and the Paul / DOG
+    smoothing filter are resolved by the same code as `wct`'s."""
+    p = _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
+    eng = engine or _engine.default_engine()
+    serial = _wct_on_device(eng, p, eng.wct_resident)
+    return ResidentCoherence(eng, p, precision, serial)

@@ -362,17 +362,22 @@ def _boxcar_len(wavelet, dj):
     return int(np.round(wavelet.deltaj0 / dj * 2))
 
 
-def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
-        significance_level=0.95, wavelet='morlet', normalize=True, precision='fp64',
-        **kwargs):
-    """Wavelet coherence (reference wavelet.py:422-528).
+def _coi(wavelet, dt, n0):
+    """Cone of influence of an n0-point series (reference wavelet.py:118-120)."""
+    coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
+    return wavelet.flambda() * wavelet.coi() * dt * coi
 
-    Returns (WCT, aWCT, coi, freq, sig).  The two transforms, the |W|^2/s and W12/s
-    products, the Gaussian time smoothing, the scale boxcar and the coherence ratio run
-    on the GPU; `sig` comes from wct_significance (GPU Monte-Carlo) when sig=True.
-    `precision` (an extension of the reference signature): 'fp64' (default) or 'fp32', the
-    arithmetic of the device pipeline, also that of the significance test; WCT and aWCT are
-    float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6)."""
+
+class _WctProblem(object):
+    """What `wct` resolves on the host before the device pipeline (reference wavelet.py:461-497):
+    the wavelet, s0 and J, the raw and standardised series, the scales, the boxcar length and the
+    requested engine precision."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+def _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
     prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     if not hasattr(wavelet, 'smooth'):
@@ -387,18 +392,41 @@ def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
     y2, y2n, _ = _standardise(y2, normalize)
     n0 = y1n.size
     sj, freq = _resolve_scales(n0, dt, dj, s0, J, wavelet, None)
-    eng = _engine.default_engine()
     klen = _boxcar_len(wavelet, dj)
     if klen < 1:
         raise ValueError('smoothing window undefined for this wavelet (deltaj0 = -1)')
+    return _WctProblem(y1=y1, y2=y2, y1n=y1n, y2n=y2n, n0=n0, dt=dt, dj=dj, s0=s0, J=J,
+                       wavelet=wavelet, sj=sj, freq=freq, klen=klen, prec=prec)
+
+
+def _wct_on_device(eng, p, call):
+    """One engine transaction of the coherence pipeline: length policy (un-padded transforms run
+    in fp64), the Paul / DOG smoothing filter, then call(y1n, y2n, dt, dj, scales, family, param,
+    boxcar_len=, precision=).  Returns the call's result; `p.prec` becomes the precision used."""
     with eng.lock:
-        if _sync_padding(eng, len(y1n)):
-            prec = _engine.F64      # un-padded transforms run in fp64
-        with _smoothing_filter(eng, wavelet, sj, dt, len(y1n)):
-            WCT, aWCT = eng.wct(y1n, y2n, dt, dj, sj, *_family_of(wavelet), boxcar_len=klen,
-                                precision=prec)
-    coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
-    coi = wavelet.flambda() * wavelet.coi() * dt * coi
+        if _sync_padding(eng, len(p.y1n)):
+            p.prec = _engine.F64      # un-padded transforms run in fp64
+        with _smoothing_filter(eng, p.wavelet, p.sj, p.dt, len(p.y1n)):
+            return call(p.y1n, p.y2n, p.dt, p.dj, p.sj, *_family_of(p.wavelet), boxcar_len=p.klen,
+                        precision=p.prec)
+
+
+def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
+        significance_level=0.95, wavelet='morlet', normalize=True, precision='fp64',
+        **kwargs):
+    """Wavelet coherence (reference wavelet.py:422-528).
+
+    Returns (WCT, aWCT, coi, freq, sig).  The two transforms, the |W|^2/s and W12/s
+    products, the Gaussian time smoothing, the scale boxcar and the coherence ratio run
+    on the GPU; `sig` comes from wct_significance (GPU Monte-Carlo) when sig=True.
+    `precision` (an extension of the reference signature): 'fp64' (default) or 'fp32', the
+    arithmetic of the device pipeline, also that of the significance test; WCT and aWCT are
+    float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6)."""
+    p = _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
+    y1, y2, wavelet, s0, J, freq = p.y1, p.y2, p.wavelet, p.s0, p.J, p.freq
+    eng = _engine.default_engine()
+    WCT, aWCT = _wct_on_device(eng, p, eng.wct)
+    coi = _coi(wavelet, dt, p.n0)
     if sig:
         a1, b1, c1 = ar1(y1)
         a2, b2, c2 = ar1(y2)
