@@ -283,8 +283,12 @@ double cwtb_last_kernel_ms(cwtb_ctx *ctx);
 int cwtb_last_launch_count(cwtb_ctx *ctx);
 /* Fills `out` (capacity n) with one int per scale of the last call:
  * log2 of the pruned transform length K' (0 if the scale used the direct small-N
- * kernel), or -log2(Nc) if the scale ran on the expansion path with a coarse grid of Nc points.
+ * kernel), or -log2(Nc) if the scale ran on the expansion path with a coarse grid of Nc points,
+ * -1 for every scale of an un-padded transform, or CWTB_PLAN_OS (-2) if it ran as an overlap-save
+ * convolution with its truncated impulse response (coarse grids have at least 2^6 points, so the
+ * codes do not overlap).
  * Returns the number written. */
+#define CWTB_PLAN_OS (-2)
 int cwtb_last_plan(cwtb_ctx *ctx, int *out, int n);
 /* Re-run the kernels of the last cwtb_cwt_dev call `iters` times and return the
  * mean device time per iteration in ms (events on the launching stream). */

@@ -113,7 +113,12 @@ struct ClassRun {   // scales sharing one execution plan
   int log2Nc = 0;   // expansion: coarse grid length
   int taps = 0;     // expansion: interpolation taps
   long long woff = 0;   // expansion: offset of the class's weight table
+  int os = 0;           // overlap-save group + 1 (0: another path)
 };
+
+// overlap-save plan of one input scale (os_plan): group + 1 (0: not overlap-save), kept taps
+// [t1 - M + 1, t1] of its impulse response, offset of its H in the context's H buffer
+struct OsRow { int grp = 0, t1 = 0, M = 0; long long hoff = 0; };
 
 struct Job {
   bool valid = false;
@@ -133,6 +138,7 @@ struct Job {
   size_t coarse_elems = 0;        // elements of the coarse buffers used by the expansion rows
   int sig_is_f32 = 0;
   bool exact = false;             // un-padded mode: N = n0 (not a power of two), Bluestein transforms
+  std::vector<OsGroup> os_groups; // overlap-save groups (uploaded to cwtb_ctx::osgrp)
 };
 
 struct BluePlan {   // chirp tables of one transform length (device memory, owned by the context)
@@ -186,6 +192,8 @@ struct cwtb_ctx {
   int dense_margin = 2;          // pruned lengths within this many octaves of Np run as dense scales
                                  // (CWTB_DENSE_MARGIN)
   int expand_min_log2R = 0;      // log2 of the smallest Np / Nc (CWTB_EXPAND_MIN_R); 0: by kernel, see build_job
+  int os_on = 1;                 // overlap-save rows (OsBody; CWTB_OS=0: off)
+  Buf osH, osgrp;                // overlap-save: DFT_L of the truncated impulse responses, group table
   Buf *ztmp = nullptr;           // intermediate of two_kernel_rows (set per stream; default Z)
   void *comm = nullptr;          // ncclComm_t of cwtb_comm_init (one rank per context)
   int comm_world = 1, comm_rank = 0;
@@ -220,6 +228,7 @@ struct cwtb_ctx {
   std::map<std::array<long long, 3>, long long> wtab_index;   // (log2R, taps, round(beta*1e6)) -> offset
   std::vector<double> wtab_host; // host mirror of wtab (tables are appended, never moved)
   size_t wtab_uploaded = 0;      // elements already on the device
+  size_t wtab_max_bytes = (size_t)256 << 20;   // CWTB_WTAB_MB: host mirror size above which the cache starts over
   Buf ctr, sig, sig2, spec, Z, Zc[3], Y, B, W, W2, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
@@ -582,7 +591,8 @@ static long long expand_weights(cwtb_ctx *c, std::vector<double> &host, int log2
 }
 
 static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const double *scales, int S,
-                     int family, double param, int precision, bool have_table, int nbatch = 1) {
+                     int family, double param, int precision, bool have_table, int nbatch = 1,
+                     const std::vector<OsRow> *os = nullptr) {
   if (n0 < 1 || S < 1 || !(dt > 0)) return fail(c, CWTB_ERR_ARG, "bad n0 / n_scales / dt");
   if (family < 0 || family > 3) return fail(c, CWTB_ERR_ARG, "unknown wavelet family");
   if (family == CWTB_TABLE && !have_table) return fail(c, CWTB_ERR_ARG, "CWTB_TABLE needs a table");
@@ -590,13 +600,6 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     return fail(c, CWTB_ERR_ARG, "Paul/DOG order must be an integer in [1, 64]");
   if (n0 > (1ll << 28)) return fail(c, CWTB_ERR_UNSUPPORTED, "signal longer than 2^28");
   job = Job();
-  // expansion weight tables are cached across calls; start over if many transform geometries
-  // have piled up more than 256 MiB of them (offsets are per job, assigned below)
-  if (c->wtab_host.size() > ((size_t)32 << 20)) {
-    c->wtab_host.clear();
-    c->wtab_index.clear();
-    c->wtab_uploaded = 0;
-  }
   job.precision = precision;
   job.n0 = n0;
   job.log2N = ilog2((unsigned long long)n0);   // pycwt/helpers.py:27-30
@@ -696,7 +699,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     d.log2K = lk;
     job.plan_log2K[j] = job.exact ? -1 : ((N < 32) ? 0 : lk);
     // ---- band-limited expansion instead of the pruned transforms (kernels.cuh: ExpandBody) ----
-    d.ip_log2Nc = 0; d.ip_kc = 0; d.ip_w = 0; d.ip_pad_ = 0; d.ip_coff = 0; d.ip_woff = 0;
+    d.ip_log2Nc = 0; d.ip_kc = 0; d.ip_w = 0; d.os_grp = 0; d.ip_coff = 0; d.ip_woff = 0;
     d.ip_beta = 0; d.ip_dc = 0;
     const double xeps = precision == CWTB_F64 ? c->expand_eps : c->expand_eps32;
     if (xeps > 0 && !job.exact && family != CWTB_TABLE && khi >= klo && job.log2N >= 9 && band_limited) {
@@ -744,15 +747,23 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
         job.plan_log2K[j] = -d.ip_log2Nc;
       }
     }
+    if (os && (*os)[j].grp) {   // overlap-save (os_plan): replaces whatever was chosen above
+      d.ip_log2Nc = 0; d.ip_kc = 0; d.ip_w = 0; d.ip_woff = 0; d.ip_beta = 0; d.ip_dc = 0;
+      d.os_grp = (*os)[j].grp;
+      job.plan_log2K[j] = CWTB_PLAN_OS;
+    }
   }
   // one descriptor per (channel, scale) row; rows of channel ch are ch*S .. ch*S+S-1
   if (nbatch > 1) {
+    int ngrp = 0;   // overlap-save groups are per channel (one signal per launch block)
+    for (int j = 0; j < S; ++j) ngrp = std::max(ngrp, ds[j].os_grp);
     ds.resize((size_t)S * nbatch);
     for (int ch = 1; ch < nbatch; ++ch)
       for (int j = 0; j < S; ++j) {
         ScaleDesc d = ds[j];
         d.chan = ch;
         d.row = ch * S + j;
+        if (d.os_grp) d.os_grp += ch * ngrp;
         ds[(size_t)ch * S + j] = d;
       }
   }
@@ -763,6 +774,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
   // exact classes first (two-kernel, then single-kernel: descending K'), expansion classes last
   // (descending coarse length, then taps / weight table)
   auto sort_key = [&](const ScaleDesc &d) -> long long {
+    if (d.os_grp) return (1ll << 41) - d.os_grp;   // overlap-save groups first, in group order
     if (!d.ip_log2Nc) return (1ll << 40) + d.log2K;
     return ((long long)(64 - d.ip_w) << 32) + ((long long)d.ip_log2Nc << 24) - (d.ip_woff & 0xffffff);
   };
@@ -775,16 +787,24 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     bool same = !job.classes.empty();
     if (same) {
       const ClassRun &b = job.classes.back();
-      same = d.ip_log2Nc ? (b.expand && b.log2Nc == d.ip_log2Nc && b.taps == d.ip_w && b.woff == d.ip_woff)
-                         : (!b.expand && b.log2K == d.log2K);
+      same = d.os_grp ? b.os == d.os_grp
+           : d.ip_log2Nc ? (b.expand && b.log2Nc == d.ip_log2Nc && b.taps == d.ip_w && b.woff == d.ip_woff)
+                         : (!b.expand && !b.os && b.log2K == d.log2K);
     }
     if (!same) {
       ClassRun cl{d.log2K, i, 0};
       if (d.ip_log2Nc) { cl.expand = 1; cl.log2Nc = d.ip_log2Nc; cl.taps = d.ip_w; cl.woff = d.ip_woff; }
+      cl.os = d.os_grp;
       job.classes.push_back(cl);
     }
     job.classes.back().count++;
-    if (d.ip_log2Nc) {
+    if (d.os_grp) {
+      if (job.classes.back().count == 1) {
+        const OsRow &o = (*os)[d.row % S];
+        job.os_groups.push_back(OsGroup{i, 0, o.t1, OsBody<4>::L - o.M + 1, o.hoff});
+      }
+      job.os_groups.back().count++;
+    } else if (d.ip_log2Nc) {
       d.ip_coff = (long long)coff;
       coff += (size_t)1 << d.ip_log2Nc;
     } else if (d.log2K <= 10 || (d.log2K <= c->direct_max_log2 && d.log2K < job.log2N)) {  // single-kernel scale
@@ -1370,10 +1390,10 @@ static int chunk_rows(const cwtb_ctx *c, unsigned N, size_t elem_bytes) {
 }
 
 static bool class_single(const cwtb_ctx *c, const Job &job, const ClassRun &cl) {
-  return !cl.expand && (cl.log2K <= 10 || (cl.log2K <= c->direct_max_log2 && cl.log2K < job.log2N));
+  return !cl.expand && !cl.os && (cl.log2K <= 10 || (cl.log2K <= c->direct_max_log2 && cl.log2K < job.log2N));
 }
 static bool class_two_kernel(const cwtb_ctx *c, const Job &job, const ClassRun &cl) {
-  return !cl.expand && !class_single(c, job, cl);
+  return !cl.expand && !cl.os && !class_single(c, job, cl);
 }
 // two-kernel class that runs as ONE persistent launch over a ring of Z buffers
 static bool class_persistent(const cwtb_ctx *c, const ClassRun &cl) {
@@ -1662,10 +1682,24 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     c->cur = c->stream;
     if (e) return e;
   }
+  // ---- overlap-save groups (kernels.cuh: OsBody): one launch on the stream of the first chain ----
+  if (!job.os_groups.empty()) {
+    if constexpr (std::is_same<T, double>::value) {
+      unsigned gx = 0;
+      for (const OsGroup &g : job.os_groups)
+        gx = std::max<unsigned>(gx, (unsigned)((job.n0 + (long long)g.hop * OsBody<4>::P - 1) /
+                                               ((long long)g.hop * OsBody<4>::P)));
+      OsArgs oa{ddesc, (const OsGroup *)c->osgrp.p, dsig, (const double2 *)c->osH.p, W, Tw<T>::get(c),
+                job.n0, N, epi};
+      if ((e = launch<OsBody<4>>(c, gx, (unsigned)job.os_groups.size(), oa))) return e;
+    } else {
+      return fail(c, CWTB_ERR_STATE, "overlap-save rows run in fp64 only");
+    }
+  }
   int chain_no = 0;
   for (int pass = 0; pass < 2; ++pass)
   for (const ClassRun &cl : job.classes) {
-    if (cl.expand) continue;
+    if (cl.expand || cl.os) continue;
     const unsigned K = 1u << cl.log2K;
     const bool single = class_single(c, job, cl);
     if (single != (pass == 0)) continue;   // pass 0: single-kernel classes, pass 1: two-kernel chains
@@ -1921,6 +1955,8 @@ int cwtb_create(int device, cwtb_ctx **out) {
   if (const char *g = getenv("CWTB_EXPAND_EPS32")) c->expand_eps32 = std::max(0.0, atof(g));
   if (const char *g = getenv("CWTB_EXPAND_MIN_R")) c->expand_min_log2R = std::min(14, std::max(2, atoi(g)));
   if (const char *g = getenv("CWTB_EXPAND_MMA")) c->expand_mma = atoi(g) != 0;
+  if (const char *g = getenv("CWTB_OS")) c->os_on = atoi(g) != 0;
+  if (const char *g = getenv("CWTB_WTAB_MB")) c->wtab_max_bytes = (size_t)std::max(0, atoi(g)) << 20;
   if (const char *g = getenv("CWTB_PLAN_REUSE")) c->plan_reuse = atoi(g) != 0;
   if (const char *g = getenv("CWTB_DENSE_MARGIN")) c->dense_margin = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_L2_PERSIST")) c->l2_persist = atoi(g);
@@ -1957,7 +1993,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   cudaStreamSynchronize(c->stream);
 #endif
   cwtb_comm_destroy(c);
-  for (Buf *b : {&c->Zxs[0], &c->Zxs[1], &c->Zxs[2], &c->Zxs[3], &c->Zxs[4], &c->Zxs[5], &c->Zxs[6], &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cin, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
+  for (Buf *b : {&c->osH, &c->osgrp, &c->Zxs[0],&c->Zxs[1], &c->Zxs[2], &c->Zxs[3], &c->Zxs[4], &c->Zxs[5], &c->Zxs[6], &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cin, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
                  &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
@@ -2044,6 +2080,162 @@ int cwtb_sync(cwtb_ctx *c) {
   return 0;
 }
 
+// ---- overlap-save planning (kernels.cuh: OsBody) ----------------------------------------------
+// Cost model, us per row of 2^20 outputs on H100 (see DESIGN.md §4): the overlap-save kernel at
+// hop = L scaled by L / hop, against the two-kernel pair the row would otherwise take.  Measured at
+// config 2 (H100 80GB HBM3, 700 W): OsBody<4> 0.337 ms for rows j = 20..47 (83..263 taps, L / hop
+// 1.09..1.35), 12.0 us per row; the dense pair 22.3-23.2 us per row.  Rows that expand by R = 4 are
+// not candidates: their expansion kernel (7.3-7.8 us per row with 16-20 taps, plus a share of the
+// coarse transform) costs less than the overlap-save kernel even at hop = L.
+static const double kOsUs = 9.5;
+static const double kTwoKernelUs = 23.2;   // dense first + second kernel (PassABody<1024> + PassBBody<1024>)
+
+struct DevTmp {   // device scratch of the planner, freed on every path out
+  void *p = nullptr;
+  ~DevTmp() { if (p) rt_free(p); }
+};
+
+// Rows that would run the two-kernel exact path, fp64 and padded, whose band [k_lo, k_hi] stays
+// clear of Nyquist: their impulse response h_j = IDFT(norm conj psi^) decays like the wavelet in
+// time.  h_j is computed by the exact path on a unit impulse (x^ = 1, into W, which the call
+// overwrites anyway), truncated to the shortest window [t1 - M + 1, t1] around t = 0 that keeps all
+// of its l1 mass but band_eps, not counting taps at the rounding noise of that computation (at most
+// max(2 * the largest tap beyond L of t = 0, 8 ulp of max|h_j|)), and taken as
+// H_j = DFT_L(h_j mod L) / L.  A row whose h_j has a tap above 128 ulp of max|h_j| beyond L of t = 0
+// (a band cut at Nyquist, Paul's one-sided spectrum) or needs M > L/2 keeps its path, as does a row
+// the cost model prices higher.  Accepted rows are grouped by M, up to four to a group.
+// Plan-time cost: one exact transform of the candidate rows and a few host round trips, once per
+// geometry (CWTB_PLAN_REUSE keeps it out of repeated calls).
+static int os_plan(cwtb_ctx *c, const Job &job, double dt, int family, double param, std::vector<OsRow> &os) {
+  constexpr int L = OsBody<4>::L, GR = 4;
+  // a window of M taps (M <= L/2: hop >= L/2 + 1) against the two-kernel pair the row leaves
+  auto os_cheaper = [](int M) { return M <= L / 2 && kOsUs * L / (double)(L - M + 1) < kTwoKernelUs; };
+  os.assign(job.S, OsRow());
+  const unsigned N = job.N;
+  if (!c->os_on || job.precision != CWTB_F64 || job.exact || family == CWTB_TABLE ||
+      !(c->band_eps > 0) || !(c->expand_eps > 0) || N < 2u * L)
+    return 0;
+  const long long half = (long long)N / 2;
+  std::vector<int> cand;      // input scales
+  std::vector<double> cs;
+  for (const ScaleDesc &d : job.descs) {
+    if (d.chan != 0 || d.k_hi < d.k_lo || d.k_lo <= -half || d.k_hi >= ((long long)N - 1) / 2) continue;
+    if (d.ip_log2Nc || (d.log2K <= 10 || (d.log2K <= c->direct_max_log2 && d.log2K < job.log2N))) continue;
+    cand.push_back(d.row);
+    cs.push_back(d.s);
+  }
+  if (cand.empty()) return 0;
+  const int nc = (int)cand.size();
+  // impulse responses: the exact path (expansion off) on x = delta, n0 = Np, into W in chunks of
+  // as many rows of Np as the call's own W holds (at least one), so that W grows by less than one row
+  const size_t wcap = (size_t)job.S * job.nbatch * job.n0;
+  const int chunk = (int)std::max<size_t>(1, wcap / N);
+  int e = ensure(c, c->W, std::max<size_t>((size_t)chunk * N, wcap) * sizeof(double2));
+  if (e) return e;
+  double2 *h = (double2 *)c->W.p;
+  DevTmp dimp, part;
+  if (rt_malloc(&dimp.p, (size_t)N * sizeof(double))) return fail(c, CWTB_ERR_NOMEM, "device allocation failed");
+  {
+    std::vector<double> delta(N, 0.0);
+    delta[0] = 1.0;
+    RT(rt_h2d(dimp.p, delta.data(), (size_t)N * sizeof(double), c->stream));
+    RT(rt_sync(c->stream));
+  }
+  const int nblk = 64;
+  if (rt_malloc(&part.p, (size_t)chunk * nblk * sizeof(double))) return fail(c, CWTB_ERR_NOMEM, "device allocation failed");
+  std::vector<double> farmax(nc, 0.0);            // largest tap beyond L of t = 0 (device)
+  std::vector<double2> win((size_t)nc * 2 * L);   // the taps within L: h[t], t = -L .. L-1 (host)
+  for (int r0 = 0; r0 < nc; r0 += chunk) {
+    const int nr = std::min(chunk, nc - r0);
+    Job imp;
+    const double xeps = c->expand_eps;
+    c->expand_eps = 0;
+    e = build_job(c, imp, (long long)N, dt, cs.data() + r0, nr, family, param, CWTB_F64, false, 1);
+    c->expand_eps = xeps;
+    if (e) return e;
+    if ((e = upload_descs(c, imp))) return e;
+    if ((e = run_job<double>(c, imp, (const double *)dimp.p, h, EPI_STORE))) return e;
+    if (N > 2u * L) {
+      AbsMaxArgs aa{h, (double *)part.p, (long long)N, (long long)L, (long long)N - L, nblk};
+      if ((e = launch<AbsMaxBody>(c, nblk, nr, aa))) return e;
+      std::vector<double> ph((size_t)nr * nblk);
+      RT(rt_d2h(ph.data(), part.p, ph.size() * sizeof(double), c->stream));
+      RT(rt_sync(c->stream));
+      for (int r = 0; r < nr; ++r)
+        for (int b = 0; b < nblk; ++b) farmax[r0 + r] = std::max(farmax[r0 + r], ph[(size_t)r * nblk + b]);
+    }
+    for (int r = 0; r < nr; ++r) {
+      RT(rt_d2h(&win[(size_t)(r0 + r) * 2 * L], h + (size_t)r * N + (N - L), L * sizeof(double2), c->stream));
+      RT(rt_d2h(&win[(size_t)(r0 + r) * 2 * L + L], h + (size_t)r * N, L * sizeof(double2), c->stream));
+    }
+    RT(rt_sync(c->stream));
+  }
+  // truncation
+  struct Acc { int r, t0, t1; };
+  std::vector<Acc> acc;
+  std::vector<double> m(2 * L), pre(2 * L + 1);
+  for (int r = 0; r < nc; ++r) {
+    const double2 *w = &win[(size_t)r * 2 * L];
+    double mx = farmax[r];
+    for (int i = 0; i < 2 * L; ++i) mx = std::max(mx, std::max(std::fabs(w[i].x), std::fabs(w[i].y)));
+    const double ulp = 2.220446049250313e-16 * mx;
+    if (!(mx > 0) || farmax[r] > 128 * ulp) continue;
+    // beyond L the response is rounding noise of its own computation: taps within L count from
+    // twice that level up (8 ulp where the far region is empty)
+    const double floor_ = std::max(2 * farmax[r], 8 * ulp);
+    double l1 = 0;
+    pre[0] = 0;
+    for (int i = 0; i < 2 * L; ++i) {
+      const double a = std::hypot(w[i].x, w[i].y);
+      l1 += a;
+      m[i] = std::max(std::fabs(w[i].x), std::fabs(w[i].y)) > floor_ ? a : 0.0;
+      pre[i + 1] = pre[i] + m[i];
+    }
+    const double tol = c->band_eps * l1;
+    int t0 = 1, t1 = 0;
+    for (int M = 1; M <= L / 2 && t0 > t1; ++M)
+      for (int a = -(M - 1); a <= 0; ++a) {   // window [a, a + M - 1] contains t = 0
+        if (pre[2 * L] - (pre[a + M + L] - pre[a + L]) <= tol) { t0 = a; t1 = a + M - 1; break; }
+      }
+    if (t0 > t1) continue;
+    if (!os_cheaper(t1 - t0 + 1)) continue;
+    acc.push_back({r, t0, t1});
+  }
+  if (acc.empty()) return 0;
+  // groups of up to GR rows of similar M; a group runs at the hop of the union of its rows' windows,
+  // so a row joins the group only while the cost model still prices that hop below the row's path.
+  // Within a group, rows in input order (the order of the class-sorted descriptors) so that H of
+  // group row i sits at hoff + i*L.
+  std::stable_sort(acc.begin(), acc.end(), [](const Acc &a, const Acc &b) { return a.t1 - a.t0 < b.t1 - b.t0; });
+  const int na = (int)acc.size();
+  std::vector<double2> hl((size_t)na * L, make_double2(0.0, 0.0));
+  long long slot = 0;
+  for (int g0 = 0, g1 = 0, grp = 1; g0 < na; g0 = g1, ++grp) {
+    int t0 = acc[g0].t0, t1 = acc[g0].t1;
+    for (g1 = g0 + 1; g1 < na && g1 - g0 < GR; ++g1) {
+      const int u0 = std::min(t0, acc[g1].t0), u1 = std::max(t1, acc[g1].t1);
+      if (!os_cheaper(u1 - u0 + 1)) break;
+      t0 = u0; t1 = u1;
+    }
+    std::sort(acc.begin() + g0, acc.begin() + g1, [&](const Acc &a, const Acc &b) { return cand[a.r] < cand[b.r]; });
+    for (int i = g0; i < g1; ++i) {
+      OsRow &o = os[cand[acc[i].r]];
+      o.grp = grp; o.t1 = t1; o.M = t1 - t0 + 1; o.hoff = (slot - (i - g0)) * L;
+      const double2 *w = &win[(size_t)acc[i].r * 2 * L];
+      for (int t = acc[i].t0; t <= acc[i].t1; ++t)
+        hl[(size_t)slot * L + ((t + L) % L)] = make_double2(w[t + L].x / L, w[t + L].y / L);
+      ++slot;
+    }
+  }
+  if ((e = ensure(c, c->osH, (size_t)na * L * sizeof(double2)))) return e;
+  DevTmp dh;
+  if (rt_malloc(&dh.p, (size_t)na * L * sizeof(double2))) return fail(c, CWTB_ERR_NOMEM, "device allocation failed");
+  RT(rt_h2d(dh.p, hl.data(), hl.size() * sizeof(double2), c->stream));
+  if ((e = fft_rows<double, -1>(c, dh.p, 0, L, L, (double2 *)c->osH.p, L, L, na))) return e;
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
 static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, int S, int family,
                    double param, int precision, const void *table, int nbatch = 1) {
   if (!c) return CWTB_ERR_ARG;
@@ -2061,8 +2253,25 @@ static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, i
   key.scales.assign(scales, scales + std::max(S, 0));
   if (c->plan_reuse && family != CWTB_TABLE && c->job.valid && key == c->plan_key) return 0;
   c->plan_key = cwtb_ctx::PlanKey();   // invalid until the new plan is complete
+  // expansion weight tables are cached across calls; start over if many transform geometries have
+  // piled up more than CWTB_WTAB_MB of them.  Only here, before any planning of this call: the
+  // tables a plan appends must stay until upload_descs has uploaded them (os_plan plans a second job
+  // in between).
+  if (c->wtab_host.size() * sizeof(double) > c->wtab_max_bytes) {
+    c->wtab_host.clear();
+    c->wtab_index.clear();
+    c->wtab_uploaded = 0;
+  }
   int e = build_job(c, c->job, n0, dt, scales, S, family, param, precision, table != nullptr, nbatch);
   if (e) return e;
+  std::vector<OsRow> os;
+  if ((e = os_plan(c, c->job, dt, family, param, os))) return e;
+  if (std::any_of(os.begin(), os.end(), [](const OsRow &o) { return o.grp != 0; })) {
+    if ((e = build_job(c, c->job, n0, dt, scales, S, family, param, precision, table != nullptr, nbatch, &os))) return e;
+    const Job &job = c->job;
+    if ((e = ensure(c, c->osgrp, job.os_groups.size() * sizeof(OsGroup)))) return e;
+    RT(rt_h2d(c->osgrp.p, job.os_groups.data(), job.os_groups.size() * sizeof(OsGroup), c->stream));
+  }
   if (family == CWTB_TABLE) {
     size_t bytes = (size_t)S * c->job.N * sizeof(double2);
     if ((e = ensure(c, c->table, bytes))) return e;

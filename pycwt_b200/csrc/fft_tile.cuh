@@ -438,14 +438,17 @@ HD void pass_mid(cx<T> *sm, const cx<T> *__restrict__ tw, Loader &ld, int tid) {
 
 // Final pass: radix R = Plan<K>::RL on K/R sub-transforms per row, lanes over b.
 // Storer interface: store(b, qlow, qstride, x[R])  with output index q = qlow + c*qstride.
-template <typename T, int K, int SIGN, class Storer, bool ROWS = false>
+// GMAJOR: lanes over the sub-transform g instead, for outputs whose contiguous global index is q
+// (a warp then stores runs of R1 consecutive q: whole 32-byte sectors; the skewed rows keep the reads
+// conflict-free).
+template <typename T, int K, int SIGN, class Storer, bool ROWS = false, bool GMAJOR = false>
 HD void pass_last(const cx<T> *sm, Storer &st, int tid) {
   using V = cx<T>;
   using LY = Lay<T, K, ROWS>;
   constexpr int NT = TileCfg<T>::NT;
   constexpr int R = Plan<K>::RL, G = K / R, P = LY::P;
   for (int idx = tid; idx < G * P; idx += NT) {
-    const int b = idx % P, g = idx / P;
+    const int b = GMAJOR ? idx / G : idx % P, g = GMAJOR ? idx % G : idx / P;
     V x[R];
 #pragma unroll
     for (int i = 0; i < R; ++i) x[i] = sm[LY::phys(b, g * R + i)];

@@ -24,7 +24,7 @@ struct ScaleDesc {
   int ip_log2Nc;   // coarse grid length Nc = 1 << ip_log2Nc  (0: exact pruned-transform path)
   int ip_kc;       // centre bin of the band (signed): the coarse grid holds the band shifted to 0
   int ip_w;        // taps of the interpolation kernel
-  int ip_pad_;
+  int os_grp;      // overlap-save group + 1 (OsBody; 0: another path)
   long long ip_coff;   // offset of this row's Nc coarse samples in the coarse buffers
   long long ip_woff;   // offset of the [taps][R] weight table of this row's class
   double ip_beta;      // Kaiser-Bessel shape parameter
@@ -488,6 +488,164 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
       }
       pass_last<T, K, SIGN, OutStorer<T>, true>(sm, st, tid);
       if (tid == 0) tb.inval();   // every thread passed wait() two barriers ago
+    }
+  }
+};
+
+// ---- Body: overlap-save rows (fp64, short impulse response) ---------------------------------
+// Row j of W is the circular convolution of the signal with h_j = IDFT(norm conj psi^) (what the
+// exact path gives for x^ = 1); the planner keeps its taps t in [t1 - M + 1, t1] (engine.cu: os_plan).
+// A CTA owns P consecutive blocks of hop = L - M + 1 outputs for a group of up to G rows sharing
+// (t1, M):
+//   y_b[i] = x[(n_b - t1 + i) mod Np] (0 past n0),  n_b = (bx*P + b) * hop,
+//   W[n_b + i - t1] = IDFT_L(DFT_L(y_b) * H_j)[i]  for t1 <= i < t1 + hop,  H_j = DFT_L(h_j mod L) / L.
+// The forward transform of the real blocks is taken once and kept in shared memory as its
+// non-negative half (X[L - k] = conj X[k]); each row of the group multiplies it by H_j while the
+// inverse transform is loaded, and stores its hop valid outputs contiguously.
+struct OsGroup {
+  int first, count;  // descriptors first .. first + count (one class of the sorted array)
+  int t1, hop;
+  long long hoff;    // H of the group's first row; the others follow, L entries each
+};
+struct OsArgs {
+  const ScaleDesc *descs;
+  const OsGroup *groups;
+  const double *sig;   // real signals, n0 samples per channel (ScaleDesc::chan)
+  const double2 *H;
+  double2 *W;
+  const double2 *tw;
+  long long n0;
+  unsigned N;
+  int epi;             // EPI_STORE / EPI_MULCONJ
+};
+
+template <int L, int R> struct OsSigLoader {
+  const double *x;
+  long long start, n0;   // start: n_0 - t1 of the tile's first block
+  unsigned nmask;
+  int hop, base, stride;
+  HD void begin(int base_, int stride_, int, int) { base = base_; stride = stride_; }
+  HD void load(int b, double2 (&v)[R]) const {
+    const long long s = start + (long long)b * hop + base;
+#pragma unroll
+    for (int i = 0; i < R; ++i) {
+      const long long n = (s + (long long)i * stride) & (long long)nmask;   // circular modulo Np
+      v[i] = make_double2(n < n0 ? ldg(&x[n]) : 0.0, 0.0);
+    }
+  }
+};
+template <int L> struct OsHalfStorer {
+  double2 *xs;   // [P][L/2 + 1]
+  template <int R> HD void store(int b, int ql, int qs, double2 (&x)[R]) const {
+#pragma unroll
+    for (int c = 0; c < R; ++c) {
+      const int q = ql + c * qs;
+      if (q <= L / 2) xs[b * (L / 2 + 1) + q] = x[c];
+    }
+  }
+};
+template <int L, int R> struct OsSpecLoader {
+  const double2 *xs, *H;
+  int base, stride;
+  double2 hv[R];
+  HD void begin(int base_, int stride_, int, int) {
+    base = base_; stride = stride_;
+#pragma unroll
+    for (int i = 0; i < R; ++i) hv[i] = ldg(&H[base + i * stride]);
+  }
+  HD void load(int b, double2 (&v)[R]) const {
+#pragma unroll
+    for (int i = 0; i < R; ++i) {
+      const int q = base + i * stride;
+      const double2 y = q <= L / 2 ? xs[b * (L / 2 + 1) + q] : cconj(xs[b * (L / 2 + 1) + L - q]);
+      v[i] = cmul(y, hv[i]);
+    }
+  }
+};
+struct OsStorer {
+  double2 *row;
+  long long nb0, n0;   // W index of tile position i of block b: nb0 + b*hop + i
+  int t1, hop, epi;
+  template <int R> HD void store(int b, int ql, int qs, double2 (&x)[R]) const {
+    const long long nb = nb0 + (long long)b * hop;
+#pragma unroll
+    for (int c = 0; c < R; ++c) {
+      const int i = ql + c * qs;
+      const long long n = nb + i;
+      if (i >= t1 && i < t1 + hop && n < n0) {
+        if (epi == EPI_STORE) st_stream(&row[n], x[c]);
+        else row[n] = cmul(row[n], cconj(x[c]));
+      }
+    }
+  }
+};
+
+template <int G> struct OsBody {
+  static constexpr int L = 1024;
+  static constexpr int NTB = TileCfg<double>::NT;
+  static constexpr int NT = NTB;
+  using Args = OsArgs;
+  using LY = Lay<double, L>;
+  static constexpr int P = LY::P;
+  static_assert(Plan<L>::NP == 3, "overlap-save phases assume a three-pass tile plan");
+  static constexpr int NPHASE = 3 + 3 * G;
+  static constexpr size_t SMEM = LY::TILE_BYTES + (size_t)P * (L / 2 + 1) * sizeof(double2);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double2 *sm = (double2 *)smraw;
+    double2 *xs = (double2 *)((char *)smraw + LY::TILE_BYTES);
+    const OsGroup g = a.groups[by];
+    const long long n_first = (long long)bx * P * g.hop;
+    if (n_first >= a.n0) return;   // whole CTA: no block of this tile holds outputs
+    if constexpr (PH == 0) {
+      OsSigLoader<L, Plan<L>::R1> ld;
+      ld.x = a.sig + (size_t)a.descs[g.first].chan * a.n0; ld.start = n_first - g.t1; ld.n0 = a.n0; ld.nmask = a.N - 1; ld.hop = g.hop;
+      tile_first<double, L, -1>(sm, a.tw, ld, tid);
+    } else if constexpr (PH == 1) {
+      tile_second<double, L, -1>(sm, a.tw, tid);
+    } else if constexpr (PH == 2) {
+      OsHalfStorer<L> st{xs};
+      pass_last<double, L, -1, OsHalfStorer<L>, false, true>(sm, st, tid);
+    } else {
+      constexpr int r = (PH - 3) / 3, step = (PH - 3) % 3;
+      if (r >= g.count) return;
+      if constexpr (step == 0) {
+        OsSpecLoader<L, Plan<L>::R1> ld;
+        ld.xs = xs; ld.H = a.H + g.hoff + (long long)r * L;
+        tile_first<double, L, +1>(sm, a.tw, ld, tid);
+      } else if constexpr (step == 1) {
+        tile_second<double, L, +1>(sm, a.tw, tid);
+      } else {
+        OsStorer st;
+        st.row = a.W + (size_t)a.descs[g.first + r].row * a.n0;
+        st.nb0 = n_first - g.t1; st.n0 = a.n0; st.t1 = g.t1; st.hop = g.hop; st.epi = a.epi;
+        pass_last<double, L, +1, OsStorer, false, true>(sm, st, tid);
+      }
+    }
+  }
+};
+
+// largest |h[t]| of rows of h over t in [lo, hi), one partial per CTA (out[by * gridDim.x + bx]):
+// the planner's test that an impulse response has no taps above its rounding floor far from t = 0
+struct AbsMaxArgs { const double2 *h; double *out; long long pitch, lo, hi; int nblk; };
+struct AbsMaxBody {
+  using Args = AbsMaxArgs;
+  static constexpr int NPHASE = 2;
+  static constexpr size_t SMEM = NT * sizeof(double);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double *sm = (double *)smraw;
+    if constexpr (PH == 0) {
+      const long long chunk = (a.hi - a.lo + a.nblk - 1) / a.nblk;
+      const long long s = a.lo + bx * chunk, e = s + chunk < a.hi ? s + chunk : a.hi;
+      double m = 0;
+      for (long long i = s + tid; i < e; i += NT) {
+        const double2 v = a.h[(size_t)by * a.pitch + i];
+        m = fmax(m, fmax(fabs(v.x), fabs(v.y)));
+      }
+      sm[tid] = m;
+    } else if (tid == 0) {
+      double m = 0;
+      for (int i = 0; i < NT; ++i) m = fmax(m, sm[i]);
+      a.out[(size_t)by * a.nblk + bx] = m;
     }
   }
 };
