@@ -156,14 +156,10 @@ struct cwtb_ctx {
   int device = 0;
   rt_stream stream{};
   rt_stream aux_stream{};        // single-kernel classes run here, concurrently with the two-kernel chains
-  rt_stream prio_stream{};       // highest-priority stream: the chain of small launches in front of the
-                                 // expansion kernels (band products + coarse transforms) -- its CTAs are
-                                 // dispatched before the pending CTAs of the big launches on the other streams
-  rt_stream prio_aux[7]{};       // the coarse transforms of different lengths are independent: they fan out
-                                 // over the priority stream and these (own intermediates Zxs[]), so that the
-                                 // chain in front of the expansion kernels is as long as its longest member,
-                                 // not their sum (CWTB_PRIO_FAN=1..8 streams)
-  int prio_fan = 4;
+  rt_stream prio_stream{};       // highest-priority stream: the coarse transforms in front of the expansion
+                                 // kernels (coarse lengths above 1024) -- its CTAs are dispatched before the
+                                 // pending CTAs of the big launches on the other streams
+  rt_stream prio_short{};        // the same priority: the coarse transforms of lengths up to 1024
   int prio_mode = 1;             // CWTB_PRIO: 0 = no priority stream, 1 = coarse chain, 2 = coarse chain and
                                  // the expansion kernels
   rt_stream chain_streams[3]{};  // two-kernel classes rotate over the engine's stream and these (own Z
@@ -194,7 +190,6 @@ struct cwtb_ctx {
   int expand_min_log2R = 0;      // log2 of the smallest Np / Nc (CWTB_EXPAND_MIN_R); 0: by kernel, see build_job
   int os_on = 1;                 // overlap-save rows (OsBody; CWTB_OS=0: off)
   Buf osH, osgrp;                // overlap-save: DFT_L of the truncated impulse responses, group table
-  Buf *ztmp = nullptr;           // intermediate of two_kernel_rows (set per stream; default Z)
   void *comm = nullptr;          // ncclComm_t of cwtb_comm_init (one rank per context)
   int comm_world = 1, comm_rank = 0;
   Buf comm_send, comm_recv;      // device staging of the host-buffer collectives
@@ -222,9 +217,8 @@ struct cwtb_ctx {
   Buf filt;                      // caller-supplied time-smoothing responses [S][N] (cwtb_set_smooth_filter)
   int filt_rows = 0;
   long long filt_n = 0;
-  Buf Zxs[7];                    // intermediates of the coarse transforms on prio_aux[]
-  Buf Zx, Cin, Cout, wtab;       // expansion path: its own transform intermediate, coarse spectra /
-                                 // samples, interpolation weight tables
+  Buf Zx, Cout, wtab;            // expansion path: intermediate of the coarse transforms, coarse samples,
+                                 // interpolation weight tables
   std::map<std::array<long long, 3>, long long> wtab_index;   // (log2R, taps, round(beta*1e6)) -> offset
   std::vector<double> wtab_host; // host mirror of wtab (tables are appended, never moved)
   size_t wtab_uploaded = 0;      // elements already on the device
@@ -280,9 +274,9 @@ struct cwtb_ctx {
   std::set<void *> pinned, devallocs;
 #ifndef CWTB_HOST_EMU
   cudaEvent_t e0{}, e1{};
-  cudaEvent_t ev_fork{}, ev_join{}, ev_joinc[3]{}, ev_coarse{};
+  cudaEvent_t ev_fork{}, ev_join{}, ev_joinc[3]{}, ev_coarse{}, ev_coarse_short{};
   cudaEvent_t ev_h2d[2]{}, ev_used[2]{};
-  cudaEvent_t ev_xband{}, ev_pj[7]{}, ev_angle{};
+  cudaEvent_t ev_angle{};
 #endif
 };
 
@@ -723,7 +717,8 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
       // coarse transform of Np/4 points): 2.866 against 2.925 ms per step on H100 at 400 W, spread 0.012 ms.
       // The scalar kernel's trade-off at R = 4 has not been measured on H100.
       const int min_log2R = c->expand_min_log2R ? c->expand_min_log2R : (mma ? 2 : 3);
-      for (int l = lmin; l <= lmin + 2 && job.log2N - l >= min_log2R; ++l) {
+      // (coarse grids of at most 2^20 points: their transforms run as one 1024-point pass pair, CoarseABody)
+      for (int l = lmin; l <= lmin + 2 && l <= 20 && job.log2N - l >= min_log2R; ++l) {
         double xi_b = 0;
         int w = expand_taps((double)hw / (double)(1ll << l), xeps, precision != CWTB_F64, max_taps, &xi_b);
         if (!w) continue;
@@ -877,7 +872,7 @@ static int two_kernel_rows(cwtb_ctx *c, const void *in, int real_in, long long i
   // rows per chunk: the intermediate of a chunk (rows_chunk_bytes, default 64 MiB) stays in L2
   // between the two kernels
   const int chunk = std::max(1, std::min(nrows, (int)std::max<size_t>(1, c->rows_chunk_bytes / ((size_t)n * sizeof(cx<T>)))));
-  Buf &Zt = c->ztmp ? *c->ztmp : c->Z;
+  Buf &Zt = c->Z;
   if ((e = ensure(c, Zt, (size_t)chunk * n * sizeof(cx<T>)))) return e;
   for (int r0 = 0; r0 < nrows; r0 += chunk) {
     const int nr = std::min(chunk, nrows - r0);
@@ -1456,6 +1451,24 @@ static int launch_persistent(cwtb_ctx *c, unsigned gm, unsigned rows, const type
 }
 #endif
 
+// One ragged launch of Body (CoarseRowsBody / CoarseABody / CoarseBBody) over the given segments:
+// a single launch unless there are more than CSEG_MAX of them
+template <class Body, typename T>
+static int launch_coarse(cwtb_ctx *c, CoarseArgs<T> a, const std::vector<CoarseSeg> &segs) {
+  for (size_t s0 = 0; s0 < segs.size(); s0 += CSEG_MAX) {
+    a.nseg = (int)std::min<size_t>(CSEG_MAX, segs.size() - s0);
+    unsigned ctas = 0;
+    for (int i = 0; i < a.nseg; ++i) {
+      a.seg[i] = segs[s0 + i];
+      a.seg[i].cta0 = (int)ctas;
+      ctas += (unsigned)Body::ctas(a.seg[i].log2Nc, a.seg[i].count);
+    }
+    int e = launch<Body>(c, ctas, 1, a);
+    if (e) return e;
+  }
+  return 0;
+}
+
 template <typename T, int TAPS>
 static int launch_expand_t(cwtb_ctx *c, const ExpandArgs<T> &a, int rows, int min_log2Nc) {
   using B = ExpandBody<T, TAPS>;
@@ -1519,7 +1532,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   int e;
   // whatever path leaves this function (also an error in the middle of the fork), the launcher
   // is back on the engine's stream afterwards
-  struct CurGuard { cwtb_ctx *c; ~CurGuard() { c->cur = c->stream; c->prof_tag = ""; c->ztmp = nullptr; } } cur_guard{c};
+  struct CurGuard { cwtb_ctx *c; ~CurGuard() { c->cur = c->stream; c->prof_tag = ""; } } cur_guard{c};
   if ((e = ensure(c, c->spec, (size_t)job.nbatch * N * sizeof(V)))) return e;
   if (!Wout) {
     if ((e = ensure(c, c->W, (size_t)S * job.n0 * sizeof(V)))) return e;
@@ -1582,100 +1595,87 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
 #else
   const bool split2 = false;
 #endif
-  // ---- expansion classes (kernels.cuh: ExpandBody): coarse band spectra of every expansion row
-  // in one launch, one batched coarse transform per coarse length, one expansion launch per class.
-  // They run on the second stream like the single-kernel classes (own transform intermediate Zx).
+  // ---- expansion classes (kernels.cuh: ExpandBody): the coarse transforms of every expansion row
+  // form their coarse spectra while they fill their tiles, in one launch for the coarse lengths up
+  // to 1024 and one launch pair for the longer ones; then one expansion launch per tap count.
   if (job.coarse_elems) {
-#ifndef CWTB_HOST_EMU
-    // the ~30 small launches in front of the expansion kernels go to the priority stream: queued
-    // behind the big launches of the other streams they would only advance in those launches' tails
     const bool prio = split && c->prio_mode > 0;
-    if (prio) RT(cudaStreamWaitEvent(c->prio_stream, c->ev_fork, 0));
+#ifndef CWTB_HOST_EMU
+    // the coarse launches go to high-priority streams: queued behind the big launches of the other
+    // streams they would only advance in those launches' tails.  Short and long coarse lengths run
+    // side by side; an expansion launch waits only for the lengths it reads.
+    if (prio) {
+      RT(cudaStreamWaitEvent(c->prio_stream, c->ev_fork, 0));
+      RT(cudaStreamWaitEvent(c->prio_short, c->ev_fork, 0));
+    }
     if (split) c->cur = prio ? c->prio_stream : c->aux_stream;
 #endif
-    if ((e = ensure(c, c->Cin, job.coarse_elems * sizeof(V)))) return e;
     if ((e = ensure(c, c->Cout, job.coarse_elems * sizeof(V)))) return e;
-    int first = -1, maxl = 0, nrows = 0;
-    for (const ClassRun &cl : job.classes)
-      if (cl.expand) {
-        if (first < 0) first = cl.first;
-        maxl = std::max(maxl, cl.log2Nc);
-        nrows += cl.count;
-      }
-    ExpandBandArgs<T> xa{ddesc, spec, (V *)c->Cin.p, fam, N, first};
-    constexpr int XPER = ExpandBandBody<T>::PER;
-    if ((e = launch<ExpandBandBody<T>>(c, ((1u << maxl) + NT * XPER - 1) / (NT * XPER), nrows, xa))) return e;
-    c->ztmp = &c->Zx;
-    c->prof_tag = "coarse:";
-#ifndef CWTB_HOST_EMU
-    const int fan = prio ? c->prio_fan : 1;   // groups of one coarse length rotate over this many streams
-    int fan_used = 1, group = 0;
-    if (fan > 1) RT(cudaEventRecord(c->ev_xband, c->prio_stream));
-#endif
-    for (size_t ci = 0; ci < job.classes.size() && !e; ++ci) {
+    // segments: consecutive expansion rows of one coarse length (their coarse rows are contiguous)
+    std::vector<CoarseSeg> short_segs, long_segs;
+    size_t zx_elems = 0;
+    for (size_t ci = 0; ci < job.classes.size(); ++ci) {
       const ClassRun &cl = job.classes[ci];
       if (!cl.expand) continue;
-      // coarse transforms: consecutive classes of one coarse length at once (rows are contiguous)
-      if (ci == 0 || !job.classes[ci - 1].expand || job.classes[ci - 1].log2Nc != cl.log2Nc) {
-        int rows = 0;
-        for (size_t cj = ci; cj < job.classes.size() && job.classes[cj].expand && job.classes[cj].log2Nc == cl.log2Nc; ++cj)
-          rows += job.classes[cj].count;
-        const long long off = job.descs[cl.first].ip_coff;
-        const unsigned Nc = 1u << cl.log2Nc;
-#ifndef CWTB_HOST_EMU
-        if (fan > 1) {
-          const int slot = group++ % fan;
-          if (slot > 0) {
-            if (slot >= fan_used) {   // first use in this call: behind the band products
-              RT(cudaStreamWaitEvent(c->prio_aux[slot - 1], c->ev_xband, 0));
-              fan_used = slot + 1;
-            }
-            c->cur = c->prio_aux[slot - 1];
-            c->ztmp = &c->Zxs[slot - 1];
-          } else {
-            c->cur = c->prio_stream;
-            c->ztmp = &c->Zx;
-          }
-        }
-#endif
-        e = fft_rows<T, +1>(c, (const V *)c->Cin.p + off, 0, Nc, Nc, (V *)c->Cout.p + off, Nc, Nc, rows);
-      }
+      if (cl.log2Nc < 6 || cl.log2Nc > 20)   // the lengths CoarseRowsBody / CoarseABody have tiles for
+        return fail(c, CWTB_ERR_STATE, "expansion: coarse length outside 2^6 .. 2^20");
+      std::vector<CoarseSeg> &v = cl.log2Nc <= 10 ? short_segs : long_segs;
+      if (ci > 0 && job.classes[ci - 1].expand && job.classes[ci - 1].log2Nc == cl.log2Nc) v.back().count += cl.count;
+      else v.push_back(CoarseSeg{cl.first, cl.count, cl.log2Nc, 0});
+      if (cl.log2Nc > 10)   // Z rows sit at the rows' offsets in C
+        zx_elems = std::max(zx_elems, (size_t)job.descs[cl.first].ip_coff + ((size_t)cl.count << cl.log2Nc));
     }
-#ifndef CWTB_HOST_EMU
-    if (fan > 1) {   // join the fan on the priority stream
-      for (int k = 1; k < fan_used; ++k) {
-        RT(cudaEventRecord(c->ev_pj[k - 1], c->prio_aux[k - 1]));
-        RT(cudaStreamWaitEvent(c->prio_stream, c->ev_pj[k - 1], 0));
-      }
-      c->cur = c->prio_stream;
-      c->ztmp = &c->Zx;
+    CoarseArgs<T> ca{};
+    ca.descs = ddesc; ca.spec = spec; ca.C = (V *)c->Cout.p; ca.tw = Tw<T>::get(c); ca.fam = fam; ca.Nx = N;
+    ca.pf_dist = c->pf_rows_b; ca.rev = c->passb_rev;
+    c->prof_tag = "coarse:";
+    if (!long_segs.empty()) {
+      if ((e = ensure(c, c->Zx, zx_elems * sizeof(V)))) return e;
+      ca.Z = (V *)c->Zx.p;
+      for (const CoarseSeg &g : long_segs)
+        if ((e = get_ntab(c, 1u << g.log2Nc, g.log2Nc, &ca.nt[g.log2Nc - 10]))) return e;
+      if ((e = launch_coarse<CoarseABody<T>>(c, ca, long_segs))) return e;
+      if ((e = launch_coarse<CoarseBBody<T>>(c, ca, long_segs))) return e;
     }
+    if (!short_segs.empty()) {
+#ifndef CWTB_HOST_EMU
+      if (prio) c->cur = c->prio_short;
 #endif
+      if ((e = launch_coarse<CoarseRowsBody<T>>(c, ca, short_segs))) return e;
+    }
     c->prof_tag = "";
 #ifndef CWTB_HOST_EMU
-    if (prio && c->prio_mode == 1) {   // expansion kernels: ordinary priority, after the coarse chain
+    if (prio) {
+      RT(cudaEventRecord(c->ev_coarse_short, c->prio_short));
       RT(cudaEventRecord(c->ev_coarse, c->prio_stream));
-      RT(cudaStreamWaitEvent(c->aux_stream, c->ev_coarse, 0));
-      c->cur = c->aux_stream;
+      c->cur = c->prio_mode == 1 ? c->aux_stream : c->prio_stream;   // 1: expansion kernels at ordinary priority
+      RT(cudaStreamWaitEvent(c->cur, c->ev_coarse_short, 0));
     }
 #endif
-    // one expansion launch per tap count: classes are sorted by taps first
-    for (size_t ci = 0; ci < job.classes.size() && !e; ++ci) {
-      const ClassRun &cl = job.classes[ci];
-      if (!cl.expand || (ci > 0 && job.classes[ci - 1].expand && job.classes[ci - 1].taps == cl.taps)) continue;
-      int rows = 0, minl = 30;
-      for (size_t cj = ci; cj < job.classes.size() && job.classes[cj].expand && job.classes[cj].taps == cl.taps; ++cj) {
-        rows += job.classes[cj].count;
-        minl = std::min(minl, job.classes[cj].log2Nc);
-      }
-      ExpandArgs<T> ea{ddesc, (const V *)c->Cout.p, (const double *)c->wtab.p, W, nt, job.n0, N, cl.first, epi,
-                       job.log2N};
-      e = launch_expand<T>(c, cl.taps, ea, rows, minl);
-    }
-    c->ztmp = nullptr;
+    // one expansion launch per tap count (classes are sorted by taps first): those that read only
+    // coarse lengths up to 1024 first, the others behind the long coarse transforms
+    for (int pass = 0; pass < 2 && !e; ++pass) {
 #ifndef CWTB_HOST_EMU
-    if (prio && c->prio_mode == 2 && !e) {   // later work of the second stream and the join follow the priority stream
-      RT(cudaEventRecord(c->ev_coarse, c->prio_stream));
+      if (pass == 1 && prio && c->prio_mode == 1) RT(cudaStreamWaitEvent(c->cur, c->ev_coarse, 0));
+#endif
+      for (size_t ci = 0; ci < job.classes.size() && !e; ++ci) {
+        const ClassRun &cl = job.classes[ci];
+        if (!cl.expand || (ci > 0 && job.classes[ci - 1].expand && job.classes[ci - 1].taps == cl.taps)) continue;
+        int rows = 0, minl = 30, maxl = 0;
+        for (size_t cj = ci; cj < job.classes.size() && job.classes[cj].expand && job.classes[cj].taps == cl.taps; ++cj) {
+          rows += job.classes[cj].count;
+          minl = std::min(minl, job.classes[cj].log2Nc);
+          maxl = std::max(maxl, job.classes[cj].log2Nc);
+        }
+        if ((maxl > 10) != (pass == 1)) continue;
+        ExpandArgs<T> ea{ddesc, (const V *)c->Cout.p, (const double *)c->wtab.p, W, nt, job.n0, N, cl.first, epi,
+                         job.log2N};
+        e = launch_expand<T>(c, cl.taps, ea, rows, minl);
+      }
+    }
+#ifndef CWTB_HOST_EMU
+    if (prio && !e) {   // later work of the second stream and the join follow the coarse chain
+      if (c->prio_mode == 2) RT(cudaEventRecord(c->ev_coarse, c->prio_stream));
       RT(cudaStreamWaitEvent(c->aux_stream, c->ev_coarse, 0));
     }
 #endif
@@ -1927,13 +1927,11 @@ int cwtb_create(int device, cwtb_ctx **out) {
     int lo = 0, hi = 0;   // numerically lower = higher priority
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
     cudaStreamCreateWithPriority(&c->prio_stream, cudaStreamNonBlocking, hi);
-    for (auto &st : c->prio_aux) cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, hi);
+    cudaStreamCreateWithPriority(&c->prio_short, cudaStreamNonBlocking, hi);
   }
-  cudaEventCreateWithFlags(&c->ev_xband, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&c->ev_angle, cudaEventDisableTiming);
-  for (auto &ev : c->ev_pj) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (const char *g = getenv("CWTB_PRIO_FAN")) c->prio_fan = std::min(8, std::max(1, atoi(g)));
   cudaEventCreateWithFlags(&c->ev_coarse, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&c->ev_coarse_short, cudaEventDisableTiming);
   for (auto &ev : c->ev_h2d) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   for (auto &ev : c->ev_used) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   if (const char *g = getenv("CWTB_BATCH_PIPELINE")) c->batch_pipeline = atoi(g) != 0;
@@ -1993,7 +1991,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   cudaStreamSynchronize(c->stream);
 #endif
   cwtb_comm_destroy(c);
-  for (Buf *b : {&c->osH, &c->osgrp, &c->Zxs[0],&c->Zxs[1], &c->Zxs[2], &c->Zxs[3], &c->Zxs[4], &c->Zxs[5], &c->Zxs[6], &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cin, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
+  for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
                  &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
@@ -2009,11 +2007,10 @@ void cwtb_destroy(cwtb_ctx *c) {
   for (auto &st : c->copy_streams) cudaStreamDestroy(st);
   cudaStreamDestroy(c->aux_stream);
   cudaStreamDestroy(c->prio_stream);
-  for (auto &st : c->prio_aux) cudaStreamDestroy(st);
-  cudaEventDestroy(c->ev_xband);
+  cudaStreamDestroy(c->prio_short);
   cudaEventDestroy(c->ev_angle);
-  for (auto &ev : c->ev_pj) cudaEventDestroy(ev);
   cudaEventDestroy(c->ev_coarse);
+  cudaEventDestroy(c->ev_coarse_short);
   for (auto &ev : c->ev_h2d) cudaEventDestroy(ev);
   for (auto &ev : c->ev_used) cudaEventDestroy(ev);
   for (void *p : c->stage_host) if (p) cudaFreeHost(p);

@@ -653,11 +653,32 @@ struct AbsMaxBody {
 // ---- Body: first kernel of the two-kernel path: K1-point transforms over r1 --------
 // (Band scales read the band buffer rather than evaluate x^ * conj(psi^) * norm while the tile is filled:
 // the evaluation slows the first kernel of Np/K' = 2 scales by more than the band-product launch it saves.)
-enum { MODE_DENSE = 0, MODE_BAND = 1, MODE_REAL = 2, MODE_CPLX = 3 };
+// MODE_COARSE: coarse spectra of expansion rows (coarse_value), rows of N = Nc points
+enum { MODE_DENSE = 0, MODE_BAND = 1, MODE_REAL = 2, MODE_CPLX = 3, MODE_COARSE = 4 };
+
+// Coarse spectrum of expansion row d at coarse index r < Nc: the band product shifted to the centre
+// bin and divided by the transform of the interpolation kernel (see "Band-limited expansion path"
+// below); zero outside the band.  Nx: length of the signal's spectrum.
+template <typename T> HD cx<T> coarse_value(const Fam &fam, const ScaleDesc &d, const cx<T> *spec, int r, unsigned Nx) {
+  const int Nc = 1 << d.ip_log2Nc;
+  const int kp = r < Nc / 2 ? r : r - Nc;       // signed offset from the centre bin
+  const int k = d.ip_kc + kp;
+  if (k < d.k_lo || k > d.k_hi) return mk<T>(0, 0);
+  const cx<T> b = band_value<T>(fam, d, spec, (unsigned)k & (Nx - 1), k, Nx);
+  // 1 / phi^(kp / Nc),  phi^(xi) = taps / I0(beta) * sinh(z) / z,  z = sqrt(beta^2 - (pi taps xi)^2)
+  const double pw = 3.14159265358979323846 * (double)d.ip_w;
+  const double x = pw * ((double)kp / (double)Nc);
+  // > 0: |xi| <= 1/4 < 1 - xi_max.  The fused multiply-add is spelled out: left to the compiler, the
+  // contraction differs between the kernels that inline this function, and so would the last bit
+  const double bb = d.ip_beta * d.ip_beta;
+  const double z = sqrt(fma(-x, x, bb));
+  const double f = d.ip_dc * (z / sinh(z));
+  return mk<T>((T)((double)b.x * f), (T)((double)b.y * f));
+}
 
 template <typename T> struct PassAArgs {
   const ScaleDesc *descs;
-  const cx<T> *spec;   // x^ (MODE_DENSE)
+  const cx<T> *spec;   // x^ (MODE_DENSE, MODE_COARSE)
   const cx<T> *Bbuf;   // band products (MODE_BAND)
   const void *in;      // T* (MODE_REAL) or cx<T>* (MODE_CPLX), rows of `in_pitch`
   cx<T> *Z;            // [ny][U][K2]
@@ -672,6 +693,7 @@ template <typename T> struct PassAArgs {
   int gauss_rec;       // dense Morlet: evaluate the Gaussian by recurrence along each thread's bins
   unsigned K2;         // row length of Z: 1024 (second kernel = PassB) or 2^20 (pre-pass of the
                        // three-level path for Np > 2^20, where the rows are transformed again)
+  unsigned Nx;         // MODE_COARSE: length of the signal's spectrum (N is the coarse length)
 };
 
 template <typename T, int K1, int MODE, int SIGN> struct PassABody {
@@ -692,7 +714,7 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
     int by, p;
     V twist0;
     HD Src(const Args &a_, int by_, int p_) : a(a_), by(by_), p(p_) {
-      if (MODE == MODE_DENSE || MODE == MODE_BAND) d = a.descs[a.first + by];
+      if (MODE == MODE_DENSE || MODE == MODE_BAND || MODE == MODE_COARSE) d = a.descs[a.first + by];
     }
     // element r = pos*K2 + r2 of the K'-point input
     HD V get(int pos, int r2) const {
@@ -710,6 +732,8 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
         // e^{2 pi i k1 p / (K1 M)} = e^{2 pi i (k1 p K2) / N}
         V w = nroot_t<T>(a.nt, (unsigned)k1 * (unsigned)p * a.K2);
         return cmul(v, w);
+      } else if (MODE == MODE_COARSE) {
+        return coarse_value<T>(a.fam, d, a.spec, (int)r, a.Nx);
       } else if (MODE == MODE_REAL) {
         const T *row = (const T *)a.in + (size_t)(a.row0 + by) * a.in_pitch;
         return mk<T>((long long)r < a.n_in ? ldg(&row[r]) : (T)0, (T)0);
@@ -756,7 +780,7 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
             TileBarrier::prefetch_l2(base + (size_t)pos * a.K2, (unsigned)(T2 * sizeof(V)));
         }
       }
-      // the same for the rows of a batched row transform (coherence smoothing, coarse transforms): the
+      // the same for the rows of a batched row transform (coherence smoothing): the
       // tile `pf_dist` blocks ahead of this one in the same row
       if (MODE == MODE_CPLX && a.pf_dist > 0 && T2 * sizeof(V) >= 256) {
         const int t = bx + a.pf_dist;
@@ -880,8 +904,9 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
 // (Kb of the Np bins) is a trigonometric polynomial of Kb terms: it is fully determined by
 // Nc >= 2 Kb samples.  Instead of running Np/K' pruned transforms of K' points each, the engine
 //   (1) forms the band product shifted to the centre bin kc and divided by the transform of the
-//       interpolation kernel (ExpandBandBody),
-//   (2) inverse-transforms it on the coarse grid of Nc points (the ordinary batched FFT), and
+//       interpolation kernel (coarse_value), while it fills the tiles of
+//   (2) the inverse transform on the coarse grid of Nc points (CoarseRowsBody, CoarseABody +
+//       CoarseBBody: the batched FFT's tiles, one launch each for all coarse lengths), and
 //   (3) expands the Nc samples to the Np output points with a polyphase Kaiser-Bessel kernel of
 //       `taps` real weights per output and re-modulates by e^{2 pi i kc n / Np} (ExpandBody):
 //         W[R m + rho] = e^{2 pi i kc n/Np} * sum_t c[m + t - (taps/2 - 1)] * h[t][rho],  R = Np / Nc.
@@ -894,41 +919,173 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
 // Cost per output point: 2*taps + 8 fp64 FMAs, one 16-byte shared-memory read, one 16-byte store --
 // a streaming kernel bounded by the W store, with no intermediate in global memory.
 // ==================================================================================================
-template <typename T> struct ExpandBandArgs {
+// ---- coarse transforms of the expansion rows: ragged launches over every coarse length ----------
+// The expansion rows of one coarse length that are consecutive in the class-sorted descriptor array
+// form a segment; their coarse rows are consecutive in C and Z (descs[].ip_coff).  A launch covers up
+// to CSEG_MAX segments; CTA bx belongs to the last segment whose cta0 <= bx and runs the tile of that
+// segment's length -- the same radix plan, twiddles and arithmetic as a per-length launch.
+struct CoarseSeg { int first, count, log2Nc, cta0; };
+constexpr int CSEG_MAX = 32;
+HD constexpr size_t cmax(size_t a, size_t b) { return a > b ? a : b; }
+template <typename T> struct CoarseArgs {
   const ScaleDesc *descs;
-  const cx<T> *spec;
-  cx<T> *Cin;       // coarse spectra, rows at descs[].ip_coff
+  const cx<T> *spec;   // x^ of the signal(s), Nx points per channel
+  cx<T> *Z;            // CoarseABody -> CoarseBBody intermediate, rows at descs[].ip_coff
+  cx<T> *C;            // coarse samples, rows at descs[].ip_coff
+  const cx<T> *tw;
   Fam fam;
-  unsigned N;
-  int first;
+  NTab nt[11];         // CoarseABody: e^{2 pi i e / Nc} for Nc = 2^(10 + i)
+  unsigned Nx;
+  int nseg;
+  int pf_dist, rev;    // CoarseBBody: PassBArgs::pf_dist, ::rev
+  CoarseSeg seg[CSEG_MAX];
 };
-template <typename T> struct ExpandBandBody {
+template <typename T> HD const CoarseSeg &coarse_seg(const CoarseArgs<T> &a, int bx) {
+  int s = 0;
+  while (s + 1 < a.nseg && bx >= a.seg[s + 1].cta0) ++s;
+  return a.seg[s];
+}
+
+// Nc <= 1024: one tile of P rows per CTA.  Phase 0 fills the tile with coarse_value, then the
+// passes of the batched row transform (RowsBody) run from shared memory.
+template <typename T> struct CoarseRowsBody {
+  static constexpr int NTB = TileCfg<T>::NT;
+  static constexpr int NT = NTB;
   using V = cx<T>;
-  using Args = ExpandBandArgs<T>;
-  static constexpr int NPHASE = 1;
-  static constexpr size_t SMEM = 0;
-  static constexpr int PER = 4;
-  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
-    const ScaleDesc d = a.descs[a.first + by];
-    const int Nc = 1 << d.ip_log2Nc;
-    const double pw = 3.14159265358979323846 * (double)d.ip_w;
+  using Args = CoarseArgs<T>;
+  template <int K> static constexpr size_t bytes() { return Lay<T, K>::BYTES; }
+  static constexpr size_t SMEM = cmax(cmax(cmax(bytes<64>(), bytes<128>()), cmax(bytes<256>(), bytes<512>())), bytes<1024>());
+  static constexpr int NPHASE = 4;
+  // CTAs of a segment of `rows` rows of 2^log2Nc points
+  HD static int ctas(int log2Nc, int rows) {
+    const int P = TileCfg<T>::TILE >> log2Nc;
+    return (rows + P - 1) / P;
+  }
+  struct Storer {
+    V *out;   // row 0 of the tile
+    int nb;   // valid rows
+    int K;
+    template <int R> HD void store(int b, int ql, int qs, V (&x)[R]) const {
+      if (b >= nb) return;
 #pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      const int r = (bx * PER + i) * NT + tid;
-      if (r >= Nc) return;
-      const int kp = r < Nc / 2 ? r : r - Nc;       // signed offset from the centre bin
-      const int k = d.ip_kc + kp;
-      V v = mk<T>(0, 0);
-      if (k >= d.k_lo && k <= d.k_hi) {
-        const V b = band_value<T>(a.fam, d, a.spec, (unsigned)k & (a.N - 1), k, a.N);
-        // 1 / phi^(kp / Nc),  phi^(xi) = taps / I0(beta) * sinh(z) / z,  z = sqrt(beta^2 - (pi taps xi)^2)
-        const double x = pw * ((double)kp / (double)Nc);
-        const double z = sqrt(d.ip_beta * d.ip_beta - x * x);      // > 0: |xi| <= 1/4 < 1 - xi_max
-        const double f = d.ip_dc * (z / sinh(z));
-        v = mk<T>((T)((double)b.x * f), (T)((double)b.y * f));
-      }
-      a.Cin[d.ip_coff + r] = v;
+      for (int c = 0; c < R; ++c) out[(size_t)b * K + ql + c * qs] = x[c];
     }
+  };
+  template <int K, int PH> HD static void tile(const Args &a, const CoarseSeg &g, int bx, int tid, V *sm) {
+    using LY = Lay<T, K>;
+    constexpr int NP = Plan<K>::NP;
+    static_assert(NP >= 2, "coarse rows: multi-pass tile plans only");
+    const int row0 = (bx - g.cta0) * LY::P;
+    const int nb = g.count - row0 < LY::P ? g.count - row0 : LY::P;
+    if constexpr (PH == 0) {
+      for (int idx = tid; idx < LY::P * K; idx += NT) {
+        const int b = idx / K, pos = idx % K;
+        V v = mk<T>(0, 0);
+        if (b < nb) v = coarse_value<T>(a.fam, a.descs[g.first + row0 + b], a.spec, pos, a.Nx);
+        sm[LY::phys(b, pos)] = v;
+      }
+    } else if constexpr (PH == 1) {
+      SmemLoader<T, K> ld;
+      ld.sm = sm;
+      tile_first<T, K, +1>(sm, a.tw, ld, tid);
+    } else if constexpr (PH == 2 && NP == 3) {
+      tile_second<T, K, +1>(sm, a.tw, tid);
+    } else if constexpr (PH == NP) {
+      Storer st{a.C + a.descs[g.first].ip_coff + (size_t)row0 * K, nb, K};
+      pass_last<T, K, +1>(sm, st, tid);
+    }
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *smraw) {
+    const CoarseSeg &g = coarse_seg(a, bx);
+    V *sm = (V *)smraw;
+    switch (g.log2Nc) {
+      case 6: tile<64, PH>(a, g, bx, tid, sm); break;
+      case 7: tile<128, PH>(a, g, bx, tid, sm); break;
+      case 8: tile<256, PH>(a, g, bx, tid, sm); break;
+      case 9: tile<512, PH>(a, g, bx, tid, sm); break;
+      case 10: tile<1024, PH>(a, g, bx, tid, sm); break;
+    }
+  }
+};
+
+// 1024 < Nc <= 2^20: the two-kernel row transform (K1 = Nc / 1024, K2 = 1024).  The first kernel is
+// PassABody in MODE_COARSE, which forms the coarse spectrum while it fills its tile.
+template <typename T> struct CoarseABody {
+  static constexpr int NTB = TileCfg<T>::NT;
+  static constexpr int NT = NTB;
+  using V = cx<T>;
+  using Args = CoarseArgs<T>;
+  template <int K1> using A = PassABody<T, K1, MODE_COARSE, +1>;
+  static constexpr size_t SMEM = cmax(cmax(cmax(cmax(A<2>::SMEM, A<4>::SMEM), cmax(A<8>::SMEM, A<16>::SMEM)),
+                                           cmax(cmax(A<32>::SMEM, A<64>::SMEM), cmax(A<128>::SMEM, A<256>::SMEM))),
+                                      cmax(A<512>::SMEM, A<1024>::SMEM));
+  static constexpr int NPHASE = 4;
+  template <int K1> HD static int per_row() { return K2C / A<K1>::T2; }
+  HD static int ctas(int log2Nc, int rows) {
+    switch (log2Nc - 10) {
+      case 1: return rows * per_row<2>();
+      case 2: return rows * per_row<4>();
+      case 3: return rows * per_row<8>();
+      case 4: return rows * per_row<16>();
+      case 5: return rows * per_row<32>();
+      case 6: return rows * per_row<64>();
+      case 7: return rows * per_row<128>();
+      case 8: return rows * per_row<256>();
+      case 9: return rows * per_row<512>();
+      case 10: return rows * per_row<1024>();
+    }
+    return 0;
+  }
+  template <int K1, int PH> HD static void tile(const Args &a, const CoarseSeg &g, int bx, int tid, void *sm) {
+    if constexpr (PH < A<K1>::NPHASE) {
+      const int local = bx - g.cta0, per = per_row<K1>();
+      PassAArgs<T> pa{};
+      pa.descs = a.descs; pa.spec = a.spec; pa.tw = a.tw; pa.fam = a.fam; pa.nt = a.nt[g.log2Nc - 10];
+      pa.Z = a.Z + a.descs[g.first].ip_coff;
+      pa.N = 1u << g.log2Nc; pa.Nx = a.Nx; pa.first = g.first; pa.zmod = 1 << 30; pa.K2 = K2C;
+      A<K1>::template phase<PH>(pa, local % per, local / per, tid, sm);
+    }
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *sm) {
+    const CoarseSeg &g = coarse_seg(a, bx);
+    switch (g.log2Nc - 10) {
+      case 1: tile<2, PH>(a, g, bx, tid, sm); break;
+      case 2: tile<4, PH>(a, g, bx, tid, sm); break;
+      case 3: tile<8, PH>(a, g, bx, tid, sm); break;
+      case 4: tile<16, PH>(a, g, bx, tid, sm); break;
+      case 5: tile<32, PH>(a, g, bx, tid, sm); break;
+      case 6: tile<64, PH>(a, g, bx, tid, sm); break;
+      case 7: tile<128, PH>(a, g, bx, tid, sm); break;
+      case 8: tile<256, PH>(a, g, bx, tid, sm); break;
+      case 9: tile<512, PH>(a, g, bx, tid, sm); break;
+      case 10: tile<1024, PH>(a, g, bx, tid, sm); break;
+    }
+  }
+};
+
+// second kernel of the same rows: PassBBody from Z into C
+template <typename T> struct CoarseBBody {
+  using B = PassBBody<T, +1>;
+  static constexpr int NTB = B::NTB;
+  static constexpr int NT = NTB;
+  using Args = CoarseArgs<T>;
+  static constexpr size_t SMEM = B::SMEM;
+  static constexpr int NPHASE = B::NPHASE;
+  HD static int per_row(int log2Nc) {
+    constexpr int P = B::LY::P;
+    return ((1 << (log2Nc - 10)) + P - 1) / P;
+  }
+  HD static int ctas(int log2Nc, int rows) { return rows * per_row(log2Nc); }
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *sm) {
+    const CoarseSeg &g = coarse_seg(a, bx);
+    const int local = bx - g.cta0, per = per_row(g.log2Nc);
+    const long long off = a.descs[g.first].ip_coff;
+    const unsigned Nc = 1u << g.log2Nc;
+    PassBArgs<T> pb{};
+    pb.Z = a.Z + off; pb.out = a.C + off; pb.tw = a.tw;
+    pb.pitch = Nc; pb.nout = Nc; pb.N = Nc; pb.post = 1.0;
+    pb.epi = EPI_STORE; pb.zmod = 1 << 30; pb.pf_dist = a.pf_dist; pb.ny = g.count; pb.ileave = 1; pb.rev = a.rev;
+    B::template phase<PH>(pb, local % per, local / per, tid, sm);
   }
 };
 
