@@ -224,6 +224,47 @@ int cwtb_coherence_row_stats(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi
  * aWCT[j,n].  Rows with weight 0 are not read.  Deterministic. */
 int cwtb_coherence_scale_avg(cwtb_ctx *ctx, const double *weights, double *out);
 
+/* ---- resident cross spectrum ----------------------------------------------------------------
+ * cwtb_xwt_resident runs what cwtb_xwt runs (same arguments without W12_out, same precision:
+ * cwtb_set_coherence_precision; un-padded transforms only in fp64, CWTB_TABLE unsupported) and
+ * keeps W12 = W1 conj(W2) (n_scales x n0, complex of the engine precision) in a device buffer of
+ * its own, the transform's W buffer handed over without a copy.  Lifetime:
+ *   - only cwtb_xwt_resident writes that buffer: it survives every other call (cwt*, xwt, wct,
+ *     wct_resident, wct_mc*, smooth, cwt_batch*);
+ *   - it dies at the next cwtb_xwt_resident or cwtb_cross_release (which frees it; so does
+ *     cwtb_destroy).  cwtb_cross_serial changes at both, and is bumped before the buffer is
+ *     written, so a cwtb_xwt_resident that fails part-way changes it too;
+ *   - afterwards no transform is resident: cwtb_get_w, cwtb_icwt_sum and the power calls return
+ *     CWTB_ERR_STATE until the next transform.
+ * cwtb_xwt itself is unchanged: its W12 stays the resident transform. */
+int cwtb_xwt_resident(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,
+                      double dt, const double *scales, int n_scales, int family, double param);
+int64_t cwtb_cross_serial(cwtb_ctx *ctx);
+int cwtb_cross_release(cwtb_ctx *ctx);
+
+/* Reading calls on a resident complex field: CWTB_FIELD_W (the resident transform's W) or
+ * CWTB_FIELD_CROSS (the cross spectrum).  They return CWTB_ERR_STATE when the field is not
+ * resident, CWTB_ERR_UNSUPPORTED for the W of a batched transform and CWTB_ERR_ARG for bad
+ * ranges.  Outputs are complex128 / double whatever the field's precision (fp32 fields are widened
+ * on the device); the reductions are deterministic (fixed partition and summation order, no
+ * atomics: repeated calls are bit-identical). */
+enum cwtb_field { CWTB_FIELD_W = 0, CWTB_FIELD_CROSS = 1 };
+/* rows [row0, row0 + nrows), nrows x n0 complex128 */
+int cwtb_field_get(cwtb_ctx *ctx, int field, int row0, int nrows, void *out);
+/* strided sub-grid, nrows x ncols complex128: out[r][c] = F[row0 + r*row_step][col0 + c*col_step],
+ * steps >= 1, every index inside the field (the checks of cwtb_coherence_window) */
+int cwtb_field_window(cwtb_ctx *ctx, int field, int row0, int nrows, int row_step, int64_t col0,
+                      int64_t ncols, int64_t col_step, void *out);
+/* Per row j, over the columns [lo[j], hi[j]) (lo / hi NULL: the whole row) where thr is NULL or
+ * re^2 + im^2 > thr[j] (in double, false for a NaN threshold): out[j] = [count, sum |F|^2,
+ * sum |F|, sum cos phi, sum sin phi] (S x 5 doubles), |F| = sqrt(re^2 + im^2), cos phi = re/|F|,
+ * sin phi = im/|F|; a zero coefficient has phase 0 (adds (1, 0)). */
+int cwtb_field_row_stats(cwtb_ctx *ctx, int field, const int64_t *lo, const int64_t *hi,
+                         const double *thr, double *out);
+/* out[n] = sum_j weights[j] * W12[j,n] (n0 complex128) over the cross spectrum.  Rows with weight
+ * 0 are not read. */
+int cwtb_cross_scale_avg(cwtb_ctx *ctx, const double *weights, void *out);
+
 /* Morlet.smooth on a caller-supplied host array (mothers.py:61-104).
  * in: n_scales x n (complex128 if is_complex else float64); out same type. */
 int cwtb_smooth(cwtb_ctx *ctx, const void *in, int is_complex, int n_scales,

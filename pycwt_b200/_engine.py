@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libcwtb200.so")
 
 MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
 F64, F32 = 0, 1
+FIELD_W, FIELD_CROSS = 0, 1      # complex fields of the cwtb_field_* calls
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -72,6 +73,13 @@ _SIGNATURES = {
     "cwtb_coherence_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P, _P]),
     "cwtb_coherence_row_stats": (_I, [_P, _P, _P, _P, _I, _P]),
     "cwtb_coherence_scale_avg": (_I, [_P, _P, _P]),
+    "cwtb_xwt_resident": (_I, [_P, _P, _P, _I64, _D, _P, _I, _I, _D]),
+    "cwtb_cross_serial": (_I64, [_P]),
+    "cwtb_cross_release": (_I, [_P]),
+    "cwtb_field_get": (_I, [_P, _I, _I, _I, _P]),
+    "cwtb_field_window": (_I, [_P, _I, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_field_row_stats": (_I, [_P, _I, _P, _P, _P, _P]),
+    "cwtb_cross_scale_avg": (_I, [_P, _P, _P]),
     "cwtb_smooth": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _P]),
     "cwtb_wct_mc": (_I, [_P, _P, _I, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
     "cwtb_wct_mc_seeded": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
@@ -576,6 +584,88 @@ class Engine(object):
             raise ValueError("coherence_scale_avg: one weight per row expected")
         out = self.result_array((3, n0), np.float64)
         self._check(self.lib.cwtb_coherence_scale_avg(self.h, _ptr(w), _ptr(out)))
+        return out
+
+    # ---- resident cross spectrum and complex-field reductions (include/cwt_b200.h) -----------
+    _cross = None            # (rows, n0) of the resident cross spectrum
+
+    @_locked
+    def xwt_resident(self, y1, y2, dt, scales, family, param, precision=F64):
+        """`xwt` with W12 kept on the device; returns the cross serial that identifies it.  No
+        transform is resident afterwards."""
+        y1 = np.ascontiguousarray(y1, dtype=np.float64)
+        y2 = np.ascontiguousarray(y2, dtype=np.float64)
+        if y1.shape != y2.shape or y1.ndim != 1:
+            raise ValueError("xwt_resident: the two series must be 1-D and of equal length")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        self._cross = None
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_xwt_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt),
+                                               _ptr(sj), sj.size, int(family), float(param)))
+        self._cross = (sj.size, y1.size)
+        return self.cross_serial()
+
+    @_locked
+    def cross_serial(self):
+        return int(self.lib.cwtb_cross_serial(self.h))
+
+    @_locked
+    def cross_release(self):
+        self._cross = None
+        self._check(self.lib.cwtb_cross_release(self.h))
+
+    def _field_shape(self, field):
+        shape = self._cross if field == FIELD_CROSS else self._resident
+        if shape is None:
+            raise EngineError("no cross spectrum resident" if field == FIELD_CROSS
+                              else "no single transform resident")
+        return shape
+
+    @_locked
+    def field_get(self, field):
+        """The whole field, complex128 [rows, n0]."""
+        rows, n0 = self._field_shape(field)
+        out = self.result_array((rows, n0), np.complex128)
+        self._check(self.lib.cwtb_field_get(self.h, int(field), 0, rows, _ptr(out)))
+        return out
+
+    @_locked
+    def field_window(self, field, row0, nrows, row_step, col0, ncols, col_step):
+        """F[row0::row_step][:nrows, col0::col_step][:, :ncols] as complex128."""
+        self._field_shape(field)
+        out = self.result_array((nrows, ncols), np.complex128)
+        self._check(self.lib.cwtb_field_window(self.h, int(field), int(row0), int(nrows), int(row_step),
+                                               int(col0), int(ncols), int(col_step), _ptr(out)))
+        return out
+
+    @_locked
+    def field_row_stats(self, field, lo, hi, thr=None):
+        """[rows, 5]: count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F over the columns
+        [lo[j], hi[j]) where thr is None or |F|^2 > thr[j]."""
+        rows, _ = self._field_shape(field)
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        if lo.shape != (rows,) or hi.shape != (rows,):
+            raise ValueError("field_row_stats: one column range per row expected")
+        if thr is not None:
+            thr = np.ascontiguousarray(thr, dtype=np.float64)
+            if thr.shape != (rows,):
+                raise ValueError("field_row_stats: one threshold per row expected")
+        out = np.empty((rows, 5), dtype=np.float64)
+        self._check(self.lib.cwtb_field_row_stats(self.h, int(field), _ptr(lo), _ptr(hi),
+                                                  None if thr is None else _ptr(thr), _ptr(out)))
+        return out
+
+    @_locked
+    def cross_scale_avg(self, weights):
+        """sum_j w_j W12[j, :] (complex128, n0)."""
+        rows, n0 = self._field_shape(FIELD_CROSS)
+        w = np.ascontiguousarray(weights, dtype=np.float64)
+        if w.shape != (rows,):
+            raise ValueError("cross_scale_avg: one weight per row expected")
+        out = self.result_array((n0,), np.complex128)
+        self._check(self.lib.cwtb_cross_scale_avg(self.h, _ptr(w), _ptr(out)))
         return out
 
     @_locked

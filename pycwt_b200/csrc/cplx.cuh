@@ -58,6 +58,16 @@ HD void sincos_hd(double x, double *s, double *c) {
 #endif
 }
 
+// re^2 + im^2 with every operation rounded (no fused multiply-add): the value numpy's
+// `re**2 + im**2` has, so that thresholds on it select the same points
+HD double norm2_rn(double re, double im) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  return __dadd_rn(__dmul_rn(re, re), __dmul_rn(im, im));
+#else
+  return re * re + im * im;
+#endif
+}
+
 // ---- DFT_R in registers: x[c] <- sum_i x[i] e^{SIGN 2 pi i * i*c/R}, natural order ----
 template <int SIGN, typename V> HD void dft2(V &a, V &b) {
   V t = csub(a, b);

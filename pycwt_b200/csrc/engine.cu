@@ -256,6 +256,17 @@ struct cwtb_ctx {
   int coh_S = 0;                 // rows resident (0: none)
   long long coh_n0 = 0;
   long long coh_serial = 0;
+  // resident cross spectrum (cwtb_xwt_resident): W12 [cross_S][cross_n0] of precision cross_prec.
+  // cwtb_xwt_resident hands its transform's W over by swapping the two buffers, so W12 is never
+  // copied and the old cross buffer becomes the next transform's W.  Nothing else writes it;
+  // cwtb_cross_release frees it.  cross_serial is bumped before every write and on release.
+  Buf cross;
+  int cross_S = 0;               // rows resident (0: none)
+  long long cross_n0 = 0;
+  int cross_prec = 0;
+  long long cross_serial = 0;
+  bool w_moved = false;          // W went to the cross spectrum: no transform resident until the
+                                 // next one writes W
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
   double last_ms = 0;
   int launches = 0;
@@ -1034,6 +1045,7 @@ static int run_job_exact(cwtb_ctx *c, const Job &job, const double *dsig, double
   if (!Wout) {
     if ((e = ensure(c, c->W, (size_t)S * job.n0 * sizeof(double2)))) return e;
     Wout = (double2 *)c->W.p;
+    c->w_moved = false;
   }
   if ((e = blue_rows(c, dsig, 1, n, (double2 *)c->spec.p, n, n, 1, -1, 1.0, n))) return e;
   const BluePlan *pl;
@@ -1537,6 +1549,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   if (!Wout) {
     if ((e = ensure(c, c->W, (size_t)S * job.n0 * sizeof(V)))) return e;
     Wout = (V *)c->W.p;
+    c->w_moved = false;
   }
   V *spec = (V *)c->spec.p;
   V *W = Wout;
@@ -1992,7 +2005,7 @@ void cwtb_destroy(cwtb_ctx *c) {
 #endif
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh, &c->cross})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2335,11 +2348,14 @@ int cwtb_bench_last(cwtb_ctx *c, int iters, double *ms_out) {
   return timed_run(c, c->job_dsig, iters, ms_out);
 }
 
+// a transform's W is on the device (cwtb_xwt_resident moves it to the cross spectrum)
+static bool w_resident(const cwtb_ctx *c) { return c->job.valid && !c->w_moved; }
+
 double cwtb_last_kernel_ms(cwtb_ctx *c) { return c ? c->last_ms : -1; }
 int cwtb_last_launch_count(cwtb_ctx *c) { return c ? c->launches : -1; }
 int64_t cwtb_padded_length(cwtb_ctx *c) { return (c && c->job.valid) ? (int64_t)c->job.N : -1; }
 int64_t cwtb_job_serial(cwtb_ctx *c) { return c ? c->serial : -1; }
-void *cwtb_w_device_ptr(cwtb_ctx *c) { return (c && c->job.valid) ? c->W.p : nullptr; }
+void *cwtb_w_device_ptr(cwtb_ctx *c) { return (c && w_resident(c)) ? c->W.p : nullptr; }
 
 int cwtb_last_plan(cwtb_ctx *c, int *out, int n) {
   if (!c || !c->job.valid || !out) return CWTB_ERR_ARG;
@@ -2348,13 +2364,12 @@ int cwtb_last_plan(cwtb_ctx *c, int *out, int n) {
   return m;
 }
 
-int cwtb_get_w(cwtb_ctx *c, void *out, int out_f64, int row0, int nrows) {
-  if (!c || !c->job.valid || !out) return fail(c, CWTB_ERR_STATE, "no transform resident");
-  const Job &job = c->job;
-  if (row0 < 0 || nrows < 0 || row0 + nrows > job.S * job.nbatch) return fail(c, CWTB_ERR_ARG, "row range");
-  const size_t cnt = (size_t)nrows * job.n0;
-  if (job.precision == CWTB_F64) {
-    const char *src = (const char *)((const double2 *)c->W.p + (size_t)row0 * job.n0);
+// Host copy of `cnt` coefficients from element `first` of a device complex field of precision
+// `prec`: complex128, or complex64 for an fp32 field with out_f64 == 0.
+static int field_to_host(cwtb_ctx *c, const void *field, int prec, size_t first, size_t cnt, void *out,
+                         int out_f64) {
+  if (prec == CWTB_F64) {
+    const char *src = (const char *)((const double2 *)field + first);
     const size_t bytes = cnt * sizeof(double2);
 #ifndef CWTB_HOST_EMU
     if (c->d2h_split > 1 && bytes >= ((size_t)64 << 20)) {
@@ -2373,13 +2388,13 @@ int cwtb_get_w(cwtb_ctx *c, void *out, int out_f64, int row0, int nrows) {
     RT(rt_d2h(out, src, bytes, c->stream));
     RT(rt_sync(c->stream));
   } else if (!out_f64) {
-    RT(rt_d2h(out, (const float2 *)c->W.p + (size_t)row0 * job.n0, cnt * sizeof(float2), c->stream));
+    RT(rt_d2h(out, (const float2 *)field + first, cnt * sizeof(float2), c->stream));
     RT(rt_sync(c->stream));
   } else {
     // complex64 on the device, complex128 for the caller: widen on the device in chunks and
     // copy each chunk out while the next one is converted (two staging halves, two streams).
     // 16 B per element over PCIe beats an 8 B copy plus a host-side conversion pass.
-    const float2 *src = (const float2 *)c->W.p + (size_t)row0 * job.n0;
+    const float2 *src = (const float2 *)field + first;
     const size_t chunk = std::min<size_t>(cnt, (size_t)8 << 20);   // elements per staging half
     int e;
     if ((e = ensure(c, c->wide, 2 * chunk * sizeof(double2)))) return e;
@@ -2399,6 +2414,13 @@ int cwtb_get_w(cwtb_ctx *c, void *out, int out_f64, int row0, int nrows) {
     RT(rt_sync(c->copy_streams[1]));
   }
   return 0;
+}
+
+int cwtb_get_w(cwtb_ctx *c, void *out, int out_f64, int row0, int nrows) {
+  if (!c || !w_resident(c) || !out) return fail(c, CWTB_ERR_STATE, "no transform resident");
+  const Job &job = c->job;
+  if (row0 < 0 || nrows < 0 || row0 + nrows > job.S * job.nbatch) return fail(c, CWTB_ERR_ARG, "row range");
+  return field_to_host(c, c->W.p, job.precision, (size_t)row0 * job.n0, (size_t)nrows * job.n0, out, out_f64);
 }
 
 int cwtb_get_signal_fft(cwtb_ctx *c, void *out) {
@@ -2577,6 +2599,7 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   const size_t cnt = (size_t)S * n0;
   int e;
   if ((e = ensure(c, c->W, cnt * sizeof(V)))) return e;
+  c->w_moved = false;
   if ((e = ensure(c, c->W2, cnt * sizeof(V)))) return e;
   if ((e = ensure(c, c->C, cnt * sizeof(V)))) return e;
   if ((e = ensure(c, c->A12, cnt * sizeof(V)))) return e;
@@ -2707,7 +2730,7 @@ int cwtb_cwt_to_host(cwtb_ctx *c, const void *signal, int signal_is_f32, int64_t
 static int reduction_rows_per_block(int rows) { return rows <= 32 ? rows : 32; }
 
 int cwtb_icwt_sum(cwtb_ctx *c, double *out) {
-  if (!c || !c->job.valid || !out) return fail(c, CWTB_ERR_STATE, "no transform resident");
+  if (!c || !w_resident(c) || !out) return fail(c, CWTB_ERR_STATE, "no transform resident");
   const Job &job = c->job;
   if (job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "icwt of a batched transform: fetch rows per channel");
   std::vector<double> rs(job.S);
@@ -2756,7 +2779,7 @@ int cwtb_icwt_sum_host(cwtb_ctx *c, const void *W, const double *scales, int n_s
 
 static int power_common(cwtb_ctx *c, double *power_out, double *mean_out, const double *row_scale,
                         const int64_t *lo, const int64_t *hi) {
-  if (!c || !c->job.valid) return fail(c, CWTB_ERR_STATE, "no transform resident");
+  if (!c || !w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
   const Job &job = c->job;
   const int R = job.S * job.nbatch;
   const size_t cnt = (size_t)R * job.n0;
@@ -2811,7 +2834,7 @@ int cwtb_global_power_ranges(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, 
 }
 
 int cwtb_scale_avg_power(cwtb_ctx *c, const double *weights, double *out) {
-  if (!c || !c->job.valid) return fail(c, CWTB_ERR_STATE, "no transform resident");
+  if (!c || !w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
   if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
   const Job &job = c->job;
   if (job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "scale average of a batched transform: fetch rows per channel");
@@ -2872,6 +2895,194 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
   return c->coh_precision == CWTB_F32
              ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out)
              : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out);
+}
+
+// ---- resident cross spectrum ----------------------------------------------------------------
+int cwtb_xwt_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt,
+                      const double *scales, int n_scales, int family, double param) {
+  if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
+  ++c->cross_serial;   // before the buffer is written: a call that fails part-way invalidates it too
+  c->cross_S = 0;
+  c->cross_n0 = 0;
+  int e = c->coh_precision == CWTB_F32
+              ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr)
+              : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr);
+  if (e) return e;
+  // W12 is the transform's W: take the buffer over.  No kernel or plan keeps W's address (every
+  // run takes it afresh from c->W), so the old cross buffer can serve as the next W.
+  std::swap(c->W, c->cross);
+  c->w_moved = true;
+  c->cross_S = n_scales;
+  c->cross_n0 = n0;
+  c->cross_prec = c->job.precision;
+  return 0;
+}
+
+int64_t cwtb_cross_serial(cwtb_ctx *c) { return c ? c->cross_serial : -1; }
+
+int cwtb_cross_release(cwtb_ctx *c) {
+  if (!c) return CWTB_ERR_ARG;
+  ++c->cross_serial;
+  c->cross_S = 0;
+  c->cross_n0 = 0;
+  if (c->cross.p) {
+#ifndef CWTB_HOST_EMU
+    RT(cudaSetDevice(c->device));
+#endif
+    RT(rt_sync(c->stream));
+    rt_free(c->cross.p);
+    c->cross.p = nullptr;
+    c->cross.bytes = 0;
+  }
+  return 0;
+}
+
+// A resident complex field of cwtb_field_*: the transform's W or the cross spectrum
+struct FieldRef {
+  const void *p;
+  int prec, S;
+  long long n0;
+};
+
+static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
+  if (!c) return CWTB_ERR_ARG;
+  if (field == CWTB_FIELD_W) {
+    if (!w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
+    if (c->job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "field of a batched transform: fetch rows per channel");
+    f = FieldRef{c->W.p, c->job.precision, c->job.S, c->job.n0};
+  } else if (field == CWTB_FIELD_CROSS) {
+    if (c->cross_S <= 0 || !c->cross.p) return fail(c, CWTB_ERR_STATE, "no cross spectrum resident");
+    f = FieldRef{c->cross.p, c->cross_prec, c->cross_S, c->cross_n0};
+  } else {
+    return fail(c, CWTB_ERR_ARG, "unknown field");
+  }
+#ifndef CWTB_HOST_EMU
+  RT(cudaSetDevice(c->device));
+#endif
+  return 0;
+}
+
+int cwtb_field_get(cwtb_ctx *c, int field, int row0, int nrows, void *out) {
+  FieldRef f;
+  int e = field_ref(c, field, f);
+  if (e) return e;
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (row0 < 0 || nrows < 0 || row0 > f.S - nrows) return fail(c, CWTB_ERR_ARG, "row range");
+  return field_to_host(c, f.p, f.prec, (size_t)row0 * f.n0, (size_t)nrows * f.n0, out, 1);
+}
+
+int cwtb_field_window(cwtb_ctx *c, int field, int row0, int nrows, int row_step, int64_t col0,
+                      int64_t ncols, int64_t col_step, void *out) {
+  FieldRef f;
+  int e = field_ref(c, field, f);
+  if (e) return e;
+  const int S = f.S;
+  const long long n0 = f.n0;
+  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
+    return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
+  if (nrows == 0 || ncols == 0) return 0;
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
+      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
+    return fail(c, CWTB_ERR_ARG, "window outside the resident field");
+  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0)   // whole rows: the fetch
+    return field_to_host(c, f.p, f.prec, (size_t)row0 * n0, (size_t)nrows * n0, out, 1);
+  const size_t m = (size_t)nrows * ncols;
+  if ((e = ensure(c, c->aux, m * sizeof(double2)))) return e;
+  double2 *o = (double2 *)c->aux.p;
+  const unsigned gx = (unsigned)((ncols + NT - 1) / NT);
+  if (f.prec == CWTB_F64) {
+    CxWindowArgs<double> a{(const double2 *)f.p, o, n0, row0, row_step, col0, col_step, ncols};
+    e = launch<CxWindowBody<double>>(c, gx, (unsigned)nrows, a);
+  } else {
+    CxWindowArgs<float> a{(const float2 *)f.p, o, n0, row0, row_step, col0, col_step, ncols};
+    e = launch<CxWindowBody<float>>(c, gx, (unsigned)nrows, a);
+  }
+  if (e) return e;
+  RT(rt_d2h(out, o, m * sizeof(double2), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+extern "C++" {
+template <typename T>
+static int field_row_stats_run(cwtb_ctx *c, const FieldRef &f, const long long *dlo, const long long *dhi,
+                               const double *dthr, double *dpart, double *dsum, int nchunk) {
+  CxRowStatsArgs<T> a{(const cx<T> *)f.p, dlo, dhi, dthr, dpart, f.n0, nchunk};
+  int e = launch<CxRowStatsBody<T>>(c, (unsigned)nchunk, (unsigned)f.S, a);
+  if (e) return e;
+  RowSumArgs r{dpart, dsum, f.S, nchunk};
+  return launch<RowSumBody<5>>(c, (unsigned)((5 * f.S + NT - 1) / NT), 1, r);
+}
+}  // extern "C++"
+
+int cwtb_field_row_stats(cwtb_ctx *c, int field, const int64_t *lo, const int64_t *hi, const double *thr,
+                         double *out) {
+  FieldRef f;
+  int e = field_ref(c, field, f);
+  if (e) return e;
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  const long long chunk = f.prec == CWTB_F64 ? CxRowStatsBody<double>::CHUNK : CxRowStatsBody<float>::CHUNK;
+  const int nchunk = (int)((n0 + chunk - 1) / chunk);
+  // aux: [lo S][hi S][thr S][partials S*nchunk*5][sums S*5], 8 bytes each
+  std::vector<long long> h(3 * (size_t)S);
+  for (int j = 0; j < S; ++j) {
+    h[j] = lo ? lo[j] : 0;
+    h[S + j] = hi ? hi[j] : n0;
+    if (h[j] < 0 || h[S + j] > n0 || h[j] > h[S + j])
+      return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
+  }
+  if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
+  const size_t npart = (size_t)S * nchunk * 5;
+  if ((e = ensure(c, c->aux, (3 * (size_t)S + npart + 5 * (size_t)S) * sizeof(double)))) return e;
+  long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
+  double *dthr = (double *)(dhi + S), *dpart = dthr + S, *dsum = dpart + npart;
+  RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
+  e = f.prec == CWTB_F64
+          ? field_row_stats_run<double>(c, f, dlo, dhi, thr ? dthr : nullptr, dpart, dsum, nchunk)
+          : field_row_stats_run<float>(c, f, dlo, dhi, thr ? dthr : nullptr, dpart, dsum, nchunk);
+  if (e) return e;
+  RT(rt_d2h(out, dsum, (size_t)S * 5 * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+int cwtb_cross_scale_avg(cwtb_ctx *c, const double *weights, void *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_CROSS, f);
+  if (e) return e;
+  if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  // aux: [weights S doubles][selected rows S ints][out n0 complex128]: rows with a zero weight are
+  // not read
+  std::vector<double> w(weights, weights + S);
+  std::vector<int> sel;
+  for (int j = 0; j < S; ++j)
+    if (w[j] != 0.0) sel.push_back(j);
+  const int nsel = (int)sel.size();
+  const size_t head = ((size_t)S + ((size_t)S + 1) / 2 + 1) & ~(size_t)1;   // 16-byte aligned output
+  w.resize(head);
+  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
+  if ((e = ensure(c, c->aux, (head + 2 * (size_t)n0) * sizeof(double)))) return e;
+  double *dw = (double *)c->aux.p;
+  double2 *dout = (double2 *)(dw + head);
+  RT(rt_h2d(dw, w.data(), head * sizeof(double), c->stream));
+  const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
+  if (f.prec == CWTB_F64) {
+    CrossScaleAvgArgs<double> a{(const double2 *)f.p, dw, (const int *)(dw + S), nsel, dout, n0};
+    e = launch<CrossScaleAvgBody<double>>(c, gx, 1, a);
+  } else {
+    CrossScaleAvgArgs<float> a{(const float2 *)f.p, dw, (const int *)(dw + S), nsel, dout, n0};
+    e = launch<CrossScaleAvgBody<float>>(c, gx, 1, a);
+  }
+  if (e) return e;
+  RT(rt_d2h(out, dout, (size_t)n0 * sizeof(double2), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
 }
 
 // WCT and aWCT of a coherence share one device buffer; aWCT starts on a 256-byte boundary, so that
@@ -3043,8 +3254,8 @@ int cwtb_coherence_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, 
   const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
   CohRowStatsArgs a{dW, dA, dlo, dhi, thr ? dthr : nullptr, dpart, n0, nchunk, want_phase != 0};
   if ((e = launch<B>(c, (unsigned)nchunk, (unsigned)S, a))) return e;
-  CohRowSumArgs r{dpart, dsum, S, nchunk};
-  if ((e = launch<CohRowSumBody>(c, (unsigned)((4 * S + NT - 1) / NT), 1, r))) return e;
+  RowSumArgs r{dpart, dsum, S, nchunk};
+  if ((e = launch<RowSumBody<4>>(c, (unsigned)((4 * S + NT - 1) / NT), 1, r))) return e;
   RT(rt_d2h(out, dsum, (size_t)S * 4 * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;

@@ -1914,7 +1914,7 @@ template <typename T> struct ScaleAvgBody {
 // Per-row sums over the columns [lo_j, hi_j) where thr is null or WCT > thr_j (false for a NaN
 // threshold): [count, sum WCT, sum cos aWCT, sum sin aWCT].  CTA (bx, j) covers the fixed chunk
 // [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j's range with 16-byte streaming loads, reduces
-// its threads' sums in a fixed order and writes its partial; CohRowSumBody adds the partials of a
+// its threads' sums in a fixed order and writes its partial; RowSumBody<4> adds the partials of a
 // row in chunk order.  No atomics: repeated calls are bit-identical.
 struct CohRowStatsArgs {
   const double *WCT, *aWCT;
@@ -1996,18 +1996,19 @@ struct CohRowStatsBody {
   }
 };
 
-// out[j][k] = sum over chunks b (in order) of part[j][b][k]
-struct CohRowSumArgs { const double *part; double *out; int rows, nchunk; };
-struct CohRowSumBody {
-  using Args = CohRowSumArgs;
+// out[j][k] = sum over chunks b (in order) of part[j][b][k], k < K (the K sums per row of
+// CohRowStatsBody and CxRowStatsBody)
+struct RowSumArgs { const double *part; double *out; int rows, nchunk; };
+template <int K> struct RowSumBody {
+  using Args = RowSumArgs;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
     const int i = bx * NT + tid;
-    if (i >= 4 * a.rows) return;
-    const double *p = a.part + (size_t)(i >> 2) * a.nchunk * 4 + (i & 3);
+    if (i >= K * a.rows) return;
+    const double *p = a.part + (size_t)(i / K) * a.nchunk * K + (i % K);
     double v = 0;
-    for (int b = 0; b < a.nchunk; ++b) v += p[(size_t)b * 4];
+    for (int b = 0; b < a.nchunk; ++b) v += p[(size_t)b * K];
     a.out[i] = v;
   }
 };
@@ -2084,6 +2085,178 @@ struct CohWindowBody {
     const size_t dst = (size_t)by * a.ncols + c;
     if (a.oW) a.oW[dst] = a.WCT[src];
     if (a.oA) a.oA[dst] = a.aWCT[src];
+  }
+};
+
+// ---- Bodies: reductions of a resident complex field (cwtb_field_*: W or the cross spectrum) ----
+// F is a [rows][n] field of cx<T>.  Every sum is formed in double, after widening.
+
+// 16 bytes of a complex field: one double2, or two float2
+template <typename T> struct CxVec16;
+template <> struct CxVec16<double> {
+  using V = double2;
+  static constexpr int E = 1;
+  HD static double re(const V &v, int) { return v.x; }
+  HD static double im(const V &v, int) { return v.y; }
+};
+template <> struct CxVec16<float> {
+  using V = float4;
+  static constexpr int E = 2;
+  HD static double re(const V &v, int e) { return (double)(e ? v.z : v.x); }
+  HD static double im(const V &v, int e) { return (double)(e ? v.w : v.y); }
+};
+
+// Per-row sums over the columns [lo_j, hi_j) where thr is null or re^2 + im^2 > thr_j (false for a
+// NaN threshold): [count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F], with cos = re / |F|,
+// sin = im / |F| and a zero coefficient counted as phase 0 (np.angle(0) == 0).  The partition is
+// CohRowStatsBody's: CTA (bx, j) covers the fixed chunk [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK)
+// of row j's range with 16-byte streaming loads, reduces its threads' sums in a fixed order and
+// writes its partial; RowSumBody<5> adds the partials of a row in chunk order.  No atomics.
+template <typename T> struct CxRowStatsArgs {
+  const cx<T> *F;
+  const long long *lo, *hi;   // per row
+  const double *thr;          // per row, or null
+  double *part;               // [rows][nchunk][5]
+  long long n;
+  int nchunk;
+};
+template <typename T> struct CxRowStatsBody {
+  using Args = CxRowStatsArgs<T>;
+  using Vec = CxVec16<T>;
+  static constexpr int NTB = 256, NPHASE = 3, K = 5;
+  static constexpr int U = 4;                                          // 16-byte loads in flight
+  static constexpr long long CHUNK = (long long)Vec::E * 32 * NTB;    // 32 loads per thread
+  static constexpr size_t SMEM = (size_t)K * (NTB + 32) * sizeof(double);
+  HD static void add(double (&s)[K], double re, double im, bool has_thr, double t) {
+    const double p = norm2_rn(re, im);
+    if (has_thr && !(p > t)) return;
+    const double m = sqrt(p);
+    s[0] += 1.0;
+    s[1] += p;
+    s[2] += m;
+    if (m > 0) {
+      s[3] += re / m;
+      s[4] += im / m;
+    } else {
+      s[3] += 1.0;
+    }
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double *sm = (double *)smraw;          // [K][NTB] thread sums, then [K][32] lane sums
+    if constexpr (PH == 0) {
+      double s[K] = {0, 0, 0, 0, 0};
+      const long long lo = a.lo[by], hi = a.hi[by];
+      const long long c0 = lo + (long long)bx * CHUNK;
+      if (c0 < hi) {
+        const long long c1 = c0 + CHUNK < hi ? c0 + CHUNK : hi;
+        const bool has_thr = a.thr != nullptr;
+        const double t = has_thr ? a.thr[by] : 0.0;
+        constexpr size_t E = Vec::E;
+        const size_t p0 = (size_t)by * a.n + c0, p1 = (size_t)by * a.n + c1;
+        const size_t v0 = (p0 + E - 1) / E, v1 = p1 / E;   // [v0, v1): whole 16-byte vectors
+        if constexpr (E == 2) {                             // an odd element at either end
+          if (tid == 0 && (p0 & 1)) add(s, a.F[p0].x, a.F[p0].y, has_thr, t);
+          if (tid == 1 && (p1 & 1) && p1 - 1 >= E * v0) add(s, a.F[p1 - 1].x, a.F[p1 - 1].y, has_thr, t);
+        }
+        const typename Vec::V *F16 = (const typename Vec::V *)a.F;
+        for (size_t q0 = v0 + (size_t)tid; q0 < v1; q0 += (size_t)NTB * U) {
+          typename Vec::V w[U] = {};
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const size_t q = q0 + (size_t)NTB * u;
+            if (q < v1) w[u] = ld_stream(F16 + q);
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            if (q0 + (size_t)NTB * u < v1) {
+#pragma unroll
+              for (int e = 0; e < (int)E; ++e) add(s, Vec::re(w[u], e), Vec::im(w[u], e), has_thr, t);
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < K; ++k) sm[k * NTB + tid] = s[k];
+    } else if constexpr (PH == 1) {
+      if (tid < K * 32) {
+        const int k = tid >> 5, l = tid & 31;
+        double v = 0;
+        for (int i = l; i < NTB; i += 32) v += sm[k * NTB + i];
+        sm[K * NTB + tid] = v;
+      }
+    } else {
+      if (tid < K) {
+        double v = 0;
+        for (int l = 0; l < 32; ++l) v += sm[K * NTB + tid * 32 + l];
+        a.part[((size_t)by * a.nchunk + bx) * K + tid] = v;
+      }
+    }
+  }
+};
+
+// out[n] = sum_j w_j F[j,n] (complex128) over the selected rows, in order: one thread per column
+// (the selected-rows pattern of CohScaleAvgBody), no atomics.
+template <typename T> struct CrossScaleAvgArgs {
+  const cx<T> *F;
+  const double *w;     // per row
+  const int *sel;      // rows with a non-zero weight, ascending (device)
+  int nsel;
+  double2 *out;        // [n]
+  long long n;
+};
+template <typename T> struct CrossScaleAvgBody {
+  using Args = CrossScaleAvgArgs<T>;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const long long n = (long long)bx * NT + tid;
+    if (n >= a.n) return;
+    double sr = 0, si = 0;
+    int i = 0;
+    for (; i + 4 <= a.nsel; i += 4) {
+      cx<T> v[4];
+      double wj[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int j = a.sel[i + u];
+        wj[u] = a.w[j];
+        v[u] = ld_stream(&a.F[(size_t)j * a.n + n]);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        sr += wj[u] * (double)v[u].x;
+        si += wj[u] * (double)v[u].y;
+      }
+    }
+    for (; i < a.nsel; ++i) {
+      const int j = a.sel[i];
+      const cx<T> v = ld_stream(&a.F[(size_t)j * a.n + n]);
+      sr += a.w[j] * (double)v.x;
+      si += a.w[j] * (double)v.y;
+    }
+    st_stream(&a.out[n], make_double2(sr, si));
+  }
+};
+
+// Strided sub-grid as complex128: out[r][c] = F[row0 + r row_step][col0 + c col_step].
+// Grid: (ceil(ncols / NT), nrows).
+template <typename T> struct CxWindowArgs {
+  const cx<T> *F;
+  double2 *out;        // [nrows][ncols]
+  long long n;
+  int row0, row_step;
+  long long col0, col_step, ncols;
+};
+template <typename T> struct CxWindowBody {
+  using Args = CxWindowArgs<T>;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long c = (long long)bx * NT + tid;
+    if (c >= a.ncols) return;
+    const size_t src = (size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + c * a.col_step;
+    const cx<T> v = a.F[src];
+    a.out[(size_t)by * a.ncols + c] = make_double2((double)v.x, (double)v.y);
   }
 };
 

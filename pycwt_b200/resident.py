@@ -14,7 +14,8 @@ then do with W (pycwt/sample/simple_sample.py:64-96) are reductions of |W|^2:
 methods evaluate those products on the device, so only O(S) or O(N) numbers cross the bus.
 The handle is valid until the next transform on the same engine.
 
-`wct_resident` does the same for the wavelet coherence (see the second half of this module).
+`wct_resident` does the same for the wavelet coherence and `xwt_resident` for the cross-wavelet
+transform (see the second half of this module).
 """
 import collections
 
@@ -23,9 +24,11 @@ import numpy as np
 from . import _engine
 from .helpers import ar1, fft, fft_kwargs
 from .wavelet import (_check_parameter_wavelet, _coi, _nan_rows, _precision, _resolve_scales,
-                      _sync_padding, _wct_on_device, _wct_problem, _wct_significance)
+                      _sync_padding, _wct_on_device, _wct_problem, _wct_significance,
+                      _xwt_on_device, _xwt_problem, _xwt_signif)
 
-__all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence']
+__all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence',
+           'xwt_resident', 'ResidentCrossWavelet']
 
 
 def _coi_ranges(wavelet, dt, n0, period):
@@ -132,13 +135,33 @@ class ResidentTransform(object):
         return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
 
     @_live
-    def global_power(self, inside_coi=False):
+    def window(self, rows=slice(None), cols=slice(None)):
+        """W[rows, cols] (complex128) for two slices with steps >= 1, gathered on the device: only
+        the sub-grid crosses the bus."""
+        return _field_window(self.engine, _engine.FIELD_W, self.shape, rows, cols)
+
+    @_live
+    def global_power(self, inside_coi=False, signif=None):
         """Time mean of |W|^2 per scale (`power.mean(axis=1)`); with `inside_coi` only over
-        the columns where the period is inside the cone of influence (NaN if there are none)."""
-        if not inside_coi:
-            return self.engine.global_power(len(self.scales))
+        the columns where the period is inside the cone of influence, with `signif` (power units,
+        as `significance()` returns it) only over the points where |W|^2 > signif[j] (none where
+        signif[j] is NaN).  NaN for a scale without points."""
+        if signif is None:
+            if not inside_coi:
+                return self.engine.global_power(len(self.scales))
+            lo, hi = self.coi_ranges()
+            return self.engine.global_power_ranges(lo, hi)
+        lo, hi = _column_ranges(self, inside_coi)
+        st = self.engine.field_row_stats(_engine.FIELD_W, lo, hi, _power_threshold(self, signif))
+        return _ratio(st[:, 1], st[:, 0])
+
+    @_live
+    def significant_fraction(self, signif):
+        """Per scale, the fraction of the points inside the cone of influence where
+        |W|^2 > signif[j] (power units); NaN for a scale without such points."""
         lo, hi = self.coi_ranges()
-        return self.engine.global_power_ranges(lo, hi)
+        st = self.engine.field_row_stats(_engine.FIELD_W, lo, hi, _power_threshold(self, signif))
+        return _ratio(st[:, 0], hi - lo)
 
     @_live
     def scale_avg_power(self, period_min, period_max, variance=1.0):
@@ -228,6 +251,46 @@ def _slice_range(s, n, name):
     return start, len(range(start, stop, step)), step
 
 
+def _field_window(engine, field, shape, rows, cols):
+    """field[rows, cols] of a resident complex field, complex128, gathered on the device."""
+    S, n0 = shape
+    r0, nr, rs = _slice_range(rows, S, 'rows')
+    c0, nc, cs = _slice_range(cols, n0, 'cols')
+    if nr == 0 or nc == 0:
+        return np.empty((nr, nc), dtype=np.complex128)
+    return engine.field_window(field, r0, nr, rs, c0, nc, cs)
+
+
+def _column_ranges(h, inside_coi):
+    """Per scale, the columns inside the cone of influence, or every column."""
+    if inside_coi:
+        return h.coi_ranges()
+    S = len(h.scales)
+    return np.zeros(S, dtype=np.int64), np.full(S, h.n0, dtype=np.int64)
+
+
+def _power_threshold(h, signif):
+    """A per-scale threshold on |F|^2: one entry per scale, none negative (NaN selects no point)."""
+    thr = np.asarray(signif, dtype=float)
+    if thr.shape != (len(h.scales),):
+        raise ValueError("signif must have one entry per scale (%d), got shape %s"
+                         % (len(h.scales), thr.shape))
+    if (thr < 0).any():
+        raise ValueError("signif must not be negative")
+    return thr
+
+
+def _mean_phase(cnt, c, s, per_scale):
+    """MeanPhase of per-scale point counts and sums of cos / sin of the phase."""
+    if not per_scale:
+        cnt, c, s = cnt.sum(), c.sum(), s.sum()
+    angle = np.where(cnt > 0, np.arctan2(s, c), np.nan)
+    strength = _ratio(np.hypot(c, s), cnt)
+    if per_scale:
+        return MeanPhase(angle, strength, cnt.astype(np.int64))
+    return MeanPhase(float(angle), float(strength), int(cnt))
+
+
 def _ratio(num, den):
     """num / den, NaN where den == 0."""
     num = np.asarray(num, dtype=float)
@@ -286,12 +349,6 @@ class ResidentCoherence(object):
             if self.engine.coherence_serial() == self._serial:
                 self.engine.coherence_release()
 
-    def _ranges(self, inside_coi):
-        if inside_coi:
-            return self.coi_ranges()
-        S = len(self.scales)
-        return np.zeros(S, dtype=np.int64), np.full(S, self.n0, dtype=np.int64)
-
     def _threshold(self, sig95):
         if sig95 is None:
             return None
@@ -343,7 +400,7 @@ class ResidentCoherence(object):
         """Mean WCT per scale over the selected points: inside the cone of influence
         (period_j <= coi[n]) if `inside_coi`, where WCT[j, n] > sig95[j] if `sig95` is given
         (false where sig95[j] is NaN).  NaN for a scale without points."""
-        lo, hi = self._ranges(inside_coi)
+        lo, hi = _column_ranges(self, inside_coi)
         st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95))
         return _ratio(st[:, 1], st[:, 0])
 
@@ -365,17 +422,10 @@ class ResidentCoherence(object):
         (arrays; NaN angle and strength where the count is 0)."""
         per = self.period
         sel = (per >= period_min) & (per < period_max)
-        lo, hi = self._ranges(inside_coi)
+        lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
         st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95), want_phase=True)
-        cnt, c, s = st[:, 0], st[:, 2], st[:, 3]
-        if not per_scale:
-            cnt, c, s = cnt.sum(), c.sum(), s.sum()
-        angle = np.where(cnt > 0, np.arctan2(s, c), np.nan)
-        strength = _ratio(np.hypot(c, s), cnt)
-        if per_scale:
-            return MeanPhase(angle, strength, cnt.astype(np.int64))
-        return MeanPhase(float(angle), float(strength), int(cnt))
+        return _mean_phase(st[:, 0], st[:, 2], st[:, 3], per_scale)
 
     @_live
     def scale_avg(self, period_min, period_max):
@@ -400,3 +450,142 @@ def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=T
     eng = engine or _engine.default_engine()
     serial = _wct_on_device(eng, p, eng.wct_resident)
     return ResidentCoherence(eng, p, precision, serial)
+
+
+# ---- resident cross spectrum -------------------------------------------------------------------
+# `xwt` hands the caller a complex128 [S, n0] field; at config 4 that is 608 MB over PCIe for about
+# 1.5 ms of GPU work.  What the reference's sample script (pycwt/sample/sample_xwt.py) and Grinsted
+# et al. (2004) do with it are |W12| against `signif`, phase arrows on a sub-grid and the circular
+# mean phase over the region where |W12| is significant.  `xwt_resident` runs the same transforms
+# as `xwt` and keeps W12 on the device, in a buffer of its own: the handle stays valid across later
+# cwt / xwt / wct / wct_resident / Monte-Carlo calls, until the next `xwt_resident` on the same
+# engine or `release()`.
+
+class ResidentCrossWavelet(object):
+    """W12 = W1 conj(W2) [S, n0] of one `xwt_resident` call, resident on the device.
+
+    `signif` arguments of the methods are in |W12| units, as `xwt` returns them (`.signif`); a
+    point is selected where |W12| > signif[j], i.e. re^2 + im^2 > signif[j]^2.  The sample
+    script's `|W12|^2 / signif > 1` convention is `signif=np.sqrt(h.signif)`.  A negative entry
+    raises ValueError, a NaN entry selects no point of its scale."""
+
+    def __init__(self, engine, problem, signif, precision, serial):
+        p = problem
+        self.engine = engine
+        self.wavelet = p.wavelet
+        self.n0 = int(p.n0)
+        self.dt = float(p.dt)
+        self.dj = p.dj
+        self.scales = p.sj
+        self.freq = p.freq
+        self.signif = signif
+        self.precision = precision
+        self._serial = serial
+        self._coi = None
+
+    @property
+    def coi(self):
+        if self._coi is None:
+            self._coi = _coi(self.wavelet, self.dt, self.n0)
+        return self._coi
+
+    @property
+    def shape(self):
+        return (len(self.scales), self.n0)
+
+    @property
+    def period(self):
+        return 1.0 / np.asarray(self.freq)
+
+    def coi_ranges(self):
+        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
+        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
+
+    # -- bookkeeping ---------------------------------------------------------------------
+    def _check_live(self):
+        if self.engine.cross_serial() != self._serial:
+            raise _engine.EngineError("this cross spectrum is no longer resident: it was released "
+                                      "or another xwt_resident has run on the same engine")
+
+    def release(self):
+        """Free the device buffer (16 or 8 bytes per scale and time point).  The handle is
+        invalid afterwards; releasing an invalid handle does nothing."""
+        with self.engine.lock:
+            if self.engine.cross_serial() == self._serial:
+                self.engine.cross_release()
+
+    def _stats(self, lo, hi, signif):
+        thr = None if signif is None else _power_threshold(self, signif) ** 2
+        return self.engine.field_row_stats(_engine.FIELD_CROSS, lo, hi, thr)
+
+    # -- the products --------------------------------------------------------------------
+    @_live
+    def cross_spectrum(self):
+        """W12 (complex128, S x n0), as returned by `xwt`: the expensive fetch."""
+        return self.engine.field_get(_engine.FIELD_CROSS)
+
+    @_live
+    def window(self, rows=slice(None), cols=slice(None)):
+        """W12[rows, cols] (complex128) for two slices with steps >= 1, gathered on the device
+        (phase arrows, a down-sampled |W12| image)."""
+        return _field_window(self.engine, _engine.FIELD_CROSS, self.shape, rows, cols)
+
+    @_live
+    def global_power(self, inside_coi=False, signif=None):
+        """Mean |W12| per scale over the selected points: inside the cone of influence if
+        `inside_coi`, where |W12| > signif[j] if `signif` is given.  NaN for a scale without
+        points."""
+        st = self._stats(*_column_ranges(self, inside_coi), signif)
+        return _ratio(st[:, 2], st[:, 0])
+
+    @_live
+    def significant_fraction(self, signif):
+        """Per scale, the fraction of the points inside the cone of influence where
+        |W12| > signif[j]; NaN for a scale without points inside the cone."""
+        lo, hi = self.coi_ranges()
+        st = self._stats(lo, hi, signif)
+        return _ratio(st[:, 0], hi - lo)
+
+    @_live
+    def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, signif=None,
+                   per_scale=False):
+        """Circular mean of angle(W12) over the points of the scales with period_min <= period <
+        period_max, inside the cone of influence if `inside_coi`, where |W12| > signif if given
+        (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
+        |sum e^{i angle}| / count, count), for the whole band or, with `per_scale`, per scale
+        (NaN angle and strength where the count is 0).  A zero coefficient has phase 0."""
+        per = self.period
+        sel = (per >= period_min) & (per < period_max)
+        lo, hi = _column_ranges(self, inside_coi)
+        lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
+        st = self._stats(lo, hi, signif)
+        return _mean_phase(st[:, 0], st[:, 3], st[:, 4], per_scale)
+
+    @_live
+    def scale_avg(self, period_min, period_max):
+        """Scale-averaged cross spectrum over period_min <= period < period_max (complex128,
+        length n0): dj * dt / Cdelta * sum_j W12[j] / s_j, Torrence & Compo (1998) eq. 24 with
+        W12 in place of |W|^2."""
+        if self.wavelet.cdelta == -1:
+            raise ValueError('Cdelta not defined for this wavelet')
+        per = self.period
+        sel = (per >= period_min) & (per < period_max)
+        if not sel.any():
+            raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
+        w = np.where(sel, 1.0 / np.asarray(self.scales, dtype=float), 0.0)
+        w = w * (self.dj * self.dt / self.wavelet.cdelta)
+        return self.engine.cross_scale_avg(w)
+
+
+def xwt_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95, wavelet='morlet',
+                 normalize=True, precision='fp64', engine=None):
+    """Same cross-wavelet transform as `xwt(y1, y2, dt, dj, s0, J, significance_level, wavelet,
+    normalize, precision)`, W12 kept on the device.
+
+    Returns a `ResidentCrossWavelet`; its `signif` is `xwt`'s fourth return value.  Scales,
+    standardisation, the un-padded fallback to fp64 and `signif` are resolved by the same code
+    as `xwt`'s.  No transform stays resident afterwards (handles of `cwt_resident` die)."""
+    p = _xwt_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
+    eng = engine or _engine.default_engine()
+    serial = _xwt_on_device(eng, p, eng.xwt_resident)
+    return ResidentCrossWavelet(eng, p, _xwt_signif(p, significance_level), precision, serial)

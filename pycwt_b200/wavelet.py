@@ -296,6 +296,17 @@ def xwt(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
     pass) run on the GPU.  Returns (W12, coi, freq, signif).  `precision` (an extension of
     the reference signature): 'fp64' (default) or 'fp32', the arithmetic of the transforms;
     W12 is complex128 either way.  Un-padded transforms run in fp64 whatever is asked."""
+    p = _xwt_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
+    eng = _engine.default_engine()
+    W12 = _xwt_on_device(eng, p, eng.xwt)
+    coi = _coi(p.wavelet, dt, p.n0)
+    return W12, coi, p.freq, _xwt_signif(p, significance_level)
+
+
+def _xwt_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
+    """What `xwt` resolves on the host before the device call (reference wavelet.py:370-394): the
+    wavelet, the raw and standardised series, the scales without the reference's all-NaN rows
+    and the requested engine precision."""
     prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     y1, y1n, std1 = _standardise(y1, normalize)
@@ -307,24 +318,31 @@ def xwt(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
     if not keep.any():
         keep[:] = True
     sj, freq = sj[keep], freq[keep]
-    eng = _engine.default_engine()
-    with eng.lock:
-        if _sync_padding(eng, n0):
-            prec = _engine.F64      # un-padded transforms run in fp64
-        W12 = eng.xwt(y1n, y2n, dt, sj, *_family_of(wavelet), precision=prec)
-    coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
-    coi = wavelet.flambda() * wavelet.coi() * dt * coi
+    return _Problem(y1=y1, y2=y2, y1n=y1n, y2n=y2n, std1=std1, std2=std2, n0=n0, dt=dt, dj=dj,
+                    wavelet=wavelet, sj=sj, freq=freq, normalize=normalize, prec=prec)
 
-    if normalize:
-        std1 = std2 = 1.
-    a1, _, _ = ar1(y1)
-    a2, _, _ = ar1(y2)
-    Pk1 = ar1_spectrum(freq * dt, a1)
-    Pk2 = ar1_spectrum(freq * dt, a2)
-    dof = wavelet.dofmin
+
+def _xwt_on_device(eng, p, call):
+    """One engine transaction of the cross transform: length policy (un-padded transforms run in
+    fp64), then call(y1n, y2n, dt, scales, family, param, precision=).  Returns the call's result;
+    `p.prec` becomes the precision used."""
+    with eng.lock:
+        if _sync_padding(eng, p.n0):
+            p.prec = _engine.F64      # un-padded transforms run in fp64
+        return call(p.y1n, p.y2n, p.dt, p.sj, *_family_of(p.wavelet), precision=p.prec)
+
+
+def _xwt_signif(p, significance_level):
+    """Significance level of |W12| per scale against the two series' red-noise spectra (reference
+    wavelet.py:404-418): the fourth return value of `xwt`."""
+    std1, std2 = (1., 1.) if p.normalize else (p.std1, p.std2)
+    a1, _, _ = ar1(p.y1)
+    a2, _, _ = ar1(p.y2)
+    Pk1 = ar1_spectrum(p.freq * p.dt, a1)
+    Pk2 = ar1_spectrum(p.freq * p.dt, a2)
+    dof = p.wavelet.dofmin
     PPF = chi2.ppf(significance_level, dof)
-    signif = (std1 * std2 * (Pk1 * Pk2) ** 0.5 * PPF / dof)
-    return W12, coi, freq, signif
+    return (std1 * std2 * (Pk1 * Pk2) ** 0.5 * PPF / dof)
 
 
 def _family_of(wavelet):
@@ -368,16 +386,18 @@ def _coi(wavelet, dt, n0):
     return wavelet.flambda() * wavelet.coi() * dt * coi
 
 
-class _WctProblem(object):
-    """What `wct` resolves on the host before the device pipeline (reference wavelet.py:461-497):
-    the wavelet, s0 and J, the raw and standardised series, the scales, the boxcar length and the
-    requested engine precision."""
+class _Problem(object):
+    """What `xwt` / `wct` resolve on the host before the device call (see `_xwt_problem` and
+    `_wct_problem`)."""
 
     def __init__(self, **kw):
         self.__dict__.update(kw)
 
 
 def _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
+    """What `wct` resolves on the host before the device pipeline (reference wavelet.py:461-497):
+    the wavelet, s0 and J, the raw and standardised series, the scales, the boxcar length and the
+    requested engine precision."""
     prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     if not hasattr(wavelet, 'smooth'):
@@ -395,8 +415,8 @@ def _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
     klen = _boxcar_len(wavelet, dj)
     if klen < 1:
         raise ValueError('smoothing window undefined for this wavelet (deltaj0 = -1)')
-    return _WctProblem(y1=y1, y2=y2, y1n=y1n, y2n=y2n, n0=n0, dt=dt, dj=dj, s0=s0, J=J,
-                       wavelet=wavelet, sj=sj, freq=freq, klen=klen, prec=prec)
+    return _Problem(y1=y1, y2=y2, y1n=y1n, y2n=y2n, n0=n0, dt=dt, dj=dj, s0=s0, J=J,
+                    wavelet=wavelet, sj=sj, freq=freq, klen=klen, prec=prec)
 
 
 def _wct_on_device(eng, p, call):
