@@ -8,7 +8,7 @@ Per precision the two paths run alternately, `--reps` times:
 For every call the script records the end-to-end time of the Python call and, for the two
 cross-transform calls, the device time of the engine's kernels (last_kernel_ms); it reports their
 median and min-max.  A separate pass records the device time of each product's kernels
-(cwtb_profile_begin / end), and the rate at which `CxRowStatsBody` reads W12 in
+(cwtb_profile_begin / end), and the rate at which `RowStatsBody<CxView>` reads W12 in
 `global_power(inside_coi=True)`: S x (columns inside the cone) x (bytes per coefficient: 16 in
 fp64, 8 in fp32) over its time, against the data sheet's 3.35 TB/s.  The card's name, power limit
 and maximum SM clock go into the output.  Needs a GPU: without one it fails.  The summary goes to
@@ -110,12 +110,12 @@ def main():
         for _ in range(5):
             eng.profile_begin()
             h.global_power(inside_coi=True)
-            ms.append(sum(r["ms"] for r in eng.profile_end() if "CxRowStats" in r["name"]))
+            ms.append(sum(r["ms"] for r in eng.profile_end() if "RowStatsBody" in r["name"]))
         kms = float(np.median(ms))
         rate = nbytes / (kms * 1e-3) / 1e12
         res["row_stats_rate"][p] = {"bytes": nbytes, "kernel_ms": kms, "kernel_ms_all": ms, "TB_s": rate,
                                     "of_data_sheet": rate / HBM_TBS}
-        print(p, "CxRowStatsBody %.1f MB in %.4f ms: %.2f TB/s, %.2f of %.2f TB/s"
+        print(p, "RowStatsBody<CxView> %.1f MB in %.4f ms: %.2f TB/s, %.2f of %.2f TB/s"
               % (nbytes / 1e6, kms, rate, rate / HBM_TBS, HBM_TBS), flush=True)
         h.release()
     if args.out:

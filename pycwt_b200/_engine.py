@@ -13,6 +13,8 @@ LIB_PATH = os.path.join(_HERE, "libcwtb200.so")
 MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
 F64, F32 = 0, 1
 FIELD_W, FIELD_CROSS = 0, 1      # complex fields of the cwtb_field_* calls
+FIELD_COH = -1                   # the resident coherence (calls of its own, not a cwtb_field)
+_NOT_RESIDENT = {FIELD_COH: "no coherence resident", FIELD_CROSS: "no cross spectrum resident"}
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -127,6 +129,27 @@ def _locked(method):
     return wrapper
 
 
+def _row_args(name, rows, lo, hi, thr):
+    """lo, hi (and thr, if given) of a per-row reduction, checked for one entry per row."""
+    lo = np.ascontiguousarray(lo, dtype=np.int64)
+    hi = np.ascontiguousarray(hi, dtype=np.int64)
+    if lo.shape != (rows,) or hi.shape != (rows,):
+        raise ValueError("%s: one column range per row expected" % name)
+    if thr is not None:
+        thr = np.ascontiguousarray(thr, dtype=np.float64)
+        if thr.shape != (rows,):
+            raise ValueError("%s: one threshold per row expected" % name)
+    return lo, hi, thr
+
+
+def _weights(name, rows, weights):
+    """Per-row weights of a scale average, checked for one entry per row."""
+    w = np.ascontiguousarray(weights, dtype=np.float64)
+    if w.shape != (rows,):
+        raise ValueError("%s: one weight per row expected" % name)
+    return w
+
+
 class Engine(object):
     """One context = one device + one stream.  Every call into the C library is made under
     `self.lock`, a re-entrant lock: compound operations of the Python surface (set the length
@@ -153,6 +176,7 @@ class Engine(object):
         self._pool_bytes = 0
         self._dead = []          # retired pinned buffers waiting for _reap()
         self._outstanding = 0    # result arrays still alive that alias pinned memory
+        self._held = {}          # (rows, n0) of the resident coherence and cross spectrum, by field
 
     def _reap(self):
         """Free the pinned buffers the finalizers retired.  Finalizers never call into the
@@ -508,8 +532,15 @@ class Engine(object):
             self._resident = None                   # several intermediates, no single transform
         return WCT, aWCT
 
-    # ---- resident coherence (its own device buffer, see include/cwt_b200.h) ------------------
-    _coherence = None        # (rows, n0) of the resident coherence
+    # ---- resident coherence and cross spectrum (device buffers of their own, see
+    # include/cwt_b200.h) and the reads of a resident field ------------------------------------
+    def _shape(self, field):
+        """(rows, n0) of the resident field: the coherence, the cross spectrum or, for any other
+        field, the transform."""
+        shape = self._held.get(field) if field in _NOT_RESIDENT else self._resident
+        if shape is None:
+            raise EngineError(_NOT_RESIDENT.get(field, "no single transform resident"))
+        return shape
 
     @_locked
     def wct_resident(self, y1, y2, dt, dj, scales, family, param, boxcar_len, precision=F64):
@@ -520,13 +551,13 @@ class Engine(object):
         if y1.shape != y2.shape or y1.ndim != 1:
             raise ValueError("wct_resident: the two series must be 1-D and of equal length")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
-        self._coherence = None
+        self._held[FIELD_COH] = None
         self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
                                                _ptr(sj), sj.size, int(family), float(param),
                                                int(boxcar_len)))
-        self._coherence = (sj.size, y1.size)
+        self._held[FIELD_COH] = (sj.size, y1.size)
         return self.coherence_serial()
 
     @_locked
@@ -535,20 +566,15 @@ class Engine(object):
 
     @_locked
     def coherence_release(self):
-        self._coherence = None
+        self._held[FIELD_COH] = None
         self._check(self.lib.cwtb_coherence_release(self.h))
-
-    def _coherence_shape(self):
-        if self._coherence is None:
-            raise EngineError("no coherence resident")
-        return self._coherence
 
     @_locked
     def coherence_window(self, row0, nrows, row_step, col0, ncols, col_step, want_wct=True,
                          want_angle=True):
         """(WCT, aWCT)[row0::row_step][:nrows, col0::col_step][:, :ncols] of the resident
         coherence; a field not asked for is None."""
-        self._coherence_shape()
+        self._shape(FIELD_COH)
         WCT = self.result_array((nrows, ncols), np.float64) if want_wct else None
         aWCT = self.result_array((nrows, ncols), np.float64) if want_angle else None
         self._check(self.lib.cwtb_coherence_window(
@@ -560,15 +586,8 @@ class Engine(object):
     def coherence_row_stats(self, lo, hi, thr=None, want_phase=False):
         """[rows, 4]: count, sum WCT, sum cos aWCT, sum sin aWCT over the columns [lo[j], hi[j])
         where thr is None or WCT > thr[j]."""
-        rows, _ = self._coherence_shape()
-        lo = np.ascontiguousarray(lo, dtype=np.int64)
-        hi = np.ascontiguousarray(hi, dtype=np.int64)
-        if lo.shape != (rows,) or hi.shape != (rows,):
-            raise ValueError("coherence_row_stats: one column range per row expected")
-        if thr is not None:
-            thr = np.ascontiguousarray(thr, dtype=np.float64)
-            if thr.shape != (rows,):
-                raise ValueError("coherence_row_stats: one threshold per row expected")
+        rows, _ = self._shape(FIELD_COH)
+        lo, hi, thr = _row_args("coherence_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 4), dtype=np.float64)
         self._check(self.lib.cwtb_coherence_row_stats(self.h, _ptr(lo), _ptr(hi),
                                                       None if thr is None else _ptr(thr),
@@ -578,16 +597,11 @@ class Engine(object):
     @_locked
     def coherence_scale_avg(self, weights):
         """[3, n0]: sum_j w_j WCT[j], sum_j w_j cos aWCT[j], sum_j w_j sin aWCT[j]."""
-        rows, n0 = self._coherence_shape()
-        w = np.ascontiguousarray(weights, dtype=np.float64)
-        if w.shape != (rows,):
-            raise ValueError("coherence_scale_avg: one weight per row expected")
+        rows, n0 = self._shape(FIELD_COH)
+        w = _weights("coherence_scale_avg", rows, weights)
         out = self.result_array((3, n0), np.float64)
         self._check(self.lib.cwtb_coherence_scale_avg(self.h, _ptr(w), _ptr(out)))
         return out
-
-    # ---- resident cross spectrum and complex-field reductions (include/cwt_b200.h) -----------
-    _cross = None            # (rows, n0) of the resident cross spectrum
 
     @_locked
     def xwt_resident(self, y1, y2, dt, scales, family, param, precision=F64):
@@ -598,12 +612,12 @@ class Engine(object):
         if y1.shape != y2.shape or y1.ndim != 1:
             raise ValueError("xwt_resident: the two series must be 1-D and of equal length")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
-        self._cross = None
+        self._held[FIELD_CROSS] = None
         self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_xwt_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt),
                                                _ptr(sj), sj.size, int(family), float(param)))
-        self._cross = (sj.size, y1.size)
+        self._held[FIELD_CROSS] = (sj.size, y1.size)
         return self.cross_serial()
 
     @_locked
@@ -612,20 +626,13 @@ class Engine(object):
 
     @_locked
     def cross_release(self):
-        self._cross = None
+        self._held[FIELD_CROSS] = None
         self._check(self.lib.cwtb_cross_release(self.h))
-
-    def _field_shape(self, field):
-        shape = self._cross if field == FIELD_CROSS else self._resident
-        if shape is None:
-            raise EngineError("no cross spectrum resident" if field == FIELD_CROSS
-                              else "no single transform resident")
-        return shape
 
     @_locked
     def field_get(self, field):
         """The whole field, complex128 [rows, n0]."""
-        rows, n0 = self._field_shape(field)
+        rows, n0 = self._shape(field)
         out = self.result_array((rows, n0), np.complex128)
         self._check(self.lib.cwtb_field_get(self.h, int(field), 0, rows, _ptr(out)))
         return out
@@ -633,7 +640,7 @@ class Engine(object):
     @_locked
     def field_window(self, field, row0, nrows, row_step, col0, ncols, col_step):
         """F[row0::row_step][:nrows, col0::col_step][:, :ncols] as complex128."""
-        self._field_shape(field)
+        self._shape(field)
         out = self.result_array((nrows, ncols), np.complex128)
         self._check(self.lib.cwtb_field_window(self.h, int(field), int(row0), int(nrows), int(row_step),
                                                int(col0), int(ncols), int(col_step), _ptr(out)))
@@ -643,15 +650,8 @@ class Engine(object):
     def field_row_stats(self, field, lo, hi, thr=None):
         """[rows, 5]: count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F over the columns
         [lo[j], hi[j]) where thr is None or |F|^2 > thr[j]."""
-        rows, _ = self._field_shape(field)
-        lo = np.ascontiguousarray(lo, dtype=np.int64)
-        hi = np.ascontiguousarray(hi, dtype=np.int64)
-        if lo.shape != (rows,) or hi.shape != (rows,):
-            raise ValueError("field_row_stats: one column range per row expected")
-        if thr is not None:
-            thr = np.ascontiguousarray(thr, dtype=np.float64)
-            if thr.shape != (rows,):
-                raise ValueError("field_row_stats: one threshold per row expected")
+        rows, _ = self._shape(field)
+        lo, hi, thr = _row_args("field_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 5), dtype=np.float64)
         self._check(self.lib.cwtb_field_row_stats(self.h, int(field), _ptr(lo), _ptr(hi),
                                                   None if thr is None else _ptr(thr), _ptr(out)))
@@ -660,10 +660,8 @@ class Engine(object):
     @_locked
     def cross_scale_avg(self, weights):
         """sum_j w_j W12[j, :] (complex128, n0)."""
-        rows, n0 = self._field_shape(FIELD_CROSS)
-        w = np.ascontiguousarray(weights, dtype=np.float64)
-        if w.shape != (rows,):
-            raise ValueError("cross_scale_avg: one weight per row expected")
+        rows, n0 = self._shape(FIELD_CROSS)
+        w = _weights("cross_scale_avg", rows, weights)
         out = self.result_array((n0,), np.complex128)
         self._check(self.lib.cwtb_cross_scale_avg(self.h, _ptr(w), _ptr(out)))
         return out

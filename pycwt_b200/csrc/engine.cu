@@ -116,6 +116,16 @@ struct ClassRun {   // scales sharing one execution plan
   int os = 0;           // overlap-save group + 1 (0: another path)
 };
 
+// A product that one call writes to a device buffer of its own and that later calls read in place
+// (cwtb_wct_resident, cwtb_xwt_resident).  serial is bumped before every write and on release.
+struct ResidentSlot {
+  Buf buf;
+  int S = 0;                     // rows resident (0: none)
+  long long n0 = 0;
+  int prec = 0;
+  long long serial = 0;
+};
+
 // overlap-save plan of one input scale (os_plan): group + 1 (0: not overlap-save), kept taps
 // [t1 - M + 1, t1] of its impulse response, offset of its H in the context's H buffer
 struct OsRow { int grp = 0, t1 = 0, M = 0; long long hoff = 0; };
@@ -249,22 +259,13 @@ struct cwtb_ctx {
   int batch_pipeline = 1;        // CWTB_BATCH_PIPELINE=0: one synchronous chunk after the other
   double *angle_host = nullptr;  // cwtb_wct: host destination of the phase angle, copied on a copy stream
                                  // as soon as it exists (before the smoothing transforms), not after them
-  // resident coherence (cwtb_wct_resident): WCT [S][n0], aWCT at coh_angle_offset(S*n0).  Only
-  // cwtb_wct_resident writes this buffer, so it outlives any other call; cwtb_coherence_release
-  // frees it.  coh_serial is bumped before every write and on release (cwtb_coherence_serial).
-  Buf coh;
-  int coh_S = 0;                 // rows resident (0: none)
-  long long coh_n0 = 0;
-  long long coh_serial = 0;
-  // resident cross spectrum (cwtb_xwt_resident): W12 [cross_S][cross_n0] of precision cross_prec.
+  // resident coherence (cwtb_wct_resident): WCT [S][n0], aWCT at coh_angle_offset(S*n0), double.
+  // Only cwtb_wct_resident writes this slot, so it outlives any other call.
+  ResidentSlot coh;
+  // resident cross spectrum (cwtb_xwt_resident): W12 [S][n0] of precision prec.
   // cwtb_xwt_resident hands its transform's W over by swapping the two buffers, so W12 is never
-  // copied and the old cross buffer becomes the next transform's W.  Nothing else writes it;
-  // cwtb_cross_release frees it.  cross_serial is bumped before every write and on release.
-  Buf cross;
-  int cross_S = 0;               // rows resident (0: none)
-  long long cross_n0 = 0;
-  int cross_prec = 0;
-  long long cross_serial = 0;
+  // copied and the old cross buffer becomes the next transform's W.  Nothing else writes it.
+  ResidentSlot cross;
   bool w_moved = false;          // W went to the cross spectrum: no transform resident until the
                                  // next one writes W
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
@@ -2005,7 +2006,7 @@ void cwtb_destroy(cwtb_ctx *c) {
 #endif
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh, &c->cross})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh.buf, &c->cross.buf})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2897,52 +2898,62 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
              : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out);
 }
 
-// ---- resident cross spectrum ----------------------------------------------------------------
+// ---- resident products and the reading calls ------------------------------------------------
+// A call that writes a slot invalidates it first, so that one failing part-way leaves none resident
+static void slot_begin(ResidentSlot &s) {
+  ++s.serial;
+  s.S = 0;
+  s.n0 = 0;
+}
+
+static int slot_release(cwtb_ctx *c, ResidentSlot &s) {
+  slot_begin(s);
+  if (s.buf.p) {
+#ifndef CWTB_HOST_EMU
+    RT(cudaSetDevice(c->device));
+#endif
+    RT(rt_sync(c->stream));
+    rt_free(s.buf.p);
+    s.buf = Buf{};
+  }
+  return 0;
+}
+
 int cwtb_xwt_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt,
                       const double *scales, int n_scales, int family, double param) {
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
   if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
-  ++c->cross_serial;   // before the buffer is written: a call that fails part-way invalidates it too
-  c->cross_S = 0;
-  c->cross_n0 = 0;
+  slot_begin(c->cross);
   int e = c->coh_precision == CWTB_F32
               ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr)
               : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr);
   if (e) return e;
   // W12 is the transform's W: take the buffer over.  No kernel or plan keeps W's address (every
   // run takes it afresh from c->W), so the old cross buffer can serve as the next W.
-  std::swap(c->W, c->cross);
+  std::swap(c->W, c->cross.buf);
   c->w_moved = true;
-  c->cross_S = n_scales;
-  c->cross_n0 = n0;
-  c->cross_prec = c->job.precision;
+  c->cross.S = n_scales;
+  c->cross.n0 = n0;
+  c->cross.prec = c->job.precision;
   return 0;
 }
 
-int64_t cwtb_cross_serial(cwtb_ctx *c) { return c ? c->cross_serial : -1; }
+int64_t cwtb_cross_serial(cwtb_ctx *c) { return c ? c->cross.serial : -1; }
+int cwtb_cross_release(cwtb_ctx *c) { return c ? slot_release(c, c->cross) : CWTB_ERR_ARG; }
 
-int cwtb_cross_release(cwtb_ctx *c) {
-  if (!c) return CWTB_ERR_ARG;
-  ++c->cross_serial;
-  c->cross_S = 0;
-  c->cross_n0 = 0;
-  if (c->cross.p) {
-#ifndef CWTB_HOST_EMU
-    RT(cudaSetDevice(c->device));
-#endif
-    RT(rt_sync(c->stream));
-    rt_free(c->cross.p);
-    c->cross.p = nullptr;
-    c->cross.bytes = 0;
-  }
-  return 0;
-}
+// WCT and aWCT of a coherence share one device buffer; aWCT starts on a 256-byte boundary, so that
+// a flat index has the same alignment in both fields (the 16-byte loads of RowStatsBody<CohView>)
+static size_t coh_angle_offset(size_t cnt) { return (cnt + 31) & ~(size_t)31; }
 
-// A resident complex field of cwtb_field_*: the transform's W or the cross spectrum
+// A resident field of the reading calls: a cwtb_field (the transform's W or the cross spectrum),
+// or the coherence under an id of its own
+static constexpr int FIELD_COH = -1;
 struct FieldRef {
+  int field;
   const void *p;
-  int prec, S;
+  int prec, S;      // prec: the complex field's element type (the coherence is double)
   long long n0;
+  size_t angle;     // coherence: aWCT's offset from WCT, in doubles
 };
 
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
@@ -2950,12 +2961,13 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   if (field == CWTB_FIELD_W) {
     if (!w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
     if (c->job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "field of a batched transform: fetch rows per channel");
-    f = FieldRef{c->W.p, c->job.precision, c->job.S, c->job.n0};
-  } else if (field == CWTB_FIELD_CROSS) {
-    if (c->cross_S <= 0 || !c->cross.p) return fail(c, CWTB_ERR_STATE, "no cross spectrum resident");
-    f = FieldRef{c->cross.p, c->cross_prec, c->cross_S, c->cross_n0};
+    f = FieldRef{field, c->W.p, c->job.precision, c->job.S, c->job.n0, 0};
   } else {
-    return fail(c, CWTB_ERR_ARG, "unknown field");
+    const bool coh = field == FIELD_COH;
+    const ResidentSlot &s = coh ? c->coh : c->cross;
+    if (s.S <= 0 || !s.buf.p)
+      return fail(c, CWTB_ERR_STATE, coh ? "no coherence resident" : "no cross spectrum resident");
+    f = FieldRef{field, s.buf.p, s.prec, s.S, s.n0, coh ? coh_angle_offset((size_t)s.S * s.n0) : 0};
   }
 #ifndef CWTB_HOST_EMU
   RT(cudaSetDevice(c->device));
@@ -2963,9 +2975,131 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   return 0;
 }
 
+// the field of a cwtb_field_* call
+static int cx_field_ref(cwtb_ctx *c, int field, FieldRef &f) {
+  if (c && field != CWTB_FIELD_W && field != CWTB_FIELD_CROSS) return fail(c, CWTB_ERR_ARG, "unknown field");
+  return field_ref(c, field, f);
+}
+
+extern "C++" {
+// fn(view) with the kernel view of a resident field (kernels.cuh)
+template <typename Fn>
+static int with_view(const FieldRef &f, int want_phase, Fn &&fn) {
+  if (f.field == FIELD_COH) {
+    const double *w = (const double *)f.p;
+    return fn(CohView{w, w + f.angle, want_phase});
+  }
+  if (f.prec == CWTB_F64) return fn(CxView<double>{(const cx<double> *)f.p});
+  return fn(CxView<float>{(const cx<float> *)f.p});
+}
+
+// Strided sub-grid into out0 / out1: the coherence's WCT / aWCT (nothing asked for: nothing to
+// do), or a complex field as complex128 into out0
+static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int row_step, int64_t col0,
+                      int64_t ncols, int64_t col_step, void *out0, void *out1) {
+  const int S = f.S;
+  const long long n0 = f.n0;
+  const bool coh = f.field == FIELD_COH;
+  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
+    return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
+  if (nrows == 0 || ncols == 0 || (!out0 && !out1)) return 0;
+  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
+      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
+    return fail(c, CWTB_ERR_ARG, "window outside the resident field");
+  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
+    const size_t off = (size_t)row0 * n0, cnt = (size_t)nrows * n0;
+    if (!coh) return field_to_host(c, f.p, f.prec, off, cnt, out0, 1);
+    const double *dW = (const double *)f.p;
+    if (out0) RT(rt_d2h(out0, dW + off, cnt * sizeof(double), c->stream));
+    if (out1) RT(rt_d2h(out1, dW + f.angle + off, cnt * sizeof(double), c->stream));
+    RT(rt_sync(c->stream));
+    return 0;
+  }
+  const size_t m = (size_t)nrows * ncols;
+  int e = ensure(c, c->aux, m * sizeof(double2));
+  if (e) return e;
+  double *o0 = (double *)c->aux.p, *o1 = o0 + m;   // a complex128 output takes both halves
+  e = with_view(f, 0, [&](auto v) {
+    WindowArgs<decltype(v)> a{v, out0 ? o0 : nullptr, out1 ? o1 : nullptr, n0, row0, row_step, col0, col_step, ncols};
+    return launch<WindowBody<decltype(v)>>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a);
+  });
+  if (e) return e;
+  const size_t bytes = m * (coh ? sizeof(double) : sizeof(double2));
+  if (out0) RT(rt_d2h(out0, o0, bytes, c->stream));
+  if (out1) RT(rt_d2h(out1, o1, bytes, c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+// The view's K sums per row over the columns [lo_j, hi_j) (every column where lo / hi is null)
+static int row_stats_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, const int64_t *hi,
+                         const double *thr, int want_phase, double *out) {
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  std::vector<long long> h(3 * (size_t)S);
+  for (int j = 0; j < S; ++j) {
+    h[j] = lo ? lo[j] : 0;
+    h[S + j] = hi ? hi[j] : n0;
+    if (h[j] < 0 || h[S + j] > n0 || h[j] > h[S + j])
+      return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
+  }
+  if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
+  return with_view(f, want_phase, [&](auto v) {
+    using B = RowStatsBody<decltype(v)>;
+    constexpr int K = B::K;
+    const int nchunk = (int)((n0 + B::CHUNK - 1) / B::CHUNK);
+    // aux: [lo S][hi S][thr S][partials S*nchunk*K][sums S*K], 8 bytes each
+    const size_t npart = (size_t)S * nchunk * K;
+    int e = ensure(c, c->aux, (3 * (size_t)S + npart + K * (size_t)S) * sizeof(double));
+    if (e) return e;
+    long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
+    double *dthr = (double *)(dhi + S), *dpart = dthr + S, *dsum = dpart + npart;
+    RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
+    typename B::Args a{v, dlo, dhi, thr ? dthr : nullptr, dpart, n0, nchunk};
+    if ((e = launch<B>(c, (unsigned)nchunk, (unsigned)S, a))) return e;
+    RowSumArgs r{dpart, dsum, S, nchunk};
+    if ((e = launch<RowSumBody<K>>(c, (unsigned)((K * S + NT - 1) / NT), 1, r))) return e;
+    RT(rt_d2h(out, dsum, (size_t)S * K * sizeof(double), c->stream));
+    RT(rt_sync(c->stream));
+    return 0;
+  });
+}
+
+// The view's NA weighted sums per column over the rows with a non-zero weight
+static int scale_avg_run(cwtb_ctx *c, const FieldRef &f, const double *weights, void *out) {
+  if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  // aux: [weights S doubles][selected rows S ints][out NA*n0 doubles, 16-byte aligned]: rows with
+  // a zero weight are not read
+  std::vector<double> w(weights, weights + S);
+  std::vector<int> sel;
+  for (int j = 0; j < S; ++j)
+    if (w[j] != 0.0) sel.push_back(j);
+  const int nsel = (int)sel.size();
+  const size_t head = ((size_t)S + ((size_t)S + 1) / 2 + 1) & ~(size_t)1;
+  w.resize(head);
+  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
+  return with_view(f, 0, [&](auto v) {
+    using B = SelScaleAvgBody<decltype(v)>;
+    const size_t nout = decltype(v)::NA * (size_t)n0;
+    int e = ensure(c, c->aux, (head + nout) * sizeof(double));
+    if (e) return e;
+    double *dw = (double *)c->aux.p, *dout = dw + head;
+    RT(rt_h2d(dw, w.data(), head * sizeof(double), c->stream));
+    typename B::Args a{v, dw, (const int *)(dw + S), nsel, dout, n0};
+    if ((e = launch<B>(c, (unsigned)((n0 + NT - 1) / NT), 1, a))) return e;
+    RT(rt_d2h(out, dout, nout * sizeof(double), c->stream));
+    RT(rt_sync(c->stream));
+    return 0;
+  });
+}
+}  // extern "C++"
+
 int cwtb_field_get(cwtb_ctx *c, int field, int row0, int nrows, void *out) {
   FieldRef f;
-  int e = field_ref(c, field, f);
+  int e = cx_field_ref(c, field, f);
   if (e) return e;
   if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
   if (row0 < 0 || nrows < 0 || row0 > f.S - nrows) return fail(c, CWTB_ERR_ARG, "row range");
@@ -2975,119 +3109,24 @@ int cwtb_field_get(cwtb_ctx *c, int field, int row0, int nrows, void *out) {
 int cwtb_field_window(cwtb_ctx *c, int field, int row0, int nrows, int row_step, int64_t col0,
                       int64_t ncols, int64_t col_step, void *out) {
   FieldRef f;
-  int e = field_ref(c, field, f);
+  int e = cx_field_ref(c, field, f);
   if (e) return e;
-  const int S = f.S;
-  const long long n0 = f.n0;
-  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
-    return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
-  if (nrows == 0 || ncols == 0) return 0;
-  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
-  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
-      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
-    return fail(c, CWTB_ERR_ARG, "window outside the resident field");
-  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0)   // whole rows: the fetch
-    return field_to_host(c, f.p, f.prec, (size_t)row0 * n0, (size_t)nrows * n0, out, 1);
-  const size_t m = (size_t)nrows * ncols;
-  if ((e = ensure(c, c->aux, m * sizeof(double2)))) return e;
-  double2 *o = (double2 *)c->aux.p;
-  const unsigned gx = (unsigned)((ncols + NT - 1) / NT);
-  if (f.prec == CWTB_F64) {
-    CxWindowArgs<double> a{(const double2 *)f.p, o, n0, row0, row_step, col0, col_step, ncols};
-    e = launch<CxWindowBody<double>>(c, gx, (unsigned)nrows, a);
-  } else {
-    CxWindowArgs<float> a{(const float2 *)f.p, o, n0, row0, row_step, col0, col_step, ncols};
-    e = launch<CxWindowBody<float>>(c, gx, (unsigned)nrows, a);
-  }
-  if (e) return e;
-  RT(rt_d2h(out, o, m * sizeof(double2), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  if (!out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, out, nullptr);
 }
-
-extern "C++" {
-template <typename T>
-static int field_row_stats_run(cwtb_ctx *c, const FieldRef &f, const long long *dlo, const long long *dhi,
-                               const double *dthr, double *dpart, double *dsum, int nchunk) {
-  CxRowStatsArgs<T> a{(const cx<T> *)f.p, dlo, dhi, dthr, dpart, f.n0, nchunk};
-  int e = launch<CxRowStatsBody<T>>(c, (unsigned)nchunk, (unsigned)f.S, a);
-  if (e) return e;
-  RowSumArgs r{dpart, dsum, f.S, nchunk};
-  return launch<RowSumBody<5>>(c, (unsigned)((5 * f.S + NT - 1) / NT), 1, r);
-}
-}  // extern "C++"
 
 int cwtb_field_row_stats(cwtb_ctx *c, int field, const int64_t *lo, const int64_t *hi, const double *thr,
                          double *out) {
   FieldRef f;
-  int e = field_ref(c, field, f);
-  if (e) return e;
-  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
-  const int S = f.S;
-  const long long n0 = f.n0;
-  const long long chunk = f.prec == CWTB_F64 ? CxRowStatsBody<double>::CHUNK : CxRowStatsBody<float>::CHUNK;
-  const int nchunk = (int)((n0 + chunk - 1) / chunk);
-  // aux: [lo S][hi S][thr S][partials S*nchunk*5][sums S*5], 8 bytes each
-  std::vector<long long> h(3 * (size_t)S);
-  for (int j = 0; j < S; ++j) {
-    h[j] = lo ? lo[j] : 0;
-    h[S + j] = hi ? hi[j] : n0;
-    if (h[j] < 0 || h[S + j] > n0 || h[j] > h[S + j])
-      return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
-  }
-  if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
-  const size_t npart = (size_t)S * nchunk * 5;
-  if ((e = ensure(c, c->aux, (3 * (size_t)S + npart + 5 * (size_t)S) * sizeof(double)))) return e;
-  long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
-  double *dthr = (double *)(dhi + S), *dpart = dthr + S, *dsum = dpart + npart;
-  RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
-  e = f.prec == CWTB_F64
-          ? field_row_stats_run<double>(c, f, dlo, dhi, thr ? dthr : nullptr, dpart, dsum, nchunk)
-          : field_row_stats_run<float>(c, f, dlo, dhi, thr ? dthr : nullptr, dpart, dsum, nchunk);
-  if (e) return e;
-  RT(rt_d2h(out, dsum, (size_t)S * 5 * sizeof(double), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  int e = cx_field_ref(c, field, f);
+  return e ? e : row_stats_run(c, f, lo, hi, thr, 0, out);
 }
 
 int cwtb_cross_scale_avg(cwtb_ctx *c, const double *weights, void *out) {
   FieldRef f;
   int e = field_ref(c, CWTB_FIELD_CROSS, f);
-  if (e) return e;
-  if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
-  const int S = f.S;
-  const long long n0 = f.n0;
-  // aux: [weights S doubles][selected rows S ints][out n0 complex128]: rows with a zero weight are
-  // not read
-  std::vector<double> w(weights, weights + S);
-  std::vector<int> sel;
-  for (int j = 0; j < S; ++j)
-    if (w[j] != 0.0) sel.push_back(j);
-  const int nsel = (int)sel.size();
-  const size_t head = ((size_t)S + ((size_t)S + 1) / 2 + 1) & ~(size_t)1;   // 16-byte aligned output
-  w.resize(head);
-  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
-  if ((e = ensure(c, c->aux, (head + 2 * (size_t)n0) * sizeof(double)))) return e;
-  double *dw = (double *)c->aux.p;
-  double2 *dout = (double2 *)(dw + head);
-  RT(rt_h2d(dw, w.data(), head * sizeof(double), c->stream));
-  const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
-  if (f.prec == CWTB_F64) {
-    CrossScaleAvgArgs<double> a{(const double2 *)f.p, dw, (const int *)(dw + S), nsel, dout, n0};
-    e = launch<CrossScaleAvgBody<double>>(c, gx, 1, a);
-  } else {
-    CrossScaleAvgArgs<float> a{(const float2 *)f.p, dw, (const int *)(dw + S), nsel, dout, n0};
-    e = launch<CrossScaleAvgBody<float>>(c, gx, 1, a);
-  }
-  if (e) return e;
-  RT(rt_d2h(out, dout, (size_t)n0 * sizeof(double2), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  return e ? e : scale_avg_run(c, f, weights, out);
 }
-
-// WCT and aWCT of a coherence share one device buffer; aWCT starts on a 256-byte boundary, so that
-// a flat index has the same alignment in both fields (the 16-byte loads of CohRowStatsBody)
-static size_t coh_angle_offset(size_t cnt) { return (cnt + 31) & ~(size_t)31; }
 
 // Coherence of two series in the engine type T into the device buffer `dst` (WCT, then aWCT at
 // coh_angle_offset), grown as needed.  `angle_host`: host destination of an early angle copy (see
@@ -3156,136 +3195,37 @@ int cwtb_wct_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n
                       const double *scales, int n_scales, int family, double param, int boxcar_len) {
   (void)dj;
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
-  ++c->coh_serial;   // before the buffer is written: a call that fails part-way invalidates it too
-  c->coh_S = 0;
-  c->coh_n0 = 0;
-  int e = wct_dispatch(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, c->coh, true, nullptr);
+  slot_begin(c->coh);
+  int e = wct_dispatch(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, c->coh.buf, true, nullptr);
   if (e) return e;
   RT(rt_sync(c->stream));
-  c->coh_S = n_scales;
-  c->coh_n0 = n0;
+  c->coh.S = n_scales;
+  c->coh.n0 = n0;
+  c->coh.prec = CWTB_F64;
   return 0;
 }
 
-int64_t cwtb_coherence_serial(cwtb_ctx *c) { return c ? c->coh_serial : -1; }
-
-int cwtb_coherence_release(cwtb_ctx *c) {
-  if (!c) return CWTB_ERR_ARG;
-  ++c->coh_serial;
-  c->coh_S = 0;
-  c->coh_n0 = 0;
-  if (c->coh.p) {
-#ifndef CWTB_HOST_EMU
-    RT(cudaSetDevice(c->device));
-#endif
-    RT(rt_sync(c->stream));
-    rt_free(c->coh.p);
-    c->coh.p = nullptr;
-    c->coh.bytes = 0;
-  }
-  return 0;
-}
-
-static int coh_ready(cwtb_ctx *c) {
-  if (!c) return CWTB_ERR_ARG;
-  if (c->coh_S <= 0 || !c->coh.p) return fail(c, CWTB_ERR_STATE, "no coherence resident");
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
-  return 0;
-}
+int64_t cwtb_coherence_serial(cwtb_ctx *c) { return c ? c->coh.serial : -1; }
+int cwtb_coherence_release(cwtb_ctx *c) { return c ? slot_release(c, c->coh) : CWTB_ERR_ARG; }
 
 int cwtb_coherence_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
                           int64_t col_step, double *WCT_out, double *aWCT_out) {
-  int e = coh_ready(c);
-  if (e) return e;
-  const int S = c->coh_S;
-  const long long n0 = c->coh_n0;
-  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
-    return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
-  if (nrows == 0 || ncols == 0 || (!WCT_out && !aWCT_out)) return 0;
-  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
-      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
-    return fail(c, CWTB_ERR_ARG, "window outside the resident coherence");
-  const size_t cnt = (size_t)S * n0;
-  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
-  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
-    const size_t off = (size_t)row0 * n0, bytes = (size_t)nrows * n0 * sizeof(double);
-    if (WCT_out) RT(rt_d2h(WCT_out, dW + off, bytes, c->stream));
-    if (aWCT_out) RT(rt_d2h(aWCT_out, dA + off, bytes, c->stream));
-    RT(rt_sync(c->stream));
-    return 0;
-  }
-  const size_t m = (size_t)nrows * ncols;
-  if ((e = ensure(c, c->aux, 2 * m * sizeof(double)))) return e;
-  double *oW = (double *)c->aux.p, *oA = oW + m;
-  CohWindowArgs a{dW, dA, WCT_out ? oW : nullptr, aWCT_out ? oA : nullptr, n0, row0, row_step, col0, col_step, ncols};
-  if ((e = launch<CohWindowBody>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a))) return e;
-  if (WCT_out) RT(rt_d2h(WCT_out, oW, m * sizeof(double), c->stream));
-  if (aWCT_out) RT(rt_d2h(aWCT_out, oA, m * sizeof(double), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  return e ? e : window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, WCT_out, aWCT_out);
 }
 
 int cwtb_coherence_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, const double *thr,
                              int want_phase, double *out) {
-  int e = coh_ready(c);
-  if (e) return e;
-  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
-  const int S = c->coh_S;
-  const long long n0 = c->coh_n0;
-  using B = CohRowStatsBody;
-  const int nchunk = (int)((n0 + B::CHUNK - 1) / B::CHUNK);
-  // aux: [lo S][hi S][thr S][partials S*nchunk*4][sums S*4], 8 bytes each
-  std::vector<long long> h(3 * (size_t)S);
-  for (int j = 0; j < S; ++j) {
-    h[j] = lo ? lo[j] : 0;
-    h[S + j] = hi ? hi[j] : n0;
-    if (h[j] < 0 || h[S + j] > n0 || h[j] > h[S + j])
-      return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
-  }
-  if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
-  const size_t npart = (size_t)S * nchunk * 4;
-  if ((e = ensure(c, c->aux, (3 * (size_t)S + npart + 4 * (size_t)S) * sizeof(double)))) return e;
-  long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
-  double *dthr = (double *)(dhi + S), *dpart = dthr + S, *dsum = dpart + npart;
-  RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
-  const size_t cnt = (size_t)S * n0;
-  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
-  CohRowStatsArgs a{dW, dA, dlo, dhi, thr ? dthr : nullptr, dpart, n0, nchunk, want_phase != 0};
-  if ((e = launch<B>(c, (unsigned)nchunk, (unsigned)S, a))) return e;
-  RowSumArgs r{dpart, dsum, S, nchunk};
-  if ((e = launch<RowSumBody<4>>(c, (unsigned)((4 * S + NT - 1) / NT), 1, r))) return e;
-  RT(rt_d2h(out, dsum, (size_t)S * 4 * sizeof(double), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  return e ? e : row_stats_run(c, f, lo, hi, thr, want_phase != 0, out);
 }
 
 int cwtb_coherence_scale_avg(cwtb_ctx *c, const double *weights, double *out) {
-  int e = coh_ready(c);
-  if (e) return e;
-  if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
-  const int S = c->coh_S;
-  const long long n0 = c->coh_n0;
-  // aux: [weights S doubles][selected rows S ints][out 3*n0]: rows with a zero weight are not read
-  std::vector<double> w(weights, weights + S);
-  std::vector<int> sel;
-  for (int j = 0; j < S; ++j)
-    if (w[j] != 0.0) sel.push_back(j);
-  const int nsel = (int)sel.size();
-  const size_t head = (size_t)S + ((size_t)S + 1) / 2;
-  w.resize(head);
-  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
-  if ((e = ensure(c, c->aux, (head + 3 * (size_t)n0) * sizeof(double)))) return e;
-  double *dw = (double *)c->aux.p, *dout = dw + head;
-  RT(rt_h2d(dw, w.data(), head * sizeof(double), c->stream));
-  const size_t cnt = (size_t)S * n0;
-  const double *dW = (const double *)c->coh.p, *dA = dW + coh_angle_offset(cnt);
-  CohScaleAvgArgs a{dW, dA, dw, (const int *)(dw + S), nsel, dout, n0};
-  if ((e = launch<CohScaleAvgBody>(c, (unsigned)((n0 + NT - 1) / NT), 1, a))) return e;
-  RT(rt_d2h(out, dout, 3 * (size_t)n0 * sizeof(double), c->stream));
-  RT(rt_sync(c->stream));
-  return 0;
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  return e ? e : scale_avg_run(c, f, weights, out);
 }
 
 int cwtb_set_coherence_precision(cwtb_ctx *c, int precision) {

@@ -1908,188 +1908,66 @@ template <typename T> struct ScaleAvgBody {
   }
 };
 
-// ---- Bodies: reductions of the resident coherence (cwtb_wct_resident) ----------------------
-// WCT and aWCT are two [rows][n] double fields whose flat indices have the same alignment.
+// ---- Bodies: reductions of a resident field (cwtb_coherence_*, cwtb_field_*) ---------------
+// One template per operation, over a view that says how the field is read and what a point adds:
+//   CohView     the resident coherence (cwtb_wct_resident): WCT and aWCT, two [rows][n] double
+//               fields whose flat indices have the same alignment
+//   CxView<T>   a [rows][n] complex field of cx<T> (W or the cross spectrum); every sum is formed
+//               in double, after widening
+// A view supplies, for RowStatsBody: K sums per row, E elements per 16-byte vector, VPT 16-byte
+// vectors per thread per chunk, load (vector q), add (element e of a vector) and add_at (element
+// p, at a chunk's odd edge); for SelScaleAvgBody: NA sums per column, Pt, point, acc and put; for
+// WindowBody: copy.
 
-// Per-row sums over the columns [lo_j, hi_j) where thr is null or WCT > thr_j (false for a NaN
-// threshold): [count, sum WCT, sum cos aWCT, sum sin aWCT].  CTA (bx, j) covers the fixed chunk
-// [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j's range with 16-byte streaming loads, reduces
-// its threads' sums in a fixed order and writes its partial; RowSumBody<4> adds the partials of a
-// row in chunk order.  No atomics: repeated calls are bit-identical.
-struct CohRowStatsArgs {
+// Row stats [count, sum WCT, sum cos aWCT, sum sin aWCT] of the points with WCT > thr_j; aWCT is
+// not read when want_phase == 0.  Scale average [sum w_j WCT, sum w_j cos aWCT, sum w_j sin aWCT]
+// as three planes of n.  Window: WCT to o0, aWCT to o1, either may be null.
+struct CohView {
   const double *WCT, *aWCT;
-  const long long *lo, *hi;   // per row
-  const double *thr;          // per row, or null
-  double *part;               // [rows][nchunk][4]
-  long long n;
-  int nchunk, want_phase;     // aWCT is not read when want_phase == 0
-};
-struct CohRowStatsBody {
-  using Args = CohRowStatsArgs;
-  static constexpr int NTB = 256, NPHASE = 3;
-  static constexpr int U = 4;                                  // 16-byte loads in flight per field
-  static constexpr long long CHUNK = 2LL * 16 * NTB;           // 16 pairs of columns per thread
-  static constexpr size_t SMEM = (size_t)4 * (NTB + 32) * sizeof(double);
-  HD static void add(double (&s)[4], double w, double ang, const Args &a, bool has_thr, double t) {
+  int want_phase;
+  static constexpr int K = 4, E = 2, VPT = 16, NA = 3;   // VPT: two loads each, one per field
+  struct Vec { double2 w, g; };
+  HD Vec load(size_t q) const {
+    Vec v{ld_stream((const double2 *)WCT + q), make_double2(0, 0)};
+    if (want_phase) v.g = ld_stream((const double2 *)aWCT + q);
+    return v;
+  }
+  HD void add1(double (&s)[K], double w, double ang, bool has_thr, double t) const {
     if (has_thr && !(w > t)) return;
     s[0] += 1.0;
     s[1] += w;
-    if (a.want_phase) {
+    if (want_phase) {
       double sn, cs;
       sincos_hd(ang, &sn, &cs);
       s[2] += cs;
       s[3] += sn;
     }
   }
-  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
-    double *sm = (double *)smraw;          // [4][NTB] thread sums, then [4][32] lane sums
-    if constexpr (PH == 0) {
-      double s[4] = {0, 0, 0, 0};
-      const long long lo = a.lo[by], hi = a.hi[by];
-      const long long c0 = lo + (long long)bx * CHUNK;
-      if (c0 < hi) {
-        const long long c1 = c0 + CHUNK < hi ? c0 + CHUNK : hi;
-        const bool has_thr = a.thr != nullptr;
-        const double t = has_thr ? a.thr[by] : 0.0;
-        const size_t p0 = (size_t)by * a.n + c0, p1 = (size_t)by * a.n + c1;
-        const size_t v0 = p0 + (p0 & 1), v1 = p1 - (p1 & 1);   // [v0, v1): whole 16-byte pairs
-        if (tid == 0 && (p0 & 1)) add(s, a.WCT[p0], a.want_phase ? a.aWCT[p0] : 0.0, a, has_thr, t);
-        if (tid == 1 && (p1 & 1) && p1 - 1 >= v0)
-          add(s, a.WCT[p1 - 1], a.want_phase ? a.aWCT[p1 - 1] : 0.0, a, has_thr, t);
-        for (size_t q0 = v0 + 2 * (size_t)tid; q0 < v1; q0 += (size_t)2 * NTB * U) {
-          double2 w[U], g[U];
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            const size_t q = q0 + (size_t)2 * NTB * u;
-            w[u] = make_double2(0, 0);
-            g[u] = w[u];
-            if (q < v1) {
-              w[u] = ld_stream((const double2 *)(a.WCT + q));
-              if (a.want_phase) g[u] = ld_stream((const double2 *)(a.aWCT + q));
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            if (q0 + (size_t)2 * NTB * u < v1) {
-              add(s, w[u].x, g[u].x, a, has_thr, t);
-              add(s, w[u].y, g[u].y, a, has_thr, t);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) sm[k * NTB + tid] = s[k];
-    } else if constexpr (PH == 1) {
-      if (tid < 4 * 32) {
-        const int k = tid >> 5, l = tid & 31;
-        double v = 0;
-        for (int i = l; i < NTB; i += 32) v += sm[k * NTB + i];
-        sm[4 * NTB + tid] = v;
-      }
-    } else {
-      if (tid < 4) {
-        double v = 0;
-        for (int l = 0; l < 32; ++l) v += sm[4 * NTB + tid * 32 + l];
-        a.part[((size_t)by * a.nchunk + bx) * 4 + tid] = v;
-      }
-    }
+  HD void add(double (&s)[K], const Vec &v, int e, bool has_thr, double t) const {
+    add1(s, e ? v.w.y : v.w.x, e ? v.g.y : v.g.x, has_thr, t);
+  }
+  HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
+    add1(s, WCT[p], want_phase ? aWCT[p] : 0.0, has_thr, t);
+  }
+  struct Pt { double w, a; };
+  HD Pt point(size_t p) const { return Pt{ld_stream(&WCT[p]), ld_stream(&aWCT[p])}; }
+  HD static void acc(double (&s)[NA], double wj, const Pt &v) {
+    double sn, cs;
+    sincos_hd(v.a, &sn, &cs);
+    s[0] += wj * v.w;
+    s[1] += wj * cs;
+    s[2] += wj * sn;
+  }
+  HD static void put(double *out, long long n, long long N, const double (&s)[NA]) {
+    st_stream(&out[n], s[0]);
+    st_stream(&out[N + n], s[1]);
+    st_stream(&out[2 * N + n], s[2]);
+  }
+  HD void copy(size_t src, double *o0, double *o1, size_t dst) const {
+    if (o0) o0[dst] = WCT[src];
+    if (o1) o1[dst] = aWCT[src];
   }
 };
-
-// out[j][k] = sum over chunks b (in order) of part[j][b][k], k < K (the K sums per row of
-// CohRowStatsBody and CxRowStatsBody)
-struct RowSumArgs { const double *part; double *out; int rows, nchunk; };
-template <int K> struct RowSumBody {
-  using Args = RowSumArgs;
-  static constexpr int NPHASE = 1;
-  static constexpr size_t SMEM = 0;
-  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
-    const int i = bx * NT + tid;
-    if (i >= K * a.rows) return;
-    const double *p = a.part + (size_t)(i / K) * a.nchunk * K + (i % K);
-    double v = 0;
-    for (int b = 0; b < a.nchunk; ++b) v += p[(size_t)b * K];
-    a.out[i] = v;
-  }
-};
-
-// Scale average of the two fields over the selected rows (the selected-rows pattern of
-// ScaleAvgBody): out[0][n] = sum_j w_j WCT[j,n], out[1][n] = sum_j w_j cos aWCT[j,n],
-// out[2][n] = sum_j w_j sin aWCT[j,n].  One thread per column adds the rows in order: no atomics.
-struct CohScaleAvgArgs {
-  const double *WCT, *aWCT;
-  const double *w;     // per row
-  const int *sel;      // rows with a non-zero weight, ascending (device)
-  int nsel;
-  double *out;         // [3][n]
-  long long n;
-};
-struct CohScaleAvgBody {
-  using Args = CohScaleAvgArgs;
-  static constexpr int NPHASE = 1;
-  static constexpr size_t SMEM = 0;
-  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
-    const long long n = (long long)bx * NT + tid;
-    if (n >= a.n) return;
-    double sw = 0, sc = 0, ss = 0;
-    int i = 0;
-    for (; i + 4 <= a.nsel; i += 4) {
-      double wv[4], av[4], wj[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int j = a.sel[i + u];
-        wj[u] = a.w[j];
-        wv[u] = ld_stream(&a.WCT[(size_t)j * a.n + n]);
-        av[u] = ld_stream(&a.aWCT[(size_t)j * a.n + n]);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        double sn, cs;
-        sincos_hd(av[u], &sn, &cs);
-        sw += wj[u] * wv[u];
-        sc += wj[u] * cs;
-        ss += wj[u] * sn;
-      }
-    }
-    for (; i < a.nsel; ++i) {
-      const int j = a.sel[i];
-      double sn, cs;
-      sincos_hd(ld_stream(&a.aWCT[(size_t)j * a.n + n]), &sn, &cs);
-      sw += a.w[j] * ld_stream(&a.WCT[(size_t)j * a.n + n]);
-      sc += a.w[j] * cs;
-      ss += a.w[j] * sn;
-    }
-    st_stream(&a.out[n], sw);
-    st_stream(&a.out[a.n + n], sc);
-    st_stream(&a.out[2 * a.n + n], ss);
-  }
-};
-
-// Strided sub-grid: out[r][c] = field[row0 + r row_step][col0 + c col_step] of either field
-// (outputs may be null).  Grid: (ceil(ncols / NT), nrows).
-struct CohWindowArgs {
-  const double *WCT, *aWCT;
-  double *oW, *oA;     // [nrows][ncols], or null
-  long long n;
-  int row0, row_step;
-  long long col0, col_step, ncols;
-};
-struct CohWindowBody {
-  using Args = CohWindowArgs;
-  static constexpr int NPHASE = 1;
-  static constexpr size_t SMEM = 0;
-  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
-    const long long c = (long long)bx * NT + tid;
-    if (c >= a.ncols) return;
-    const size_t src = (size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + c * a.col_step;
-    const size_t dst = (size_t)by * a.ncols + c;
-    if (a.oW) a.oW[dst] = a.WCT[src];
-    if (a.oA) a.oA[dst] = a.aWCT[src];
-  }
-};
-
-// ---- Bodies: reductions of a resident complex field (cwtb_field_*: W or the cross spectrum) ----
-// F is a [rows][n] field of cx<T>.  Every sum is formed in double, after widening.
 
 // 16 bytes of a complex field: one double2, or two float2
 template <typename T> struct CxVec16;
@@ -2106,28 +1984,16 @@ template <> struct CxVec16<float> {
   HD static double im(const V &v, int e) { return (double)(e ? v.w : v.y); }
 };
 
-// Per-row sums over the columns [lo_j, hi_j) where thr is null or re^2 + im^2 > thr_j (false for a
-// NaN threshold): [count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F], with cos = re / |F|,
-// sin = im / |F| and a zero coefficient counted as phase 0 (np.angle(0) == 0).  The partition is
-// CohRowStatsBody's: CTA (bx, j) covers the fixed chunk [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK)
-// of row j's range with 16-byte streaming loads, reduces its threads' sums in a fixed order and
-// writes its partial; RowSumBody<5> adds the partials of a row in chunk order.  No atomics.
-template <typename T> struct CxRowStatsArgs {
+// Row stats [count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F] of the points with
+// re^2 + im^2 > thr_j, with cos = re / |F|, sin = im / |F| and a zero coefficient counted as phase
+// 0 (np.angle(0) == 0).  Scale average sum_j w_j F[j,n] as complex128.  Window: complex128 to o0.
+template <typename T> struct CxView {
   const cx<T> *F;
-  const long long *lo, *hi;   // per row
-  const double *thr;          // per row, or null
-  double *part;               // [rows][nchunk][5]
-  long long n;
-  int nchunk;
-};
-template <typename T> struct CxRowStatsBody {
-  using Args = CxRowStatsArgs<T>;
-  using Vec = CxVec16<T>;
-  static constexpr int NTB = 256, NPHASE = 3, K = 5;
-  static constexpr int U = 4;                                          // 16-byte loads in flight
-  static constexpr long long CHUNK = (long long)Vec::E * 32 * NTB;    // 32 loads per thread
-  static constexpr size_t SMEM = (size_t)K * (NTB + 32) * sizeof(double);
-  HD static void add(double (&s)[K], double re, double im, bool has_thr, double t) {
+  using V16 = CxVec16<T>;
+  using Vec = typename V16::V;
+  static constexpr int K = 5, E = V16::E, VPT = 32, NA = 2;
+  HD Vec load(size_t q) const { return ld_stream((const Vec *)F + q); }
+  HD static void add1(double (&s)[K], double re, double im, bool has_thr, double t) {
     const double p = norm2_rn(re, im);
     if (has_thr && !(p > t)) return;
     const double m = sqrt(p);
@@ -2141,36 +2007,75 @@ template <typename T> struct CxRowStatsBody {
       s[3] += 1.0;
     }
   }
+  HD void add(double (&s)[K], const Vec &v, int e, bool has_thr, double t) const {
+    add1(s, V16::re(v, e), V16::im(v, e), has_thr, t);
+  }
+  HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
+    add1(s, F[p].x, F[p].y, has_thr, t);
+  }
+  using Pt = cx<T>;
+  HD Pt point(size_t p) const { return ld_stream(&F[p]); }
+  HD static void acc(double (&s)[NA], double wj, const Pt &v) {
+    s[0] += wj * (double)v.x;
+    s[1] += wj * (double)v.y;
+  }
+  HD static void put(double *out, long long n, long long, const double (&s)[NA]) {
+    st_stream((double2 *)out + n, make_double2(s[0], s[1]));
+  }
+  HD void copy(size_t src, double *o0, double *, size_t dst) const {
+    const cx<T> v = F[src];
+    ((double2 *)o0)[dst] = make_double2((double)v.x, (double)v.y);
+  }
+};
+
+// Per-row sums of a view over the columns [lo_j, hi_j) where thr is null or the view's point
+// passes thr_j (false for a NaN threshold).  CTA (bx, j) covers the fixed chunk
+// [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j's range with 16-byte streaming loads, reduces
+// its threads' sums in a fixed order and writes its partial; RowSumBody<K> adds the partials of a
+// row in chunk order.  No atomics: repeated calls are bit-identical.
+template <typename View> struct RowStatsArgs {
+  View f;
+  const long long *lo, *hi;   // per row
+  const double *thr;          // per row, or null
+  double *part;               // [rows][nchunk][K]
+  long long n;
+  int nchunk;
+};
+template <typename View> struct RowStatsBody {
+  using Args = RowStatsArgs<View>;
+  static constexpr int NTB = 256, NPHASE = 3, K = View::K;
+  static constexpr int U = 4;                                              // 16-byte loads in flight
+  static constexpr long long CHUNK = (long long)View::E * View::VPT * NTB;
+  static constexpr size_t SMEM = (size_t)K * (NTB + 32) * sizeof(double);
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
     double *sm = (double *)smraw;          // [K][NTB] thread sums, then [K][32] lane sums
     if constexpr (PH == 0) {
-      double s[K] = {0, 0, 0, 0, 0};
+      double s[K] = {};
       const long long lo = a.lo[by], hi = a.hi[by];
       const long long c0 = lo + (long long)bx * CHUNK;
       if (c0 < hi) {
         const long long c1 = c0 + CHUNK < hi ? c0 + CHUNK : hi;
         const bool has_thr = a.thr != nullptr;
         const double t = has_thr ? a.thr[by] : 0.0;
-        constexpr size_t E = Vec::E;
+        constexpr size_t E = View::E;
         const size_t p0 = (size_t)by * a.n + c0, p1 = (size_t)by * a.n + c1;
         const size_t v0 = (p0 + E - 1) / E, v1 = p1 / E;   // [v0, v1): whole 16-byte vectors
         if constexpr (E == 2) {                             // an odd element at either end
-          if (tid == 0 && (p0 & 1)) add(s, a.F[p0].x, a.F[p0].y, has_thr, t);
-          if (tid == 1 && (p1 & 1) && p1 - 1 >= E * v0) add(s, a.F[p1 - 1].x, a.F[p1 - 1].y, has_thr, t);
+          if (tid == 0 && (p0 & 1)) a.f.add_at(s, p0, has_thr, t);
+          if (tid == 1 && (p1 & 1) && p1 - 1 >= E * v0) a.f.add_at(s, p1 - 1, has_thr, t);
         }
-        const typename Vec::V *F16 = (const typename Vec::V *)a.F;
         for (size_t q0 = v0 + (size_t)tid; q0 < v1; q0 += (size_t)NTB * U) {
-          typename Vec::V w[U] = {};
+          typename View::Vec w[U] = {};
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const size_t q = q0 + (size_t)NTB * u;
-            if (q < v1) w[u] = ld_stream(F16 + q);
+            if (q < v1) w[u] = a.f.load(q);
           }
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             if (q0 + (size_t)NTB * u < v1) {
 #pragma unroll
-              for (int e = 0; e < (int)E; ++e) add(s, Vec::re(w[u], e), Vec::im(w[u], e), has_thr, t);
+              for (int e = 0; e < (int)E; ++e) a.f.add(s, w[u], e, has_thr, t);
             }
           }
         }
@@ -2194,69 +2099,80 @@ template <typename T> struct CxRowStatsBody {
   }
 };
 
-// out[n] = sum_j w_j F[j,n] (complex128) over the selected rows, in order: one thread per column
-// (the selected-rows pattern of CohScaleAvgBody), no atomics.
-template <typename T> struct CrossScaleAvgArgs {
-  const cx<T> *F;
+// out[j][k] = sum over chunks b (in order) of part[j][b][k], k < K (the K sums per row of
+// RowStatsBody)
+struct RowSumArgs { const double *part; double *out; int rows, nchunk; };
+template <int K> struct RowSumBody {
+  using Args = RowSumArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const int i = bx * NT + tid;
+    if (i >= K * a.rows) return;
+    const double *p = a.part + (size_t)(i / K) * a.nchunk * K + (i % K);
+    double v = 0;
+    for (int b = 0; b < a.nchunk; ++b) v += p[(size_t)b * K];
+    a.out[i] = v;
+  }
+};
+
+// The view's NA weighted sums over the selected rows (the selected-rows pattern of ScaleAvgBody),
+// four rows at a time: one thread per column adds the rows in order, no atomics.
+template <typename View> struct SelScaleAvgArgs {
+  View f;
   const double *w;     // per row
   const int *sel;      // rows with a non-zero weight, ascending (device)
   int nsel;
-  double2 *out;        // [n]
+  double *out;         // NA doubles per column, laid out by View::put
   long long n;
 };
-template <typename T> struct CrossScaleAvgBody {
-  using Args = CrossScaleAvgArgs<T>;
+template <typename View> struct SelScaleAvgBody {
+  using Args = SelScaleAvgArgs<View>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
     const long long n = (long long)bx * NT + tid;
     if (n >= a.n) return;
-    double sr = 0, si = 0;
+    double s[View::NA] = {};
     int i = 0;
     for (; i + 4 <= a.nsel; i += 4) {
-      cx<T> v[4];
+      typename View::Pt v[4];
       double wj[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int j = a.sel[i + u];
         wj[u] = a.w[j];
-        v[u] = ld_stream(&a.F[(size_t)j * a.n + n]);
+        v[u] = a.f.point((size_t)j * a.n + n);
       }
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        sr += wj[u] * (double)v[u].x;
-        si += wj[u] * (double)v[u].y;
-      }
+      for (int u = 0; u < 4; ++u) View::acc(s, wj[u], v[u]);
     }
     for (; i < a.nsel; ++i) {
       const int j = a.sel[i];
-      const cx<T> v = ld_stream(&a.F[(size_t)j * a.n + n]);
-      sr += a.w[j] * (double)v.x;
-      si += a.w[j] * (double)v.y;
+      View::acc(s, a.w[j], a.f.point((size_t)j * a.n + n));
     }
-    st_stream(&a.out[n], make_double2(sr, si));
+    View::put(a.out, n, a.n, s);
   }
 };
 
-// Strided sub-grid as complex128: out[r][c] = F[row0 + r row_step][col0 + c col_step].
-// Grid: (ceil(ncols / NT), nrows).
-template <typename T> struct CxWindowArgs {
-  const cx<T> *F;
-  double2 *out;        // [nrows][ncols]
+// Strided sub-grid: out[r][c] = field[row0 + r row_step][col0 + c col_step], written by the
+// view's copy.  Grid: (ceil(ncols / NT), nrows).
+template <typename View> struct WindowArgs {
+  View f;
+  double *o0, *o1;     // [nrows][ncols] outputs (see the view)
   long long n;
   int row0, row_step;
   long long col0, col_step, ncols;
 };
-template <typename T> struct CxWindowBody {
-  using Args = CxWindowArgs<T>;
+template <typename View> struct WindowBody {
+  using Args = WindowArgs<View>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
     const long long c = (long long)bx * NT + tid;
     if (c >= a.ncols) return;
     const size_t src = (size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + c * a.col_step;
-    const cx<T> v = a.F[src];
-    a.out[(size_t)by * a.ncols + c] = make_double2((double)v.x, (double)v.y);
+    a.f.copy(src, a.o0, a.o1, (size_t)by * a.ncols + c);
   }
 };
 

@@ -60,44 +60,28 @@ def _live(method):
     return wrapper
 
 
-class ResidentTransform(object):
-    """W[S, n0] of one `cwt_resident` call, resident on the device."""
+class _Resident(object):
+    """What the handles of one resident [S, n0] product share.  A subclass names its frequency
+    attribute (`_FREQ`), the engine method that returns its product's serial (`_SERIAL`) and the
+    message once that serial has moved on (`_GONE`)."""
 
-    def __init__(self, engine, wavelet, n0, dt, dj, sj, freqs, precision, serial):
+    def __init__(self, engine, wavelet, n0, dt, dj, sj, precision, serial):
         self.engine = engine
         self.wavelet = wavelet
         self.n0 = int(n0)
         self.dt = float(dt)
         self.dj = dj
         self.scales = sj
-        self.freqs = freqs
         self.precision = precision
         self._serial = serial
-        self.npad = fft_kwargs(range(self.n0))['n']       # transform length (helpers.py:15-30)
         self._coi = None
-        self._fftfreqs = None
 
-    # O(n0) host arrays of the `cwt` return tuple, built on first use
+    # O(n0) host array of the `cwt` return tuple, built on first use
     @property
     def coi(self):
         if self._coi is None:
-            n0 = self.n0
-            coi = (n0 / 2 - np.abs(np.arange(0, n0) - (n0 - 1) / 2))
-            self._coi = self.wavelet.flambda() * self.wavelet.coi() * self.dt * coi   # wavelet.py:118-120
+            self._coi = _coi(self.wavelet, self.dt, self.n0)
         return self._coi
-
-    @property
-    def fftfreqs(self):
-        if self._fftfreqs is None:
-            npad = self.npad
-            self._fftfreqs = (2 * np.pi * fft.fftfreq(npad, self.dt))[1:npad // 2] / (2 * np.pi)
-        return self._fftfreqs
-
-    # -- bookkeeping ---------------------------------------------------------------------
-    def _check_live(self):
-        if self.engine.job_serial() != self._serial:
-            raise _engine.EngineError("this transform is no longer resident: another transform "
-                                      "has run on the same engine")
 
     @property
     def shape(self):
@@ -105,7 +89,61 @@ class ResidentTransform(object):
 
     @property
     def period(self):
-        return 1.0 / np.asarray(self.freqs)
+        return 1.0 / np.asarray(getattr(self, self._FREQ))
+
+    def coi_ranges(self):
+        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
+        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
+
+    def _check_live(self):
+        if getattr(self.engine, self._SERIAL)() != self._serial:
+            raise _engine.EngineError(self._GONE)
+
+    def _band(self, period_min, period_max):
+        """The scales with period_min <= period < period_max."""
+        per = self.period
+        return (per >= period_min) & (per < period_max)
+
+    def _band_weights(self, period_min, period_max, factor=1.0):
+        """(band, factor * dj * dt / Cdelta / s_j on the band and 0 elsewhere): the weights of
+        TC98 eq. 24 (simple_sample.py:87-91)."""
+        if self.wavelet.cdelta == -1:
+            raise ValueError('Cdelta not defined for this wavelet')
+        sel = self._band(period_min, period_max)
+        w = np.where(sel, 1.0 / np.asarray(self.scales, dtype=float), 0.0)
+        return sel, w * (factor * self.dj * self.dt / self.wavelet.cdelta)
+
+
+class _ResidentSlot(_Resident):
+    """A product in a device buffer of its own, freed by the engine method `_RELEASE`."""
+
+    def release(self):
+        """Free the device buffer (16 bytes per scale and time point for a coherence, 16 or 8
+        for a cross spectrum).  The handle is invalid afterwards; releasing an invalid handle
+        does nothing."""
+        with self.engine.lock:
+            if getattr(self.engine, self._SERIAL)() == self._serial:
+                getattr(self.engine, self._RELEASE)()
+
+
+class ResidentTransform(_Resident):
+    """W[S, n0] of one `cwt_resident` call, resident on the device."""
+
+    _FREQ, _SERIAL = 'freqs', 'job_serial'
+    _GONE = "this transform is no longer resident: another transform has run on the same engine"
+
+    def __init__(self, engine, wavelet, n0, dt, dj, sj, freqs, precision, serial):
+        super(ResidentTransform, self).__init__(engine, wavelet, n0, dt, dj, sj, precision, serial)
+        self.freqs = freqs
+        self.npad = fft_kwargs(range(self.n0))['n']       # transform length (helpers.py:15-30)
+        self._fftfreqs = None
+
+    @property
+    def fftfreqs(self):
+        if self._fftfreqs is None:
+            npad = self.npad
+            self._fftfreqs = (2 * np.pi * fft.fftfreq(npad, self.dt))[1:npad // 2] / (2 * np.pi)
+        return self._fftfreqs
 
     # -- the products --------------------------------------------------------------------
     @_live
@@ -129,10 +167,6 @@ class ResidentTransform(object):
             if variance is not None:
                 rs = rs / float(variance)
         return self.engine.power(len(self.scales), self.n0, rs)
-
-    def coi_ranges(self):
-        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
-        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
 
     @_live
     def window(self, rows=slice(None), cols=slice(None)):
@@ -167,12 +201,7 @@ class ResidentTransform(object):
     def scale_avg_power(self, period_min, period_max, variance=1.0):
         """Scale-averaged power over period_min <= period < period_max (TC98 eq. 24 as in
         simple_sample.py:87-91): variance * dj * dt / Cdelta * sum_j |W_j|^2 / s_j."""
-        if self.wavelet.cdelta == -1:
-            raise ValueError('Cdelta not defined for this wavelet')
-        per = self.period
-        sel = (per >= period_min) & (per < period_max)
-        w = np.where(sel, 1.0 / np.asarray(self.scales, dtype=float), 0.0)
-        w = w * (variance * self.dj * self.dt / self.wavelet.cdelta)
+        _, w = self._band_weights(period_min, period_max, variance)
         return self.engine.scale_avg_power(w)
 
     @_live
@@ -299,55 +328,21 @@ def _ratio(num, den):
         return np.where(den > 0, num / np.where(den > 0, den, 1.0), np.nan)
 
 
-class ResidentCoherence(object):
+class ResidentCoherence(_ResidentSlot):
     """WCT and aWCT [S, n0] of one `wct_resident` call, resident on the device."""
+
+    _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence_serial', 'coherence_release'
+    _GONE = ("this coherence is no longer resident: it was released or another wct_resident has "
+             "run on the same engine")
 
     def __init__(self, engine, problem, precision, serial):
         p = problem
-        self.engine = engine
-        self.wavelet = p.wavelet
-        self.n0 = int(p.n0)
-        self.dt = float(p.dt)
-        self.dj = p.dj
+        super(ResidentCoherence, self).__init__(engine, p.wavelet, p.n0, p.dt, p.dj, p.sj,
+                                                precision, serial)
         self.s0 = p.s0
         self.J = p.J
-        self.scales = p.sj
         self.freq = p.freq
-        self.precision = precision
         self._y = (np.array(p.y1, copy=True), np.array(p.y2, copy=True))   # raw series, for ar1
-        self._serial = serial
-        self._coi = None
-
-    @property
-    def coi(self):
-        if self._coi is None:
-            self._coi = _coi(self.wavelet, self.dt, self.n0)
-        return self._coi
-
-    @property
-    def shape(self):
-        return (len(self.scales), self.n0)
-
-    @property
-    def period(self):
-        return 1.0 / np.asarray(self.freq)
-
-    def coi_ranges(self):
-        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
-        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
-
-    # -- bookkeeping ---------------------------------------------------------------------
-    def _check_live(self):
-        if self.engine.coherence_serial() != self._serial:
-            raise _engine.EngineError("this coherence is no longer resident: it was released or "
-                                      "another wct_resident has run on the same engine")
-
-    def release(self):
-        """Free the device buffer (16 bytes per scale and time point).  The handle is invalid
-        afterwards; releasing an invalid handle does nothing."""
-        with self.engine.lock:
-            if self.engine.coherence_serial() == self._serial:
-                self.engine.coherence_release()
 
     def _threshold(self, sig95):
         if sig95 is None:
@@ -420,8 +415,7 @@ class ResidentCoherence(object):
         (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
         |sum e^{i aWCT}| / count, count), for the whole band or, with `per_scale`, per scale
         (arrays; NaN angle and strength where the count is 0)."""
-        per = self.period
-        sel = (per >= period_min) & (per < period_max)
+        sel = self._band(period_min, period_max)
         lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
         st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95), want_phase=True)
@@ -431,8 +425,7 @@ class ResidentCoherence(object):
     def scale_avg(self, period_min, period_max):
         """Two length-n0 series over the scales with period_min <= period < period_max: the mean
         WCT and the circular mean phase atan2(sum sin aWCT, sum cos aWCT)."""
-        per = self.period
-        sel = (per >= period_min) & (per < period_max)
+        sel = self._band(period_min, period_max)
         if not sel.any():
             raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
         out = self.engine.coherence_scale_avg(sel.astype(float))
@@ -461,7 +454,7 @@ def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=T
 # cwt / xwt / wct / wct_resident / Monte-Carlo calls, until the next `xwt_resident` on the same
 # engine or `release()`.
 
-class ResidentCrossWavelet(object):
+class ResidentCrossWavelet(_ResidentSlot):
     """W12 = W1 conj(W2) [S, n0] of one `xwt_resident` call, resident on the device.
 
     `signif` arguments of the methods are in |W12| units, as `xwt` returns them (`.signif`); a
@@ -469,50 +462,16 @@ class ResidentCrossWavelet(object):
     script's `|W12|^2 / signif > 1` convention is `signif=np.sqrt(h.signif)`.  A negative entry
     raises ValueError, a NaN entry selects no point of its scale."""
 
+    _FREQ, _SERIAL, _RELEASE = 'freq', 'cross_serial', 'cross_release'
+    _GONE = ("this cross spectrum is no longer resident: it was released or another xwt_resident "
+             "has run on the same engine")
+
     def __init__(self, engine, problem, signif, precision, serial):
         p = problem
-        self.engine = engine
-        self.wavelet = p.wavelet
-        self.n0 = int(p.n0)
-        self.dt = float(p.dt)
-        self.dj = p.dj
-        self.scales = p.sj
+        super(ResidentCrossWavelet, self).__init__(engine, p.wavelet, p.n0, p.dt, p.dj, p.sj,
+                                                   precision, serial)
         self.freq = p.freq
         self.signif = signif
-        self.precision = precision
-        self._serial = serial
-        self._coi = None
-
-    @property
-    def coi(self):
-        if self._coi is None:
-            self._coi = _coi(self.wavelet, self.dt, self.n0)
-        return self._coi
-
-    @property
-    def shape(self):
-        return (len(self.scales), self.n0)
-
-    @property
-    def period(self):
-        return 1.0 / np.asarray(self.freq)
-
-    def coi_ranges(self):
-        """Columns inside the cone of influence, per scale (see `_coi_ranges`)."""
-        return _coi_ranges(self.wavelet, self.dt, self.n0, self.period)
-
-    # -- bookkeeping ---------------------------------------------------------------------
-    def _check_live(self):
-        if self.engine.cross_serial() != self._serial:
-            raise _engine.EngineError("this cross spectrum is no longer resident: it was released "
-                                      "or another xwt_resident has run on the same engine")
-
-    def release(self):
-        """Free the device buffer (16 or 8 bytes per scale and time point).  The handle is
-        invalid afterwards; releasing an invalid handle does nothing."""
-        with self.engine.lock:
-            if self.engine.cross_serial() == self._serial:
-                self.engine.cross_release()
 
     def _stats(self, lo, hi, signif):
         thr = None if signif is None else _power_threshold(self, signif) ** 2
@@ -554,8 +513,7 @@ class ResidentCrossWavelet(object):
         (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
         |sum e^{i angle}| / count, count), for the whole band or, with `per_scale`, per scale
         (NaN angle and strength where the count is 0).  A zero coefficient has phase 0."""
-        per = self.period
-        sel = (per >= period_min) & (per < period_max)
+        sel = self._band(period_min, period_max)
         lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
         st = self._stats(lo, hi, signif)
@@ -566,14 +524,9 @@ class ResidentCrossWavelet(object):
         """Scale-averaged cross spectrum over period_min <= period < period_max (complex128,
         length n0): dj * dt / Cdelta * sum_j W12[j] / s_j, Torrence & Compo (1998) eq. 24 with
         W12 in place of |W|^2."""
-        if self.wavelet.cdelta == -1:
-            raise ValueError('Cdelta not defined for this wavelet')
-        per = self.period
-        sel = (per >= period_min) & (per < period_max)
+        sel, w = self._band_weights(period_min, period_max)
         if not sel.any():
             raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
-        w = np.where(sel, 1.0 / np.asarray(self.scales, dtype=float), 0.0)
-        w = w * (self.dj * self.dt / self.wavelet.cdelta)
         return self.engine.cross_scale_avg(w)
 
 
