@@ -264,34 +264,73 @@ def test_resident_transform_products(pycwt):
     check_resident_products(pycwt.default_engine(), TOL64)
 
 
-def test_resident_products_full_size(pycwt):
-    """North-star size: the reductions agree with NumPy on rows fetched from the device,
-    and the fp32 transform comes back as complex128 through the widening fetch."""
-    n = 2 ** 20
-    x = chirp(n)
-    r = pycwt.cwt_resident(x, 1.0, 1 / 16, 2.0, 255, pycwt.Morlet(6))
-    glbl = r.global_power()
-    savg = r.scale_avg_power(16.0, 64.0, variance=1.0)
-    inside = r.global_power(inside_coi=True)
+def _check_full_size_reductions(pycwt, precision):
+    """Every reduction of the resident transform against longdouble sums of the rows fetched from the
+    same handle (the fp32 engine: of its complex64 values; its reductions add in double too)."""
+    from pycwt_b200 import _engine
+    n = 2 ** 20 - 5                      # PowerBody's last round of columns is partial
+    x = chirp(n) + 0.1 * np.random.RandomState(17).randn(n)
+    if precision == _engine.F32:
+        x = x.astype(np.float32)
+    # 300 rows: 10 blocks of icwt atomics (the last one partial); the cone leaves no column to the
+    # largest scales (NaN rows of the inside-COI spectrum)
+    r = pycwt.cwt_resident(x, 1.0, 1 / 16, 2.0, 299, pycwt.Morlet(6))
     eng = r.engine
-    rows = [0, 100, 255]
-    per = r.period
+    S = len(r.scales)
+    assert S == 300 and r.precision == precision
+    glbl = r.global_power()
+    inside = r.global_power(inside_coi=True)
+    savg = r.scale_avg_power(8.0, 128.0, variance=1.0)
+    # TC98 eq. 24 weights, stated here from the oracle's mother: dj dt / (Cdelta s_j) on the band
+    per = orc.Morlet(6).flambda() * r.scales
+    sel = (per >= 8.0) & (per < 128.0)
+    w = np.where(sel, r.dj * r.dt / (orc.Morlet(6).cdelta * r.scales), 0.0)
+    assert sel.sum() > 32                # more than one block of rows: the atomic path
+    red = eng.icwt_sum()
     lo, hi = r.coi_ranges()
-    for j in rows:
-        Wj = np.empty((1, n), dtype=np.complex128)
-        eng._check(eng.lib.cwtb_get_w(eng.h, Wj.ctypes.data, 1, j, 1))
-        p = np.abs(Wj[0]) ** 2
-        assert abs(glbl[j] / p.mean() - 1) < 1e-12
+    LD = np.longdouble
+    gp_ref, in_ref = np.empty(S), np.full(S, np.nan)
+    sa_ref, ic_ref, ic_abs = np.zeros(n, LD), np.zeros(n, LD), np.zeros(n, LD)
+    Wj = np.empty((1, n), dtype=np.complex64 if precision == _engine.F32 else np.complex128)
+    for j in range(S):
+        eng._check(eng.lib.cwtb_get_w(eng.h, Wj.ctypes.data, 1 if precision == _engine.F64 else 0, j, 1))
+        re_, im_ = Wj[0].real.astype(LD), Wj[0].imag.astype(LD)
+        p = re_ * re_ + im_ * im_
+        gp_ref[j] = p.sum() / n
+        if hi[j] > lo[j]:
+            in_ref[j] = p[lo[j]:hi[j]].sum() / (hi[j] - lo[j])
+        if w[j]:
+            sa_ref += LD(w[j]) * p
+        t = re_ / np.sqrt(LD(r.scales[j]))
+        ic_ref += t
+        ic_abs += np.abs(t)
+    assert np.isnan(in_ref).any() and not np.isnan(in_ref).all()
+    assert np.array_equal(np.isnan(inside), np.isnan(in_ref))
+    ok = ~np.isnan(in_ref)
+    e_gp = np.abs(glbl / gp_ref - 1).max()
+    e_in = np.abs(inside[ok] / in_ref[ok] - 1).max()
+    e_sa = float((np.abs(savg - sa_ref) / sa_ref).max())
+    e_ic = float((np.abs(red - ic_ref) / ic_abs).max())
+    print("full-size reductions, precision %d: global %.1e, inside COI %.1e, scale average %.1e, icwt %.1e"
+          % (precision, e_gp, e_in, e_sa, e_ic))
+    assert e_gp < 1e-13 and e_in < 1e-13 and e_sa < 1e-13 and e_ic < 1e-13
+    # the cone's column ranges, and the icwt scaling on top of the row sum
+    per = r.period
+    assert np.array_equal(sel, (per >= 8.0) & (per < 128.0))
+    for j in (0, 100, 255):
         assert np.array_equal(np.nonzero(per[j] <= r.coi)[0][[0, -1]], [lo[j], hi[j] - 1])
-        assert abs(inside[j] / p[lo[j]:hi[j]].mean() - 1) < 1e-12
-    sel = np.nonzero((per >= 16.0) & (per < 64.0))[0]
-    acc = np.zeros(n)
-    for j in sel:
-        Wj = np.empty((1, n), dtype=np.complex128)
-        eng._check(eng.lib.cwtb_get_w(eng.h, Wj.ctypes.data, 1, int(j), 1))
-        acc += np.abs(Wj[0]) ** 2 / r.scales[j]
-    acc *= r.dj * r.dt / r.wavelet.cdelta
-    assert relerr(savg, acc) < 1e-12
+    fac = r.dj * np.sqrt(r.dt) / (r.wavelet.cdelta * r.wavelet.psi(0))
+    assert relerr(r.icwt(), fac * red) < 1e-15
+
+
+def test_resident_products_full_size(pycwt, monkeypatch):
+    """North-star size: the reductions -- global spectrum (also inside the COI), scale average over
+    more than 32 rows, icwt sum -- agree with longdouble sums of the rows fetched from the device, in
+    the fp64 and the fp32 engine."""
+    from pycwt_b200 import _engine
+    _check_full_size_reductions(pycwt, _engine.F64)
+    monkeypatch.setenv("CWTB_PRECISION", "fp32")
+    _check_full_size_reductions(pycwt, _engine.F32)
 
 
 def test_fp32_fetch_widening_large(pycwt, monkeypatch):

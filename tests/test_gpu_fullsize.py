@@ -26,6 +26,37 @@ def _oracle_rows(x, dt, mother, sj, rows):
     return orc.cwt(x, dt, wavelet=mother, freqs=fr, workers=-1)[0]
 
 
+# Per-row bounds of config 2, by the row's class in last_plan (error / max|W_ref[j]|): expansion rows at
+# the expansion tolerance, exact and overlap-save rows at 1e-14 (DESIGN 6).  Measured on H100 against the
+# fp64 oracle: 5.2e-14, 6.4e-15 and 2.7e-15.  The exact rows 0..19 (s = 2 .. 4.8) lie above the chirp's
+# band, where the oracle's own rounding is of the order of the bound; they are also checked against the
+# longdouble reference of test_gpu_row_parity.py (measured: 6.0e-15).
+C2_OUT_OF_BAND = 20
+C2_BOUND = {"expansion": 5e-13, "exact": 1e-14, "overlap-save": 1e-14}
+
+
+def _row_class(p):
+    return "expansion" if p < -2 else ("overlap-save" if p == -2 else "exact")
+
+
+def _check_config2_rows(x, c, sj, plan, err, W):
+    from test_gpu_row_parity import ref_rows, row_err
+    worst = {}
+    for j, p in enumerate(plan):
+        k = _row_class(p)
+        worst[k] = max(worst.get(k, 0.0), float(err[j]))
+    print("config 2 per-row error by class: %s" % ", ".join("%s %.2e" % kv for kv in sorted(worst.items())))
+    bad = [(j, _row_class(plan[j]), float(err[j])) for j in range(len(plan))
+           if err[j] > C2_BOUND[_row_class(plan[j])]]
+    assert not bad, bad
+    rows = np.arange(C2_OUT_OF_BAND)
+    e = row_err(W[rows], ref_rows(x, c["dt"], sj[rows], 0, c["f0"]))
+    print("config 2 rows 0..%d (above the chirp's band): against the longdouble reference %.2e, against "
+          "the fp64 oracle %.2e" % (C2_OUT_OF_BAND - 1, e.max(), err[rows].max()))
+    assert all(_row_class(plan[j]) == "exact" for j in rows), plan[:C2_OUT_OF_BAND]
+    assert (e < C2_BOUND["exact"]).all(), e
+
+
 def test_config2_every_row(pycwt):
     """Config 2 (the bench's input: chirp N = 2^20, s0 = 2, dj = 1/16, 256 scales, Morlet(6), fp64):
     all 256 rows of W and of |W|^2 against the oracle."""
@@ -48,15 +79,15 @@ def test_config2_every_row(pycwt):
         pmax = max(pmax, float(pr.max()))
         d = np.abs(W[rows] - Wr).max(axis=1)
         dp = np.abs(np.abs(W[rows]) ** 2 - pr).max(axis=1)
-        diffs.append((rows, d, dp))
-    for rows, d, dp in diffs:
+        diffs.append((rows, d, dp, np.abs(Wr).max(axis=1)))
+    for rows, d, dp, _ in diffs:
         worst = max(worst, float(d.max()) / wmax)
         worst_p = max(worst_p, float(dp.max()) / pmax)
     print("config 2: max|dW|/max|W| = %.2e, power %.2e" % (worst, worst_p))
     assert worst < TOL64 and worst_p < TOL64
-    # per-row: no row may hide behind the global maximum by more than its own scale allows
-    for rows, d, dp in diffs:
-        assert (d / wmax < TOL64).all()
+    # per row, against the row's own maximum, with the bound of the row's class
+    err = np.concatenate([d / rmax for rows, d, dp, rmax in diffs])
+    _check_config2_rows(x, c, sj, plan, err, W)
     ref_fft = np.fft.fft(x)[1:c["n"] // 2] / np.sqrt(c["n"])
     assert relerr(fft, ref_fft) < 1e-12
 
