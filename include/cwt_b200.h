@@ -190,7 +190,7 @@ int cwtb_xwt(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,
 /* Wavelet coherence of two signals (Morlet smoothing operator):
  *   WCT = |S(W12/s)|^2 / (S(|W1|^2/s) * S(|W2|^2/s)),  aWCT = angle(W12),
  * S = Gaussian time filter exp(-0.5*(s/dt)^2*k^2) (FFT, zero-pad to Np) followed
- * by a boxcar of `boxcar_len` taps with half-weight ends along the scale axis
+ * by a boxcar of `boxcar_len` >= 1 taps with half-weight ends along the scale axis
  * (helpers.py:176-191, scipy convolve2d 'same' alignment).
  * WCT_out, aWCT_out: n_scales x n0 doubles (either may be NULL). */
 int cwtb_wct(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t n0,

@@ -2537,7 +2537,8 @@ static int upload_signal_f64(cwtb_ctx *c, Buf &b, const double *y, long long n0)
   return 0;
 }
 
-// boxcar with half-weight end taps, normalised (helpers.py:176-191)
+// boxcar with half-weight end taps, normalised (helpers.py:176-191), followed by one unit tap
+// (the one-tap window of wct_core's path for boxcars longer than 64 taps)
 static int upload_window(cwtb_ctx *c, int K) {
   if (K < 1) return fail(c, CWTB_ERR_ARG, "boxcar length must be >= 1");
   std::vector<double> w(K, 1.0);
@@ -2546,6 +2547,7 @@ static int upload_window(cwtb_ctx *c, int K) {
   double sum = 0;
   for (double v : w) sum += v;
   for (double &v : w) v /= sum;
+  w.push_back(1.0);
   return upload_doubles(c, c->win, w);
 }
 
@@ -2620,11 +2622,21 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
 #endif
   if ((e = smooth_time<T>(c, (V *)c->C.p, S, n0, job.N, d_g))) return e;
   if ((e = smooth_time<T>(c, (V *)c->A12.p, S, n0, job.N, d_g))) return e;
-  WctFinalArgs<T> fa{(const V *)c->C.p, (const V *)c->A12.p, (const double *)c->win.p, dWCT,
-                     dmask, dhist, n0, S, K, maxscale, nbins};
-  if (K > 64) return fail(c, CWTB_ERR_UNSUPPORTED, "scale boxcar longer than 64 taps");
   const int rows_out = dWCT ? S : maxscale;
   if (rows_out <= 0) return 0;
+  WctFinalArgs<T> fa{(const V *)c->C.p, (const V *)c->A12.p, (const double *)c->win.p, dWCT,
+                     dmask, dhist, n0, S, K, maxscale, nbins};
+  if (K > 64) {
+    // longer than the fused kernel stages: the scale boxcar of both fields into W and W2 (dead
+    // since WctPrepBody), then the ratio through the fused kernel with the unit tap at win + K
+    BoxcarArgs<T> b1{fa.C, (V *)c->W.p, fa.win, n0, S, K}, b2{fa.A12, (V *)c->W2.p, fa.win, n0, S, K};
+    if ((e = launch<BoxcarBody<T>>(c, gx, rows_out, b1))) return e;
+    if ((e = launch<BoxcarBody<T>>(c, gx, rows_out, b2))) return e;
+    fa.C = (const V *)c->W.p;
+    fa.A12 = (const V *)c->W2.p;
+    fa.win += K;
+    fa.K = 1;
+  }
   using F16 = WctFinalBody<T, 16>;
   const unsigned fx = (unsigned)((n0 + F16::CW - 1) / F16::CW), fy = (unsigned)((rows_out + F16::RS - 1) / F16::RS);
   return K <= 16 ? launch<F16>(c, fx, fy, fa) : launch<WctFinalBody<T, 64>>(c, fx, fy, fa);
@@ -3289,8 +3301,8 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
     if ((e = launch<R2CBody>(c, (unsigned)((cnt + NT - 1) / NT), 1, ra))) return e;
   }
   if ((e = smooth_time<double>(c, X, S, n, N, (const double *)c->rowd.p + S))) return e;
-  BoxcarArgs ba{X, Y, (const double *)c->win.p, n, S, boxcar_len};
-  if ((e = launch<BoxcarBody>(c, (unsigned)((n + NT - 1) / NT), S, ba))) return e;
+  BoxcarArgs<double> ba{X, Y, (const double *)c->win.p, n, S, boxcar_len};
+  if ((e = launch<BoxcarBody<double>>(c, (unsigned)((n + NT - 1) / NT), S, ba))) return e;
   if (is_complex) {
     RT(rt_d2h(out, Y, cnt * sizeof(double2), c->stream));
     RT(rt_sync(c->stream));

@@ -1682,33 +1682,32 @@ template <typename T> struct NoiseBody {
 
 // ---- Body: scale-axis boxcar (mothers.py:100-102; scipy convolve2d 'same', zero fill) ------
 //   out[i] = sum_t win[t] * in[i - (t - off)],  off = (K-1)//2, rows outside [0, m) are zero
-struct BoxcarArgs {
-  const double2 *in;
-  double2 *out;
+// Sums in the engine type T, like WctFinalBody; any K (no shared memory).
+template <typename T> struct BoxcarArgs {
+  const cx<T> *in;
+  cx<T> *out;
   const double *win;
   long long n;
   int rows, K;
 };
-HD double2 boxcar_at(const double2 *in, const double *win, int K, int rows, long long n, int i, long long col) {
-  const int off = (K - 1) / 2;
-  double re = 0, im = 0;
-  for (int t = 0; t < K; ++t) {
-    const int q = i - (t - off);
-    if (q < 0 || q >= rows) continue;
-    const double2 v = in[(size_t)q * n + col];
-    re += win[t] * v.x;
-    im += win[t] * v.y;
-  }
-  return make_double2(re, im);
-}
-struct BoxcarBody {
-  using Args = BoxcarArgs;
+template <typename T> struct BoxcarBody {
+  using Args = BoxcarArgs<T>;
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
     const long long n = (long long)bx * NT + tid;
     if (n >= a.n) return;
-    a.out[(size_t)by * a.n + n] = boxcar_at(a.in, a.win, a.K, a.rows, a.n, by, n);
+    const int off = (a.K - 1) / 2;
+    T re = 0, im = 0;
+    for (int t = 0; t < a.K; ++t) {
+      const int q = by - (t - off);
+      if (q < 0 || q >= a.rows) continue;
+      const cx<T> v = a.in[(size_t)q * a.n + n];
+      const T w = (T)a.win[t];
+      re += w * v.x;
+      im += w * v.y;
+    }
+    a.out[(size_t)by * a.n + n] = mk<T>(re, im);
   }
 };
 

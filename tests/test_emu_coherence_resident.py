@@ -262,14 +262,14 @@ def test_lifetime(api, emu, precision):
     h2.release()                              # idempotent
 
 
-def test_failed_call_invalidates_the_old_handle(api, emu):
+def test_refused_boxcar_invalidates_the_old_handle(api, emu):
     from pycwt_b200 import _engine
     y1, y2, dt, kw = ao_baltic()
     h = api.wct_resident(y1, y2, dt, **kw)
     before = emu.coherence_serial()
     with pytest.raises(_engine.EngineError):
-        # an odd boxcar that the engine refuses (longer than 64 taps): fails after the serial bump
-        emu.wct_resident(y1, y2, dt, 1 / 12, h.scales, 0, 6.0, 65)
+        # a boxcar of no taps, refused when the window is uploaded: fails after the serial bump
+        emu.wct_resident(y1, y2, dt, 1 / 12, h.scales, 0, 6.0, 0)
     assert emu.coherence_serial() != before
     with pytest.raises(_engine.EngineError):
         h.global_coherence()

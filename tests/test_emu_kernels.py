@@ -274,7 +274,9 @@ def check_unpadded_mode(eng, tol):
         assert relerr(m.smooth(g["Wr"], 1.0, 0.25, g["sj"]), g["Sr"]) < tol
         assert relerr(m.smooth(g["Wc"], 1.0, 0.25, g["sj"]), g["Sc"]) < tol
         WCT, aWCT, _, _, _ = pycwt.wct(g["y1"], g["y2"], float(g["dt"]), dj=1 / 12, sig=False, wavelet=m)
-        assert relerr(WCT, g["WCT"]) < 100 * tol and relerr(aWCT, g["aWCT"]) < 100 * tol
+        # (measured 3e-15 and 1e-14; the fixture itself is within 2e-16 kappa of the longdouble
+        # coherence, test_gpu_coherence_parity.py)
+        assert relerr(WCT, g["WCT"]) < tol and relerr(aWCT, g["aWCT"]) < tol
         np.random.seed(4321)
         sig95 = pycwt.wct_significance(0.2, 0.1, 1.0, 0.5, 2.0, 10, 0.95, m, mc_count=5,
                                        progress=False, cache=False)

@@ -57,14 +57,14 @@ def _conj_psi_ld(family, param, f):
     return mag * {0: -1, 1: 1j, 2: 1, 3: -1j}[m % 4]
 
 
-def ref_rows(x, dt, scales, family, param, n0=None):
-    """Rows W[j, :n0] of the transform of x (zero-padded to the next power of two) at the fp64 scales,
-    as full-length band products computed in longdouble; complex128 result.  Paul's response is finite
+def ref_rows(x, dt, scales, family, param, n0=None, npad=None):
+    """Rows W[j, :n0] of the transform of x (zero-padded to the next power of two, or to `npad`) at the
+    fp64 scales, as full-length band products computed in longdouble; complex128 result.  Paul's response is finite
     everywhere here, as in the engine (the reference's inf * 0 = NaN rows, s pi / dt > 709.78, are
     dropped by the Python layer, pycwt_b200/wavelet.py: _nan_rows)."""
     x = np.asarray(x, dtype=np.float64)
     n0 = x.size if n0 is None else n0
-    Np = orc.next_pow2(x.size)
+    Np = npad or orc.next_pow2(x.size)
     X = np.fft.fft(x.astype(LD), Np)
     k = (np.fft.fftfreq(Np) * Np).astype(LD)                   # signed bins, exact
     omega = 2 * PI_L * k / (LD(Np) * LD(dt))
