@@ -117,7 +117,11 @@ def test_config2_widest_band_mode(pycwt):
 
 @pytest.mark.parametrize("family", ["paul", "dog"])
 def test_config3_every_row_fp32(pycwt, monkeypatch, family):
-    """Config 3: Paul(4) / DOG(2), N = 2^18, 128 scales, float32 chirp, fp32 engine; every row."""
+    """Config 3: Paul(4) / DOG(2), N = 2^18, 128 scales, float32 chirp, fp32 engine; every row against
+    the oracle at the contract's 1e-5 of max|W|, and every row against its own scale sigma_j (the row's
+    maximum, or its rms response to white noise of the signal's energy where that is larger: rows
+    outside the chirp's band) with the per-row bounds of test_gpu_fp32_row_parity.py."""
+    from test_gpu_fp32_row_parity import EXACT32, EXPAND32, ref32, sigma_err
     monkeypatch.setenv("CWTB_PRECISION", "fp32")
     c = wl.C3
     p = c[family]
@@ -132,6 +136,13 @@ def test_config3_every_row_fp32(pycwt, monkeypatch, family):
     print("config 3 %s: max|dW|/max|W| = %.2e (worst row %d)" % (family, err, int(rows.argmax())))
     assert err < TOL32 and (rows < TOL32).all()
     assert relerr(np.abs(W) ** 2, np.abs(Wr) ** 2) < TOL32
+    plan = np.array(pycwt.default_engine().last_plan(len(sj)))
+    fam = 1 if family == "paul" else 2
+    e = sigma_err(W, *ref32(x, c["dt"], sj, fam, float(p["m"])))
+    bound = np.where(plan < 0, EXPAND32, EXACT32)
+    print("config 3 %s per row / sigma_j: expansion rows %.2e, exact rows %.2e"
+          % (family, e[plan < 0].max(initial=0), e[plan >= 0].max(initial=0)))
+    assert (e <= bound).all(), [(j, int(plan[j]), float(e[j])) for j in np.flatnonzero(e > bound)]
 
 
 def test_config4_xwt_wct_every_row(pycwt):
