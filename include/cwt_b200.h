@@ -242,6 +242,24 @@ int cwtb_xwt_resident(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t
 int64_t cwtb_cross_serial(cwtb_ctx *ctx);
 int cwtb_cross_release(cwtb_ctx *ctx);
 
+/* ---- partial and multiple wavelet coherence of three series (Mihanovic et al. 2009; Ng & Chan
+ * 2012) -------------------------------------------------------------------------------------------
+ * y, x1, x2: three signals of n0 samples (standardised by the caller as for cwtb_wct).  With S the
+ * smoothing operator of cwtb_wct (same boxcar_len, same time filter, cwtb_set_smooth_filter
+ * included), S_a = S(|W_a|^2/s) and S_ab = S(W_a conj(W_b)/s):
+ *   RP2 = |S_y1 S_2 - S_y2 S_21|^2 / ((S_y S_2 - |S_y2|^2) (S_1 S_2 - |S_12|^2))   (y with x1, x2 removed)
+ *   RM2 = 1 - det G3 / (S_y (S_1 S_2 - |S_12|^2))                                  (y on x1 and x2)
+ * G3 the 3 x 3 smoothed spectral matrix.  RP2_out, RM2_out: n_scales x n0 doubles, either may be
+ * NULL.  No clamping: a denominator that is zero or rounds to <= 0 gives inf or NaN; both measures
+ * are ill-conditioned where x1 and x2 are nearly coherent (|S_12|^2 -> S_1 S_2).  The smoothed fields
+ * are combined in double in both precisions.  Precision: cwtb_set_coherence_precision; un-padded
+ * transforms only in fp64, CWTB_TABLE unsupported.  Lifetime: the resident coherence and cross
+ * spectrum are not written (their handles survive the call); afterwards no transform is resident
+ * (cwtb_get_w, cwtb_icwt_sum and the power calls return CWTB_ERR_STATE until the next transform). */
+int cwtb_wct3(cwtb_ctx *ctx, const double *y, const double *x1, const double *x2, int64_t n0,
+              double dt, double dj, const double *scales, int n_scales, int family, double param,
+              int boxcar_len, double *RP2_out, double *RM2_out);
+
 /* Reading calls on a resident complex field: CWTB_FIELD_W (the resident transform's W) or
  * CWTB_FIELD_CROSS (the cross spectrum).  They return CWTB_ERR_STATE when the field is not
  * resident, CWTB_ERR_UNSUPPORTED for the W of a batched transform and CWTB_ERR_ARG for bad

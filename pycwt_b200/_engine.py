@@ -70,6 +70,7 @@ _SIGNATURES = {
     "cwtb_xwt": (_I, [_P, _P, _P, _I64, _D, _P, _I, _I, _D, _P]),
     "cwtb_wct": (_I, [_P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_wct_resident": (_I, [_P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I]),
+    "cwtb_wct3": (_I, [_P, _P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_coherence_serial": (_I64, [_P]),
     "cwtb_coherence_release": (_I, [_P]),
     "cwtb_coherence_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P, _P]),
@@ -531,6 +532,27 @@ class Engine(object):
                                           _ptr(aWCT) if want_angle else None))
             self._resident = None                   # several intermediates, no single transform
         return WCT, aWCT
+
+    @_locked
+    def wct3(self, y, x1, x2, dt, dj, scales, family, param, boxcar_len, want_partial=True,
+             want_multiple=True, precision=F64):
+        """(RP2, RM2): partial coherence of y with x1 (x2 removed) and multiple coherence of y on
+        x1 and x2, float64 [S, n0]; a measure not asked for is None.  No transform is resident
+        afterwards; the resident coherence and cross spectrum are left alone."""
+        ys = [np.ascontiguousarray(v, dtype=np.float64) for v in (y, x1, x2)]
+        if any(v.ndim != 1 or v.shape != ys[0].shape for v in ys):
+            raise ValueError("wct3: the three series must be 1-D and of equal length")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        RP2 = self.result_array((sj.size, ys[0].size), np.float64) if want_partial else None
+        RM2 = self.result_array((sj.size, ys[0].size), np.float64) if want_multiple else None
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct3(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]), ys[0].size,
+                                       float(dt), float(dj), _ptr(sj), sj.size, int(family),
+                                       float(param), int(boxcar_len),
+                                       _ptr(RP2) if want_partial else None,
+                                       _ptr(RM2) if want_multiple else None))
+        return RP2, RM2
 
     # ---- resident coherence and cross spectrum (device buffers of their own, see
     # include/cwt_b200.h) and the reads of a resident field ------------------------------------

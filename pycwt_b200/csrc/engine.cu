@@ -233,7 +233,7 @@ struct cwtb_ctx {
   std::vector<double> wtab_host; // host mirror of wtab (tables are appended, never moved)
   size_t wtab_uploaded = 0;      // elements already on the device
   size_t wtab_max_bytes = (size_t)256 << 20;   // CWTB_WTAB_MB: host mirror size above which the cache starts over
-  Buf ctr, sig, sig2, spec, Z, Zc[3], Y, B, W, W2, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
+  Buf ctr, sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
   // geometry and settings reuses it (planning + descriptor upload: ~0.3 ms for 256 scales, several ms
@@ -266,8 +266,8 @@ struct cwtb_ctx {
   // cwtb_xwt_resident hands its transform's W over by swapping the two buffers, so W12 is never
   // copied and the old cross buffer becomes the next transform's W.  Nothing else writes it.
   ResidentSlot cross;
-  bool w_moved = false;          // W went to the cross spectrum: no transform resident until the
-                                 // next one writes W
+  bool w_moved = false;          // W went to the cross spectrum, or cwtb_wct3 wrote a smoothed field
+                                 // into it: no transform resident until the next one writes W
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
   double last_ms = 0;
   int launches = 0;
@@ -2005,7 +2005,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   cudaStreamSynchronize(c->stream);
 #endif
   cwtb_comm_destroy(c);
-  for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->descs, &c->table, &c->scratch,
+  for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
                  &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh.buf, &c->cross.buf})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
@@ -2642,6 +2642,54 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   return K <= 16 ? launch<F16>(c, fx, fy, fa) : launch<WctFinalBody<T, 64>>(c, fx, fy, fa);
 }
 
+// three transforms + partial / multiple coherence in the engine type T; outputs are device
+// pointers (either may be null) and double for every T.  Device memory per scale-point: the three
+// transforms W, W2, W3 (the crosses are written over them), the two auto fields C, A12 and the
+// smoothing buffer F.
+template <typename T>
+static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, const T *dx2, int K,
+                     double *dRP2, double *dRM2) {
+  using V = cx<T>;
+  const int S = job.S;
+  const long long n0 = job.n0;
+  const size_t cnt = (size_t)S * n0;
+  int e;
+  for (Buf *b : {&c->W, &c->W2, &c->W3, &c->C, &c->A12})
+    if ((e = ensure(c, *b, cnt * sizeof(V)))) return e;
+  c->w_moved = false;
+  if ((e = run_job<T>(c, job, dy, (V *)c->W.p, EPI_STORE))) return e;
+  if ((e = run_job<T>(c, job, dx1, (V *)c->W2.p, EPI_STORE))) return e;
+  if ((e = run_job<T>(c, job, dx2, (V *)c->W3.p, EPI_STORE))) return e;
+  const double *d_scale = (const double *)c->rowd.p;      // [S] scales, then [S] g
+  const double *d_g = d_scale + S;
+  V *f[5] = {(V *)c->C.p, (V *)c->A12.p, (V *)c->W.p, (V *)c->W2.p, (V *)c->W3.p};
+  Wct3PrepArgs<T> pa{f[2], f[3], f[4], d_scale, f[0], f[1], f[2], f[3], f[4], n0};
+  const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
+  if ((e = launch<Wct3PrepBody<T>>(c, gx, S, pa))) return e;
+  for (V *x : f)
+    if ((e = smooth_time<T>(c, x, S, n0, job.N, d_g))) return e;
+  const double *win = (const double *)c->win.p;
+  if (K > 64) {
+    // longer than the fused kernel stages: the scale boxcar of each field into the buffer the
+    // previous field left (the first into F, free after the smoothing), then the fused kernel
+    // with the unit tap at win + K
+    V *dst = (V *)c->F.p;
+    for (V *&x : f) {
+      BoxcarArgs<T> b{x, dst, win, n0, S, K};
+      if ((e = launch<BoxcarBody<T>>(c, gx, S, b))) return e;
+      std::swap(x, dst);
+    }
+    win += K;
+    K = 1;
+  }
+  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, n0, S, K};
+  using F16 = Wct3FinalBody<T, 16, 32, 16>;
+  using F64K = Wct3FinalBody<T, 64, 64, 8>;
+  if (K <= 16)
+    return launch<F16>(c, (unsigned)((n0 + F16::CW - 1) / F16::CW), (unsigned)((S + F16::RS - 1) / F16::RS), fa);
+  return launch<F64K>(c, (unsigned)((n0 + F64K::CW - 1) / F64K::CW), (unsigned)((S + F64K::RS - 1) / F64K::RS), fa);
+}
+
 // the engine precision of T, and host series (double) as device series of type T: the fp32
 // coherence converts on the device, so that its inputs are the fp64 inputs rounded
 template <typename T> constexpr int prec_of() { return sizeof(T) == 8 ? CWTB_F64 : CWTB_F32; }
@@ -3199,6 +3247,53 @@ int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
 #ifndef CWTB_HOST_EMU
   if (early_angle) RT(rt_sync(c->copy_streams[0]));
 #endif
+  return 0;
+}
+
+// ---- partial and multiple coherence of three series ------------------------------------------
+extern "C++" {
+template <typename T>
+static int wct3_run(cwtb_ctx *c, const double *y, const double *x1, const double *x2, int64_t n0, double dt,
+                    const double *scales, int n_scales, int family, double param, int boxcar_len,
+                    double *dRP2, double *dRM2) {
+  int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
+  if (e) return e;
+  if ((e = upload_series<T>(c, c->sig, y, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig2, x1, n0))) return e;
+  if ((e = upload_series<T>(c, c->sig3, x2, n0))) return e;
+  if ((e = upload_window(c, boxcar_len))) return e;
+  if ((e = upload_row_tables(c, c->job))) return e;
+  c->launches = 0;
+  if ((e = time_begin(c))) return e;
+  e = wct3_core<T>(c, c->job, (const T *)c->sig.p, (const T *)c->sig2.p, (const T *)c->sig3.p,
+                   boxcar_len, dRP2, dRM2);
+  c->w_moved = true;   // W holds a smoothed field now, not a transform
+  if (e) return e;
+  if ((e = time_end(c))) return e;
+  c->job_dsig = nullptr;
+  return 0;
+}
+}  // extern "C++"
+
+int cwtb_wct3(cwtb_ctx *c, const double *y, const double *x1, const double *x2, int64_t n0, double dt,
+              double dj, const double *scales, int n_scales, int family, double param, int boxcar_len,
+              double *RP2_out, double *RM2_out) {
+  (void)dj;
+  if (!c || !y || !x1 || !x2) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct3 needs an analytic wavelet family");
+  if (n0 < 1 || n_scales < 1) return fail(c, CWTB_ERR_ARG, "bad n0 / n_scales");
+  const size_t cnt = (size_t)n_scales * n0;
+  // outputs in aux: RP2, then RM2
+  int e = ensure(c, c->aux, 2 * cnt * sizeof(double));
+  if (e) return e;
+  double *dRP2 = RP2_out ? (double *)c->aux.p : nullptr, *dRM2 = RM2_out ? (double *)c->aux.p + cnt : nullptr;
+  e = c->coh_precision == CWTB_F32
+          ? wct3_run<float>(c, y, x1, x2, n0, dt, scales, n_scales, family, param, boxcar_len, dRP2, dRM2)
+          : wct3_run<double>(c, y, x1, x2, n0, dt, scales, n_scales, family, param, boxcar_len, dRP2, dRM2);
+  if (e) return e;
+  if (RP2_out) RT(rt_d2h(RP2_out, dRP2, cnt * sizeof(double), c->stream));
+  if (RM2_out) RT(rt_d2h(RM2_out, dRM2, cnt * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
   return 0;
 }
 

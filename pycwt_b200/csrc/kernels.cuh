@@ -1800,6 +1800,141 @@ template <typename T, int KMAX_> struct WctFinalBody {
   }
 };
 
+// ---- Body: partial / multiple coherence inputs of three series y, x1, x2 -------------------
+//   A  = (|Wy|^2 + i |W1|^2) / s,   B = |W2|^2 / s   (real autos packed as in WctPrepBody)
+//   Xy1 = Wy conj(W1) / s,   Xy2 = Wy conj(W2) / s,   X12 = W1 conj(W2) / s
+// Each point's three coefficients are read once; the crosses may be written over the transforms
+// (Xy1 over Wy, Xy2 over W1, X12 over W2): every thread reads its point before it writes it.
+template <typename T> struct Wct3PrepArgs {
+  const cx<T> *Wy, *W1, *W2;
+  const double *scale;   // per row
+  cx<T> *A, *B, *Xy1, *Xy2, *X12;
+  long long n;
+};
+template <typename T> struct Wct3PrepBody {
+  using Args = Wct3PrepArgs<T>;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long n = (long long)bx * NT + tid;
+    if (n >= a.n) return;
+    const size_t i = (size_t)by * a.n + n;
+    const cx<T> wy = a.Wy[i], w1 = a.W1[i], w2 = a.W2[i];
+    const T s = (T)a.scale[by];
+    const cx<T> y1 = cmul(wy, cconj(w1)), y2 = cmul(wy, cconj(w2)), x12 = cmul(w1, cconj(w2));
+    a.A[i] = mk<T>((wy.x * wy.x + wy.y * wy.y) / s, (w1.x * w1.x + w1.y * w1.y) / s);
+    a.B[i] = mk<T>((w2.x * w2.x + w2.y * w2.y) / s, (T)0);
+    a.Xy1[i] = mk<T>(y1.x / s, y1.y / s);
+    a.Xy2[i] = mk<T>(y2.x / s, y2.y / s);
+    a.X12[i] = mk<T>(x12.x / s, x12.y / s);
+  }
+};
+
+// ---- Body: scale boxcar of the five time-smoothed fields of Wct3PrepBody, then
+//   RP2 = |Sy1 S2 - Sy2 conj(S12)|^2 / ((Sy S2 - |Sy2|^2) (S1 S2 - |S12|^2))       (partial)
+//   RM2 = (S2 |Sy1|^2 + S1 |Sy2|^2 - 2 Re(Sy1 S12 conj(Sy2))) / (Sy (S1 S2 - |S12|^2))  (multiple)
+// The second is 1 - det G3 / (Sy (S1 S2 - |S12|^2)) with the 1 - x cancelled exactly.  No clamping:
+// a zero or negative denominator gives inf / NaN.  The fields are widened to double when they are
+// staged, and the boxcar sums and the combination run in double for every T: in fp32 the
+// differences above cancel badly, and the kernel is bound by its global reads, not by arithmetic.
+// Tile: RS output rows x CW columns; phase 0 stages the RS + K - 1 input rows of the five fields
+// for these columns, phase 1 gives each of the NT = (RS / RG) CW threads RG consecutive rows of
+// one column.
+template <typename T> struct Wct3FinalArgs {
+  const cx<T> *A, *B, *Xy1, *Xy2, *X12;   // time-smoothed fields
+  const double *win;
+  double *RP2, *RM2;                     // [rows][n], either may be null
+  long long n;
+  int rows, K;
+};
+template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
+  using Args = Wct3FinalArgs<T>;
+  using V = cx<T>;
+  static constexpr int NPHASE = 2;
+  static constexpr int NF = 5, RS = RS_, CW = CW_, KMAX = KMAX_, RG = 4;
+  static_assert((RS / RG) * CW == NT, "one task per thread");
+  static constexpr size_t PLANE = (size_t)(RS + KMAX - 1) * CW;   // double2 per staged field
+  static constexpr size_t SMEM = NF * PLANE * sizeof(double2) + KMAX * sizeof(double);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    const int K = a.K, off = (K - 1) / 2;
+    const int nrow = RS + K - 1;
+    double2 *st = (double2 *)smraw;                   // NF planes [nrow][CW]
+    double *sw = (double *)(st + NF * PLANE);
+    const int i0 = by * RS;
+    const long long n0 = (long long)bx * CW;
+    if (i0 >= a.rows) return;
+    const int qlo = i0 + off - K + 1;
+    if constexpr (PH == 0) {
+      const V *src[NF] = {a.A, a.B, a.Xy1, a.Xy2, a.X12};
+      for (int idx = tid; idx < nrow * CW; idx += NT) {
+        const int r = idx / CW, col = idx % CW;
+        const int q = qlo + r;
+        const long long n = n0 + col;
+        const bool in = q >= 0 && q < a.rows && n < a.n;
+        const size_t g = in ? (size_t)q * a.n + n : 0;
+#pragma unroll
+        for (int f = 0; f < NF; ++f) {
+          double2 v = mk<double>(0.0, 0.0);
+          if (in) {
+            const V x = src[f][g];
+            v = mk<double>((double)x.x, (double)x.y);
+          }
+          st[f * PLANE + idx] = v;
+        }
+      }
+      for (int t = tid; t < K; t += NT) sw[t] = a.win[t];
+    } else {
+      const int task = tid, col = task % CW, grp = task / CW;
+      const long long n = n0 + col;
+      if (n >= a.n) return;
+      double acc[NF][2][RG];
+#pragma unroll
+      for (int f = 0; f < NF; ++f)
+#pragma unroll
+        for (int e = 0; e < RG; ++e) acc[f][0][e] = acc[f][1][e] = 0.0;
+      // staged row u feeds output row i0 + RG grp + e with tap t = e + K - 1 - (u - RG grp)
+      for (int du = 0; du < K + RG - 1; ++du) {
+        const int u = RG * grp + du;
+        double2 v[NF];
+#pragma unroll
+        for (int f = 0; f < NF; ++f) v[f] = st[f * PLANE + u * CW + col];
+#pragma unroll
+        for (int e = 0; e < RG; ++e) {
+          const int t = e + K - 1 - du;
+          if (t >= 0 && t < K) {
+            const double w = sw[t];
+#pragma unroll
+            for (int f = 0; f < NF; ++f) {
+              acc[f][0][e] += w * v[f].x;
+              acc[f][1][e] += w * v[f].y;
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < RG; ++e) {
+        const int i = i0 + RG * grp + e;
+        if (i >= a.rows) break;
+        const double Sy = acc[0][0][e], S1 = acc[0][1][e], S2 = acc[1][0][e];
+        const double2 Sy1 = mk<double>(acc[2][0][e], acc[2][1][e]);
+        const double2 Sy2 = mk<double>(acc[3][0][e], acc[3][1][e]);
+        const double2 S12 = mk<double>(acc[4][0][e], acc[4][1][e]);
+        const double ny1 = Sy1.x * Sy1.x + Sy1.y * Sy1.y, ny2 = Sy2.x * Sy2.x + Sy2.y * Sy2.y;
+        const double d12 = S1 * S2 - (S12.x * S12.x + S12.y * S12.y);
+        const size_t o = (size_t)i * a.n + n;
+        if (a.RP2) {
+          const double2 u = csub(cscale(Sy1, S2), cmul(Sy2, cconj(S12)));
+          a.RP2[o] = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
+        }
+        if (a.RM2) {
+          const double2 z = cmul(cmul(Sy1, S12), cconj(Sy2));
+          a.RM2[o] = (S2 * ny1 + S1 * ny2 - 2.0 * z.x) / (Sy * d12);
+        }
+      }
+    }
+  }
+};
+
 // ---- Body: |W|^2 and its row means (SURVEY 8f: device-side derived products) ---------------
 template <typename T> struct PowerArgs {
   const cx<T> *W;

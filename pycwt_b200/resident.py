@@ -342,7 +342,7 @@ class ResidentCoherence(_ResidentSlot):
         self.s0 = p.s0
         self.J = p.J
         self.freq = p.freq
-        self._y = (np.array(p.y1, copy=True), np.array(p.y2, copy=True))   # raw series, for ar1
+        self._y = tuple(np.array(y, copy=True) for y in p.ys)   # raw series, for ar1
 
     def _threshold(self, sig95):
         if sig95 is None:
@@ -439,7 +439,7 @@ def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=T
 
     Returns a `ResidentCoherence`.  Scales, boxcar, un-padded fallback to fp64 and the Paul / DOG
     smoothing filter are resolved by the same code as `wct`'s."""
-    p = _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
+    p = _wct_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
     eng = engine or _engine.default_engine()
     serial = _wct_on_device(eng, p, eng.wct_resident)
     return ResidentCoherence(eng, p, precision, serial)

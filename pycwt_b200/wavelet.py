@@ -394,10 +394,11 @@ class _Problem(object):
         self.__dict__.update(kw)
 
 
-def _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
-    """What `wct` resolves on the host before the device pipeline (reference wavelet.py:461-497):
-    the wavelet, s0 and J, the raw and standardised series, the scales, the boxcar length and the
-    requested engine precision."""
+def _wct_problem(series, dt, dj, s0, J, wavelet, normalize, precision):
+    """What `wct` (two series) and `partial_wct` / `multiple_wct` (three) resolve on the host before
+    the device pipeline (reference wavelet.py:461-497): the wavelet, s0 and J, the raw and
+    standardised series (`ys`, `yns`), the scales, the boxcar length and the requested engine
+    precision."""
     prec = _coherence_precision(precision)
     wavelet = _check_parameter_wavelet(wavelet)
     if not hasattr(wavelet, 'smooth'):
@@ -407,28 +408,28 @@ def _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision):
     if s0 == -1:
         s0 = 2 * dt / wavelet.flambda()
     if J == -1:
-        J = int(np.round(np.log2(y1.size * dt / s0) / dj))  # y1.size: ndarray required, as in the reference
-    y1, y1n, _ = _standardise(y1, normalize)
-    y2, y2n, _ = _standardise(y2, normalize)
-    n0 = y1n.size
+        J = int(np.round(np.log2(series[0].size * dt / s0) / dj))  # .size: ndarray required, as in the reference
+    ys, yns = zip(*[_standardise(y, normalize)[:2] for y in series])
+    n0 = yns[0].size
     sj, freq = _resolve_scales(n0, dt, dj, s0, J, wavelet, None)
     klen = _boxcar_len(wavelet, dj)
     if klen < 1:
         raise ValueError('smoothing window undefined for this wavelet (deltaj0 = -1)')
-    return _Problem(y1=y1, y2=y2, y1n=y1n, y2n=y2n, n0=n0, dt=dt, dj=dj, s0=s0, J=J,
+    return _Problem(ys=ys, yns=yns, n0=n0, dt=dt, dj=dj, s0=s0, J=J,
                     wavelet=wavelet, sj=sj, freq=freq, klen=klen, prec=prec)
 
 
-def _wct_on_device(eng, p, call):
+def _wct_on_device(eng, p, call, **kw):
     """One engine transaction of the coherence pipeline: length policy (un-padded transforms run
-    in fp64), the Paul / DOG smoothing filter, then call(y1n, y2n, dt, dj, scales, family, param,
-    boxcar_len=, precision=).  Returns the call's result; `p.prec` becomes the precision used."""
+    in fp64), the Paul / DOG smoothing filter, then call(*yns, dt, dj, scales, family, param,
+    boxcar_len=, precision=, **kw).  Returns the call's result; `p.prec` becomes the precision
+    used."""
     with eng.lock:
-        if _sync_padding(eng, len(p.y1n)):
+        if _sync_padding(eng, len(p.yns[0])):
             p.prec = _engine.F64      # un-padded transforms run in fp64
-        with _smoothing_filter(eng, p.wavelet, p.sj, p.dt, len(p.y1n)):
-            return call(p.y1n, p.y2n, p.dt, p.dj, p.sj, *_family_of(p.wavelet), boxcar_len=p.klen,
-                        precision=p.prec)
+        with _smoothing_filter(eng, p.wavelet, p.sj, p.dt, len(p.yns[0])):
+            return call(*p.yns, p.dt, p.dj, p.sj, *_family_of(p.wavelet), boxcar_len=p.klen,
+                        precision=p.prec, **kw)
 
 
 def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
@@ -442,8 +443,8 @@ def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
     `precision` (an extension of the reference signature): 'fp64' (default) or 'fp32', the
     arithmetic of the device pipeline, also that of the significance test; WCT and aWCT are
     float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6)."""
-    p = _wct_problem(y1, y2, dt, dj, s0, J, wavelet, normalize, precision)
-    y1, y2, wavelet, s0, J, freq = p.y1, p.y2, p.wavelet, p.s0, p.J, p.freq
+    p = _wct_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
+    (y1, y2), wavelet, s0, J, freq = p.ys, p.wavelet, p.s0, p.J, p.freq
     eng = _engine.default_engine()
     WCT, aWCT = _wct_on_device(eng, p, eng.wct)
     coi = _coi(wavelet, dt, p.n0)
@@ -456,6 +457,46 @@ def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
     else:
         sig = np.asarray([0])
     return WCT, aWCT, coi, freq, sig
+
+
+def partial_wct(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
+                precision='fp64'):
+    """Partial wavelet coherence of `y` with `x1` once `x2` is accounted for (Mihanovic et al.
+    2009; Ng & Chan 2012).  An extension: the reference has no three-series coherence.
+
+    With S the smoothing operator of `wct`, S_a = S(|W_a|^2 / s), S_ab = S(W_a conj(W_b) / s):
+        RP2 = |S_y1 S_2 - S_y2 S_21|^2 / ((S_y S_2 - |S_y2|^2) (S_1 S_2 - |S_12|^2))
+            = |g_y1 - g_y2 g_21|^2 / ((1 - R2_y2) (1 - R2_12)),   g_ab = S_ab / sqrt(S_a S_b).
+    Returns (RP2, coi, freq); RP2 is float64 [S, n0] in either `precision` ('fp64' default, or
+    'fp32': the arithmetic of the transforms and smoothing; the smoothed fields are combined in
+    double either way).  Scales, boxcar, un-padded fallback to fp64 and the Paul / DOG smoothing
+    filter are resolved as in `wct`, with the same errors.  RP2 lies in [0, 1] up to rounding and
+    is not clamped: where a denominator is zero or rounds to <= 0 it is inf or NaN.  Where x1 and
+    x2 are nearly coherent (R2_12 -> 1) the measure is ill-conditioned: its rounding error grows
+    like 1 / ((1 - R2_y2) (1 - R2_12)).  No significance test."""
+    return _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial=True)
+
+
+def multiple_wct(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
+                 precision='fp64'):
+    """Multiple wavelet coherence: how much of `y` the series `x1` and `x2` explain together
+    (Ng & Chan 2012).  An extension: the reference has no three-series coherence.
+
+    With the smoothed fields of `partial_wct`:
+        RM2 = (R2_y1 + R2_y2 - 2 Re(g_y1 g_12 g_2y)) / (1 - R2_12)
+            = 1 - det G3 / (S_y (S_1 S_2 - |S_12|^2)),   G3 the 3 x 3 smoothed spectral matrix.
+    Returns (RM2, coi, freq), RM2 float64 [S, n0]; `precision`, scales, errors and the absence of
+    clamping as in `partial_wct`.  RM2 >= max(R2_y1, R2_y2) up to rounding, and
+    1 - RM2 = (1 - R2_y2) (1 - RP2).  Ill-conditioned where x1 and x2 are nearly coherent: the
+    rounding error grows like 1 / (1 - R2_12).  No significance test."""
+    return _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial=False)
+
+
+def _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial):
+    p = _wct_problem((y, x1, x2), dt, dj, s0, J, wavelet, normalize, precision)
+    eng = _engine.default_engine()
+    RP2, RM2 = _wct_on_device(eng, p, eng.wct3, want_partial=partial, want_multiple=not partial)
+    return (RP2 if partial else RM2), _coi(p.wavelet, dt, p.n0), p.freq
 
 
 def _mc_problem(dt, dj, s0, J, wavelet):
