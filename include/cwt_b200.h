@@ -312,6 +312,32 @@ int cwtb_wct_mc_seeded(cwtb_ctx *ctx, uint64_t seed, int64_t first_pair, int n_p
 int cwtb_mc_surrogates(cwtb_ctx *ctx, uint64_t seed, int64_t first_pair, int n_pairs, int64_t n0,
                        double *out);
 
+/* ---- Monte-Carlo significance of the partial and multiple coherence (cwtb_wct3) ------------- */
+/* Null: three mutually independent white-noise series of n0 samples per triple, not standardised,
+ * each triple through the whole cwtb_wct3 pipeline (same smoothing, boxcar, time filter table).
+ * Accumulates, over `n_triples` triples, hist_partial[s, b] += 1 for RP2 and hist_multiple[s, b] += 1
+ * for RM2 with b = clamp(floor(R2*nbins), 0, nbins-1), for rows s < maxscale and points with
+ * mask[s, n] != 0; a non-finite R2 (a zero denominator) is not counted.  Either histogram may be
+ * NULL (its measure is then not evaluated), not both; each is n_scales x nbins int64, accumulated
+ * into (not cleared).  `noise`: host array [n_triples][3][n0] of doubles (y, x1, x2 of each triple).
+ * Precision, errors and lifetime as cwtb_wct3: the resident coherence and cross spectrum survive
+ * the call; afterwards no transform is resident. */
+int cwtb_wct3_mc(cwtb_ctx *ctx, const double *noise, int n_triples, int64_t n0, double dt,
+                 const double *scales, int n_scales, int family, double param, int boxcar_len,
+                 const uint8_t *mask, int maxscale, int nbins, int64_t *hist_partial,
+                 int64_t *hist_multiple);
+/* The same with the triples drawn on the device: series r (0 = y, 1 = x1, 2 = x2) of triple
+ * first_triple + i is a pure function of (seed, triple number, r), from the Philox4x32-10 stream of
+ * cwtb_wct_mc_seeded with a tag bit of its own, so triple t and pair t of one seed share no series
+ * and no split over calls, ranks or GPUs changes a triple. */
+int cwtb_wct3_mc_seeded(cwtb_ctx *ctx, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0,
+                        double dt, const double *scales, int n_scales, int family, double param,
+                        int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                        int64_t *hist_partial, int64_t *hist_multiple);
+/* Test hook: the triples of the seeded mode, out[n_triples][3][n0]. */
+int cwtb_mc_surrogates3(cwtb_ctx *ctx, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0,
+                        double *out);
+
 /* ---- batched transform of independent channels (SURVEY 8d config 5) ------- */
 /* X: host [n_chan, n0] (float or double).  The per-channel transforms stay on
  * the device; `power_out` (may be NULL) receives the per-channel global wavelet

@@ -14,8 +14,19 @@ grouped into the three transforms, Wct3PrepBody, the five smoothing passes and W
 gives the final kernel's HBM rate from the bytes it must move (five fields read once, one float64
 output written) against the data sheet's 3.35 TB/s.  The results of the paths are compared at the
 timed size.  The card's name, power limit and maximum SM clock go into the output, with the SM
-clock read right after the timed loop.  Needs a GPU: without one it fails.  The summary goes to
-stdout; `--out FILE` also writes the full record as JSON.
+clock read right after the timed loop.
+
+Monte-Carlo leg, at config 4's Monte-Carlo geometry (surrogates of 49152 samples padded to 65536,
+145 scales, K = 14): per precision, `--mc-count` triples of `wct3_significance` in seeded and in
+host-RNG mode, alternating with as many pairs of the two-series `wct_significance` in the same two
+modes, `--mc-reps` times; call time and the device time of the engine's Monte-Carlo call.  Then the
+per-kernel device times of one seeded triple (noise, three transforms, prep, five smoothings, the
+final kernel with both histograms), and the final kernel of the output path (`Engine.wct3` with both
+outputs) at the same geometry, per row, to show what the histograms' atomics cost against the
+stores of the output path.
+
+Needs a GPU: without one it fails.  The summary goes to stdout; `--out FILE` also writes the full
+record as JSON.
 
     python profiles/partial_coherence.py --out /tmp/partial_coherence.json
 """
@@ -83,9 +94,73 @@ def kernel_groups(rec, S, n0, esize):
             "sum_ms": ms(rec), "launches": len(rec)}
 
 
+def mc_groups(rec):
+    """Device ms of one Monte-Carlo triple by stage; the final kernel's ms per output row."""
+    names = [r["name"] for r in rec]
+    ms = lambda rs: float(sum(r["ms"] for r in rs))        # noqa: E731
+    ip = next(i for i, s in enumerate(names) if s.startswith("Wct3PrepBody"))
+    iF = next(i for i, s in enumerate(names) if s.startswith("Wct3FinalBody"))
+    noise = [r for r in rec[:ip] if r["name"].startswith("NoiseBody")]
+    return {"noise_ms": ms(noise), "transforms_ms": ms(rec[:ip]) - ms(noise), "prep_ms": ms(rec[ip:ip + 1]),
+            "smoothing_ms": ms(rec[ip + 1:iF]), "final_ms": ms(rec[iF:iF + 1]), "final_name": names[iF],
+            "final_rows": int(rec[iF].get("rows", 0)), "sum_ms": ms(rec), "launches": len(rec)}
+
+
+def mc_leg(eng, count, reps, res):
+    from pycwt_b200 import wavelet as wv
+    c4 = workloads.C4
+    dt, dj, s0, J = c4["dt"], c4["dj"], c4["s0"], c4["J"]
+    mother = pycwt.Morlet(6)
+    prob = wv._mc_problem(dt, dj, s0, J, mother)
+    res["mc"] = {"config": {"N": prob["N"], "scales": int(prob["sj"].size), "maxscale": prob["maxscale"],
+                            "count": count}, "timing": {}, "kernels": {}}
+    for p in ("fp64", "fp32"):
+        paths = {
+            "triples_seeded": lambda s: pycwt.wct3_significance(0.3, 0.5, 0.2, dt, dj, s0, J, mc_count=count,
+                                                                progress=False, seed=s, precision=p),
+            "triples_host": lambda s: pycwt.wct3_significance(0.3, 0.5, 0.2, dt, dj, s0, J, mc_count=count,
+                                                              progress=False, precision=p),
+            "pairs_seeded": lambda s: wv._wct_significance(0.3, 0.5, dt, dj, s0, J, mc_count=count, progress=False,
+                                                           cache=False, seed=s, precision=p),
+            "pairs_host": lambda s: wv._wct_significance(0.3, 0.5, dt, dj, s0, J, mc_count=count, progress=False,
+                                                         cache=False, precision=p),
+        }
+        for f in paths.values():                          # warm-up
+            f(1)
+        t = {}
+        for rep in range(reps):
+            np.random.seed(rep)
+            for k, f in paths.items():
+                t0 = time.perf_counter()
+                f(100 + rep)
+                t.setdefault(k + "_call_s", []).append(time.perf_counter() - t0)
+                t.setdefault(k + "_device_s", []).append(eng.last_kernel_ms() * 1e-3)
+        res["mc"]["timing"][p] = {k: stats(v) for k, v in t.items()}
+        res["mc"]["timing"][p]["sm_clock_after"] = sm_clock()
+        print("mc", p, json.dumps({k: round(v["median"], 4) for k, v in res["mc"]["timing"][p].items()
+                                   if isinstance(v, dict)}), flush=True)
+
+        eng.profile_begin()
+        pycwt.wct3_significance(0.3, 0.5, 0.2, dt, dj, s0, J, mc_count=1, progress=False, seed=7, precision=p)
+        mc = mc_groups(eng.profile_end())
+        # the output path's final kernel at the same geometry (both outputs), for its per-row cost
+        noise = eng.mc_surrogates3(7, 0, 1, prob["N"])[0]
+        eng.profile_begin()
+        eng.wct3(*noise, dt, dj, prob["sj"], _engine.MORLET, 6.0, 14, precision=_engine.F64 if p == "fp64" else _engine.F32)
+        out = mc_groups(eng.profile_end())
+        res["mc"]["kernels"][p] = {"mc_triple": mc, "output_path": out,
+                                   "final_ms_per_row_mc": mc["final_ms"] / prob["maxscale"],
+                                   "final_ms_per_row_output": out["final_ms"] / prob["sj"].size}
+        print("mc", p, "kernels", json.dumps({k: (round(v, 5) if isinstance(v, float) else v)
+                                              for k, v in res["mc"]["kernels"][p].items()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--mc-count", type=int, default=200, help="triples (and pairs) per Monte-Carlo call")
+    ap.add_argument("--mc-reps", type=int, default=3)
+    ap.add_argument("--mc-only", action="store_true", help="only the Monte-Carlo leg")
     ap.add_argument("--out", default=None, help="JSON file for the full record (default: stdout only)")
     args = ap.parse_args()
     if _engine.device_count() <= 0:
@@ -98,7 +173,7 @@ def main():
     res = {"card": card(), "config": {"n": int(n0), "scales": S, "boxcar": 14}, "timing": {},
            "kernels": {}, "checks": {}}
     out64 = {}
-    for p in ("fp64", "fp32"):
+    for p in (() if args.mc_only else ("fp64", "fp32")):
         paths = {
             "multiple": lambda: pycwt.multiple_wct(y, x1, x2, DT, precision=p, **kw)[0],
             "partial": lambda: pycwt.partial_wct(y, x1, x2, DT, precision=p, **kw)[0],
@@ -139,6 +214,8 @@ def main():
             (np.abs((1 - outs["multiple"])
                     - (1 - pycwt.wct(y, x2, DT, sig=False, precision=p, **kw)[0]) * (1 - outs["partial"])) * D12).max())
     print("checks", json.dumps(res["checks"]), flush=True)
+    if args.mc_count > 0:
+        mc_leg(eng, args.mc_count, args.mc_reps, res)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as f:

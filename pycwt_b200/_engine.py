@@ -87,6 +87,10 @@ _SIGNATURES = {
     "cwtb_wct_mc": (_I, [_P, _P, _I, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
     "cwtb_wct_mc_seeded": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
     "cwtb_mc_surrogates": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_wct3_mc": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P, _P]),
+    "cwtb_wct3_mc_seeded": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I,
+                                 _P, _P]),
+    "cwtb_mc_surrogates3": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -744,6 +748,63 @@ class Engine(object):
         out = np.empty((int(n_pairs), 2, int(n0)), dtype=np.float64)
         self._check(self.lib.cwtb_mc_surrogates(self.h, int(seed) & (2 ** 64 - 1), int(first_pair),
                                                 int(n_pairs), int(n0), _ptr(out)))
+        return out
+
+    @staticmethod
+    def _mc3_hists(name, S, nbins, hist_partial, hist_multiple):
+        """The two histograms of a three-series Monte-Carlo call, checked; at least one given."""
+        if hist_partial is None and hist_multiple is None:
+            raise ValueError("%s: no histogram given" % name)
+        for h in (hist_partial, hist_multiple):
+            if h is not None and not (h.dtype == np.int64 and h.flags.c_contiguous and h.shape == (S, nbins)):
+                raise ValueError("%s: histograms must be C-contiguous int64 [%d, %d]" % (name, S, nbins))
+        return [None if h is None else _ptr(h) for h in (hist_partial, hist_multiple)]
+
+    @_locked
+    def wct3_mc(self, noise, dt, scales, family, param, boxcar_len, mask, maxscale, nbins,
+                hist_partial, hist_multiple, precision=F64):
+        """Monte-Carlo histograms of the partial (RP2) and multiple (RM2) coherence of the
+        surrogate triples noise[n_triples, 3, n0] (y, x1, x2), accumulated into the given
+        histograms [S, nbins] (either may be None)."""
+        noise = np.ascontiguousarray(noise, dtype=np.float64)
+        if noise.ndim != 3 or noise.shape[1] != 3:
+            raise ValueError("wct3_mc: surrogates must be [triples, 3, n0]")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        if mask.shape != (sj.size, noise.shape[2]):
+            raise ValueError("wct3_mc: mask must be [scales, n0]")
+        hp, hm = self._mc3_hists("wct3_mc", sj.size, nbins, hist_partial, hist_multiple)
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct3_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2], float(dt),
+                                          _ptr(sj), sj.size, int(family), float(param), int(boxcar_len),
+                                          _ptr(mask), int(maxscale), int(nbins), hp, hm))
+        return hist_partial, hist_multiple
+
+    @_locked
+    def wct3_mc_seeded(self, seed, first_triple, n_triples, n0, dt, scales, family, param, boxcar_len,
+                       mask, maxscale, nbins, hist_partial, hist_multiple, precision=F64):
+        """`wct3_mc` with the triples drawn on the device (Philox stream keyed by (seed, triple
+        number), disjoint from the pairs of `wct_mc_seeded`)."""
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        if mask.shape != (sj.size, int(n0)):
+            raise ValueError("wct3_mc_seeded: mask must be [scales, n0]")
+        hp, hm = self._mc3_hists("wct3_mc_seeded", sj.size, nbins, hist_partial, hist_multiple)
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct3_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_triple),
+                                                 int(n_triples), int(n0), float(dt), _ptr(sj), sj.size,
+                                                 int(family), float(param), int(boxcar_len), _ptr(mask),
+                                                 int(maxscale), int(nbins), hp, hm))
+        return hist_partial, hist_multiple
+
+    @_locked
+    def mc_surrogates3(self, seed, first_triple, n_triples, n0):
+        """The triples of the seeded mode, float64 [n_triples, 3, n0]."""
+        out = np.empty((int(n_triples), 3, int(n0)), dtype=np.float64)
+        self._check(self.lib.cwtb_mc_surrogates3(self.h, int(seed) & (2 ** 64 - 1), int(first_triple),
+                                                 int(n_triples), int(n0), _ptr(out)))
         return out
 
     @_locked

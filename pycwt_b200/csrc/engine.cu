@@ -2643,12 +2643,14 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
 }
 
 // three transforms + partial / multiple coherence in the engine type T; outputs are device
-// pointers (either may be null) and double for every T.  Device memory per scale-point: the three
-// transforms W, W2, W3 (the crosses are written over them), the two auto fields C, A12 and the
-// smoothing buffer F.
+// pointers (either may be null) and double for every T.  With both outputs null (Monte-Carlo mode)
+// only the rows below maxscale are finished, into the histograms dhP / dhM (either may be null).
+// Device memory per scale-point: the three transforms W, W2, W3 (the crosses are written over
+// them), the two auto fields C, A12 and the smoothing buffer F.
 template <typename T>
 static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, const T *dx2, int K,
-                     double *dRP2, double *dRM2) {
+                     double *dRP2, double *dRM2, const unsigned char *dmask = nullptr, int maxscale = 0,
+                     int nbins = 0, unsigned long long *dhP = nullptr, unsigned long long *dhM = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2668,6 +2670,8 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
   if ((e = launch<Wct3PrepBody<T>>(c, gx, S, pa))) return e;
   for (V *x : f)
     if ((e = smooth_time<T>(c, x, S, n0, job.N, d_g))) return e;
+  const int rows_out = dRP2 || dRM2 ? S : maxscale;
+  if (rows_out <= 0) return 0;
   const double *win = (const double *)c->win.p;
   if (K > 64) {
     // longer than the fused kernel stages: the scale boxcar of each field into the buffer the
@@ -2676,18 +2680,18 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
     V *dst = (V *)c->F.p;
     for (V *&x : f) {
       BoxcarArgs<T> b{x, dst, win, n0, S, K};
-      if ((e = launch<BoxcarBody<T>>(c, gx, S, b))) return e;
+      if ((e = launch<BoxcarBody<T>>(c, gx, rows_out, b))) return e;
       std::swap(x, dst);
     }
     win += K;
     K = 1;
   }
-  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, n0, S, K};
+  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dmask, dhP, dhM, n0, S, K, maxscale, nbins};
   using F16 = Wct3FinalBody<T, 16, 32, 16>;
   using F64K = Wct3FinalBody<T, 64, 64, 8>;
   if (K <= 16)
-    return launch<F16>(c, (unsigned)((n0 + F16::CW - 1) / F16::CW), (unsigned)((S + F16::RS - 1) / F16::RS), fa);
-  return launch<F64K>(c, (unsigned)((n0 + F64K::CW - 1) / F64K::CW), (unsigned)((S + F64K::RS - 1) / F64K::RS), fa);
+    return launch<F16>(c, (unsigned)((n0 + F16::CW - 1) / F16::CW), (unsigned)((rows_out + F16::RS - 1) / F16::RS), fa);
+  return launch<F64K>(c, (unsigned)((n0 + F64K::CW - 1) / F64K::CW), (unsigned)((rows_out + F64K::RS - 1) / F64K::RS), fa);
 }
 
 // the engine precision of T, and host series (double) as device series of type T: the fp32
@@ -3411,13 +3415,16 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
   return 0;
 }
 
-// common part of the two Monte-Carlo entry points: `noise` host surrogates [n_pairs][2][n0], or
-// null -> drawn on the device from (seed, pair0 + i); coherence in the engine type T
+// common part of the Monte-Carlo entry points, for surrogate units of nser = 2 series (coherence,
+// one histogram) or 3 (partial and multiple coherence, hist[0] and hist[1], either may be null):
+// `noise` host surrogates [n_units][nser][n0], or null -> drawn on the device from
+// (seed, unit0 + i); coherence in the engine type T
 extern "C++" {
 template <typename T>
-static int wct_mc_run(cwtb_ctx *c, const double *noise, unsigned long long seed, long long pair0, int n_pairs,
-                      int64_t n0, double dt, const double *scales, int n_scales, int family, double param,
-                      int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
+static int mc_run(cwtb_ctx *c, int nser, const double *noise, unsigned long long seed, long long unit0,
+                  int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                  double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                  int64_t *const hist[2]) {
   int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_window(c, boxcar_len))) return e;
@@ -3425,61 +3432,75 @@ static int wct_mc_run(cwtb_ctx *c, const double *noise, unsigned long long seed,
   const size_t cnt = (size_t)n_scales * n0;
   if ((e = ensure(c, c->mask, cnt))) return e;
   RT(rt_h2d(c->mask.p, mask, cnt, c->stream));
+  const int nh = nser == 2 ? 1 : 2;                 // histograms: one per measure
   const size_t hb = (size_t)n_scales * nbins * sizeof(unsigned long long);
-  if ((e = ensure(c, c->hist, hb))) return e;
-  RT(rt_memset(c->hist.p, 0, hb, c->stream));
-  // surrogates of at most `batch` pairs are resident at a time
-  // (host surrogates stay double on the device; an fp32 run rounds one pair at a time into sig)
-  const int batch = noise ? n_pairs : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_pairs, ((size_t)256 << 20) / ((size_t)2 * n0 * sizeof(double))));
+  if ((e = ensure(c, c->hist, nh * hb))) return e;
+  RT(rt_memset(c->hist.p, 0, nh * hb, c->stream));
+  unsigned long long *dh[2] = {nullptr, nullptr};
+  for (int k = 0; k < nh; ++k)
+    if (hist[k]) dh[k] = (unsigned long long *)c->hist.p + (size_t)k * n_scales * nbins;
+  // surrogates of at most `batch` units are resident at a time
+  // (host surrogates stay double on the device; an fp32 run rounds one unit at a time into sig)
+  const size_t usz = (size_t)nser * n0;             // samples per unit
+  const int batch = noise ? n_units : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_units, ((size_t)256 << 20) / (usz * sizeof(double))));
   const size_t nsz = noise ? sizeof(double) : sizeof(T);
-  if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * 2 * n0 * nsz))) return e;
-  if (noise) RT(rt_h2d(c->noise.p, noise, (size_t)n_pairs * 2 * n0 * sizeof(double), c->stream));
-  if (noise && sizeof(T) != 8 && (e = ensure(c, c->sig, (size_t)2 * n0 * sizeof(T)))) return e;
+  if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * usz * nsz))) return e;
+  if (noise) RT(rt_h2d(c->noise.p, noise, (size_t)n_units * usz * sizeof(double), c->stream));
+  if (noise && sizeof(T) != 8 && (e = ensure(c, c->sig, usz * sizeof(T)))) return e;
   RT(rt_sync(c->stream));
   c->launches = 0;
   if ((e = time_begin(c))) return e;
-  for (int i0 = 0; i0 < n_pairs; i0 += batch) {
-    const int nb = std::min(batch, n_pairs - i0);
+  for (int i0 = 0; i0 < n_units; i0 += batch) {
+    const int nb = std::min(batch, n_units - i0);
     if (!noise) {
-      NoiseArgs<T> na{(T *)c->noise.p, seed, pair0 + i0, (long long)n0, nb};
-      if ((e = launch<NoiseBody<T>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * nb), na))) return e;
+      NoiseArgs<T> na{(T *)c->noise.p, seed, unit0 + i0, (long long)n0, nb, nser};
+      if ((e = launch<NoiseBody<T>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * nb), na))) return e;
     }
     for (int i = 0; i < nb; ++i) {
       const T *a;
       if constexpr (sizeof(T) == 8) {
-        a = (const T *)c->noise.p + (size_t)i * 2 * n0;
+        a = (const T *)c->noise.p + (size_t)i * usz;
       } else if (noise) {
-        if ((e = to_f32(c, (const double *)c->noise.p + (size_t)i * 2 * n0, (float *)c->sig.p, 2 * n0))) return e;
+        if ((e = to_f32(c, (const double *)c->noise.p + (size_t)i * usz, (float *)c->sig.p, (long long)usz))) return e;
         a = (const T *)c->sig.p;
       } else {
-        a = (const T *)c->noise.p + (size_t)i * 2 * n0;
+        a = (const T *)c->noise.p + (size_t)i * usz;
       }
-      if ((e = wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, (const unsigned char *)c->mask.p,
-                           maxscale, nbins, (unsigned long long *)c->hist.p)))
-        return e;
+      const unsigned char *dmask = (const unsigned char *)c->mask.p;
+      e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0])
+                    : wct3_core<T>(c, c->job, a, a + n0, a + 2 * n0, boxcar_len, nullptr, nullptr, dmask, maxscale,
+                                   nbins, dh[0], dh[1]);
+      if (nser == 3) c->w_moved = true;   // W holds a smoothed field now, not a transform
+      if (e) return e;
     }
   }
   if ((e = time_end(c))) return e;
   c->job_dsig = nullptr;
   std::vector<unsigned long long> h((size_t)n_scales * nbins);
-  RT(rt_d2h(h.data(), c->hist.p, hb, c->stream));
-  RT(rt_sync(c->stream));
-  for (size_t i = 0; i < h.size(); ++i) hist[i] += (int64_t)h[i];
+  for (int k = 0; k < nh; ++k) {
+    if (!hist[k]) continue;
+    RT(rt_d2h(h.data(), dh[k], hb, c->stream));
+    RT(rt_sync(c->stream));
+    for (size_t i = 0; i < h.size(); ++i) hist[k][i] += (int64_t)h[i];
+  }
   return 0;
 }
 }  // extern "C++"
 
-static int wct_mc_core(cwtb_ctx *c, const double *noise, unsigned long long seed, long long pair0, int n_pairs,
-                       int64_t n0, double dt, const double *scales, int n_scales, int family, double param,
-                       int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
-  if (!c || !mask || !hist || n_pairs < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
-    return fail(c, CWTB_ERR_ARG, "wct_mc: bad argument");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc needs an analytic wavelet family");
+static int mc_core(cwtb_ctx *c, int nser, const double *noise, unsigned long long seed, long long unit0,
+                   int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                   double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                   int64_t *const hist[2]) {
+  if (!c || !mask || !(hist[0] || hist[1]) || n_units < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
+    return fail(c, CWTB_ERR_ARG, nser == 2 ? "wct_mc: bad argument" : "wct3_mc: bad argument");
+  if (family == CWTB_TABLE)
+    return fail(c, CWTB_ERR_UNSUPPORTED, nser == 2 ? "wct_mc needs an analytic wavelet family"
+                                                   : "wct3_mc needs an analytic wavelet family");
   return c->coh_precision == CWTB_F32
-             ? wct_mc_run<float>(c, noise, seed, pair0, n_pairs, n0, dt, scales, n_scales, family, param,
-                                 boxcar_len, mask, maxscale, nbins, hist)
-             : wct_mc_run<double>(c, noise, seed, pair0, n_pairs, n0, dt, scales, n_scales, family, param,
-                                  boxcar_len, mask, maxscale, nbins, hist);
+             ? mc_run<float>(c, nser, noise, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+                             boxcar_len, mask, maxscale, nbins, hist)
+             : mc_run<double>(c, nser, noise, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+                              boxcar_len, mask, maxscale, nbins, hist);
 }
 
 int cwtb_wct_mc(cwtb_ctx *c, const double *noise, int n_pairs, int64_t n0, double dt, double dj,
@@ -3487,27 +3508,56 @@ int cwtb_wct_mc(cwtb_ctx *c, const double *noise, int n_pairs, int64_t n0, doubl
                 const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
   (void)dj;
   if (!noise) return fail(c, CWTB_ERR_ARG, "wct_mc: null surrogates");
-  return wct_mc_core(c, noise, 0, 0, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
-                     maxscale, nbins, hist);
+  int64_t *const h[2] = {hist, nullptr};
+  return mc_core(c, 2, noise, 0, 0, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
+                 maxscale, nbins, h);
 }
 
 int cwtb_wct_mc_seeded(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pairs, int64_t n0, double dt,
                        const double *scales, int n_scales, int family, double param, int boxcar_len,
                        const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
-  return wct_mc_core(c, nullptr, seed, first_pair, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len,
-                     mask, maxscale, nbins, hist);
+  int64_t *const h[2] = {hist, nullptr};
+  return mc_core(c, 2, nullptr, seed, first_pair, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len,
+                 mask, maxscale, nbins, h);
 }
 
-// test hook: the surrogates of the seeded mode, [n_pairs][2][n0] to the host
-int cwtb_mc_surrogates(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pairs, int64_t n0, double *out) {
-  if (!c || !out || n_pairs < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, "mc_surrogates: bad argument");
-  int e = ensure(c, c->noise, (size_t)n_pairs * 2 * n0 * sizeof(double));
+int cwtb_wct3_mc(cwtb_ctx *c, const double *noise, int n_triples, int64_t n0, double dt, const double *scales,
+                 int n_scales, int family, double param, int boxcar_len, const uint8_t *mask, int maxscale,
+                 int nbins, int64_t *hist_partial, int64_t *hist_multiple) {
+  if (!noise) return fail(c, CWTB_ERR_ARG, "wct3_mc: null surrogates");
+  int64_t *const h[2] = {hist_partial, hist_multiple};
+  return mc_core(c, 3, noise, 0, 0, n_triples, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
+                 maxscale, nbins, h);
+}
+
+int cwtb_wct3_mc_seeded(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0, double dt,
+                        const double *scales, int n_scales, int family, double param, int boxcar_len,
+                        const uint8_t *mask, int maxscale, int nbins, int64_t *hist_partial,
+                        int64_t *hist_multiple) {
+  int64_t *const h[2] = {hist_partial, hist_multiple};
+  return mc_core(c, 3, nullptr, seed, first_triple, n_triples, n0, dt, scales, n_scales, family, param,
+                 boxcar_len, mask, maxscale, nbins, h);
+}
+
+// test hooks: the surrogates of the seeded mode, [n_units][nser][n0] to the host
+static int mc_surrogates(cwtb_ctx *c, int nser, uint64_t seed, int64_t unit0, int n_units, int64_t n0, double *out) {
+  if (!c || !out || n_units < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, "mc_surrogates: bad argument");
+  const size_t bytes = (size_t)n_units * nser * n0 * sizeof(double);
+  int e = ensure(c, c->noise, bytes);
   if (e) return e;
-  NoiseArgs<double> na{(double *)c->noise.p, seed, first_pair, (long long)n0, n_pairs};
-  if ((e = launch<NoiseBody<double>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(2 * n_pairs), na))) return e;
-  RT(rt_d2h(out, c->noise.p, (size_t)n_pairs * 2 * n0 * sizeof(double), c->stream));
+  NoiseArgs<double> na{(double *)c->noise.p, seed, unit0, (long long)n0, n_units, nser};
+  if ((e = launch<NoiseBody<double>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * n_units), na))) return e;
+  RT(rt_d2h(out, c->noise.p, bytes, c->stream));
   RT(rt_sync(c->stream));
   return 0;
+}
+
+int cwtb_mc_surrogates(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pairs, int64_t n0, double *out) {
+  return mc_surrogates(c, 2, seed, first_pair, n_pairs, n0, out);
+}
+
+int cwtb_mc_surrogates3(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0, double *out) {
+  return mc_surrogates(c, 3, seed, first_triple, n_triples, n0, out);
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

@@ -1630,18 +1630,23 @@ template <typename T> struct WctPrepBody {
 
 // ---- Body: white-noise surrogates on the device (seeded mode of the Monte-Carlo significance) ----
 // Counter-based Philox4x32-10 (Salmon et al. 2011): sample pair (2j, 2j+1) of series `ser` of
-// surrogate pair `pair` is a pure function of (seed, pair, ser, j) -- independent of the launch
-// geometry, of the rank that draws it and of how the pairs are batched.  Two 53-bit uniforms ->
+// surrogate unit `unit` (a pair of the coherence test, a triple of the partial / multiple
+// coherence test) is a pure function of (seed, unit, ser, j) -- independent of the launch
+// geometry, of the rank that draws it and of how the units are batched.  Two 53-bit uniforms ->
 // two standard normals (Box-Muller).  The reference's surrogates are white noise as well
 // (helpers.py:146-173 filters a length-1 axis, SURVEY 8a row 10); this mode reproduces their
 // distribution, not numpy's bit stream (the host-RNG mode does that).  The draw is in double for
 // every T: the fp32 surrogates are the fp64 ones rounded.
+// Counter words: (j lo, j hi, unit lo, c3).  Pairs: c3 = (unit hi << 1) | ser.  Triples:
+// c3 = 2^31 | (unit hi << 2) | ser, a tag bit that pairs below 2^62 never set, so triple t and pair
+// t of one seed share no series.
 template <typename T> struct NoiseArgs {
-  T *out;                   // [n_pairs][2][n]
+  T *out;                   // [n_units][nser][n]
   unsigned long long seed;
-  long long pair0;          // global index of the first pair
+  long long unit0;          // global index of the first unit
   long long n;
-  int n_pairs;
+  int n_units;
+  int nser;                 // 2 (pairs) or 3 (triples)
 };
 HD void philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0, unsigned k1, unsigned (&o)[4]) {
 #pragma unroll
@@ -1662,11 +1667,12 @@ template <typename T> struct NoiseBody {
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
     const long long j = (long long)bx * NT + tid;        // sample pair index
     if (2 * j >= a.n) return;
-    const long long pair = a.pair0 + by / 2;
-    const int ser = by & 1;
+    const long long unit = a.unit0 + by / a.nser;
+    const int ser = by % a.nser;
+    const unsigned hi = (unsigned)((unsigned long long)unit >> 32);
+    const unsigned c3 = a.nser == 2 ? (hi << 1) | (unsigned)ser : 0x80000000u | (hi << 2) | (unsigned)ser;
     unsigned o[4];
-    philox4x32_10((unsigned)j, (unsigned)((unsigned long long)j >> 32), (unsigned)pair,
-                  ((unsigned)((unsigned long long)pair >> 32) << 1) | (unsigned)ser,
+    philox4x32_10((unsigned)j, (unsigned)((unsigned long long)j >> 32), (unsigned)unit, c3,
                   (unsigned)a.seed, (unsigned)(a.seed >> 32), o);
     // uniforms in (0, 1): 53 bits from two words, offset by half an ulp so that log() is finite
     const double u1 = ((double)(o[0] >> 5) * 67108864.0 + (double)(o[1] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
@@ -1840,13 +1846,30 @@ template <typename T> struct Wct3PrepBody {
 // Tile: RS output rows x CW columns; phase 0 stages the RS + K - 1 input rows of the five fields
 // for these columns, phase 1 gives each of the NT = (RS / RG) CW threads RG consecutive rows of
 // one column.
+// Monte-Carlo mode (RP2 and RM2 both null): only the rows below maxscale and only the measures
+// whose histogram is given; a measure's histogram counts floor(R2 nbins), clamped to
+// [0, nbins - 1], over the points with mask != 0.  A non-finite R2 (a zero denominator) is not
+// counted.
 template <typename T> struct Wct3FinalArgs {
   const cx<T> *A, *B, *Xy1, *Xy2, *X12;   // time-smoothed fields
   const double *win;
   double *RP2, *RM2;                     // [rows][n], either may be null
+  const unsigned char *mask;             // [rows][n], Monte-Carlo mode
+  unsigned long long *histP, *histM;     // [rows][nbins], either may be null
   long long n;
-  int rows, K;
+  int rows, K, maxscale, nbins;
 };
+// one count for R2 in its row's histogram; non-finite R2 is skipped before any conversion to int
+HD void hist_count(unsigned long long *hist, int row, int nbins, double r2) {
+  if (!isfinite(r2)) return;
+  const double x = floor(r2 * nbins);
+  const int bin = x < 0.0 ? 0 : (x >= (double)nbins ? nbins - 1 : (int)x);
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  atomicAdd(&hist[(size_t)row * nbins + bin], 1ull);
+#else
+  hist[(size_t)row * nbins + bin] += 1ull;
+#endif
+}
 template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
   using Args = Wct3FinalArgs<T>;
   using V = cx<T>;
@@ -1862,7 +1885,8 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
     double *sw = (double *)(st + NF * PLANE);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    if (i0 >= a.rows) return;
+    const int rows_out = a.RP2 || a.RM2 ? a.rows : a.maxscale;
+    if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
       const V *src[NF] = {a.A, a.B, a.Xy1, a.Xy2, a.X12};
@@ -1914,7 +1938,7 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
 #pragma unroll
       for (int e = 0; e < RG; ++e) {
         const int i = i0 + RG * grp + e;
-        if (i >= a.rows) break;
+        if (i >= rows_out) break;
         const double Sy = acc[0][0][e], S1 = acc[0][1][e], S2 = acc[1][0][e];
         const double2 Sy1 = mk<double>(acc[2][0][e], acc[2][1][e]);
         const double2 Sy2 = mk<double>(acc[3][0][e], acc[3][1][e]);
@@ -1922,13 +1946,18 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
         const double ny1 = Sy1.x * Sy1.x + Sy1.y * Sy1.y, ny2 = Sy2.x * Sy2.x + Sy2.y * Sy2.y;
         const double d12 = S1 * S2 - (S12.x * S12.x + S12.y * S12.y);
         const size_t o = (size_t)i * a.n + n;
-        if (a.RP2) {
+        const bool binned = (a.histP || a.histM) && i < a.maxscale && a.mask[o];
+        if (a.RP2 || (a.histP && binned)) {
           const double2 u = csub(cscale(Sy1, S2), cmul(Sy2, cconj(S12)));
-          a.RP2[o] = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
+          const double rp = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
+          if (a.RP2) a.RP2[o] = rp;
+          if (a.histP && binned) hist_count(a.histP, i, a.nbins, rp);
         }
-        if (a.RM2) {
+        if (a.RM2 || (a.histM && binned)) {
           const double2 z = cmul(cmul(Sy1, S12), cconj(Sy2));
-          a.RM2[o] = (S2 * ny1 + S1 * ny2 - 2.0 * z.x) / (Sy * d12);
+          const double rm = (S2 * ny1 + S1 * ny2 - 2.0 * z.x) / (Sy * d12);
+          if (a.RM2) a.RM2[o] = rm;
+          if (a.histM && binned) hist_count(a.histM, i, a.nbins, rm);
         }
       }
     }

@@ -203,17 +203,18 @@ def cwt_batch_sharded(X, dt, scales, family, param, precision, engine, comm=None
     return gather_rows(power, X.shape[0], comm, device)
 
 
-def surrogate_pair(seed, index, N, al1, al2):
-    """Surrogate pair number `index` of a sharded Monte-Carlo run: white noise like the
-    reference's `rednoise` output (helpers.py:146-173 filters a length-1 axis, SURVEY 8a row
-    10), from an RNG stream keyed by (seed, index) so that the pair does not depend on which
+def surrogate_pair(seed, index, N, *als):
+    """Surrogate unit number `index` of a sharded Monte-Carlo run, one series per coefficient in
+    `als` (a pair for the coherence, a triple for the partial / multiple coherence): white noise
+    like the reference's `rednoise` output (helpers.py:146-173 filters a length-1 axis, SURVEY 8a
+    row 10), from an RNG stream keyed by (seed, index) so that the unit does not depend on which
     rank draws it."""
     rs = np.random.RandomState([int(seed) & 0x7fffffff, int(index)])
 
     def white(al):
         tau = 0 if al == 0 else int(np.ceil(-2 / np.log(np.abs(al))))
         return rs.randn(N + tau)[tau:]
-    return white(al1), white(al2)
+    return tuple(white(al) for al in als)
 
 
 def wct_significance_sharded(al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet='morlet',
@@ -241,6 +242,33 @@ def wct_significance_sharded(al1, al2, dt, dj, s0, J, significance_level=0.95, w
                                 range(lo, hi), progress=False, engine=engine, precision=prec)
     hist = sum_over_ranks(hist, comm, device)
     return wv._mc_levels(prob, hist, significance_level)
+
+
+def wct3_significance_sharded(al_y, al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet='morlet',
+                              mc_count=300, seed=0, engine=None, comm=None, device=None, device_rng=False,
+                              precision='fp64'):
+    """`wavelet.wct3_significance` with the surrogate triples block-partitioned over the ranks:
+    every rank accumulates the histograms of the partial and of the multiple coherence of its
+    triples, ONE all-reduce of both ([2, S, 1000] int64) combines them and every rank evaluates
+    the levels.  The result is independent of the world size.  Host RNG (`device_rng=False`):
+    triple i is `surrogate_pair(seed, i, N, al_y, al1, al2)`; device RNG: the Philox triples of
+    (seed, i).  Returns (sig_partial, sig_multiple)."""
+    from . import wavelet as wv
+    mother, prec = wv._wct3_mc_setup(wavelet, dj, precision)
+    comm = _as_comm(comm)
+    rank, world = _rank_world(comm)
+    prob = wv._mc_problem(dt, dj, s0, J, mother)
+    lo, hi = shard_range(mc_count, rank, world)
+    if device_rng:
+        hist = wv._mc_histogram_seeded(prob, dt, dj, mother, seed, lo, hi - lo, engine=engine,
+                                       precision=prec, nser=3)
+    else:
+        hist = wv._mc_histogram(prob, dt, dj, mother,
+                                lambda i: surrogate_pair(seed, i, prob['N'], al_y, al1, al2),
+                                range(lo, hi), progress=False, engine=engine, precision=prec, nser=3)
+    hist = sum_over_ranks(hist, comm, device)
+    return (wv._mc_levels(prob, hist[0], significance_level),
+            wv._mc_levels(prob, hist[1], significance_level))
 
 
 def scale_rows(n_scales, rank, world, layout='cyclic'):

@@ -473,7 +473,7 @@ def partial_wct(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize
     filter are resolved as in `wct`, with the same errors.  RP2 lies in [0, 1] up to rounding and
     is not clamped: where a denominator is zero or rounds to <= 0 it is inf or NaN.  Where x1 and
     x2 are nearly coherent (R2_12 -> 1) the measure is ill-conditioned: its rounding error grows
-    like 1 / ((1 - R2_y2) (1 - R2_12)).  No significance test."""
+    like 1 / ((1 - R2_y2) (1 - R2_12)).  Significance levels: `wct3_significance`."""
     return _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial=True)
 
 
@@ -488,7 +488,8 @@ def multiple_wct(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normaliz
     Returns (RM2, coi, freq), RM2 float64 [S, n0]; `precision`, scales, errors and the absence of
     clamping as in `partial_wct`.  RM2 >= max(R2_y1, R2_y2) up to rounding, and
     1 - RM2 = (1 - R2_y2) (1 - RP2).  Ill-conditioned where x1 and x2 are nearly coherent: the
-    rounding error grows like 1 / (1 - R2_12).  No significance test."""
+    rounding error grows like 1 / (1 - R2_12).  Significance levels: `wct3_significance` (RM2 has a
+    higher null level than the two-series coherence, since RM2 >= R2_y1 at every point)."""
     return _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial=False)
 
 
@@ -518,30 +519,36 @@ def _mc_problem(dt, dj, s0, J, wavelet):
 
 
 def _mc_histogram(prob, dt, dj, wavelet, draw, indices, progress=False, engine=None,
-                  precision=_engine.F64):
-    """1000-bin histograms of the coherence of the surrogate pairs draw(i), i in `indices`
-    (reference wavelet.py:609-630), accumulated on the GPU: int64 [S, nbins].  `precision`:
-    engine precision of the coherence."""
+                  precision=_engine.F64, nser=2):
+    """1000-bin histograms of the coherence of the surrogate units draw(i), i in `indices`
+    (reference wavelet.py:609-630), accumulated on the GPU.  `nser` = 2: draw(i) is a pair, the
+    result the coherence histogram int64 [S, nbins].  `nser` = 3: draw(i) is a triple (y, x1, x2),
+    the result int64 [2, S, nbins], the histograms of the partial and of the multiple coherence.
+    `precision`: engine precision of the coherence."""
     N, sj, nbins = prob['N'], prob['sj'], prob['nbins']
-    hist = np.zeros((sj.size, nbins), dtype=np.int64)
+    hist = np.zeros((nser - 1, sj.size, nbins), dtype=np.int64)
     eng = engine or _engine.default_engine()
     fam = _family_of(wavelet)
     indices = list(indices)
-    batch = max(1, min(len(indices), int((256 << 20) // (16 * N)) or 1))
+    batch = max(1, min(len(indices), int((256 << 20) // (8 * nser * N)) or 1))
     bar = tqdm(total=len(indices), disable=not progress)
     for b0 in range(0, len(indices), batch):
         idx = indices[b0:b0 + batch]
-        noise = np.empty((len(idx), 2, N))
+        noise = np.empty((len(idx), nser, N))
         for k, i in enumerate(idx):
-            noise[k, 0], noise[k, 1] = draw(i)
+            noise[k] = draw(i)
         with eng.lock:
             prec = _engine.F64 if _sync_padding(eng, N) else precision
             with _smoothing_filter(eng, wavelet, sj, dt, N):
-                eng.wct_mc(noise, dt, dj, sj, fam[0], fam[1], _boxcar_len(wavelet, dj), prob['mask'],
-                           prob['maxscale'], nbins, hist, precision=prec)
+                if nser == 2:
+                    eng.wct_mc(noise, dt, dj, sj, fam[0], fam[1], _boxcar_len(wavelet, dj), prob['mask'],
+                               prob['maxscale'], nbins, hist[0], precision=prec)
+                else:
+                    eng.wct3_mc(noise, dt, sj, fam[0], fam[1], _boxcar_len(wavelet, dj), prob['mask'],
+                                prob['maxscale'], nbins, hist[0], hist[1], precision=prec)
         bar.update(len(idx))
     bar.close()
-    return hist
+    return hist[0] if nser == 2 else hist
 
 
 def _mc_levels(prob, hist, significance_level):
@@ -558,19 +565,22 @@ def _mc_levels(prob, hist, significance_level):
 
 
 def _mc_histogram_seeded(prob, dt, dj, wavelet, seed, first, count, engine=None,
-                         precision=_engine.F64):
+                         precision=_engine.F64, nser=2):
     """The same histograms with the surrogates drawn on the device (Philox stream keyed by
-    (seed, pair number)): no host RNG, no noise H2D."""
+    (seed, pair or triple number)): no host RNG, no noise H2D."""
     sj, nbins = prob['sj'], prob['nbins']
-    hist = np.zeros((sj.size, nbins), dtype=np.int64)
+    hist = np.zeros((nser - 1, sj.size, nbins), dtype=np.int64)
     eng = engine or _engine.default_engine()
     fam = _family_of(wavelet)
+    args = (prob['N'], dt, sj, fam[0], fam[1], _boxcar_len(wavelet, dj), prob['mask'], prob['maxscale'], nbins)
     with eng.lock:
         prec = _engine.F64 if _sync_padding(eng, prob['N']) else precision
         with _smoothing_filter(eng, wavelet, sj, dt, prob['N']):
-            eng.wct_mc_seeded(seed, first, count, prob['N'], dt, sj, fam[0], fam[1], _boxcar_len(wavelet, dj),
-                              prob['mask'], prob['maxscale'], nbins, hist, precision=prec)
-    return hist
+            if nser == 2:
+                eng.wct_mc_seeded(seed, first, count, *args, hist[0], precision=prec)
+            else:
+                eng.wct3_mc_seeded(seed, first, count, *args, hist[0], hist[1], precision=prec)
+    return hist[0] if nser == 2 else hist
 
 
 def wct_significance(al1, al2, dt, dj, s0, J, significance_level=0.95,
@@ -630,6 +640,57 @@ def _wct_significance(al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet=
     if cache:
         np.savetxt('{}/{}.gz'.format(cache_dir, cache_file), sig95)
     return sig95
+
+
+def _wct3_mc_setup(wavelet, dj, precision):
+    """(wavelet, engine precision) of a three-series Monte-Carlo run, with the errors of
+    `partial_wct` / `multiple_wct`."""
+    prec = _coherence_precision(precision)
+    wavelet = _check_parameter_wavelet(wavelet)
+    if not hasattr(wavelet, 'smooth'):
+        raise AttributeError("'{}' object has no attribute 'smooth'".format(type(wavelet).__name__))
+    if _boxcar_len(wavelet, dj) < 1:
+        raise ValueError('smoothing window undefined for this wavelet (deltaj0 = -1)')
+    _family_of(wavelet)
+    return wavelet, prec
+
+
+def wct3_significance(al_y, al1, al2, dt, dj, s0, J, significance_level=0.95, wavelet='morlet',
+                      mc_count=300, progress=True, seed=None, precision='fp64'):
+    """Monte-Carlo significance levels of `partial_wct` and `multiple_wct` per scale.  An
+    extension: the reference has no three-series coherence.
+
+    Returns (sig_partial, sig_multiple), float64 [J + 1] each, with the conventions of
+    `wct_significance`: the `significance_level` quantile of the 1000-bin histogram of every row
+    with points outside the cone of influence of the surrogates, 0 for a row without any.
+
+    Null: three mutually independent white-noise series of N = ceil(6 s0 2^(J dj) / dt) samples
+    per triple (`rednoise`, which is white noise as in the reference; `al_y`, `al1`, `al2` only
+    set how many draws it discards), not standardised, each triple through the whole pipeline of
+    `partial_wct` / `multiple_wct`.  This null does not keep a coherence between x1 and x2.  A
+    point whose RP2 or RM2 is not finite (a zero denominator) is not counted.
+
+    Default (`seed=None`): the triples are drawn on the host with numpy's global RNG, one set-up
+    draw rednoise(N, al_y, 1), then rednoise(N, al_y), rednoise(N, al1), rednoise(N, al2) per
+    triple, so a run seeded through np.random is reproducible.  With an integer `seed` the triples
+    come from the device's counter-based Philox stream, keyed by (seed, triple number) and disjoint
+    from the pairs of `wct_significance(seed=)`.  `precision`: 'fp64' (default) or 'fp32', the
+    arithmetic of the surrogates' transforms and smoothing; the levels are float64 either way.
+    Errors as in `partial_wct`.  No on-disk cache."""
+    wavelet, prec = _wct3_mc_setup(wavelet, dj, precision)
+    prob = _mc_problem(dt, dj, s0, J, wavelet)
+    N = prob['N']
+    if seed is None:
+        rednoise(N, al_y, 1)  # set-up draw, as in wct_significance
+
+        def draw(i):
+            return rednoise(N, al_y, 1), rednoise(N, al1, 1), rednoise(N, al2, 1)
+
+        hist = _mc_histogram(prob, dt, dj, wavelet, draw, range(mc_count), progress, precision=prec,
+                             nser=3)
+    else:
+        hist = _mc_histogram_seeded(prob, dt, dj, wavelet, seed, 0, mc_count, precision=prec, nser=3)
+    return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
 
 
 def _smooth_device(W, dt, dj, scales, deltaj0, wavelet=None):
