@@ -1,6 +1,6 @@
 """A/B builds of the engine with compile-time switches:
 
-    python profiles/micro/build_variant.py TAG -DCWTB_PASSA_ASYNC=0 [...]
+    python profiles/micro/build_variant.py TAG -DCWTB_UNROLL_A=8 [...]
 
 writes pycwt_b200/variants/libcwtb200_TAG.so (git-ignored like every built library; it travels to
 the GPU box with the snapshot).  Load it with `_engine.Engine(0, lib_path=...)`; the scripts under

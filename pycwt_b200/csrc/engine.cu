@@ -76,14 +76,6 @@ __device__ __forceinline__ void run_phases(const typename Body::Args &a, void *s
     run_phases<Body, PH + 1>(a, sm);
   }
 }
-template <class Body, int PH>
-__device__ __forceinline__ void run_phases_at(const typename Body::Args &a, int bx, int by, void *sm) {
-  Body::template phase<PH>(a, bx, by, (int)threadIdx.x, sm);
-  if constexpr (PH + 1 < Body::NPHASE) {
-    __syncthreads();
-    run_phases_at<Body, PH + 1>(a, bx, by, sm);
-  }
-}
 template <class Body>
 __global__ void __launch_bounds__(BodyNT<Body>::value, BodyMinB<Body>::value) k_run(const __grid_constant__ typename Body::Args a) {
   extern __shared__ __align__(16) unsigned char smraw[];
@@ -105,6 +97,10 @@ struct Buf {
   void *p = nullptr;
   size_t bytes = 0;
 };
+
+// longest pruned length K' that one kernel transforms (up to 2^10 SingleBody, above DirectBody);
+// longer ones run through the two-kernel path
+constexpr int DIRECT_MAX_LOG2 = 13;
 
 struct ClassRun {   // scales sharing one execution plan
   int log2K;        // exact path: pruned length K' = 1 << log2K
@@ -183,10 +179,7 @@ struct cwtb_ctx {
                                  // (cwtb_set_coherence_precision)
   std::map<unsigned, BluePlan> blue;
   long long serial = 0;          // counts transforms: identifies what is resident (cwtb_job_serial)
-  int two_streams = 1;           // CWTB_STREAMS=1 disables the overlap
-  int three_streams = 1;         // CWTB_STREAMS=2: single-kernel classes only
-  rt_stream copy_streams[4]{};   // large D2H copies are split over several streams / copy engines
-  int d2h_split = 1;             // CWTB_D2H_SPLIT
+  rt_stream copy_streams[2]{};   // device->host copies that overlap the kernels or each other
   std::string err;
   double band_eps = 1e-16;
   double band_eps32 = 1e-9;      // fp32 engine: pruning threshold matched to the arithmetic (fp32
@@ -205,22 +198,11 @@ struct cwtb_ctx {
   Buf comm_send, comm_recv;      // device staging of the host-buffer collectives
   int group = 0;   // rows per two-kernel chunk; 0 = as many as fit in group_bytes of Z (CWTB_GROUP)
   size_t group_bytes = (size_t)512 << 20;
-  size_t rows_chunk_bytes = (size_t)256 << 20;  // CWTB_ROWS_CHUNK_MB: launches of >= 8 waves beat keeping the
-                                                // intermediate in L2 (50 MB on H100)
-  int l2_persist = 0;
-  int direct_max_log2 = 13;
-  int fused = 0;     // experimental: two-kernel scales through one persistent kernel (CWTB_FUSED=1)
-  int ring = 3;      // Z ring slots of the fused kernel
-  int pipe_ahead = 2;   // CWTB_FUSED=2: scales the first kernel runs in front of the second (CWTB_AHEAD)
   int num_sms = 132;
   int pf_dist = 132;   // PassB: L2 prefetch distance in tiles, one per SM of an H100 (CWTB_PF_DIST)
-  int gauss_rec = 1;   // dense Morlet scales: Gaussian by recurrence (CWTB_GAUSS_REC=0: exp per bin)
   int pf_rows_a = 32, pf_rows_b = 32;   // the same for the batched row transforms (CWTB_PF_ROWS_A / _B)
   int pf_dist_a = 132;  // PassA (band): L2 prefetch distance in tiles (CWTB_PF_DIST_A)
-  int k2_512_max_log2 = 16;  // largest K' that uses the 512-point second pass (CWTB_K2_512_MAX)
-  int passb_rev = 1;    // second kernel walks the rows of a launch last-to-first (CWTB_PASSB_REV)
-  int k2_band_log2 = 9; // second-pass length of the pruned two-kernel scales: 2^9 or 2^10 (CWTB_K2_BAND)
-  size_t batch_bytes = (size_t)4 << 30;   // coefficients per chunk of cwtb_cwt_batch  // K' <= 2^13 handled by one kernel (K' > 1024: DirectBody)
+  size_t batch_bytes = (size_t)4 << 30;   // coefficients per chunk of cwtb_cwt_batch
   double2 *tw64 = nullptr;
   float2 *tw32 = nullptr;
   std::map<unsigned, NTabDev> ntabs;
@@ -233,7 +215,7 @@ struct cwtb_ctx {
   std::vector<double> wtab_host; // host mirror of wtab (tables are appended, never moved)
   size_t wtab_uploaded = 0;      // elements already on the device
   size_t wtab_max_bytes = (size_t)256 << 20;   // CWTB_WTAB_MB: host mirror size above which the cache starts over
-  Buf ctr, sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
+  Buf sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
   // geometry and settings reuses it (planning + descriptor upload: ~0.3 ms for 256 scales, several ms
@@ -273,8 +255,8 @@ struct cwtb_ctx {
   int launches = 0;
   std::set<const void *> configured;
   // per-launch event profiling (cwtb_profile_last)
-  bool profiling = false;
-  int prof_saved_streams = 1;
+  bool profiling = false;        // also puts a transform's kernels on one stream (run_job): per-kernel times
+                                 // are not blurred by overlap
   const char *prof_tag = "";     // prefix of the kernel names recorded while profiling: "fwd:" (forward
                                  // transform of the signal), "coarse:" (coarse-grid transforms of the
                                  // expansion path); W-writing launches carry no tag
@@ -292,8 +274,6 @@ struct cwtb_ctx {
 #endif
 };
 
-static int fail(cwtb_ctx *c, int code, const std::string &msg);
-static void apply_l2_policy(cwtb_ctx *c);
 static int fail(cwtb_ctx *c, int code, const std::string &msg) {
   if (c) c->err = msg;
   return code;
@@ -304,31 +284,6 @@ static int fail(cwtb_ctx *c, int code, const std::string &msg) {
     if (e_ != 0) return fail(c, CWTB_ERR_CUDA, std::string(#call) + ": " + rt_errstr(e_));   \
   } while (0)
 
-// Keep the Z buffer (intermediate of the two-kernel scales) resident in L2: persisting access
-// policy window on the engine's stream; everything else keeps the default policy and W is
-// written with streaming stores.  Re-applied whenever Z is (re)allocated.
-static void apply_l2_policy(cwtb_ctx *c) {
-#ifndef CWTB_HOST_EMU
-  if (!c->l2_persist || !c->Z.p) return;
-  int max_persist = 0, max_window = 0;
-  cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, c->device);
-  cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, c->device);
-  if (max_persist <= 0 || max_window <= 0) return;
-  const size_t want = std::min<size_t>(c->Z.bytes, (size_t)max_persist);
-  cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want);
-  cudaStreamAttrValue v{};
-  v.accessPolicyWindow.base_ptr = c->Z.p;
-  v.accessPolicyWindow.num_bytes = std::min<size_t>(c->Z.bytes, (size_t)max_window);
-  v.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)want / (double)v.accessPolicyWindow.num_bytes);
-  v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-  v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-  cudaStreamSetAttribute(c->stream, cudaStreamAttributeAccessPolicyWindow, &v);
-  cudaGetLastError();
-#else
-  (void)c;
-#endif
-}
-
 static int ensure(cwtb_ctx *c, Buf &b, size_t bytes) {
   if (b.bytes >= bytes && b.p) return 0;
   if (b.p) rt_free(b.p);
@@ -336,7 +291,6 @@ static int ensure(cwtb_ctx *c, Buf &b, size_t bytes) {
   b.bytes = 0;
   if (rt_malloc(&b.p, bytes) != 0) return fail(c, CWTB_ERR_NOMEM, "device allocation failed");
   b.bytes = bytes;
-  if (&b == &c->Z) apply_l2_policy(c);
   return 0;
 }
 
@@ -685,9 +639,9 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     long long lo = std::min<long long>(klo, 0), hi = std::max<long long>(khi, 0);
     if (khi < klo) { lo = 0; hi = 0; }
     int lk = std::max(5, ilog2((unsigned long long)(hi - lo + 1)));
-    if (lk > c->direct_max_log2) {  // two-kernel path: negative part must be a multiple of K2
+    if (lk > DIRECT_MAX_LOG2) {  // two-kernel path: negative part must be a multiple of K2
       lo = -((-lo + K2C - 1) / K2C) * K2C;
-      lk = std::max(c->direct_max_log2 + 1, ilog2((unsigned long long)(hi - lo + 1)));
+      lk = std::max(DIRECT_MAX_LOG2 + 1, ilog2((unsigned long long)(hi - lo + 1)));
     }
     if (lk > 20) lk = job.log2N;   // pruned lengths above 2^20 are not built: treat as dense
     const bool band_limited = lk < job.log2N;   // (before the promotion below: such a scale may still expand)
@@ -814,7 +768,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     } else if (d.ip_log2Nc) {
       d.ip_coff = (long long)coff;
       coff += (size_t)1 << d.ip_log2Nc;
-    } else if (d.log2K <= 10 || (d.log2K <= c->direct_max_log2 && d.log2K < job.log2N)) {  // single-kernel scale
+    } else if (d.log2K <= 10 || (d.log2K <= DIRECT_MAX_LOG2 && d.log2K < job.log2N)) {  // single-kernel scale
       d.boff = (long long)boff;
       boff += (size_t)1 << d.log2K;
     }
@@ -869,6 +823,10 @@ static int dispatch_passA(cwtb_ctx *c, int log2K1, const PassAArgs<T> &a, int ny
   return fail(c, CWTB_ERR_UNSUPPORTED, "transform longer than 2^20 per row is not supported yet");
 }
 
+// Z bytes per launch pair of two_kernel_rows: launches of >= 8 waves beat keeping the
+// intermediate in L2 (50 MB on H100)
+constexpr size_t ROWS_CHUNK_BYTES = (size_t)256 << 20;
+
 // Rows of length n (1024 < n <= 2^20) through PassA<REAL|CPLX> + PassB, in chunks that fit the
 // Z buffer.  Input row g becomes sub-transform g % ileave of output row out_row0 + g / ileave
 // (ileave = 1: plain rows).  Output rows are renamed through descs[first + outer].row if given.
@@ -881,16 +839,15 @@ static int two_kernel_rows(cwtb_ctx *c, const void *in, int real_in, long long i
   NTab nt;
   int e = get_ntab(c, n, l2, &nt);
   if (e) return e;
-  // rows per chunk: the intermediate of a chunk (rows_chunk_bytes, default 64 MiB) stays in L2
-  // between the two kernels
-  const int chunk = std::max(1, std::min(nrows, (int)std::max<size_t>(1, c->rows_chunk_bytes / ((size_t)n * sizeof(cx<T>)))));
+  // rows per chunk: the intermediate of a chunk is at most ROWS_CHUNK_BYTES
+  const int chunk = std::max(1, std::min(nrows, (int)std::max<size_t>(1, ROWS_CHUNK_BYTES / ((size_t)n * sizeof(cx<T>)))));
   Buf &Zt = c->Z;
   if ((e = ensure(c, Zt, (size_t)chunk * n * sizeof(cx<T>)))) return e;
   for (int r0 = 0; r0 < nrows; r0 += chunk) {
     const int nr = std::min(chunk, nrows - r0);
     PassAArgs<T> a{};
     a.in = in; a.Z = (cx<T> *)Zt.p; a.tw = Tw<T>::get(c); a.nt = nt;
-    a.in_pitch = in_pitch; a.n_in = n_in; a.N = n; a.first = 0; a.zmod = 1 << 30; a.K2 = K2C;
+    a.in_pitch = in_pitch; a.n_in = n_in; a.N = n; a.first = 0; a.K2 = K2C;
     a.row0 = (ileave > 1 ? 0 : out_row0) + r0;   // interleaved input rows are numbered from 0
     a.pf_dist = c->pf_rows_a;
     e = real_in ? dispatch_passA<T, SIGN, MODE_REAL>(c, l2 - 10, a, nr)
@@ -899,8 +856,8 @@ static int two_kernel_rows(cwtb_ctx *c, const void *in, int real_in, long long i
     PassBArgs<T> b{};
     b.Z = (const cx<T> *)Zt.p; b.out = out; b.tw = Tw<T>::get(c); b.descs = descs;
     b.pitch = out_pitch; b.nout = nout; b.N = n; b.first = first;
-    b.epi = grow ? EPI_GAUSS : epi; b.grow = grow; b.post = post; b.zmod = 1 << 30;
-    b.pf_dist = c->pf_rows_b; b.ny = nr; b.ileave = ileave; b.rev = c->passb_rev;
+    b.epi = grow ? EPI_GAUSS : epi; b.grow = grow; b.post = post;
+    b.pf_dist = c->pf_rows_b; b.ny = nr; b.ileave = ileave;
     if (ileave > 1) { b.row0 = out_row0; b.by0 = r0; } else { b.row0 = out_row0 + r0; b.by0 = 0; }
     e = launch<PassBBody<T, SIGN>>(c, (n / K2C + Lay<T, K2C>::P - 1) / Lay<T, K2C>::P, nr, b);
     if (e) return e;
@@ -950,7 +907,7 @@ static int fft_rows(cwtb_ctx *c, const void *in, int real_in, long long in_pitch
     const int nr = std::min(chunk, nrows - r0);
     PassAArgs<T> a{};
     a.in = in; a.Z = (cx<T> *)c->Y.p; a.tw = Tw<T>::get(c); a.nt = nt;
-    a.in_pitch = in_pitch; a.n_in = n_in; a.N = n; a.first = 0; a.row0 = r0; a.zmod = 1 << 30; a.K2 = Nsub;
+    a.in_pitch = in_pitch; a.n_in = n_in; a.N = n; a.first = 0; a.row0 = r0; a.K2 = Nsub;
     e = real_in ? dispatch_passA<T, SIGN, MODE_REAL>(c, l0, a, nr)
                 : dispatch_passA<T, SIGN, MODE_CPLX>(c, l0, a, nr);
     if (e) return e;
@@ -1071,317 +1028,6 @@ static int run_job_exact(cwtb_ctx *c, const Job &job, const double *dsig, double
   return 0;
 }
 
-// ======================================================================================
-// fused persistent two-pass kernel: PassA and PassB tiles of every scale of one class run in
-// ONE launch.  A global tile queue is consumed in the order
-//     A(0) A(1) B(0) A(2) B(1) ... A(n-1) B(n-2) B(n-1)
-// (A(s)/B(s) = all tiles of scale s); B(s) waits for the A(s) tiles through a global counter,
-// A(s) waits for B(s-ring) before reusing its Z slot.  Z is a ring of `ring` scale buffers
-// (ring * 16 MiB at Np = 2^20) that lives in L2, so the intermediate never goes to HBM and
-// there are no per-scale launch tails.
-// ======================================================================================
-template <typename T> struct FusedArgs {
-  PassAArgs<T> a;
-  PassBArgs<T> b;
-  unsigned *ctr;    // [0] queue head, [1 .. n] doneA, [1+n .. 2n] doneB
-  int nscales, ring;
-  unsigned tilesA, tilesB;
-};
-
-// position t of the queue -> (isB, scale, tile)
-HD void fused_decode(unsigned t, int n, unsigned TA, unsigned TB, int *isB, int *s, unsigned *tile) {
-  if (t < TA) { *isB = 0; *s = 0; *tile = t; return; }
-  t -= TA;
-  const unsigned per = TA + TB;
-  const unsigned blk = t / per, off = t % per;
-  if ((int)blk < n - 1) {
-    if (off < TA) { *isB = 0; *s = (int)blk + 1; *tile = off; }
-    else { *isB = 1; *s = (int)blk; *tile = off - TA; }
-  } else {  // tail: B(n-1)
-    *isB = 1; *s = n - 1; *tile = t - (unsigned)(n - 1) * per;
-  }
-}
-
-#ifndef CWTB_HOST_EMU
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-template <typename T, int K1, int MODE>
-__global__ void __launch_bounds__(TileCfg<T>::NT, 3) k_fused(const __grid_constant__ FusedArgs<T> f) {
-  extern __shared__ __align__(16) unsigned char smraw[];
-  __shared__ unsigned s_t;
-  using A = PassABody<T, K1, MODE, +1>;
-  using B = PassBBody<T, +1>;
-  const int n = f.nscales;
-  const unsigned total = (unsigned)n * (f.tilesA + f.tilesB);
-  unsigned *doneA = f.ctr + 1, *doneB = f.ctr + 1 + n;
-  for (;;) {
-    __syncthreads();  // previous tile's shared memory is free
-    if (threadIdx.x == 0) s_t = atomicAdd(f.ctr, 1u);
-    __syncthreads();
-    const unsigned t = s_t;
-    if (t >= total) break;
-    int isB, s;
-    unsigned tile;
-    fused_decode(t, n, f.tilesA, f.tilesB, &isB, &s, &tile);
-    if (threadIdx.x == 0) {
-      if (isB) {
-        while (ld_acquire_u32(&doneA[s]) < f.tilesA) __nanosleep(100);
-      } else if (s >= f.ring) {
-        while (ld_acquire_u32(&doneB[s - f.ring]) < f.tilesB) __nanosleep(100);
-      }
-      asm volatile("fence.proxy.async;" ::: "memory");
-    }
-    __syncthreads();
-    if (isB) run_phases_at<B, 0>(f.b, (int)tile, s, smraw);
-    else run_phases_at<A, 0>(f.a, (int)tile, s, smraw);
-    __syncthreads();
-    if (threadIdx.x == 0)   // release-add, no L1 invalidate (see k_pipe)
-      asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(isB ? &doneB[s] : &doneA[s]), "r"(1u) : "memory");
-  }
-}
-#endif
-
-template <typename T, int K1, int MODE>
-static int launch_fused(cwtb_ctx *c, const PassAArgs<T> &a, const PassBArgs<T> &b, int nscales) {
-  using A = PassABody<T, K1, MODE, +1>;
-  using B = PassBBody<T, +1>;
-  FusedArgs<T> f;
-  f.a = a; f.b = b;
-  f.nscales = nscales;
-  f.ring = c->ring;
-  f.a.zmod = f.b.zmod = c->ring;
-  const unsigned M = a.N / ((unsigned)K1 * K2C);
-  f.tilesA = M * (K2C / A::T2);
-  f.tilesB = (a.N / K2C + Lay<T, K2C>::P - 1) / Lay<T, K2C>::P;
-  int e = ensure(c, c->ctr, (size_t)(1 + 2 * nscales) * sizeof(unsigned));
-  if (e) return e;
-  f.ctr = (unsigned *)c->ctr.p;
-  RT(rt_memset(c->ctr.p, 0, (size_t)(1 + 2 * nscales) * sizeof(unsigned), c->stream));
-#ifdef CWTB_HOST_EMU
-  std::vector<unsigned char> sm(std::max(A::SMEM, B::SMEM) + 64);
-  const unsigned total = (unsigned)nscales * (f.tilesA + f.tilesB);
-  for (unsigned t = 0; t < total; ++t) {
-    int isB, s;
-    unsigned tile;
-    fused_decode(t, nscales, f.tilesA, f.tilesB, &isB, &s, &tile);
-    if (isB) emu_phases<B, 0>(f.b, (int)tile, s, sm.data());
-    else emu_phases<A, 0>(f.a, (int)tile, s, sm.data());
-  }
-  c->launches++;
-  return 0;
-#else
-  const size_t smem = std::max(A::SMEM, B::SMEM);
-  auto kern = k_fused<T, K1, MODE>;
-  const void *fn = (const void *)kern;
-  if (!c->configured.count(fn)) {
-    RT(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    c->configured.insert(fn);
-  }
-  int occ = 0;
-  RT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, TileCfg<T>::NT, smem));
-  if (occ < 1) return fail(c, CWTB_ERR_CUDA, "fused kernel does not fit on an SM");
-  const unsigned total = (unsigned)nscales * (f.tilesA + f.tilesB);
-  const unsigned grid = std::min<unsigned>(total, (unsigned)(occ * c->num_sms));
-  int ev = -1;
-  if (c->profiling) {
-    ev = (int)c->prof.size() * 2;
-    while ((int)c->prof_events.size() < ev + 2) {
-      cudaEvent_t e2;
-      RT(cudaEventCreate(&e2));
-      c->prof_events.push_back(e2);
-    }
-    c->prof.push_back({body_name(__PRETTY_FUNCTION__), grid, (unsigned)nscales, ev});
-    RT(cudaEventRecord(c->prof_events[ev], c->stream));
-  }
-  kern<<<grid, TileCfg<T>::NT, smem, c->stream>>>(f);
-  RT(cudaGetLastError());
-  if (ev >= 0) RT(cudaEventRecord(c->prof_events[ev + 1], c->stream));
-  c->launches++;
-  return 0;
-#endif
-}
-
-template <typename T, int MODE>
-static int dispatch_fused(cwtb_ctx *c, int log2K1, const PassAArgs<T> &a, const PassBArgs<T> &b, int n) {
-  switch (log2K1) {
-    case 1: return launch_fused<T, 2, MODE>(c, a, b, n);
-    case 2: return launch_fused<T, 4, MODE>(c, a, b, n);
-    case 3: return launch_fused<T, 8, MODE>(c, a, b, n);
-    case 4: return launch_fused<T, 16, MODE>(c, a, b, n);
-    case 5: return launch_fused<T, 32, MODE>(c, a, b, n);
-    case 6: return launch_fused<T, 64, MODE>(c, a, b, n);
-    case 7: return launch_fused<T, 128, MODE>(c, a, b, n);
-    case 8: return launch_fused<T, 256, MODE>(c, a, b, n);
-    case 9: return launch_fused<T, 512, MODE>(c, a, b, n);
-    case 10: return launch_fused<T, 1024, MODE>(c, a, b, n);
-  }
-  return fail(c, CWTB_ERR_UNSUPPORTED, "transform longer than 2^20 per row is not supported yet");
-}
-
-// ======================================================================================
-// Pipelined persistent two-pass kernel (CWTB_FUSED=2): like k_fused, but built so that the
-// bookkeeping stays off the critical path.
-//   * static schedule: CTA b runs tiles b, b + grid, b + 2 grid, ... of the global order
-//         A(0) .. A(ahead-1) | A(ahead) B(0) | A(ahead+1) B(1) | ... | B(n-ahead) .. B(n-1)
-//     (no queue atomic); the first kernel runs `ahead` scales in front of the second one, so the
-//     tiles a B(s) tile depends on were handed out >= ahead*tilesA positions earlier -- more than
-//     the number of resident CTAs for ahead = 2 -- and the dependency wait almost never blocks;
-//   * a CTA tests a dependency once per scale (not per tile): counters doneA[s] / doneB[s];
-//   * completion is published by the LAST thread of the CTA (fence + relaxed add) while the
-//     first warp already issues the next tile's bulk copies.
-// Z is a ring of `ring` >= ahead + 2 scale buffers (16 MiB each at Np = 2^20) that stays in L2:
-// the second kernel's tile loads hit L2 and the intermediate never reaches HBM.
-// ======================================================================================
-template <typename T> struct PipeArgs {
-  PassAArgs<T> a;
-  PassBArgs<T> b;
-  unsigned *ctr;    // [0 .. n) doneA, [n .. 2n) doneB
-  int nscales, ring, ahead;
-  unsigned tilesA, tilesB;
-};
-
-HD void pipe_decode(unsigned t, int n, int ahead, unsigned TA, unsigned TB, int *isB, int *s, unsigned *tile) {
-  const int na = ahead < n ? ahead : n;
-  if (t < (unsigned)na * TA) { *isB = 0; *s = (int)(t / TA); *tile = t % TA; return; }
-  t -= (unsigned)na * TA;
-  const unsigned per = TA + TB;
-  const int nmid = n - na;
-  if (t < (unsigned)nmid * per) {
-    const unsigned blk = t / per, off = t % per;
-    if (off < TA) { *isB = 0; *s = na + (int)blk; *tile = off; }
-    else { *isB = 1; *s = (int)blk; *tile = off - TA; }
-    return;
-  }
-  t -= (unsigned)nmid * per;
-  *isB = 1; *s = nmid + (int)(t / TB); *tile = t % TB;
-}
-
-#ifndef CWTB_HOST_EMU
-template <typename T, int K1, int MODE>
-__global__ void __launch_bounds__(TileCfg<T>::NT, 3) k_pipe(const __grid_constant__ PipeArgs<T> f) {
-  extern __shared__ __align__(16) unsigned char smraw[];
-  using A = PassABody<T, K1, MODE, +1>;
-  using B = PassBBody<T, +1>;
-  const int n = f.nscales;
-  const unsigned total = (unsigned)n * (f.tilesA + f.tilesB);
-  unsigned *doneA = f.ctr, *doneB = f.ctr + n;
-  int okA = -1, okB = -1;    // dependencies already seen complete by this CTA
-  for (unsigned t = blockIdx.x; t < total; t += gridDim.x) {
-    int isB, s;
-    unsigned tile;
-    pipe_decode(t, n, f.ahead, f.tilesA, f.tilesB, &isB, &s, &tile);
-    const int dep = isB ? s : s - f.ring;          // A(s) reuses the slot of B(s - ring)
-    if (dep >= 0 && dep > (isB ? okA : okB)) {
-      if (threadIdx.x == 0) {
-        const unsigned *flag = isB ? &doneA[dep] : &doneB[dep];
-        const unsigned want = isB ? f.tilesA : f.tilesB;
-        while (ld_acquire_u32(flag) < want) __nanosleep(64);
-        asm volatile("fence.proxy.async;" ::: "memory");
-      }
-      __syncthreads();
-      if (isB) okA = dep; else okB = dep;
-    }
-    if (isB) run_phases_at<B, 0>(f.b, (int)tile, s, smraw);
-    else run_phases_at<A, 0>(f.a, (int)tile, s, smraw);
-    __syncthreads();   // shared memory is free again; every store of the tile has been issued
-    if (threadIdx.x == blockDim.x - 1) {
-      // release-add: orders the tile's stores (made visible to this thread by the barrier) before
-      // the count.  NOT __threadfence(): a gpu-scope fence also invalidates the SM's L1
-      // (SASS CCTL.IVALL) -- once per tile that evicts the twiddle / root tables of every
-      // resident CTA; the release form compiles to MEMBAR.ALL.GPU + REDG only.
-      asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(isB ? &doneB[s] : &doneA[s]), "r"(1u) : "memory");
-    }
-  }
-}
-#endif
-
-template <typename T, int K1, int MODE>
-static int launch_pipe(cwtb_ctx *c, const PassAArgs<T> &a, const PassBArgs<T> &b, int nscales) {
-  using A = PassABody<T, K1, MODE, +1>;
-  using B = PassBBody<T, +1>;
-  PipeArgs<T> f;
-  f.a = a; f.b = b;
-  f.nscales = nscales;
-  f.ring = c->ring;
-  f.ahead = std::max(1, std::min(c->pipe_ahead, c->ring - 1));
-  f.a.zmod = f.b.zmod = c->ring;
-  f.b.rev = 0; f.b.pf_dist = 0; f.a.pf_dist = 0;
-  const unsigned M = a.N / ((unsigned)K1 * K2C);
-  f.tilesA = M * (K2C / A::T2);
-  f.tilesB = (a.N / K2C + Lay<T, K2C>::P - 1) / Lay<T, K2C>::P;
-  int e = ensure(c, c->ctr, (size_t)(2 * nscales) * sizeof(unsigned));
-  if (e) return e;
-  f.ctr = (unsigned *)c->ctr.p;
-  RT(rt_memset(c->ctr.p, 0, (size_t)(2 * nscales) * sizeof(unsigned), c->cur));
-#ifdef CWTB_HOST_EMU
-  std::vector<unsigned char> sm(std::max(A::SMEM, B::SMEM) + 64);
-  const unsigned total = (unsigned)nscales * (f.tilesA + f.tilesB);
-  std::vector<int> seenA(nscales, 0), seenB(nscales, 0);
-  for (unsigned t = 0; t < total; ++t) {
-    int isB, s;
-    unsigned tile;
-    pipe_decode(t, nscales, f.ahead, f.tilesA, f.tilesB, &isB, &s, &tile);
-    // the sequential emulation checks the schedule's invariants instead of waiting
-    if (isB && seenA[s] != (int)f.tilesA) return fail(c, CWTB_ERR_STATE, "pipe schedule: B before its A tiles");
-    if (!isB && s >= f.ring && seenB[s - f.ring] != (int)f.tilesB)
-      return fail(c, CWTB_ERR_STATE, "pipe schedule: Z slot reused before its B tiles");
-    if (isB) { emu_phases<B, 0>(f.b, (int)tile, s, sm.data()); seenB[s]++; }
-    else { emu_phases<A, 0>(f.a, (int)tile, s, sm.data()); seenA[s]++; }
-  }
-  c->launches++;
-  return 0;
-#else
-  const size_t smem = std::max(A::SMEM, B::SMEM);
-  auto kern = k_pipe<T, K1, MODE>;
-  const void *fn = (const void *)kern;
-  if (!c->configured.count(fn)) {
-    RT(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    c->configured.insert(fn);
-  }
-  int occ = 0;
-  RT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, TileCfg<T>::NT, smem));
-  if (occ < 1) return fail(c, CWTB_ERR_CUDA, "pipelined kernel does not fit on an SM");
-  const unsigned total = (unsigned)nscales * (f.tilesA + f.tilesB);
-  // every CTA must be resident (they wait for one another): at most occ per SM
-  const unsigned grid = std::min<unsigned>(total, (unsigned)(occ * c->num_sms));
-  int ev = -1;
-  if (c->profiling) {
-    ev = (int)c->prof.size() * 2;
-    while ((int)c->prof_events.size() < ev + 2) {
-      cudaEvent_t e2;
-      RT(cudaEventCreate(&e2));
-      c->prof_events.push_back(e2);
-    }
-    char nm[64];
-    snprintf(nm, sizeof nm, "PipeAB<%s, %d, %d>", sizeof(T) == 8 ? "double" : "float", K1, MODE);
-    c->prof.push_back({nm, grid, (unsigned)nscales, ev});
-    RT(cudaEventRecord(c->prof_events[ev], c->cur));
-  }
-  kern<<<grid, TileCfg<T>::NT, smem, c->cur>>>(f);
-  RT(cudaGetLastError());
-  if (ev >= 0) RT(cudaEventRecord(c->prof_events[ev + 1], c->cur));
-  c->launches++;
-  return 0;
-#endif
-}
-
-template <typename T, int MODE>
-static int dispatch_pipe(cwtb_ctx *c, int log2K1, const PassAArgs<T> &a, const PassBArgs<T> &b, int n) {
-  switch (log2K1) {
-    case 4: return launch_pipe<T, 16, MODE>(c, a, b, n);
-    case 5: return launch_pipe<T, 32, MODE>(c, a, b, n);
-    case 6: return launch_pipe<T, 64, MODE>(c, a, b, n);
-    case 7: return launch_pipe<T, 128, MODE>(c, a, b, n);
-    case 8: return launch_pipe<T, 256, MODE>(c, a, b, n);
-    case 9: return launch_pipe<T, 512, MODE>(c, a, b, n);
-    case 10: return launch_pipe<T, 1024, MODE>(c, a, b, n);
-  }
-  return fail(c, CWTB_ERR_UNSUPPORTED, "pipelined two-pass kernel: unsupported first-pass length");
-}
-
 template <typename T, int K>
 static int launch_single(cwtb_ctx *c, const SingleArgs<T> &a, int count) {
   constexpr int P = Lay<T, K>::P;
@@ -1397,15 +1043,11 @@ static int chunk_rows(const cwtb_ctx *c, unsigned N, size_t elem_bytes) {
   return (int)std::max<size_t>(1, std::min<size_t>(g, 32768));
 }
 
-static bool class_single(const cwtb_ctx *c, const Job &job, const ClassRun &cl) {
-  return !cl.expand && !cl.os && (cl.log2K <= 10 || (cl.log2K <= c->direct_max_log2 && cl.log2K < job.log2N));
+static bool class_single(const Job &job, const ClassRun &cl) {
+  return !cl.expand && !cl.os && (cl.log2K <= 10 || (cl.log2K <= DIRECT_MAX_LOG2 && cl.log2K < job.log2N));
 }
-static bool class_two_kernel(const cwtb_ctx *c, const Job &job, const ClassRun &cl) {
-  return !cl.expand && !cl.os && !class_single(c, job, cl);
-}
-// two-kernel class that runs as ONE persistent launch over a ring of Z buffers
-static bool class_persistent(const cwtb_ctx *c, const ClassRun &cl) {
-  return c->fused == 1 || (c->fused == 2 && cl.log2K >= 14 && cl.log2K <= 20 && cl.count <= 256);
+static bool class_two_kernel(const Job &job, const ClassRun &cl) {
+  return !cl.expand && !cl.os && !class_single(job, cl);
 }
 
 // Which band-chunk region / Z buffer / stream a two-kernel class uses: its position among the
@@ -1414,17 +1056,17 @@ static int job_chain_region(const cwtb_ctx *c, const Job &job, const ClassRun &c
   int idx = 0;
   for (const ClassRun &o : job.classes) {
     if (&o == &cl) break;
-    if (class_two_kernel(c, job, o)) ++idx;
+    if (class_two_kernel(job, o)) ++idx;
   }
   return idx % std::max(1, c->n_chains);
 }
 
 // elements of one band-chunk region: the largest chunk of band products of any two-kernel class
-static size_t band_chunk_elems(const cwtb_ctx *c, const Job &job, int G) {
+static size_t band_chunk_elems(const Job &job, int G) {
   size_t bchunk = 0;
   for (const ClassRun &cl : job.classes)
-    if (class_two_kernel(c, job, cl) && cl.log2K < job.log2N)
-      bchunk = std::max(bchunk, (size_t)(class_persistent(c, cl) ? cl.count : std::min(G, cl.count)) << cl.log2K);
+    if (class_two_kernel(job, cl) && cl.log2K < job.log2N)
+      bchunk = std::max(bchunk, (size_t)std::min(G, cl.count) << cl.log2K);
   return bchunk;
 }
 
@@ -1574,7 +1216,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   NTab nt;
   if ((e = get_ntab(c, N, job.log2N, &nt))) return e;
   const int G = chunk_rows(c, N, sizeof(V));
-  const size_t bchunk = band_chunk_elems(c, job, G);   // two regions: one per chain stream
+  const size_t bchunk = band_chunk_elems(job, G);   // two regions: one per chain stream
   if ((e = ensure(c, c->B, (job.b_single + (size_t)std::max(1, c->n_chains) * bchunk) * sizeof(V)))) return e;
   V *Bbuf = (V *)c->B.p;
 
@@ -1583,7 +1225,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   {
     int first = -1, maxlk = 0, nrows = 0;
     for (const ClassRun &cl : job.classes)
-      if (class_single(c, job, cl)) {
+      if (class_single(job, cl)) {
         if (first < 0) first = cl.first;
         maxlk = std::max(maxlk, cl.log2K);
         nrows += cl.count;
@@ -1596,18 +1238,15 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     }
   }
   // The single-kernel classes (independent of the two-kernel chains: different W rows, read-only
-  // band products) run on a second stream so that their CTAs fill the tails of the chains.
-  const bool split = c->two_streams != 0;
+  // band products) run on a second stream so that their CTAs fill the tails of the chains.  While
+  // profiling, every launch stays on the engine's stream.
+  const bool split = !c->profiling;
 #ifndef CWTB_HOST_EMU
-  const bool split2 = split && c->three_streams && !c->fused;
   if (split) {
     RT(cudaEventRecord(c->ev_fork, c->stream));
     RT(cudaStreamWaitEvent(c->aux_stream, c->ev_fork, 0));
-    if (split2)
-      for (int k = 1; k < c->n_chains; ++k) RT(cudaStreamWaitEvent(c->chain_streams[k - 1], c->ev_fork, 0));
+    for (int k = 1; k < c->n_chains; ++k) RT(cudaStreamWaitEvent(c->chain_streams[k - 1], c->ev_fork, 0));
   }
-#else
-  const bool split2 = false;
 #endif
   // ---- expansion classes (kernels.cuh: ExpandBody): the coarse transforms of every expansion row
   // form their coarse spectra while they fill their tiles, in one launch for the coarse lengths up
@@ -1641,7 +1280,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     }
     CoarseArgs<T> ca{};
     ca.descs = ddesc; ca.spec = spec; ca.C = (V *)c->Cout.p; ca.tw = Tw<T>::get(c); ca.fam = fam; ca.Nx = N;
-    ca.pf_dist = c->pf_rows_b; ca.rev = c->passb_rev;
+    ca.pf_dist = c->pf_rows_b;
     c->prof_tag = "coarse:";
     if (!long_segs.empty()) {
       if ((e = ensure(c, c->Zx, zx_elems * sizeof(V)))) return e;
@@ -1710,12 +1349,11 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
       return fail(c, CWTB_ERR_STATE, "overlap-save rows run in fp64 only");
     }
   }
-  int chain_no = 0;
   for (int pass = 0; pass < 2; ++pass)
   for (const ClassRun &cl : job.classes) {
     if (cl.expand || cl.os) continue;
     const unsigned K = 1u << cl.log2K;
-    const bool single = class_single(c, job, cl);
+    const bool single = class_single(job, cl);
     if (single != (pass == 0)) continue;   // pass 0: single-kernel classes, pass 1: two-kernel chains
     if (single) {
 #ifndef CWTB_HOST_EMU
@@ -1752,8 +1390,8 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
         const int ng = std::min(gy, cl.count - g0);
         PassAArgs<T> a{};
         a.descs = ddesc; a.spec = spec; a.Bbuf = Bbuf; a.Z = (V *)c->Y.p; a.tw = Tw<T>::get(c);
-        a.fam = fam; a.nt = nt; a.N = N; a.first = cl.first + g0; a.row0 = 0; a.zmod = 1 << 30;
-        a.pf_dist = 0; a.K2 = Nsub; a.gauss_rec = c->gauss_rec;
+        a.fam = fam; a.nt = nt; a.N = N; a.first = cl.first + g0; a.row0 = 0;
+        a.pf_dist = 0; a.K2 = Nsub;
         if ((e = dispatch_passA<T, +1, MODE_DENSE>(c, l0, a, ng))) return e;
         if ((e = two_kernel_rows<T, +1>(c, c->Y.p, 0, Nsub, Nsub, W, job.n0, Nsub, ng << l0, job.n0, nullptr, 1.0,
                                          1 << l0, ddesc, cl.first + g0, 0, epi)))
@@ -1761,50 +1399,39 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
       }
       continue;
     }
-    const bool persistent = class_persistent(c, cl);
-    const int chunk = persistent ? cl.count : G;   // persistent: the whole class in one launch
     // successive two-kernel classes rotate over the chains, each with its own stream, Z buffer
     // and band-chunk region (descriptor offsets already point into the right region)
-    const int chain = split2 ? job_chain_region(c, job, cl) : 0;
+#ifdef CWTB_HOST_EMU
+    const int chain = 0;   // the emulation runs every launch in order: one Z buffer serves all classes
+#else
+    const int chain = split ? job_chain_region(c, job, cl) : 0;
+#endif
     Buf &Zb = chain > 0 ? c->Zc[chain - 1] : c->Z;
-    if ((e = ensure(c, Zb, (size_t)(persistent ? c->ring : G) * N * sizeof(V)))) return e;
+    if ((e = ensure(c, Zb, (size_t)G * N * sizeof(V)))) return e;
 #ifndef CWTB_HOST_EMU
     c->cur = chain > 0 ? c->chain_streams[chain - 1] : c->stream;
 #endif
-    ++chain_no;
-    for (int g0 = 0; g0 < cl.count; g0 += chunk) {
-      const int ng = std::min(chunk, cl.count - g0);
+    for (int g0 = 0; g0 < cl.count; g0 += G) {
+      const int ng = std::min(G, cl.count - g0);
       PassAArgs<T> a{};
       a.descs = ddesc; a.spec = spec; a.Bbuf = Bbuf; a.Z = (V *)Zb.p; a.tw = Tw<T>::get(c);
-      a.fam = fam; a.nt = nt; a.N = N; a.first = cl.first + g0; a.row0 = 0; a.zmod = 1 << 30;
+      a.fam = fam; a.nt = nt; a.N = N; a.first = cl.first + g0; a.row0 = 0;
       // band scales: second pass of 512 points (full 128-byte output runs, conflict-free tile);
       // dense scales keep 1024 so that K1 = N/K2 <= 1024
       // (fp32: the 512-point tile has an odd row pitch, its rows would not be 16-byte aligned)
       constexpr bool k512_ok = (Lay<T, 512, true>::PITCH * sizeof(V)) % 16 == 0;
       // 512 pays up to K' = 2^16 (measured per class: first kernel + second kernel per row)
-      const int l2k = (dense || persistent || cl.log2K > c->k2_512_max_log2 || !k512_ok) ? 10 : c->k2_band_log2;
-      a.pf_dist = c->pf_dist_a; a.K2 = 1u << l2k; a.gauss_rec = c->gauss_rec;
+      const int l2k = (dense || cl.log2K > 16 || !k512_ok) ? 10 : 9;
+      a.pf_dist = c->pf_dist_a; a.K2 = 1u << l2k;
       PassBArgs<T> b{};
       b.Z = (const V *)Zb.p; b.out = W; b.tw = Tw<T>::get(c); b.descs = ddesc;
       b.pitch = job.n0; b.nout = job.n0; b.N = N; b.first = cl.first + g0; b.row0 = 0;
-      b.epi = epi; b.grow = nullptr; b.post = 1.0; b.zmod = 1 << 30;
-      b.pf_dist = c->pf_dist; b.ny = ng; b.rev = c->passb_rev;
+      b.epi = epi; b.grow = nullptr; b.post = 1.0;
+      b.pf_dist = c->pf_dist; b.ny = ng;
       if (!dense) {
         BandArgs<T> ba{ddesc, spec, Bbuf, fam, N, cl.first + g0};
         if ((e = launch<BandBody<T>>(c, (K + NT * BandBody<T>::PER - 1) / (NT * BandBody<T>::PER), ng, ba)))
           return e;
-      }
-      if (c->fused == 2 && persistent) {
-        e = dense ? dispatch_pipe<T, MODE_DENSE>(c, cl.log2K - 10, a, b, ng)
-                  : dispatch_pipe<T, MODE_BAND>(c, cl.log2K - 10, a, b, ng);
-        if (e) return e;
-        continue;
-      }
-      if (c->fused == 1) {
-        e = dense ? dispatch_fused<T, MODE_DENSE>(c, cl.log2K - 10, a, b, ng)
-                  : dispatch_fused<T, MODE_BAND>(c, cl.log2K - 10, a, b, ng);
-        if (e) return e;
-        continue;
       }
       e = dense ? dispatch_passA<T, +1, MODE_DENSE>(c, cl.log2K - l2k, a, ng)
                 : dispatch_passA<T, +1, MODE_BAND>(c, cl.log2K - l2k, a, ng);
@@ -1819,16 +1446,14 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     }
     c->cur = c->stream;
   }
-  (void)chain_no;
 #ifndef CWTB_HOST_EMU
   if (split) {   // join: later work on the main stream sees every row of W
     RT(cudaEventRecord(c->ev_join, c->aux_stream));
     RT(cudaStreamWaitEvent(c->stream, c->ev_join, 0));
-    if (split2)
-      for (int k = 1; k < c->n_chains; ++k) {
-        RT(cudaEventRecord(c->ev_joinc[k - 1], c->chain_streams[k - 1]));
-        RT(cudaStreamWaitEvent(c->stream, c->ev_joinc[k - 1], 0));
-      }
+    for (int k = 1; k < c->n_chains; ++k) {
+      RT(cudaEventRecord(c->ev_joinc[k - 1], c->chain_streams[k - 1]));
+      RT(cudaStreamWaitEvent(c->stream, c->ev_joinc[k - 1], 0));
+    }
   }
 #endif
   return 0;
@@ -1837,13 +1462,13 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
 // band-buffer offsets of the two-kernel scales depend on the chunk position; set them here
 static void assign_chunk_offsets(cwtb_ctx *c, Job &job) {
   const int G = chunk_rows(c, job.N, job.precision == CWTB_F64 ? sizeof(double2) : sizeof(float2));
-  const size_t bchunk = band_chunk_elems(c, job, G);
+  const size_t bchunk = band_chunk_elems(job, G);
   for (const ClassRun &cl : job.classes) {
-    if (!class_two_kernel(c, job, cl) || cl.log2K == job.log2N) continue;
+    if (!class_two_kernel(job, cl) || cl.log2K == job.log2N) continue;
     const size_t region = (size_t)job_chain_region(c, job, cl) * bchunk;
     for (int i = 0; i < cl.count; ++i)
       job.descs[cl.first + i].boff =
-          (long long)(job.b_single + region + (size_t)(class_persistent(c, cl) ? i : i % G) * ((size_t)1 << cl.log2K));
+          (long long)(job.b_single + region + (size_t)(i % G) * ((size_t)1 << cl.log2K));
   }
 }
 
@@ -1954,13 +1579,10 @@ int cwtb_create(int device, cwtb_ctx **out) {
   for (auto &ev : c->ev_joinc) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-  if (const char *g = getenv("CWTB_STREAMS")) { c->two_streams = atoi(g) >= 2; c->three_streams = atoi(g) >= 3; }
-  if (const char *g = getenv("CWTB_D2H_SPLIT")) c->d2h_split = std::min(4, std::max(1, atoi(g)));
 #endif
   c->cur = c->stream;
   if (const char *g = getenv("CWTB_GROUP")) c->group = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_GROUP_MB")) c->group_bytes = (size_t)std::max(1, atoi(g)) << 20;
-  if (const char *g = getenv("CWTB_ROWS_CHUNK_MB")) c->rows_chunk_bytes = (size_t)std::max(1, atoi(g)) << 20;
   if (const char *g = getenv("CWTB_BAND_EPS")) c->band_eps = atof(g);
   if (const char *g = getenv("CWTB_BAND_EPS32")) c->band_eps32 = atof(g);
   if (const char *g = getenv("CWTB_EXPAND_EPS")) c->expand_eps = std::max(0.0, atof(g));
@@ -1971,26 +1593,16 @@ int cwtb_create(int device, cwtb_ctx **out) {
   if (const char *g = getenv("CWTB_WTAB_MB")) c->wtab_max_bytes = (size_t)std::max(0, atoi(g)) << 20;
   if (const char *g = getenv("CWTB_PLAN_REUSE")) c->plan_reuse = atoi(g) != 0;
   if (const char *g = getenv("CWTB_DENSE_MARGIN")) c->dense_margin = std::max(0, atoi(g));
-  if (const char *g = getenv("CWTB_L2_PERSIST")) c->l2_persist = atoi(g);
-  if (const char *g = getenv("CWTB_FUSED")) c->fused = atoi(g);
   if (const char *g = getenv("CWTB_PF_DIST")) c->pf_dist = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_CHAINS")) c->n_chains = std::min(4, std::max(1, atoi(g)));
   if (const char *g = getenv("CWTB_FFT_PAD")) c->pad_pow2 = atoi(g) != 0;
   if (const char *g = getenv("CWTB_PF_ROWS_A")) c->pf_rows_a = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_PF_ROWS_B")) c->pf_rows_b = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_PF_DIST_A")) c->pf_dist_a = std::max(0, atoi(g));
-  if (const char *g = getenv("CWTB_K2_BAND")) c->k2_band_log2 = atoi(g) == 10 ? 10 : 9;
-  if (const char *g = getenv("CWTB_K2_512_MAX")) c->k2_512_max_log2 = std::min(19, atoi(g));
-  if (const char *g = getenv("CWTB_PASSB_REV")) c->passb_rev = atoi(g) != 0;
-  if (const char *g = getenv("CWTB_GAUSS_REC")) c->gauss_rec = atoi(g);
   if (const char *g = getenv("CWTB_BATCH_MB")) c->batch_bytes = (size_t)std::max(1, atoi(g)) << 20;
-  if (const char *g = getenv("CWTB_RING")) c->ring = std::max(1, atoi(g));
-  else if (c->fused == 2) c->ring = 4;
-  if (const char *g = getenv("CWTB_AHEAD")) c->pipe_ahead = std::max(1, atoi(g));
 #ifndef CWTB_HOST_EMU
   cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device);
 #endif
-  if (const char *g = getenv("CWTB_DIRECT_MAX")) c->direct_max_log2 = std::min(13, std::max(10, atoi(g)));
   int e = init_tables(c);
   if (e == 0) e = rt_sync(c->stream) ? CWTB_ERR_CUDA : 0;
   if (e) { delete c; return e; }
@@ -2005,7 +1617,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   cudaStreamSynchronize(c->stream);
 #endif
   cwtb_comm_destroy(c);
-  for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->ctr, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
+  for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
                  &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh.buf, &c->cross.buf})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
@@ -2131,7 +1743,7 @@ static int os_plan(cwtb_ctx *c, const Job &job, double dt, int family, double pa
   std::vector<double> cs;
   for (const ScaleDesc &d : job.descs) {
     if (d.chan != 0 || d.k_hi < d.k_lo || d.k_lo <= -half || d.k_hi >= ((long long)N - 1) / 2) continue;
-    if (d.ip_log2Nc || (d.log2K <= 10 || (d.log2K <= c->direct_max_log2 && d.log2K < job.log2N))) continue;
+    if (d.ip_log2Nc || (d.log2K <= 10 || (d.log2K <= DIRECT_MAX_LOG2 && d.log2K < job.log2N))) continue;
     cand.push_back(d.row);
     cs.push_back(d.s);
   }
@@ -2370,23 +1982,7 @@ int cwtb_last_plan(cwtb_ctx *c, int *out, int n) {
 static int field_to_host(cwtb_ctx *c, const void *field, int prec, size_t first, size_t cnt, void *out,
                          int out_f64) {
   if (prec == CWTB_F64) {
-    const char *src = (const char *)((const double2 *)field + first);
-    const size_t bytes = cnt * sizeof(double2);
-#ifndef CWTB_HOST_EMU
-    if (c->d2h_split > 1 && bytes >= ((size_t)64 << 20)) {
-      RT(rt_sync(c->stream));   // kernels done
-      const int ns = c->d2h_split;
-      const size_t piece = ((bytes / ns) + 255) & ~(size_t)255;
-      for (int i = 0; i < ns; ++i) {
-        const size_t off = (size_t)i * piece;
-        if (off >= bytes) break;
-        RT(rt_d2h((char *)out + off, src + off, std::min(piece, bytes - off), c->copy_streams[i]));
-      }
-      for (int i = 0; i < ns; ++i) RT(rt_sync(c->copy_streams[i]));
-      return 0;
-    }
-#endif
-    RT(rt_d2h(out, src, bytes, c->stream));
+    RT(rt_d2h(out, (const double2 *)field + first, cnt * sizeof(double2), c->stream));
     RT(rt_sync(c->stream));
   } else if (!out_f64) {
     RT(rt_d2h(out, (const float2 *)field + first, cnt * sizeof(float2), c->stream));
@@ -2731,7 +2327,7 @@ static bool single_kernel_rows(const cwtb_ctx *c, const Job &job, int *r0) {
   const int S = job.S;
   int lo = S, cnt = 0;
   for (const ClassRun &cl : job.classes) {
-    if (!(cl.expand || class_single(c, job, cl))) continue;
+    if (!(cl.expand || class_single(job, cl))) continue;
     for (int i = cl.first; i < cl.first + cl.count; ++i) {
       lo = std::min(lo, job.descs[i].row);
       ++cnt;
@@ -2749,7 +2345,7 @@ int cwtb_cwt_to_host(cwtb_ctx *c, const void *signal, int signal_is_f32, int64_t
 #ifndef CWTB_HOST_EMU
   // fp64, analytic family, forked streams: the device->host copy of the rows the single-kernel
   // chain produced starts as soon as that chain is done, while the two-kernel chains still run
-  if (precision == CWTB_F64 && family != CWTB_TABLE && c->two_streams && !c->profiling) {
+  if (precision == CWTB_F64 && family != CWTB_TABLE && !c->profiling) {
     int e = prepare(c, n0, dt, scales, n_scales, family, param, precision, nullptr);
     if (e) return e;
     const Job &job = c->job;
@@ -3601,10 +3197,7 @@ int cwtb_profile_last(cwtb_ctx *c, char *out, size_t cap) {
 #else
   c->prof.clear();
   c->profiling = true;
-  const int ts = c->two_streams;
-  c->two_streams = 0;   // kernels one after the other: per-kernel times are not blurred by overlap
   int e = timed_run(c, c->job_dsig, 1, nullptr);
-  c->two_streams = ts;
   c->profiling = false;
   if (e) return e;
   return profile_report(c, out, cap);
@@ -3617,15 +3210,12 @@ int cwtb_profile_begin(cwtb_ctx *c) {
   if (!c) return CWTB_ERR_ARG;
   c->prof.clear();
   c->profiling = true;
-  c->prof_saved_streams = c->two_streams;
-  c->two_streams = 0;
   return 0;
 }
 int cwtb_profile_end(cwtb_ctx *c, char *out, size_t cap) {
   if (!c || !out || cap < 2) return CWTB_ERR_ARG;
   if (!c->profiling) return fail(c, CWTB_ERR_STATE, "profile_end without profile_begin");
   c->profiling = false;
-  c->two_streams = c->prof_saved_streams;
   return profile_report(c, out, cap);
 }
 

@@ -58,15 +58,7 @@ constexpr int NT = CWTB_NT;  // threads per CTA
 // Pass twiddle tables: for a pass of radix R on sub-transforms of length L the factor
 // w_L^{j c} (c = 1..R-1, j < L/R) is stored at  tw[tw_offset(L) + (c-1)*(L/R) + j], i.e. lanes
 // (consecutive j) read consecutive entries.  Each L has one radix in the plans below.
-#ifndef CWTB_PLAN1024_R32
-#define CWTB_PLAN1024_R32 0
-#endif
-#ifndef CWTB_PLAN256_3PASS
-#define CWTB_PLAN256_3PASS 1
-#endif
-HD constexpr int tw_radix(int L) {
-  return L == 32 ? 4 : (L == 256 ? (CWTB_PLAN256_3PASS ? 4 : 16) : ((L == 1024 && CWTB_PLAN1024_R32) ? 32 : 8));
-}
+HD constexpr int tw_radix(int L) { return (L == 32 || L == 256) ? 4 : 8; }
 HD constexpr int tw_count(int L) { return (tw_radix(L) - 1) * (L / tw_radix(L)); }
 HD constexpr int tw_offset(int L) {
   return L == 32 ? 0 : (L == 64 ? tw_count(32) : tw_offset(L / 2) + tw_count(L / 2));
@@ -97,17 +89,9 @@ CWTB_PLAN(16, 16, 1, 1)
 CWTB_PLAN(32, 4, 8, 1)
 CWTB_PLAN(64, 8, 8, 1)
 CWTB_PLAN(128, 8, 16, 1)
-#if CWTB_PLAN256_3PASS
 CWTB_PLAN(256, 4, 8, 8)
-#else
-CWTB_PLAN(256, 16, 16, 1)
-#endif
 CWTB_PLAN(512, 8, 8, 8)
-#if CWTB_PLAN1024_R32
-CWTB_PLAN(1024, 32, 32, 1)
-#else
 CWTB_PLAN(1024, 8, 8, 16)
-#endif
 #undef CWTB_PLAN
 
 // Shared-memory layout of the tile: [b][pos] with a row pitch chosen so that both
@@ -118,15 +102,9 @@ template <typename T, int K, bool ROWS = false> struct Lay {
   static constexpr int Q = TileCfg<T>::Q;
   // For P < Q one pad element is inserted after every 16 positions (pos + pos/16), which shifts
   // the second position of a quarter-warp onto the free bank groups -> conflict-free in every
-  // pass.  ROWS = true marks tiles whose rows are filled by bulk-async (TMA) copies: with the
-  // skew a row arrives as K/16 copies of 16 elements (CHUNKED); that needs 16-byte aligned
-  // chunk starts, i.e. 16-byte elements (fp64) -- fp32 row tiles stay unskewed (one contiguous
-  // copy per row, 2-way conflict on the last pass's reads when P = Q/2).
-#ifndef CWTB_ROWS_SKEW
-#define CWTB_ROWS_SKEW 0
-#endif
-  static constexpr bool SKEW = (P < Q) && (!ROWS || (CWTB_ROWS_SKEW && sizeof(T) == 8));
-  static constexpr bool CHUNKED = ROWS && SKEW;
+  // pass.  ROWS = true marks tiles whose rows are filled by bulk-async (TMA) copies: they stay
+  // unskewed (one contiguous copy per row, 2-way conflict on the last pass's reads when P = Q/2).
+  static constexpr bool SKEW = (P < Q) && !ROWS;
   static constexpr int KS = SKEW ? K + K / 16 : K;
   static constexpr int PITCH = (P < Q) ? (KS - (KS % Q) + 2 + ((KS % Q) > 2 ? Q : 0)) : K + 1;
   static constexpr int ELEMS = P * PITCH;
@@ -138,12 +116,6 @@ template <typename T, int K, bool ROWS = false> struct Lay {
 // ---- bulk asynchronous copy (TMA, cp.async.bulk) global -> shared with an mbarrier --------
 // One thread arms the barrier with the expected byte count and issues the copies; every
 // thread then waits on the barrier's phase.  Host emulation: plain memcpy, wait is a no-op.
-HD void warp_sync() {
-#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
-  __syncwarp();
-#endif
-}
-
 #ifdef CWTB_HOST_EMU
 inline long long &emu_bulk_copy_faults() {   // misaligned bulk copies seen by the emulation
   static long long n = 0;
@@ -211,13 +183,10 @@ struct TileBarrier {
 
 // Ampere-style asynchronous copy global -> shared of one element (8 or 16 bytes) that bypasses the
 // register file: a thread can have its whole share of a tile in flight at once instead of
-// compiler-sized batches of loads followed by stores.  Off by default for the first kernel of the band
-// scales: the element-wise LDGSTS scatter costs more than the extra loads in flight gain, against
-// batches of four LDG.128 + STS.128 (CWTB_PASSA_ASYNC=1 builds it in).  cp_async_wait() makes the thread's own
+// compiler-sized batches of loads followed by stores.  Not used for the first kernel of the band
+// scales: there the element-wise LDGSTS scatter costs more than the extra loads in flight gain, against
+// batches of four LDG.128 + STS.128.  cp_async_wait() makes the thread's own
 // copies visible to itself; the CTA barrier that follows publishes them.  Host emulation: plain copy.
-#ifndef CWTB_PASSA_ASYNC
-#define CWTB_PASSA_ASYNC 0
-#endif
 template <typename V> HD void cp_async(V *dst, const V *src) {
 #if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
   static_assert(sizeof(V) == 16 || sizeof(V) == 8, "cp_async: 8- or 16-byte elements");

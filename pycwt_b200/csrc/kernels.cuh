@@ -390,14 +390,11 @@ template <typename T> struct PassBArgs {
   unsigned N;
   int first, row0;
   int epi;
-  int zmod;                // Z slot of row `by` is by % zmod
   int pf_dist;             // L2 prefetch distance in tiles (0 = off)
   int ny;                  // gridDim.y of this launch (rows)
   int by0;                 // global index of this launch's first Z row (interleave bookkeeping)
   int ileave;              // > 1: Z row `by` is sub-transform by % ileave of output row by / ileave
                            // (final index n*ileave + by % ileave): three-level path, Np > 2^20
-  int rev;                 // rows are processed last-to-first: the first kernel wrote the last rows
-                           // of Z most recently, they are the ones still resident in L2
 };
 
 // K2 = 1024 leaves P = TILE/K2 = Q/2 transforms per tile (64-byte output runs, 2-way bank
@@ -419,8 +416,10 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
   static constexpr bool ROWS_ALIGNED = (LY::PITCH * sizeof(V)) % 16 == 0;
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
     static_assert(ROWS_ALIGNED, "PassB: tile rows must start on 16-byte boundaries");
+    // rows run last-to-first: the first kernel wrote the last rows of Z most recently, they are
+    // the ones still resident in L2
     const int ey = by;                   // position in execution order
-    if (a.rev) by = a.ny - 1 - ey;
+    by = a.ny - 1 - ey;
     V *sm = (V *)smraw;
     const int U = (int)(a.N / K);
     const int u0 = bx * LY::P;
@@ -428,20 +427,8 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
     tb.bar = (unsigned long long *)((char *)smraw + LY::TILE_BYTES);
     if constexpr (PH == 0) {
       const int nvalid = (U - u0) < LY::P ? (U - u0) : LY::P;
-      const V *src = a.Z + (size_t)(by % a.zmod) * a.N + (size_t)u0 * K;
-      if constexpr (LY::CHUNKED) {
-        // skewed rows (compile-time option CWTB_ROWS_SKEW): 16-element pieces issued by the
-        // lanes of warp 0 after lane 0 has armed the barrier
-        if (tid < 32) {
-          if (tid == 0) tb.init_and_expect((unsigned)(nvalid * K * sizeof(V)));
-          warp_sync();
-          constexpr int NCH = K / 16;
-          for (int i = tid; i < nvalid * NCH; i += 32) {
-            const int b = i / NCH, ch = i % NCH;
-            tb.copy(sm + LY::phys(b, 16 * ch), src + (size_t)b * K + 16 * ch, (unsigned)(16 * sizeof(V)));
-          }
-        }
-      } else if (tid == 0) {
+      const V *src = a.Z + (size_t)by * a.N + (size_t)u0 * K;
+      if (tid == 0) {
         // one thread arms the barrier and issues one bulk copy per row
         tb.init_and_expect((unsigned)(nvalid * K * sizeof(V)));
         for (int b = 0; b < nvalid; ++b)
@@ -454,9 +441,9 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
         int pe = ey;
         const int tiles = (U + LY::P - 1) / LY::P;
         while (t >= tiles && pe + 1 < a.ny) { t -= tiles; ++pe; }
-        const int py = a.rev ? a.ny - 1 - pe : pe;
+        const int py = a.ny - 1 - pe;
         if (t < tiles && t * LY::P + LY::P <= U)
-          TileBarrier::prefetch_l2(a.Z + (size_t)(py % a.zmod) * a.N + (size_t)t * LY::P * K,
+          TileBarrier::prefetch_l2(a.Z + (size_t)py * a.N + (size_t)t * LY::P * K,
                                    (unsigned)(LY::P * K * sizeof(V)));
       }
       for (int b = nvalid; b < LY::P; ++b)
@@ -688,9 +675,7 @@ template <typename T> struct PassAArgs {
   long long in_pitch, n_in;
   unsigned N;
   int first, row0;
-  int zmod;            // Z slot of row `by` is by % zmod (ring of Z buffers in the fused kernel)
   int pf_dist;         // L2 prefetch distance in tiles for the band-product rows (0 = off)
-  int gauss_rec;       // dense Morlet: evaluate the Gaussian by recurrence along each thread's bins
   unsigned K2;         // row length of Z: 1024 (second kernel = PassB) or 2^20 (pre-pass of the
                        // three-level path for Np > 2^20, where the rows are transformed again)
   unsigned Nx;         // MODE_COARSE: length of the signal's spectrum (N is the coarse length)
@@ -751,7 +736,7 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
     const int r20 = (bx % NTILE2) * T2;
     const int M = (int)(a.N / ((unsigned)K1 * a.K2));
     ZStorer<T, SIGN> st;
-    st.Z = a.Z + (size_t)(by % a.zmod) * a.N;
+    st.Z = a.Z + (size_t)by * a.N;
     st.nt = a.nt;
     st.p = p;
     st.M = M;
@@ -791,7 +776,7 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
               TileBarrier::prefetch_l2(row + (size_t)pos * a.K2, (unsigned)(T2 * sizeof(V)));
         }
       }
-      if (MODE == MODE_DENSE && a.fam.family == 0 && a.gauss_rec && T2 <= NT) {
+      if (MODE == MODE_DENSE && a.fam.family == 0 && T2 <= NT) {
         // Morlet, dense scale: a thread's bins are k0, k0 + D, k0 + 2D, ... (D = (NT/T2)*K2), so
         //   g(k + D) = g(k) * rho(k),  rho(k + D) = rho(k) * exp(-a^2),  a = s * w_D,
         // replaces the exp per bin by two multiplies.  Re-seeded with exact exp() when the
@@ -852,24 +837,6 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
             sm[LY::phys(b, pos)] = v;
           }
         }
-      } else if (CWTB_PASSA_ASYNC && MODE == MODE_BAND) {
-        // band products are copied as they are (multi-pass plans apply the twist in pass 1):
-        // asynchronous copies, the thread's 32 elements in flight together
-        const V *base = a.Bbuf + src.d.boff + r20;
-        for (int idx = tid; idx < K1 * T2; idx += NT) {
-          const int b = idx % T2, pos = idx / T2;
-          cp_async(&sm[LY::phys(b, pos)], base + (size_t)pos * a.K2 + b);
-        }
-        cp_async_wait();
-      } else if (CWTB_PASSA_ASYNC && MODE == MODE_CPLX) {
-        const V *row = (const V *)a.in + (size_t)(a.row0 + by) * a.in_pitch;
-        for (int idx = tid; idx < K1 * T2; idx += NT) {
-          const int b = idx % T2, pos = idx / T2;
-          const unsigned r = (unsigned)pos * a.K2 + (unsigned)(r20 + b);
-          if ((long long)r < a.n_in) cp_async(&sm[LY::phys(b, pos)], row + r);
-          else sm[LY::phys(b, pos)] = mk<T>(0, 0);
-        }
-        cp_async_wait();
       } else {
         // (the compiler batches four loads per round trip on its own; eight in flight measured ...)
         CWTB_PRAGMA_UNROLL_A
@@ -937,7 +904,7 @@ template <typename T> struct CoarseArgs {
   NTab nt[11];         // CoarseABody: e^{2 pi i e / Nc} for Nc = 2^(10 + i)
   unsigned Nx;
   int nseg;
-  int pf_dist, rev;    // CoarseBBody: PassBArgs::pf_dist, ::rev
+  int pf_dist;         // CoarseBBody: PassBArgs::pf_dist
   CoarseSeg seg[CSEG_MAX];
 };
 template <typename T> HD const CoarseSeg &coarse_seg(const CoarseArgs<T> &a, int bx) {
@@ -1042,7 +1009,7 @@ template <typename T> struct CoarseABody {
       PassAArgs<T> pa{};
       pa.descs = a.descs; pa.spec = a.spec; pa.tw = a.tw; pa.fam = a.fam; pa.nt = a.nt[g.log2Nc - 10];
       pa.Z = a.Z + a.descs[g.first].ip_coff;
-      pa.N = 1u << g.log2Nc; pa.Nx = a.Nx; pa.first = g.first; pa.zmod = 1 << 30; pa.K2 = K2C;
+      pa.N = 1u << g.log2Nc; pa.Nx = a.Nx; pa.first = g.first; pa.K2 = K2C;
       A<K1>::template phase<PH>(pa, local % per, local / per, tid, sm);
     }
   }
@@ -1084,7 +1051,7 @@ template <typename T> struct CoarseBBody {
     PassBArgs<T> pb{};
     pb.Z = a.Z + off; pb.out = a.C + off; pb.tw = a.tw;
     pb.pitch = Nc; pb.nout = Nc; pb.N = Nc; pb.post = 1.0;
-    pb.epi = EPI_STORE; pb.zmod = 1 << 30; pb.pf_dist = a.pf_dist; pb.ny = g.count; pb.ileave = 1; pb.rev = a.rev;
+    pb.epi = EPI_STORE; pb.pf_dist = a.pf_dist; pb.ny = g.count; pb.ileave = 1;
     B::template phase<PH>(pb, local % per, local / per, tid, sm);
   }
 };
