@@ -338,6 +338,32 @@ int cwtb_wct3_mc_seeded(cwtb_ctx *ctx, uint64_t seed, int64_t first_triple, int 
 int cwtb_mc_surrogates3(cwtb_ctx *ctx, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0,
                         double *out);
 
+/* ---- Monte-Carlo significance against phase-randomised surrogates of the data -------------- */
+/* Null: the data themselves with their Fourier phases randomised (Theiler et al. 1992; multivariate
+ * form Prichard & Theiler 1994).  With X = FFT_n0(x) at the series' own length, unit u of a series
+ * in phase group g is x' = Re IFFT_n0(X'), X'_k = X_k e^{i phi(u,g,k)} for 1 <= k < n0/2,
+ * X'_{n0-k} = conj(X'_k), X'_0 = X_0 and, for even n0, X'_{n0/2} = X_{n0/2}: every series keeps its
+ * power spectrum, mean and variance; series of one group share phi and keep their cross spectrum and
+ * coherence; series of different groups become independent.  phi = 2 pi U, U uniform in (0, 1) from
+ * the Philox4x32-10 stream keyed by `seed`, a pure function of (seed, u, g, k) with a counter tag of
+ * its own (no counter of cwtb_wct_mc_seeded / cwtb_wct3_mc_seeded recurs for 0 <= u < 2^61), so no
+ * split over calls, ranks or GPUs changes a unit.  Transforms and rotation run in fp64; an fp32
+ * coherence gets the fp64 surrogates rounded.
+ * series: host [nser][n0] doubles, nser = 2 or 3; group[nser]: phase group (>= 0) of each series.
+ * nser = 2: hist_a = coherence histogram, hist_b must be NULL.
+ * nser = 3 (y, x1, x2): hist_a = partial, hist_b = multiple, either may be NULL, not both.
+ * Everything else (mask, maxscale, nbins, accumulate-into, precision, smoothing filter, lifetime of
+ * resident results) as cwtb_wct_mc_seeded / cwtb_wct3_mc_seeded.
+ * CWTB_ERR_ARG: nser not 2 or 3, a negative group or unit number, n0 < 4, a null pointer;
+ * CWTB_ERR_UNSUPPORTED: CWTB_TABLE wavelets, n0 > 2^26, or n0 > 2^24 that is not a power of two. */
+int cwtb_wct_mc_phase(cwtb_ctx *ctx, const double *series, int nser, const int *group, uint64_t seed,
+                      int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                      int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                      int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b);
+/* Test hook: the surrogates themselves, out[n_units][nser][n0]. */
+int cwtb_mc_phase_surrogates(cwtb_ctx *ctx, const double *series, int nser, const int *group,
+                             uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out);
+
 /* ---- batched transform of independent channels (SURVEY 8d config 5) ------- */
 /* X: host [n_chan, n0] (float or double).  The per-channel transforms stay on
  * the device; `power_out` (may be NULL) receives the per-channel global wavelet

@@ -12,6 +12,7 @@ from ._engine import Engine, EngineError, default_engine, device_count  # noqa: 
 from .resident import cwt_resident, ResidentTransform  # noqa: F401  (extension, SURVEY 8f)
 from .resident import wct_resident, ResidentCoherence  # noqa: F401  (extension)
 from .wavelet import partial_wct, multiple_wct, wct3_significance  # noqa: F401  (extension)
+from .wavelet import wct_surrogate_significance, wct3_surrogate_significance  # noqa: F401  (extension)
 from .resident import xwt_resident, ResidentCrossWavelet  # noqa: F401  (extension)
 
 __all__ = ['cwt', 'icwt', 'significance', 'xwt', 'wct', 'wct_significance',

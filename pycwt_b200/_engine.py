@@ -91,6 +91,9 @@ _SIGNATURES = {
     "cwtb_wct3_mc_seeded": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I,
                                  _P, _P]),
     "cwtb_mc_surrogates3": (_I, [_P, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_wct_mc_phase": (_I, [_P, _P, _I, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I,
+                                _P, _P]),
+    "cwtb_mc_phase_surrogates": (_I, [_P, _P, _I, _P, ctypes.c_uint64, _I64, _I, _I64, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -805,6 +808,52 @@ class Engine(object):
         out = np.empty((int(n_triples), 3, int(n0)), dtype=np.float64)
         self._check(self.lib.cwtb_mc_surrogates3(self.h, int(seed) & (2 ** 64 - 1), int(first_triple),
                                                  int(n_triples), int(n0), _ptr(out)))
+        return out
+
+    @staticmethod
+    def _phase_inputs(name, series, groups):
+        """The data [nser, n0] and the phase groups of a phase-randomised Monte-Carlo call."""
+        series = np.ascontiguousarray(series, dtype=np.float64)
+        groups = np.ascontiguousarray(groups, dtype=np.int32)
+        if series.ndim != 2 or series.shape[0] not in (2, 3) or groups.shape != (series.shape[0],):
+            raise ValueError("%s: series must be [2 or 3, n0] with one phase group each" % name)
+        if not np.isfinite(series).all():
+            raise ValueError("%s: non-finite sample" % name)
+        return series, groups
+
+    @_locked
+    def wct_mc_phase(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+                     mask, maxscale, nbins, hist_a, hist_b=None, precision=F64):
+        """Monte-Carlo histograms of `n_units` phase-randomised surrogate units of `series`
+        [nser, n0] (cwtb_wct_mc_phase): series of equal `groups` number share the random phases and
+        keep their coherence.  Two series: `hist_a` the coherence histogram.  Three (y, x1, x2):
+        `hist_a` the partial, `hist_b` the multiple coherence, either may be None.  Accumulated
+        into the histograms [S, nbins]."""
+        series, groups = self._phase_inputs("wct_mc_phase", series, groups)
+        nser, n0 = series.shape
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        if mask.shape != (sj.size, n0):
+            raise ValueError("wct_mc_phase: mask must be [scales, n0]")
+        if nser == 2 and hist_b is not None:
+            raise ValueError("wct_mc_phase: two series have one histogram")
+        ha, hb = self._mc3_hists("wct_mc_phase", sj.size, nbins, hist_a, hist_b)
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct_mc_phase(self.h, _ptr(series), nser, _ptr(groups), int(seed) & (2 ** 64 - 1),
+                                               int(first_unit), int(n_units), n0, float(dt), _ptr(sj), sj.size,
+                                               int(family), float(param), int(boxcar_len), _ptr(mask),
+                                               int(maxscale), int(nbins), ha, hb))
+        return hist_a, hist_b
+
+    @_locked
+    def mc_phase_surrogates(self, series, groups, seed, first_unit, n_units):
+        """The surrogate units of `wct_mc_phase`, float64 [n_units, nser, n0]."""
+        series, groups = self._phase_inputs("mc_phase_surrogates", series, groups)
+        out = np.empty((int(n_units),) + series.shape, dtype=np.float64)
+        self._check(self.lib.cwtb_mc_phase_surrogates(self.h, _ptr(series), series.shape[0], _ptr(groups),
+                                                      int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
+                                                      series.shape[1], _ptr(out)))
         return out
 
     @_locked

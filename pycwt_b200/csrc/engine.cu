@@ -215,7 +215,7 @@ struct cwtb_ctx {
   std::vector<double> wtab_host; // host mirror of wtab (tables are appended, never moved)
   size_t wtab_uploaded = 0;      // elements already on the device
   size_t wtab_max_bytes = (size_t)256 << 20;   // CWTB_WTAB_MB: host mirror size above which the cache starts over
-  Buf sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY;
+  Buf sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY, pspec, prot;
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
   // geometry and settings reuses it (planning + descriptor upload: ~0.3 ms for 256 scales, several ms
@@ -259,7 +259,8 @@ struct cwtb_ctx {
                                  // are not blurred by overlap
   const char *prof_tag = "";     // prefix of the kernel names recorded while profiling: "fwd:" (forward
                                  // transform of the signal), "coarse:" (coarse-grid transforms of the
-                                 // expansion path); W-writing launches carry no tag
+                                 // expansion path), "data:" / "phase:" (spectra of the data and generation of
+                                 // their phase-randomised surrogates); W-writing launches carry no tag
   struct ProfRec { std::string name; unsigned gx, gy; int ev; };
   std::vector<ProfRec> prof;
 #ifndef CWTB_HOST_EMU
@@ -1618,7 +1619,7 @@ void cwtb_destroy(cwtb_ctx *c) {
 #endif
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->coh.buf, &c->cross.buf})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -3013,11 +3014,35 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
 
 // common part of the Monte-Carlo entry points, for surrogate units of nser = 2 series (coherence,
 // one histogram) or 3 (partial and multiple coherence, hist[0] and hist[1], either may be null):
-// `noise` host surrogates [n_units][nser][n0], or null -> drawn on the device from
-// (seed, unit0 + i); coherence in the engine type T
+// `noise` host surrogates [n_units][nser][n0]; or `phase` groups -> phase-randomised surrogates of
+// the data whose spectra are in c->pspec, drawn on the device from (seed, unit0 + i); or neither ->
+// white noise drawn on the device from (seed, unit0 + i); coherence in the engine type T
+struct PhaseSrc { int group[3]; };
+
 extern "C++" {
+// nb surrogate units of the data spectra c->pspec [nser][n0] into out [nb][nser][n0]: rotation,
+// inverse transform at length n0 (in place: every row transform reads its chunk of rows into a
+// work buffer before it stores them) and real part.  c->prot holds nb * nser * n0 double2.
 template <typename T>
-static int mc_run(cwtb_ctx *c, int nser, const double *noise, unsigned long long seed, long long unit0,
+static int phase_units(cwtb_ctx *c, const PhaseSrc &ph, int nser, unsigned long long seed, long long unit0, int nb,
+                       int64_t n0, T *out) {
+  const int rows = nser * nb;
+  double2 *R = (double2 *)c->prot.p;
+  struct Tag { cwtb_ctx *c; ~Tag() { c->prof_tag = ""; } } tag{c};
+  c->prof_tag = "phase:";                 // profiles tell the generator's row transforms from the pipeline's
+  PhaseRotArgs ra{(const double2 *)c->pspec.p, R, seed, unit0, (long long)n0, nser, {ph.group[0], ph.group[1], ph.group[2]}};
+  int e = launch<PhaseRotBody>(c, (unsigned)((n0 / 2 + 1 + NT - 1) / NT), (unsigned)rows, ra);
+  if (e) return e;
+  e = (n0 & (n0 - 1)) ? blue_rows(c, R, 0, n0, R, n0, (unsigned)n0, rows, +1, 1.0, n0)
+                      : fft_rows<double, +1>(c, R, 0, n0, n0, R, n0, (unsigned)n0, rows);
+  if (e) return e;
+  const long long cnt = (long long)rows * n0;
+  RealPartArgs<T> pa{R, out, cnt, 1.0 / (double)n0};
+  return launch<RealPartBody<T>>(c, (unsigned)((cnt + NT - 1) / NT), 1, pa);
+}
+
+template <typename T>
+static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed, long long unit0,
                   int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                   double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                   int64_t *const hist[2]) {
@@ -3038,9 +3063,12 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, unsigned long long
   // surrogates of at most `batch` units are resident at a time
   // (host surrogates stay double on the device; an fp32 run rounds one unit at a time into sig)
   const size_t usz = (size_t)nser * n0;             // samples per unit
-  const int batch = noise ? n_units : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_units, ((size_t)256 << 20) / (usz * sizeof(double))));
+  // (the rotated spectra of a batch of phase-randomised units take 16 B per sample)
+  const size_t resident = phase ? sizeof(double2) : sizeof(double);
+  const int batch = noise ? n_units : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_units, ((size_t)256 << 20) / (usz * resident)));
   const size_t nsz = noise ? sizeof(double) : sizeof(T);
   if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * usz * nsz))) return e;
+  if (phase && (e = ensure(c, c->prot, (size_t)std::max(batch, 1) * usz * sizeof(double2)))) return e;
   if (noise) RT(rt_h2d(c->noise.p, noise, (size_t)n_units * usz * sizeof(double), c->stream));
   if (noise && sizeof(T) != 8 && (e = ensure(c, c->sig, usz * sizeof(T)))) return e;
   RT(rt_sync(c->stream));
@@ -3048,7 +3076,9 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, unsigned long long
   if ((e = time_begin(c))) return e;
   for (int i0 = 0; i0 < n_units; i0 += batch) {
     const int nb = std::min(batch, n_units - i0);
-    if (!noise) {
+    if (phase) {
+      if ((e = phase_units<T>(c, *phase, nser, seed, unit0 + i0, nb, n0, (T *)c->noise.p))) return e;
+    } else if (!noise) {
       NoiseArgs<T> na{(T *)c->noise.p, seed, unit0 + i0, (long long)n0, nb, nser};
       if ((e = launch<NoiseBody<T>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * nb), na))) return e;
     }
@@ -3083,8 +3113,8 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, unsigned long long
 }
 }  // extern "C++"
 
-static int mc_core(cwtb_ctx *c, int nser, const double *noise, unsigned long long seed, long long unit0,
-                   int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+static int mc_core(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed,
+                   long long unit0, int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                    double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                    int64_t *const hist[2]) {
   if (!c || !mask || !(hist[0] || hist[1]) || n_units < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
@@ -3093,9 +3123,9 @@ static int mc_core(cwtb_ctx *c, int nser, const double *noise, unsigned long lon
     return fail(c, CWTB_ERR_UNSUPPORTED, nser == 2 ? "wct_mc needs an analytic wavelet family"
                                                    : "wct3_mc needs an analytic wavelet family");
   return c->coh_precision == CWTB_F32
-             ? mc_run<float>(c, nser, noise, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+             ? mc_run<float>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
                              boxcar_len, mask, maxscale, nbins, hist)
-             : mc_run<double>(c, nser, noise, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+             : mc_run<double>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
                               boxcar_len, mask, maxscale, nbins, hist);
 }
 
@@ -3105,7 +3135,7 @@ int cwtb_wct_mc(cwtb_ctx *c, const double *noise, int n_pairs, int64_t n0, doubl
   (void)dj;
   if (!noise) return fail(c, CWTB_ERR_ARG, "wct_mc: null surrogates");
   int64_t *const h[2] = {hist, nullptr};
-  return mc_core(c, 2, noise, 0, 0, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
+  return mc_core(c, 2, noise, nullptr, 0, 0, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
                  maxscale, nbins, h);
 }
 
@@ -3113,7 +3143,7 @@ int cwtb_wct_mc_seeded(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pai
                        const double *scales, int n_scales, int family, double param, int boxcar_len,
                        const uint8_t *mask, int maxscale, int nbins, int64_t *hist) {
   int64_t *const h[2] = {hist, nullptr};
-  return mc_core(c, 2, nullptr, seed, first_pair, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len,
+  return mc_core(c, 2, nullptr, nullptr, seed, first_pair, n_pairs, n0, dt, scales, n_scales, family, param, boxcar_len,
                  mask, maxscale, nbins, h);
 }
 
@@ -3122,7 +3152,7 @@ int cwtb_wct3_mc(cwtb_ctx *c, const double *noise, int n_triples, int64_t n0, do
                  int nbins, int64_t *hist_partial, int64_t *hist_multiple) {
   if (!noise) return fail(c, CWTB_ERR_ARG, "wct3_mc: null surrogates");
   int64_t *const h[2] = {hist_partial, hist_multiple};
-  return mc_core(c, 3, noise, 0, 0, n_triples, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
+  return mc_core(c, 3, noise, nullptr, 0, 0, n_triples, n0, dt, scales, n_scales, family, param, boxcar_len, mask,
                  maxscale, nbins, h);
 }
 
@@ -3131,7 +3161,7 @@ int cwtb_wct3_mc_seeded(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_
                         const uint8_t *mask, int maxscale, int nbins, int64_t *hist_partial,
                         int64_t *hist_multiple) {
   int64_t *const h[2] = {hist_partial, hist_multiple};
-  return mc_core(c, 3, nullptr, seed, first_triple, n_triples, n0, dt, scales, n_scales, family, param,
+  return mc_core(c, 3, nullptr, nullptr, seed, first_triple, n_triples, n0, dt, scales, n_scales, family, param,
                  boxcar_len, mask, maxscale, nbins, h);
 }
 
@@ -3154,6 +3184,69 @@ int cwtb_mc_surrogates(cwtb_ctx *c, uint64_t seed, int64_t first_pair, int n_pai
 
 int cwtb_mc_surrogates3(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_triples, int64_t n0, double *out) {
   return mc_surrogates(c, 3, seed, first_triple, n_triples, n0, out);
+}
+
+// ---- phase-randomised surrogates of the data (PhaseRotBody) -----------------------------------
+// argument checks shared by the two entry points, then the spectra of the nser series at their own
+// length into c->pspec (fp64; the reals are staged in c->prot)
+static int phase_spectra(cwtb_ctx *c, const char *name, const double *series, int nser, const int *group,
+                         int64_t first_unit, int n_units, int64_t n0, PhaseSrc *ph) {
+  const std::string nm(name);
+  if (!c || !series || !group || (nser != 2 && nser != 3) || n0 < 4 || n_units < 0 || first_unit < 0 ||
+      first_unit > (1ll << 61) - n_units)
+    return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  for (int r = 0; r < nser; ++r) {
+    if (group[r] < 0) return fail(c, CWTB_ERR_ARG, nm + ": negative phase group");
+    ph->group[r] = group[r];
+  }
+  const bool pow2 = (n0 & (n0 - 1)) == 0;
+  if (n0 > (pow2 ? 1ll << 26 : 1ll << 24))
+    return fail(c, CWTB_ERR_UNSUPPORTED, nm + ": series longer than 2^26 (2^24 if the length is not 2^k)");
+#ifndef CWTB_HOST_EMU
+  RT(cudaSetDevice(c->device));
+#endif
+  const size_t cnt = (size_t)nser * n0;
+  int e;
+  if ((e = ensure(c, c->pspec, cnt * sizeof(double2)))) return e;
+  if ((e = ensure(c, c->prot, cnt * sizeof(double)))) return e;
+  RT(rt_h2d(c->prot.p, series, cnt * sizeof(double), c->stream));
+  c->prof_tag = "data:";
+  e = pow2 ? fft_rows<double, -1>(c, c->prot.p, 1, n0, n0, (double2 *)c->pspec.p, n0, (unsigned)n0, nser)
+           : blue_rows(c, c->prot.p, 1, n0, (double2 *)c->pspec.p, n0, (unsigned)n0, nser, -1, 1.0, n0);
+  c->prof_tag = "";
+  if (e) return e;
+  RT(rt_sync(c->stream));   // `series` is the caller's again
+  return 0;
+}
+
+int cwtb_wct_mc_phase(cwtb_ctx *c, const double *series, int nser, const int *group, uint64_t seed,
+                      int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                      int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                      int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b) {
+  if (nser == 2 && hist_b) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: two series have one histogram");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc_phase needs an analytic wavelet family");
+  if (!mask || !(hist_a || hist_b)) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: bad argument");
+  PhaseSrc ph{};
+  int e = phase_spectra(c, "wct_mc_phase", series, nser, group, first_unit, n_units, n0, &ph);
+  if (e) return e;
+  int64_t *const h[2] = {hist_a, hist_b};
+  return mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                 boxcar_len, mask, maxscale, nbins, h);
+}
+
+int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const int *group, uint64_t seed,
+                             int64_t first_unit, int n_units, int64_t n0, double *out) {
+  if (!out || n_units < 1) return fail(c, CWTB_ERR_ARG, "mc_phase_surrogates: bad argument");
+  PhaseSrc ph{};
+  int e = phase_spectra(c, "mc_phase_surrogates", series, nser, group, first_unit, n_units, n0, &ph);
+  if (e) return e;
+  const size_t cnt = (size_t)n_units * nser * n0;
+  if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
+  if ((e = ensure(c, c->prot, cnt * sizeof(double2)))) return e;
+  if ((e = phase_units<double>(c, ph, nser, seed, first_unit, n_units, n0, (double *)c->noise.p))) return e;
+  RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

@@ -1653,6 +1653,70 @@ template <typename T> struct NoiseBody {
   }
 };
 
+// ---- Body: phase-randomised surrogates of the data (Theiler et al. 1992; Prichard & Theiler 1994) --
+// For a real series x of length n with X = FFT_n(x) (the series' own length, not padded), surrogate
+// unit u of a series in phase group g is x' = Re IFFT_n(X') with
+//   X'_k = X_k e^{i phi(u,g,k)} for 1 <= k < n/2,   X'_{n-k} = conj(X'_k),   X'_0 = X_0,
+//   X'_{n/2} = X_{n/2} for even n.
+// |X'| = |X| bin by bin: the power spectrum, the mean and the variance of the series are kept.
+// Series of one group share phi, so their cross spectrum X_a conj(X_b), hence their coherence, is
+// kept too; series of different groups get independent phases.  phi = 2 pi U, U uniform in (0, 1)
+// (53 bits of one Philox4x32-10 block, NoiseBody's conversion), a pure function of (seed, u, g, k):
+// independent of the launch geometry, of the batching, of the rank and of which series uses it.
+// Counter words: (k, g, u lo, 2^31 | (u hi << 2) | 3).  The white-noise pairs never set bit 31 of the
+// last word (units below 2^62) and the triples never set both of its low bits (ser <= 2), so for
+// 0 <= u < 2^61 no counter coincides with one of NoiseBody's.  k < 2^32 and 0 <= g < 2^31.
+// One thread per bin pair (k, n - k) of one series of one unit: the Hermitian half is written, not
+// recomputed.  fp64 whatever the coherence precision.
+struct PhaseRotArgs {
+  const double2 *spec;      // [nser][n] spectra of the data
+  double2 *out;             // [n_units][nser][n] rotated spectra
+  unsigned long long seed;
+  long long unit0;          // global index of the first unit
+  long long n;
+  int nser;
+  int group[3];             // phase group of each series
+};
+struct PhaseRotBody {
+  using Args = PhaseRotArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long k = (long long)bx * NT + tid;
+    if (2 * k > a.n) return;
+    const int ser = by % a.nser;
+    const double2 *src = a.spec + (size_t)ser * a.n;
+    double2 *dst = a.out + (size_t)by * a.n;
+    if (k == 0 || 2 * k == a.n) {   // mean and Nyquist bin stay
+      dst[k] = src[k];
+      return;
+    }
+    const unsigned long long unit = (unsigned long long)(a.unit0 + by / a.nser);
+    unsigned o[4];
+    philox4x32_10((unsigned)k, (unsigned)a.group[ser], (unsigned)unit, 0x80000000u | ((unsigned)(unit >> 32) << 2) | 3u,
+                  (unsigned)a.seed, (unsigned)(a.seed >> 32), o);
+    const double u = ((double)(o[0] >> 5) * 67108864.0 + (double)(o[1] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
+    double sn, cs;
+    sincospi_hd(2.0 * u, &sn, &cs);
+    const double2 x = src[k];
+    const double2 r = make_double2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
+    dst[k] = r;
+    dst[a.n - k] = make_double2(r.x, -r.y);
+  }
+};
+
+// ---- Body: out[i] = (T)(Re in[i] * f): the surrogates of the inverse transform, in the engine type --
+template <typename T> struct RealPartArgs { const double2 *in; T *out; long long count; double f; };
+template <typename T> struct RealPartBody {
+  using Args = RealPartArgs<T>;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const long long i = (long long)bx * NT + tid;
+    if (i < a.count) a.out[i] = (T)(a.in[i].x * a.f);
+  }
+};
+
 // ---- Body: scale-axis boxcar (mothers.py:100-102; scipy convolve2d 'same', zero fill) ------
 //   out[i] = sum_t win[t] * in[i - (t - off)],  off = (K-1)//2, rows outside [0, m) are zero
 // Sums in the engine type T, like WctFinalBody; any K (no shared memory).

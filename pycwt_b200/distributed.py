@@ -271,6 +271,40 @@ def wct3_significance_sharded(al_y, al1, al2, dt, dj, s0, J, significance_level=
             wv._mc_levels(prob, hist[1], significance_level))
 
 
+def _surrogate_significance_sharded(series, groups, dt, dj, s0, J, significance_level, wavelet, normalize,
+                                    mc_count, seed, engine, comm, device, precision):
+    from . import wavelet as wv
+    p, prob = wv._surrogate_problem(series, dt, dj, s0, J, wavelet, normalize, precision)
+    comm = _as_comm(comm)
+    rank, world = _rank_world(comm)
+    lo, hi = shard_range(mc_count, rank, world)
+    hist = wv._surrogate_histogram(p, prob, groups, seed, lo, hi - lo, engine=engine)
+    hist = sum_over_ranks(hist, comm, device)
+    return [wv._mc_levels(prob, h, significance_level) for h in hist]
+
+
+def wct_surrogate_significance_sharded(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
+                                       wavelet='morlet', normalize=True, mc_count=300, seed=0, engine=None,
+                                       comm=None, device=None, precision='fp64'):
+    """`wavelet.wct_surrogate_significance` with the phase-randomised surrogate pairs
+    block-partitioned over the ranks: every rank holds the data, draws pairs (seed, i) of its block
+    on its GPU and accumulates their histogram, ONE all-reduce combines them and every rank
+    evaluates the levels.  The result is independent of the world size."""
+    return _surrogate_significance_sharded((y1, y2), (0, 1), dt, dj, s0, J, significance_level, wavelet,
+                                           normalize, mc_count, seed, engine, comm, device, precision)[0]
+
+
+def wct3_surrogate_significance_sharded(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
+                                        wavelet='morlet', normalize=True, mc_count=300, seed=0, engine=None,
+                                        comm=None, device=None, precision='fp64', conditional=True):
+    """`wavelet.wct3_surrogate_significance` with the surrogate triples block-partitioned over the
+    ranks, as `wct_surrogate_significance_sharded`; one all-reduce of both histograms.  Returns
+    (sig_partial, sig_multiple), independent of the world size."""
+    return tuple(_surrogate_significance_sharded((y, x1, x2), (0, 1, 1) if conditional else (0, 1, 2), dt, dj,
+                                                 s0, J, significance_level, wavelet, normalize, mc_count,
+                                                 seed, engine, comm, device, precision))
+
+
 def scale_rows(n_scales, rank, world, layout='cyclic'):
     """Scales owned by `rank`: 'cyclic' (j = rank, rank + world, ...) balances the cost -- the small
     scales (wide bands, two-kernel transforms) cost 4x the large ones, a contiguous block would give

@@ -500,11 +500,13 @@ def _wct3(y, x1, x2, dt, dj, s0, J, wavelet, normalize, precision, partial):
     return (RP2 if partial else RM2), _coi(p.wavelet, dt, p.n0), p.freq
 
 
-def _mc_problem(dt, dj, s0, J, wavelet):
+def _mc_problem(dt, dj, s0, J, wavelet, N=None):
     """Geometry of the Monte-Carlo coherence problem (reference wavelet.py:588-607): surrogate
-    length, scales, cone-of-influence mask, last valid scale and the sig95 template."""
-    ms = s0 * (2 ** (J * dj)) / dt
-    N = int(np.ceil(ms * 6))
+    length, scales, cone-of-influence mask, last valid scale and the sig95 template.  `N`: the
+    surrogate length; by default the reference's, derived from the largest scale."""
+    if N is None:
+        ms = s0 * (2 ** (J * dj)) / dt
+        N = int(np.ceil(ms * 6))
     sj = s0 * 2 ** (np.arange(0, J + 1) * dj)
     freq = 1 / (wavelet.flambda() * sj)
     coi = (N / 2 - np.abs(np.arange(0, N) - (N - 1) / 2))
@@ -690,6 +692,106 @@ def wct3_significance(al_y, al1, al2, dt, dj, s0, J, significance_level=0.95, wa
                              nser=3)
     else:
         hist = _mc_histogram_seeded(prob, dt, dj, wavelet, seed, 0, mc_count, precision=prec, nser=3)
+    return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
+
+
+def _surrogate_problem(series, dt, dj, s0, J, wavelet, normalize, precision):
+    """(p, prob) of a Monte-Carlo run against phase-randomised surrogates of `series`: the
+    `_wct_problem` of the data and the Monte-Carlo geometry of their own length and cone of
+    influence."""
+    p = _wct_problem(series, dt, dj, s0, J, wavelet, normalize, precision)
+    if any(y.size != p.n0 for y in p.yns):
+        raise ValueError('the series must have the same length')
+    if not all(np.isfinite(y).all() for y in p.yns):
+        raise ValueError('the series must be finite: phase randomisation transforms every sample')
+    _family_of(p.wavelet)
+    return p, _mc_problem(dt, dj, p.s0, p.J, p.wavelet, N=p.n0)
+
+
+def _surrogate_histogram(p, prob, groups, seed, first, count, engine=None):
+    """Histograms int64 [nser - 1, S, nbins] of the coherence (two series) or of the partial and
+    multiple coherence (three) of the surrogate units first .. first + count - 1 of the
+    standardised data `p.yns`, drawn and accumulated on the device in one transaction."""
+    nser = len(p.yns)
+    hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
+    eng = engine or _engine.default_engine()
+
+    def call(*a, boxcar_len, precision):
+        dt, _, sj, family, param = a[nser:]
+        eng.wct_mc_phase(np.stack(a[:nser]), groups, seed, first, count, dt, sj, family, param, boxcar_len,
+                         prob['mask'], prob['maxscale'], prob['nbins'], *hist, precision=precision)
+
+    _wct_on_device(eng, p, call)
+    return hist
+
+
+def _surrogate_seed(seed):
+    """`seed`, or one draw from numpy's global RNG (so np.random.seed makes a run repeatable)."""
+    return int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+
+
+def wct_surrogate_significance(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
+                               wavelet='morlet', normalize=True, mc_count=300, seed=None,
+                               precision='fp64'):
+    """Monte-Carlo significance level of the wavelet coherence of `y1` and `y2` per scale, against
+    phase-randomised surrogates of the data themselves.  An extension: the reference tests against
+    white noise only (`wct_significance`).
+
+    Null: each surrogate pair is the two standardised series with the Fourier phases of each
+    replaced by independent uniform random phases (Theiler et al. 1992), at the series' own length
+    n0: X'_k = X_k e^{i phi_k} for 1 <= k < n0/2, Hermitian completion, mean and Nyquist bin kept.
+    Every surrogate keeps the power spectrum, mean and variance of its series exactly; the two are
+    independent of each other.  Each pair goes through the whole pipeline of `wct`.
+
+    The arguments are those of `wct`, resolved the same way (scales, boxcar, standardisation,
+    `precision`, errors), so the result, float64 [J + 1], lines up row for row with the WCT of the
+    same arguments: `WCT > sig[:, None]`.  The geometry is the data's: the histograms count the
+    points inside the cone of influence of an n0-point record.  Conventions of `wct_significance`:
+    the `significance_level` quantile of the 1000-bin histogram, NaN from the last row with such
+    points on, 0 for a row without any.
+
+    The surrogates are drawn on the device from a counter-based Philox stream keyed by (`seed`,
+    pair number), in one device transaction (no progress bar); `seed=None` takes one draw from
+    numpy's global RNG as the seed, so `np.random.seed` makes a run repeatable.  Transforms of the
+    surrogate generator run in fp64 whatever `precision`.  A non-finite sample or series of unequal
+    lengths raise ValueError.  No on-disk cache (the key would have to hash the data).
+
+    Phase randomisation assumes a stationary record and treats it as circular: a strong trend or a
+    mismatch between the two ends is spread over all frequencies of the surrogates and biases the
+    level, so detrend the series first (as the samples do).  The surrogates are Gaussian-like
+    whatever the data's amplitude distribution (no amplitude adjustment)."""
+    p, prob = _surrogate_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
+    hist = _surrogate_histogram(p, prob, (0, 1), _surrogate_seed(seed), 0, mc_count)
+    return _mc_levels(prob, hist[0], significance_level)
+
+
+def wct3_surrogate_significance(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
+                                wavelet='morlet', normalize=True, mc_count=300, seed=None,
+                                precision='fp64', conditional=True):
+    """Monte-Carlo significance levels of `partial_wct` and `multiple_wct` per scale, against
+    phase-randomised surrogates of the data themselves.  Returns (sig_partial, sig_multiple),
+    float64 [J + 1] each, row for row with the RP2 / RM2 of the same arguments.
+
+    Null, `conditional=True` (default): in every surrogate triple x1 and x2 are rotated by the SAME
+    random phases and y by phases of its own (Prichard & Theiler 1994).  x1 and x2 keep their power
+    spectra and their cross spectrum, hence their coherence and phase relation, exactly; y keeps
+    its power spectrum and is independent of both.  This is the null of "y is unrelated to x1 and
+    x2, which are related to each other as in the data", the one RP2 and RM2 need where x1 and x2
+    share a driver.  `conditional=False`: three independent sets of phases, the data-coloured
+    counterpart of `wct3_significance`'s null (no coherence between x1 and x2 is kept).
+
+    Everything else as `wct_surrogate_significance`: arguments and errors of `partial_wct`, the
+    data's length and cone of influence, the conventions of `wct_significance` for the levels, a
+    point whose RP2 or RM2 is not finite is not counted, Philox stream keyed by (`seed`, triple
+    number), `seed=None` draws the seed from numpy's global RNG, no cache, no progress bar.
+
+    Phase randomisation assumes a stationary record and treats it as circular: a strong trend or a
+    mismatch between the two ends is spread over all frequencies of the surrogates and biases the
+    level, so detrend the series first (as the samples do).  The surrogates are Gaussian-like
+    whatever the data's amplitude distribution (no amplitude adjustment)."""
+    p, prob = _surrogate_problem((y, x1, x2), dt, dj, s0, J, wavelet, normalize, precision)
+    hist = _surrogate_histogram(p, prob, (0, 1, 1) if conditional else (0, 1, 2), _surrogate_seed(seed),
+                                0, mc_count)
     return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
 
 
