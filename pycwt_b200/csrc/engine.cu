@@ -20,9 +20,8 @@
 #include <vector>
 
 #include <cuda_runtime.h>
-#ifndef CWTB_HOST_EMU
 #include <dlfcn.h>
-#endif
+#include <initializer_list>
 
 #include "../../include/cwt_b200.h"
 #include "kernels.cuh"
@@ -38,8 +37,13 @@ template <class B> struct BodyNT<B, std::void_t<decltype(B::NTB)>> { static cons
 // ======================================================================================
 // runtime abstraction
 // ======================================================================================
+// Everything the host code asks of the CUDA runtime goes through these wrappers, so that the
+// emulation build runs the same host control flow.  There, streams and events are plain handles:
+// every launch runs to completion in the order it is issued, which satisfies every wait, so
+// recording, waiting and synchronising do nothing and no time elapses.
 #ifdef CWTB_HOST_EMU
 typedef int rt_stream;
+typedef int rt_event;
 static inline int rt_malloc(void **p, size_t n) { *p = malloc(n ? n : 1); return *p ? 0 : 1; }
 static inline int rt_free(void *p) { free(p); return 0; }
 static inline int rt_host_alloc(void **p, size_t n) { *p = malloc(n ? n : 1); return *p ? 0 : 1; }
@@ -49,8 +53,25 @@ static inline int rt_d2h(void *d, const void *s, size_t n, rt_stream) { memcpy(d
 static inline int rt_memset(void *d, int v, size_t n, rt_stream) { memset(d, v, n); return 0; }
 static inline int rt_sync(rt_stream) { return 0; }
 static inline const char *rt_errstr(int) { return "emulation error"; }
+static inline int rt_event_create(rt_event *e) { *e = 0; return 0; }
+static inline int rt_event_create_sync(rt_event *e) { *e = 0; return 0; }
+static inline int rt_event_destroy(rt_event) { return 0; }
+static inline int rt_record(rt_event, rt_stream) { return 0; }
+static inline int rt_wait(rt_stream, rt_event) { return 0; }
+static inline int rt_event_sync(rt_event) { return 0; }
+static inline int rt_elapsed_ms(float *ms, rt_event, rt_event) { *ms = 0; return 0; }
+static inline int rt_stream_create(rt_stream *s) { *s = 0; return 0; }
+static inline int rt_stream_create_highest(std::initializer_list<rt_stream *> ss) {
+  for (rt_stream *s : ss) *s = 0;
+  return 0;
+}
+static inline int rt_stream_destroy(rt_stream) { return 0; }
+static inline int rt_set_device(int) { return 0; }
+static inline int rt_device_count(int *n) { *n = 1; return 0; }
+static inline int rt_sm_count(int *, int) { return 0; }   // keeps the caller's value
 #else
 typedef cudaStream_t rt_stream;
+typedef cudaEvent_t rt_event;
 static inline int rt_malloc(void **p, size_t n) { return (int)cudaMalloc(p, n ? n : 1); }
 static inline int rt_free(void *p) { return (int)cudaFree(p); }
 static inline int rt_host_alloc(void **p, size_t n) { return (int)cudaHostAlloc(p, n ? n : 1, cudaHostAllocDefault); }
@@ -64,6 +85,28 @@ static inline int rt_d2h(void *d, const void *s, size_t n, rt_stream st) {
 static inline int rt_memset(void *d, int v, size_t n, rt_stream st) { return (int)cudaMemsetAsync(d, v, n, st); }
 static inline int rt_sync(rt_stream st) { return (int)cudaStreamSynchronize(st); }
 static inline const char *rt_errstr(int e) { return cudaGetErrorString((cudaError_t)e); }
+static inline int rt_event_create(rt_event *e) { return (int)cudaEventCreate(e); }
+static inline int rt_event_create_sync(rt_event *e) { return (int)cudaEventCreateWithFlags(e, cudaEventDisableTiming); }
+static inline int rt_event_destroy(rt_event e) { return (int)cudaEventDestroy(e); }
+static inline int rt_record(rt_event e, rt_stream st) { return (int)cudaEventRecord(e, st); }
+static inline int rt_wait(rt_stream st, rt_event e) { return (int)cudaStreamWaitEvent(st, e, 0); }
+static inline int rt_event_sync(rt_event e) { return (int)cudaEventSynchronize(e); }
+static inline int rt_elapsed_ms(float *ms, rt_event e0, rt_event e1) { return (int)cudaEventElapsedTime(ms, e0, e1); }
+static inline int rt_stream_create(rt_stream *s) { return (int)cudaStreamCreateWithFlags(s, cudaStreamNonBlocking); }
+// streams of the device's highest priority; every one is created, the first error is returned
+static inline int rt_stream_create_highest(std::initializer_list<rt_stream *> ss) {
+  int lo = 0, hi = 0;   // numerically lower = higher priority
+  int e = (int)cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  for (rt_stream *s : ss) {
+    const int r = (int)cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, hi);
+    if (!e) e = r;
+  }
+  return e;
+}
+static inline int rt_stream_destroy(rt_stream st) { return (int)cudaStreamDestroy(st); }
+static inline int rt_set_device(int d) { return (int)cudaSetDevice(d); }
+static inline int rt_device_count(int *n) { return (int)cudaGetDeviceCount(n); }
+static inline int rt_sm_count(int *n, int d) { return (int)cudaDeviceGetAttribute(n, cudaDevAttrMultiProcessorCount, d); }
 
 template <class B, class = void> struct BodyMinB { static constexpr int value = CWTB_MINB; };
 template <class B> struct BodyMinB<B, std::void_t<decltype(B::MINB)>> { static constexpr int value = B::MINB; };
@@ -263,16 +306,12 @@ struct cwtb_ctx {
                                  // their phase-randomised surrogates); W-writing launches carry no tag
   struct ProfRec { std::string name; unsigned gx, gy; int ev; };
   std::vector<ProfRec> prof;
-#ifndef CWTB_HOST_EMU
-  std::vector<cudaEvent_t> prof_events;
-#endif
+  std::vector<rt_event> prof_events;
   std::set<void *> pinned, devallocs;
-#ifndef CWTB_HOST_EMU
-  cudaEvent_t e0{}, e1{};
-  cudaEvent_t ev_fork{}, ev_join{}, ev_joinc[3]{}, ev_coarse{}, ev_coarse_short{};
-  cudaEvent_t ev_h2d[2]{}, ev_used[2]{};
-  cudaEvent_t ev_angle{};
-#endif
+  rt_event e0{}, e1{};
+  rt_event ev_fork{}, ev_join{}, ev_joinc[3]{}, ev_coarse{}, ev_coarse_short{};
+  rt_event ev_h2d[2]{}, ev_used[2]{};
+  rt_event ev_angle{};
 };
 
 static int fail(cwtb_ctx *c, int code, const std::string &msg) {
@@ -318,46 +357,57 @@ static std::string body_name(const char *pretty) {
   return s;
 }
 
-template <class Body>
-static int launch(cwtb_ctx *c, unsigned gx, unsigned gy, const typename Body::Args &a) {
+constexpr unsigned MAX_ROWS = 65535;   // gridDim.y: rows of one launch
+
+// What every launch of Body shares: an empty grid launches nothing, at most MAX_ROWS rows,
+// and while profiling the launch is recorded under the body's name between an event pair.
+// `dispatch()` launches on c->cur and returns 0 or an error.
+template <class Body, class Dispatch>
+static int launch_rec(cwtb_ctx *c, unsigned gx, unsigned gy, Dispatch &&dispatch) {
   if (gx == 0 || gy == 0) return 0;
-#ifdef CWTB_HOST_EMU
-  std::vector<unsigned char> smv(Body::SMEM + 64);
-  unsigned char *sm = smv.data();
-  sm += (16 - ((unsigned long long)sm & 15)) & 15;   // 16-byte aligned base, like the device's
-  for (unsigned by = 0; by < gy; ++by)
-    for (unsigned bx = 0; bx < gx; ++bx) emu_phases<Body, 0>(a, (int)bx, (int)by, sm);
-  c->launches++;
-  if (emu_bulk_copy_faults() != 0) {
-    emu_bulk_copy_faults() = 0;
-    return fail(c, CWTB_ERR_CUDA, "emulation: bulk-async copy with a misaligned address or size");
-  }
-  return 0;
-#else
-  const void *fn = (const void *)k_run<Body>;
-  if (Body::SMEM > 48 * 1024 && !c->configured.count(fn)) {
-    RT(cudaFuncSetAttribute(k_run<Body>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Body::SMEM));
-    c->configured.insert(fn);
-  }
-  // gridDim.y is limited to 65535
-  if (gy > 65535) return fail(c, CWTB_ERR_ARG, "too many rows in one launch");
+  if (gy > MAX_ROWS) return fail(c, CWTB_ERR_ARG, "too many rows in one launch");
   int ev = -1;
   if (c->profiling) {
     ev = (int)c->prof.size() * 2;
     while ((int)c->prof_events.size() < ev + 2) {
-      cudaEvent_t e;
-      RT(cudaEventCreate(&e));
+      rt_event e;
+      RT(rt_event_create(&e));
       c->prof_events.push_back(e);
     }
     c->prof.push_back({std::string(c->prof_tag) + body_name(__PRETTY_FUNCTION__), gx, gy, ev});
-    RT(cudaEventRecord(c->prof_events[ev], c->cur));
+    RT(rt_record(c->prof_events[ev], c->cur));
   }
-  k_run<Body><<<dim3(gx, gy), BodyNT<Body>::value, Body::SMEM, c->cur>>>(a);
-  RT(cudaGetLastError());
-  if (ev >= 0) RT(cudaEventRecord(c->prof_events[ev + 1], c->cur));
+  int e = dispatch();
+  if (e) return e;
+  if (ev >= 0) RT(rt_record(c->prof_events[ev + 1], c->cur));
   c->launches++;
   return 0;
+}
+
+template <class Body>
+static int launch(cwtb_ctx *c, unsigned gx, unsigned gy, const typename Body::Args &a) {
+  return launch_rec<Body>(c, gx, gy, [&]() -> int {
+#ifdef CWTB_HOST_EMU
+    std::vector<unsigned char> smv(Body::SMEM + 64);
+    unsigned char *sm = smv.data();
+    sm += (16 - ((unsigned long long)sm & 15)) & 15;   // 16-byte aligned base, like the device's
+    for (unsigned by = 0; by < gy; ++by)
+      for (unsigned bx = 0; bx < gx; ++bx) emu_phases<Body, 0>(a, (int)bx, (int)by, sm);
+    if (emu_bulk_copy_faults() != 0) {
+      emu_bulk_copy_faults() = 0;
+      return fail(c, CWTB_ERR_CUDA, "emulation: bulk-async copy with a misaligned address or size");
+    }
+#else
+    const void *fn = (const void *)k_run<Body>;
+    if (Body::SMEM > 48 * 1024 && !c->configured.count(fn)) {
+      RT(cudaFuncSetAttribute(k_run<Body>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Body::SMEM));
+      c->configured.insert(fn);
+    }
+    k_run<Body><<<dim3(gx, gy), BodyNT<Body>::value, Body::SMEM, c->cur>>>(a);
+    RT(cudaGetLastError());
 #endif
+    return 0;
+  });
 }
 
 // ======================================================================================
@@ -1075,7 +1125,6 @@ static size_t band_chunk_elems(const Job &job, int G) {
 // one CTA per resident slot (occupancy x SMs), each looping over the rows x gm tiles of the launch
 template <class Body>
 static int launch_persistent(cwtb_ctx *c, unsigned gm, unsigned rows, const typename Body::Args &a) {
-  if (gm == 0 || rows == 0) return 0;
   auto kern = k_persist<Body>;
   const void *fn = (const void *)kern;
   if (!c->configured.count(fn)) {
@@ -1088,22 +1137,11 @@ static int launch_persistent(cwtb_ctx *c, unsigned gm, unsigned rows, const type
   const unsigned long long total = (unsigned long long)gm * rows;
   if (total > 0xffffffffull) return fail(c, CWTB_ERR_ARG, "too many tiles in one launch");
   const unsigned grid = (unsigned)std::min<unsigned long long>(total, (unsigned long long)occ * c->num_sms);
-  int ev = -1;
-  if (c->profiling) {
-    ev = (int)c->prof.size() * 2;
-    while ((int)c->prof_events.size() < ev + 2) {
-      cudaEvent_t e;
-      RT(cudaEventCreate(&e));
-      c->prof_events.push_back(e);
-    }
-    c->prof.push_back({std::string(c->prof_tag) + body_name(__PRETTY_FUNCTION__), grid, rows, ev});
-    RT(cudaEventRecord(c->prof_events[ev], c->cur));
-  }
-  kern<<<grid, Body::NTB, Body::SMEM, c->cur>>>(a, gm, (unsigned)total);
-  RT(cudaGetLastError());
-  if (ev >= 0) RT(cudaEventRecord(c->prof_events[ev + 1], c->cur));
-  c->launches++;
-  return 0;
+  return launch_rec<Body>(c, grid, rows, [&]() -> int {
+    kern<<<grid, Body::NTB, Body::SMEM, c->cur>>>(a, gm, (unsigned)total);
+    RT(cudaGetLastError());
+    return 0;
+  });
 }
 #endif
 
@@ -1144,8 +1182,6 @@ static int launch_expand_t(cwtb_ctx *c, const ExpandArgs<T> &a, int rows, int mi
       return launch_persistent<ExpandMmaBody<TAPS>>(c, gm, rows, a);
     }
   }
-#endif
-#ifndef CWTB_HOST_EMU
   if constexpr (TAPS > 16) {
     return fail(c, CWTB_ERR_STATE, "expansion: tap counts above 16 exist on the tensor-core kernel only");
   } else
@@ -1242,28 +1278,24 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   // band products) run on a second stream so that their CTAs fill the tails of the chains.  While
   // profiling, every launch stays on the engine's stream.
   const bool split = !c->profiling;
-#ifndef CWTB_HOST_EMU
   if (split) {
-    RT(cudaEventRecord(c->ev_fork, c->stream));
-    RT(cudaStreamWaitEvent(c->aux_stream, c->ev_fork, 0));
-    for (int k = 1; k < c->n_chains; ++k) RT(cudaStreamWaitEvent(c->chain_streams[k - 1], c->ev_fork, 0));
+    RT(rt_record(c->ev_fork, c->stream));
+    RT(rt_wait(c->aux_stream, c->ev_fork));
+    for (int k = 1; k < c->n_chains; ++k) RT(rt_wait(c->chain_streams[k - 1], c->ev_fork));
   }
-#endif
   // ---- expansion classes (kernels.cuh: ExpandBody): the coarse transforms of every expansion row
   // form their coarse spectra while they fill their tiles, in one launch for the coarse lengths up
   // to 1024 and one launch pair for the longer ones; then one expansion launch per tap count.
   if (job.coarse_elems) {
     const bool prio = split && c->prio_mode > 0;
-#ifndef CWTB_HOST_EMU
     // the coarse launches go to high-priority streams: queued behind the big launches of the other
     // streams they would only advance in those launches' tails.  Short and long coarse lengths run
     // side by side; an expansion launch waits only for the lengths it reads.
     if (prio) {
-      RT(cudaStreamWaitEvent(c->prio_stream, c->ev_fork, 0));
-      RT(cudaStreamWaitEvent(c->prio_short, c->ev_fork, 0));
+      RT(rt_wait(c->prio_stream, c->ev_fork));
+      RT(rt_wait(c->prio_short, c->ev_fork));
     }
     if (split) c->cur = prio ? c->prio_stream : c->aux_stream;
-#endif
     if ((e = ensure(c, c->Cout, job.coarse_elems * sizeof(V)))) return e;
     // segments: consecutive expansion rows of one coarse length (their coarse rows are contiguous)
     std::vector<CoarseSeg> short_segs, long_segs;
@@ -1292,26 +1324,20 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
       if ((e = launch_coarse<CoarseBBody<T>>(c, ca, long_segs))) return e;
     }
     if (!short_segs.empty()) {
-#ifndef CWTB_HOST_EMU
       if (prio) c->cur = c->prio_short;
-#endif
       if ((e = launch_coarse<CoarseRowsBody<T>>(c, ca, short_segs))) return e;
     }
     c->prof_tag = "";
-#ifndef CWTB_HOST_EMU
     if (prio) {
-      RT(cudaEventRecord(c->ev_coarse_short, c->prio_short));
-      RT(cudaEventRecord(c->ev_coarse, c->prio_stream));
+      RT(rt_record(c->ev_coarse_short, c->prio_short));
+      RT(rt_record(c->ev_coarse, c->prio_stream));
       c->cur = c->prio_mode == 1 ? c->aux_stream : c->prio_stream;   // 1: expansion kernels at ordinary priority
-      RT(cudaStreamWaitEvent(c->cur, c->ev_coarse_short, 0));
+      RT(rt_wait(c->cur, c->ev_coarse_short));
     }
-#endif
     // one expansion launch per tap count (classes are sorted by taps first): those that read only
     // coarse lengths up to 1024 first, the others behind the long coarse transforms
     for (int pass = 0; pass < 2 && !e; ++pass) {
-#ifndef CWTB_HOST_EMU
-      if (pass == 1 && prio && c->prio_mode == 1) RT(cudaStreamWaitEvent(c->cur, c->ev_coarse, 0));
-#endif
+      if (pass == 1 && prio && c->prio_mode == 1) RT(rt_wait(c->cur, c->ev_coarse));
       for (size_t ci = 0; ci < job.classes.size() && !e; ++ci) {
         const ClassRun &cl = job.classes[ci];
         if (!cl.expand || (ci > 0 && job.classes[ci - 1].expand && job.classes[ci - 1].taps == cl.taps)) continue;
@@ -1327,12 +1353,10 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
         e = launch_expand<T>(c, cl.taps, ea, rows, minl);
       }
     }
-#ifndef CWTB_HOST_EMU
     if (prio && !e) {   // later work of the second stream and the join follow the coarse chain
-      if (c->prio_mode == 2) RT(cudaEventRecord(c->ev_coarse, c->prio_stream));
-      RT(cudaStreamWaitEvent(c->aux_stream, c->ev_coarse, 0));
+      if (c->prio_mode == 2) RT(rt_record(c->ev_coarse, c->prio_stream));
+      RT(rt_wait(c->aux_stream, c->ev_coarse));
     }
-#endif
     c->cur = c->stream;
     if (e) return e;
   }
@@ -1357,9 +1381,7 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     const bool single = class_single(job, cl);
     if (single != (pass == 0)) continue;   // pass 0: single-kernel classes, pass 1: two-kernel chains
     if (single) {
-#ifndef CWTB_HOST_EMU
       if (split) c->cur = c->aux_stream;
-#endif
       // ---- single kernel: pruned K'-point transforms from the band products ----
       SingleArgs<T> sa{ddesc, Bbuf, W, Tw<T>::get(c), nt, job.n0, N, cl.first, epi};
       switch (cl.log2K) {
@@ -1402,16 +1424,10 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     }
     // successive two-kernel classes rotate over the chains, each with its own stream, Z buffer
     // and band-chunk region (descriptor offsets already point into the right region)
-#ifdef CWTB_HOST_EMU
-    const int chain = 0;   // the emulation runs every launch in order: one Z buffer serves all classes
-#else
     const int chain = split ? job_chain_region(c, job, cl) : 0;
-#endif
     Buf &Zb = chain > 0 ? c->Zc[chain - 1] : c->Z;
     if ((e = ensure(c, Zb, (size_t)G * N * sizeof(V)))) return e;
-#ifndef CWTB_HOST_EMU
     c->cur = chain > 0 ? c->chain_streams[chain - 1] : c->stream;
-#endif
     for (int g0 = 0; g0 < cl.count; g0 += G) {
       const int ng = std::min(G, cl.count - g0);
       PassAArgs<T> a{};
@@ -1447,16 +1463,14 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     }
     c->cur = c->stream;
   }
-#ifndef CWTB_HOST_EMU
   if (split) {   // join: later work on the main stream sees every row of W
-    RT(cudaEventRecord(c->ev_join, c->aux_stream));
-    RT(cudaStreamWaitEvent(c->stream, c->ev_join, 0));
+    RT(rt_record(c->ev_join, c->aux_stream));
+    RT(rt_wait(c->stream, c->ev_join));
     for (int k = 1; k < c->n_chains; ++k) {
-      RT(cudaEventRecord(c->ev_joinc[k - 1], c->chain_streams[k - 1]));
-      RT(cudaStreamWaitEvent(c->stream, c->ev_joinc[k - 1], 0));
+      RT(rt_record(c->ev_joinc[k - 1], c->chain_streams[k - 1]));
+      RT(rt_wait(c->stream, c->ev_joinc[k - 1]));
     }
   }
-#endif
   return 0;
 }
 
@@ -1494,24 +1508,43 @@ static int upload_descs(cwtb_ctx *c, Job &job) {
   return 0;
 }
 
+// Device time of a kernel sequence on the engine's stream: time_begin in front of it, time_stop
+// behind it, time_read once the stream has been synchronised past the stop.  time_end stops, waits
+// and reads; a caller whose copies overlap the sequence's tail reads only after they are synchronised.
+static int time_begin(cwtb_ctx *c) {
+  RT(rt_record(c->e0, c->stream));
+  return 0;
+}
+static int time_stop(cwtb_ctx *c) {
+  RT(rt_record(c->e1, c->stream));
+  return 0;
+}
+static int time_read(cwtb_ctx *c, double *ms) {
+  float f = 0;
+  RT(rt_elapsed_ms(&f, c->e0, c->e1));
+  *ms = f;
+  return 0;
+}
+static int time_end(cwtb_ctx *c, double *ms) {
+  int e = time_stop(c);
+  if (e) return e;
+  RT(rt_event_sync(c->e1));
+  return time_read(c, ms);
+}
+
 static int timed_run(cwtb_ctx *c, const void *dsig, int iters, double *ms_out) {
   const Job &job = c->job;
   c->launches = 0;
-#ifndef CWTB_HOST_EMU
-  RT(cudaEventRecord(c->e0, c->stream));
-#endif
+  int e = time_begin(c);
+  if (e) return e;
   for (int it = 0; it < iters; ++it) {
-    int e = job.precision == CWTB_F64 ? run_job<double>(c, job, (const double *)dsig)
-                                      : run_job<float>(c, job, (const float *)dsig);
+    e = job.precision == CWTB_F64 ? run_job<double>(c, job, (const double *)dsig)
+                                  : run_job<float>(c, job, (const float *)dsig);
     if (e) return e;
   }
-  float ms = 0;
-#ifndef CWTB_HOST_EMU
-  RT(cudaEventRecord(c->e1, c->stream));
-  RT(cudaEventSynchronize(c->e1));
-  RT(cudaEventElapsedTime(&ms, c->e0, c->e1));
-#endif
-  if (ms_out) *ms_out = (double)ms / iters;
+  double ms = 0;
+  if ((e = time_end(c, &ms))) return e;
+  if (ms_out) *ms_out = ms / iters;
   c->launches /= std::max(1, iters);
   return 0;
 }
@@ -1542,13 +1575,9 @@ const char *cwtb_version(void) {
 }
 
 int cwtb_device_count(void) {
-#ifdef CWTB_HOST_EMU
-  return 1;
-#else
   int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
+  if (rt_device_count(&n) != 0) return 0;
   return n;
-#endif
 }
 
 int cwtb_create(int device, cwtb_ctx **out) {
@@ -1556,31 +1585,24 @@ int cwtb_create(int device, cwtb_ctx **out) {
   *out = nullptr;
   cwtb_ctx *c = new cwtb_ctx();
   c->device = device;
-#ifndef CWTB_HOST_EMU
-  if (cudaSetDevice(device) != cudaSuccess) { delete c; return CWTB_ERR_CUDA; }
-  if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return CWTB_ERR_CUDA; }
-  cudaEventCreate(&c->e0);
-  cudaEventCreate(&c->e1);
-  for (auto &st : c->copy_streams) cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&c->aux_stream, cudaStreamNonBlocking);
-  {
-    int lo = 0, hi = 0;   // numerically lower = higher priority
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    cudaStreamCreateWithPriority(&c->prio_stream, cudaStreamNonBlocking, hi);
-    cudaStreamCreateWithPriority(&c->prio_short, cudaStreamNonBlocking, hi);
-  }
-  cudaEventCreateWithFlags(&c->ev_angle, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&c->ev_coarse, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&c->ev_coarse_short, cudaEventDisableTiming);
-  for (auto &ev : c->ev_h2d) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  for (auto &ev : c->ev_used) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (rt_set_device(device) != 0) { delete c; return CWTB_ERR_CUDA; }
+  if (rt_stream_create(&c->stream) != 0) { delete c; return CWTB_ERR_CUDA; }
+  rt_event_create(&c->e0);
+  rt_event_create(&c->e1);
+  for (auto &st : c->copy_streams) rt_stream_create(&st);
+  rt_stream_create(&c->aux_stream);
+  rt_stream_create_highest({&c->prio_stream, &c->prio_short});
+  rt_event_create_sync(&c->ev_angle);
+  rt_event_create_sync(&c->ev_coarse);
+  rt_event_create_sync(&c->ev_coarse_short);
+  for (auto &ev : c->ev_h2d) rt_event_create_sync(&ev);
+  for (auto &ev : c->ev_used) rt_event_create_sync(&ev);
   if (const char *g = getenv("CWTB_BATCH_PIPELINE")) c->batch_pipeline = atoi(g) != 0;
   if (const char *g = getenv("CWTB_PRIO")) c->prio_mode = std::min(2, std::max(0, atoi(g)));
-  for (auto &st : c->chain_streams) cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
-  for (auto &ev : c->ev_joinc) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-#endif
+  for (auto &st : c->chain_streams) rt_stream_create(&st);
+  for (auto &ev : c->ev_joinc) rt_event_create_sync(&ev);
+  rt_event_create_sync(&c->ev_fork);
+  rt_event_create_sync(&c->ev_join);
   c->cur = c->stream;
   if (const char *g = getenv("CWTB_GROUP")) c->group = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_GROUP_MB")) c->group_bytes = (size_t)std::max(1, atoi(g)) << 20;
@@ -1601,9 +1623,7 @@ int cwtb_create(int device, cwtb_ctx **out) {
   if (const char *g = getenv("CWTB_PF_ROWS_B")) c->pf_rows_b = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_PF_DIST_A")) c->pf_dist_a = std::max(0, atoi(g));
   if (const char *g = getenv("CWTB_BATCH_MB")) c->batch_bytes = (size_t)std::max(1, atoi(g)) << 20;
-#ifndef CWTB_HOST_EMU
-  cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device);
-#endif
+  rt_sm_count(&c->num_sms, device);
   int e = init_tables(c);
   if (e == 0) e = rt_sync(c->stream) ? CWTB_ERR_CUDA : 0;
   if (e) { delete c; return e; }
@@ -1613,10 +1633,8 @@ int cwtb_create(int device, cwtb_ctx **out) {
 
 void cwtb_destroy(cwtb_ctx *c) {
   if (!c) return;
-#ifndef CWTB_HOST_EMU
-  cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->stream);
-#endif
+  rt_set_device(c->device);
+  rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
                  &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf})
@@ -1627,25 +1645,23 @@ void cwtb_destroy(cwtb_ctx *c) {
   if (c->tw32) rt_free(c->tw32);
   for (void *p : c->pinned) rt_host_free(p);
   for (void *p : c->devallocs) rt_free(p);
-#ifndef CWTB_HOST_EMU
-  cudaEventDestroy(c->e0);
-  cudaEventDestroy(c->e1);
-  cudaStreamDestroy(c->stream);
-  for (auto &st : c->copy_streams) cudaStreamDestroy(st);
-  cudaStreamDestroy(c->aux_stream);
-  cudaStreamDestroy(c->prio_stream);
-  cudaStreamDestroy(c->prio_short);
-  cudaEventDestroy(c->ev_angle);
-  cudaEventDestroy(c->ev_coarse);
-  cudaEventDestroy(c->ev_coarse_short);
-  for (auto &ev : c->ev_h2d) cudaEventDestroy(ev);
-  for (auto &ev : c->ev_used) cudaEventDestroy(ev);
-  for (void *p : c->stage_host) if (p) cudaFreeHost(p);
-  for (auto &st : c->chain_streams) cudaStreamDestroy(st);
-  for (auto &ev : c->ev_joinc) cudaEventDestroy(ev);
-  cudaEventDestroy(c->ev_fork);
-  cudaEventDestroy(c->ev_join);
-#endif
+  rt_event_destroy(c->e0);
+  rt_event_destroy(c->e1);
+  rt_stream_destroy(c->stream);
+  for (auto &st : c->copy_streams) rt_stream_destroy(st);
+  rt_stream_destroy(c->aux_stream);
+  rt_stream_destroy(c->prio_stream);
+  rt_stream_destroy(c->prio_short);
+  rt_event_destroy(c->ev_angle);
+  rt_event_destroy(c->ev_coarse);
+  rt_event_destroy(c->ev_coarse_short);
+  for (auto &ev : c->ev_h2d) rt_event_destroy(ev);
+  for (auto &ev : c->ev_used) rt_event_destroy(ev);
+  for (void *p : c->stage_host) if (p) rt_host_free(p);
+  for (auto &st : c->chain_streams) rt_stream_destroy(st);
+  for (auto &ev : c->ev_joinc) rt_event_destroy(ev);
+  rt_event_destroy(c->ev_fork);
+  rt_event_destroy(c->ev_join);
   delete c;
 }
 
@@ -1865,9 +1881,7 @@ static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, i
   if (!c) return CWTB_ERR_ARG;
   if (precision != CWTB_F64 && precision != CWTB_F32) return fail(c, CWTB_ERR_ARG, "bad precision");
   if (!scales) return fail(c, CWTB_ERR_ARG, "null scales");
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   if (nbatch < 1 || (long long)nbatch * S > 60000) return fail(c, CWTB_ERR_ARG, "batch too large for one launch");
   ++c->serial;   // whatever was resident is about to be replaced
   cwtb_ctx::PlanKey key;
@@ -2053,9 +2067,7 @@ int cwtb_fft_c2c(cwtb_ctx *c, const void *in, void *out, int64_t n, int batch, i
   const bool pow2 = (n & (n - 1)) == 0;
   if (!pow2 && precision != CWTB_F64) return fail(c, CWTB_ERR_UNSUPPORTED, "fft_c2c: lengths other than 2^k run in fp64");
   if (!pow2 && n > (1ll << 24)) return fail(c, CWTB_ERR_UNSUPPORTED, "fft_c2c: non power-of-two n > 2^24");
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   const size_t cnt = (size_t)n * batch;
   const size_t esz = precision == CWTB_F64 ? sizeof(double2) : sizeof(float2);
   int e;
@@ -2097,25 +2109,6 @@ int cwtb_fft_c2c(cwtb_ctx *c, const void *in, void *out, int64_t n, int batch, i
 }  // extern "C"
 
 extern "C" {
-
-// device time of a kernel sequence on the engine's stream -> cwtb_last_kernel_ms
-static int time_begin(cwtb_ctx *c) {
-#ifndef CWTB_HOST_EMU
-  RT(cudaEventRecord(c->e0, c->stream));
-#endif
-  c->last_ms = 0;
-  return 0;
-}
-static int time_end(cwtb_ctx *c) {
-#ifndef CWTB_HOST_EMU
-  float ms = 0;
-  RT(cudaEventRecord(c->e1, c->stream));
-  RT(cudaEventSynchronize(c->e1));
-  RT(cudaEventElapsedTime(&ms, c->e0, c->e1));
-  c->last_ms = ms;
-#endif
-  return 0;
-}
 
 // ---- helpers for the post-processing entry points ---------------------------------------
 static int upload_doubles(cwtb_ctx *c, Buf &b, const std::vector<double> &v) {
@@ -2210,13 +2203,11 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   WctPrepArgs<T> pa{(const V *)c->W.p, (const V *)c->W2.p, d_scale, (V *)c->C.p, (V *)c->A12.p, daWCT, n0};
   const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
   if ((e = launch<WctPrepBody<T>>(c, gx, S, pa))) return e;
-#ifndef CWTB_HOST_EMU
   if (c->angle_host && daWCT) {   // the angle is final here: its 8 B per point cross PCIe under the smoothing
-    RT(cudaEventRecord(c->ev_angle, c->stream));
-    RT(cudaStreamWaitEvent(c->copy_streams[0], c->ev_angle, 0));
-    RT(cudaMemcpyAsync(c->angle_host, daWCT, cnt * sizeof(double), cudaMemcpyDeviceToHost, c->copy_streams[0]));
+    RT(rt_record(c->ev_angle, c->stream));
+    RT(rt_wait(c->copy_streams[0], c->ev_angle));
+    RT(rt_d2h(c->angle_host, daWCT, cnt * sizeof(double), c->copy_streams[0]));
   }
-#endif
   if ((e = smooth_time<T>(c, (V *)c->C.p, S, n0, job.N, d_g))) return e;
   if ((e = smooth_time<T>(c, (V *)c->A12.p, S, n0, job.N, d_g))) return e;
   const int rows_out = dWCT ? S : maxscale;
@@ -2343,7 +2334,6 @@ int cwtb_cwt_to_host(cwtb_ctx *c, const void *signal, int signal_is_f32, int64_t
                      const double *scales, int n_scales, int family, double param, int precision,
                      void *out, int out_f64) {
   if (!c || !signal || !out) return fail(c, CWTB_ERR_ARG, "null argument");
-#ifndef CWTB_HOST_EMU
   // fp64, analytic family, forked streams: the device->host copy of the rows the single-kernel
   // chain produced starts as soon as that chain is done, while the two-kernel chains still run
   if (precision == CWTB_F64 && family != CWTB_TABLE && !c->profiling) {
@@ -2364,24 +2354,20 @@ int cwtb_cwt_to_host(cwtb_ctx *c, const void *signal, int signal_is_f32, int64_t
       c->job_dsig = c->sig.p;
       c->job.sig_is_f32 = 0;
       c->launches = 0;
-      RT(cudaEventRecord(c->e0, c->stream));
+      if ((e = time_begin(c))) return e;
       if ((e = run_job<double>(c, job, (const double *)c->sig.p))) return e;
-      RT(cudaEventRecord(c->e1, c->stream));
+      if ((e = time_stop(c))) return e;
       const size_t rowb = (size_t)n0 * sizeof(double2);
       const char *W = (const char *)c->W.p;
-      RT(cudaStreamWaitEvent(c->copy_streams[0], c->ev_join, 0));   // single-kernel chain done
+      RT(rt_wait(c->copy_streams[0], c->ev_join));   // single-kernel chain done
       RT(rt_d2h((char *)out + (size_t)r0 * rowb, W + (size_t)r0 * rowb, (size_t)(n_scales - r0) * rowb, c->copy_streams[0]));
       RT(rt_d2h(out, W, (size_t)r0 * rowb, c->stream));               // after every chain has joined
       RT(rt_sync(c->copy_streams[0]));
       RT(rt_sync(c->stream));
-      float ms = 0;
-      RT(cudaEventElapsedTime(&ms, c->e0, c->e1));
-      c->last_ms = ms;
-      return 0;
+      return time_read(c, &c->last_ms);
     }
     // not eligible: fall through to the plain sequence (prepare runs again, cheap)
   }
-#endif
   int e = cwtb_cwt(c, signal, signal_is_f32, n0, dt, scales, n_scales, family, param, precision, nullptr);
   if (e) return e;
   return cwtb_get_w(c, out, out_f64, 0, n_scales);
@@ -2542,7 +2528,7 @@ static int xwt_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, 
   if ((e = time_begin(c))) return e;
   if ((e = run_job<T>(c, c->job, (const T *)c->sig.p, nullptr, EPI_STORE))) return e;
   if ((e = run_job<T>(c, c->job, (const T *)c->sig2.p, nullptr, EPI_MULCONJ))) return e;
-  if ((e = time_end(c))) return e;
+  if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
   if (W12_out) return cwtb_get_w(c, W12_out, 1, 0, n_scales);
   RT(rt_sync(c->stream));
@@ -2570,9 +2556,7 @@ static void slot_begin(ResidentSlot &s) {
 static int slot_release(cwtb_ctx *c, ResidentSlot &s) {
   slot_begin(s);
   if (s.buf.p) {
-#ifndef CWTB_HOST_EMU
-    RT(cudaSetDevice(c->device));
-#endif
+    RT(rt_set_device(c->device));
     RT(rt_sync(c->stream));
     rt_free(s.buf.p);
     s.buf = Buf{};
@@ -2630,9 +2614,7 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
       return fail(c, CWTB_ERR_STATE, coh ? "no coherence resident" : "no cross spectrum resident");
     f = FieldRef{field, s.buf.p, s.prec, s.S, s.n0, coh ? coh_angle_offset((size_t)s.S * s.n0) : 0};
   }
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   return 0;
 }
 
@@ -2813,7 +2795,7 @@ static int wct_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, 
                   want_angle ? dA : nullptr, nullptr, 0, 0, nullptr);
   c->angle_host = nullptr;
   if (e) return e;
-  if ((e = time_end(c))) return e;
+  if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
   return 0;
 }
@@ -2833,21 +2815,14 @@ int cwtb_wct(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
              double *WCT_out, double *aWCT_out) {
   (void)dj;
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
-  bool early_angle = false;
-#ifndef CWTB_HOST_EMU
-  early_angle = aWCT_out != nullptr;
-#endif
   int e = wct_dispatch(c, y1, y2, n0, dt, scales, n_scales, family, param, boxcar_len, c->aux,
-                       aWCT_out != nullptr, early_angle ? aWCT_out : nullptr);
+                       aWCT_out != nullptr, aWCT_out);
   if (e) return e;
   const size_t cnt = (size_t)n_scales * n0;
-  const double *dW = (const double *)c->aux.p, *dA = dW + coh_angle_offset(cnt);
+  const double *dW = (const double *)c->aux.p;
   if (WCT_out) RT(rt_d2h(WCT_out, dW, cnt * sizeof(double), c->stream));
-  if (aWCT_out && !early_angle) RT(rt_d2h(aWCT_out, dA, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
-#ifndef CWTB_HOST_EMU
-  if (early_angle) RT(rt_sync(c->copy_streams[0]));
-#endif
+  if (aWCT_out) RT(rt_sync(c->copy_streams[0]));
   return 0;
 }
 
@@ -2870,7 +2845,7 @@ static int wct3_run(cwtb_ctx *c, const double *y, const double *x1, const double
                    boxcar_len, dRP2, dRM2);
   c->w_moved = true;   // W holds a smoothed field now, not a transform
   if (e) return e;
-  if ((e = time_end(c))) return e;
+  if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
   return 0;
 }
@@ -2950,9 +2925,7 @@ int cwtb_set_smooth_filter(cwtb_ctx *c, const double *table, int n_rows, int64_t
     c->filt_n = 0;
     return 0;
   }
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   const size_t bytes = (size_t)n_rows * (size_t)n * sizeof(double);
   int e = ensure(c, c->filt, bytes);
   if (e) return e;
@@ -2974,9 +2947,7 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
   if (!c || !in || !out || !scales || n_scales < 1 || n < 1 || !(dt > 0))
     return fail(c, CWTB_ERR_ARG, "smooth: bad argument");
   if (n > (1ll << 26)) return fail(c, CWTB_ERR_UNSUPPORTED, "smooth: rows longer than 2^26");
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   const int S = n_scales;
   const size_t cnt = (size_t)S * n;
   if (!c->pad_pow2 && n > (1ll << 24)) return fail(c, CWTB_ERR_UNSUPPORTED, "smooth: un-padded rows longer than 2^24");
@@ -3063,9 +3034,12 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
   // surrogates of at most `batch` units are resident at a time
   // (host surrogates stay double on the device; an fp32 run rounds one unit at a time into sig)
   const size_t usz = (size_t)nser * n0;             // samples per unit
-  // (the rotated spectra of a batch of phase-randomised units take 16 B per sample)
+  // (the rotated spectra of a batch of phase-randomised units take 16 B per sample; a batch drawn on
+  // the device is one launch of nser rows per unit)
   const size_t resident = phase ? sizeof(double2) : sizeof(double);
-  const int batch = noise ? n_units : (int)std::max<size_t>(1, std::min<size_t>((size_t)n_units, ((size_t)256 << 20) / (usz * resident)));
+  const int batch = noise ? n_units
+                          : (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_units, ((size_t)256 << 20) / (usz * resident),
+                                                                       (size_t)(MAX_ROWS / nser)}));
   const size_t nsz = noise ? sizeof(double) : sizeof(T);
   if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * usz * nsz))) return e;
   if (phase && (e = ensure(c, c->prot, (size_t)std::max(batch, 1) * usz * sizeof(double2)))) return e;
@@ -3100,7 +3074,7 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
       if (e) return e;
     }
   }
-  if ((e = time_end(c))) return e;
+  if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
   std::vector<unsigned long long> h((size_t)n_scales * nbins);
   for (int k = 0; k < nh; ++k) {
@@ -3165,14 +3139,19 @@ int cwtb_wct3_mc_seeded(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_
                  boxcar_len, mask, maxscale, nbins, h);
 }
 
-// test hooks: the surrogates of the seeded mode, [n_units][nser][n0] to the host
+// test hooks: the surrogates of the seeded mode, [n_units][nser][n0] to the host, drawn in launches
+// of at most MAX_ROWS / nser units like mc_run's
 static int mc_surrogates(cwtb_ctx *c, int nser, uint64_t seed, int64_t unit0, int n_units, int64_t n0, double *out) {
   if (!c || !out || n_units < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, "mc_surrogates: bad argument");
-  const size_t bytes = (size_t)n_units * nser * n0 * sizeof(double);
+  const size_t usz = (size_t)nser * n0, bytes = (size_t)n_units * usz * sizeof(double);
   int e = ensure(c, c->noise, bytes);
   if (e) return e;
-  NoiseArgs<double> na{(double *)c->noise.p, seed, unit0, (long long)n0, n_units, nser};
-  if ((e = launch<NoiseBody<double>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * n_units), na))) return e;
+  const int batch = (int)(MAX_ROWS / nser);
+  for (int i0 = 0; i0 < n_units; i0 += batch) {
+    const int nb = std::min(batch, n_units - i0);
+    NoiseArgs<double> na{(double *)c->noise.p + (size_t)i0 * usz, seed, unit0 + i0, (long long)n0, nb, nser};
+    if ((e = launch<NoiseBody<double>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * nb), na))) return e;
+  }
   RT(rt_d2h(out, c->noise.p, bytes, c->stream));
   RT(rt_sync(c->stream));
   return 0;
@@ -3202,9 +3181,7 @@ static int phase_spectra(cwtb_ctx *c, const char *name, const double *series, in
   const bool pow2 = (n0 & (n0 - 1)) == 0;
   if (n0 > (pow2 ? 1ll << 26 : 1ll << 24))
     return fail(c, CWTB_ERR_UNSUPPORTED, nm + ": series longer than 2^26 (2^24 if the length is not 2^k)");
-#ifndef CWTB_HOST_EMU
-  RT(cudaSetDevice(c->device));
-#endif
+  RT(rt_set_device(c->device));
   const size_t cnt = (size_t)nser * n0;
   int e;
   if ((e = ensure(c, c->pspec, cnt * sizeof(double2)))) return e;
@@ -3240,10 +3217,15 @@ int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const 
   PhaseSrc ph{};
   int e = phase_spectra(c, "mc_phase_surrogates", series, nser, group, first_unit, n_units, n0, &ph);
   if (e) return e;
-  const size_t cnt = (size_t)n_units * nser * n0;
+  const size_t usz = (size_t)nser * n0, cnt = (size_t)n_units * usz;
+  const int batch = (int)(MAX_ROWS / nser);   // units per launch, like mc_run's
   if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
-  if ((e = ensure(c, c->prot, cnt * sizeof(double2)))) return e;
-  if ((e = phase_units<double>(c, ph, nser, seed, first_unit, n_units, n0, (double *)c->noise.p))) return e;
+  if ((e = ensure(c, c->prot, (size_t)std::min(batch, n_units) * usz * sizeof(double2)))) return e;
+  for (int i0 = 0; i0 < n_units; i0 += batch) {
+    const int nb = std::min(batch, n_units - i0);
+    if ((e = phase_units<double>(c, ph, nser, seed, first_unit + i0, nb, n0, (double *)c->noise.p + (size_t)i0 * usz)))
+      return e;
+  }
   RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;
@@ -3253,17 +3235,12 @@ int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const 
 // Writes one line per kernel type: "name,launches,total_ms,rows" (rows = sum of gridDim.y, i.e.
 // scale rows processed) into `out`.  Returns the number of bytes written (<= cap-1) or < 0.
 static int profile_report(cwtb_ctx *c, char *out, size_t cap) {
-#ifdef CWTB_HOST_EMU
-  (void)c;
-  if (cap) out[0] = 0;
-  return 0;
-#else
   RT(rt_sync(c->stream));
   std::map<std::string, std::array<double, 3>> agg;
   std::vector<std::string> order;
   for (auto &r : c->prof) {
     float ms = 0;
-    RT(cudaEventElapsedTime(&ms, c->prof_events[r.ev], c->prof_events[r.ev + 1]));
+    RT(rt_elapsed_ms(&ms, c->prof_events[r.ev], c->prof_events[r.ev + 1]));
     if (!agg.count(r.name)) order.push_back(r.name);
     auto &a = agg[r.name];
     a[0] += 1; a[1] += ms; a[2] += r.gy;
@@ -3279,22 +3256,16 @@ static int profile_report(cwtb_ctx *c, char *out, size_t cap) {
   memcpy(out, txt.data(), m);
   out[m] = 0;
   return (int)m;
-#endif
 }
 
 int cwtb_profile_last(cwtb_ctx *c, char *out, size_t cap) {
   if (!c || !c->job.valid || !c->job_dsig || !out || cap < 2) return fail(c, CWTB_ERR_STATE, "no transform to profile");
-#ifdef CWTB_HOST_EMU
-  out[0] = 0;
-  return 0;
-#else
   c->prof.clear();
   c->profiling = true;
   int e = timed_run(c, c->job_dsig, 1, nullptr);
   c->profiling = false;
   if (e) return e;
   return profile_report(c, out, cap);
-#endif
 }
 
 // Profile ANY sequence of calls (xwt, wct, wct_mc, smooth ...): between begin and end every kernel
@@ -3314,7 +3285,6 @@ int cwtb_profile_end(cwtb_ctx *c, char *out, size_t cap) {
 
 // Batched transform of independent channels: chunks of channels share every kernel launch
 // (one descriptor row per (channel, scale)).  X: host [n_chan][n0].
-#ifndef CWTB_HOST_EMU
 // Per-row sums of |W|^2 of the resident chunk into dsum (device, R doubles, zeroed by the caller), on
 // the engine's stream, no synchronisation.
 static int launch_row_power(cwtb_ctx *c, double *dsum) {
@@ -3341,9 +3311,9 @@ static int cwt_batch_pipelined(cwtb_ctx *c, const void *X, int x_is_f32, int n_c
   if (c->stage_bytes < chunk_bytes) {
     RT(rt_sync(c->stream));
     for (auto &p : c->stage_host) {
-      if (p) RT(cudaFreeHost(p));
+      if (p) RT(rt_host_free(p));
       p = nullptr;
-      RT(cudaHostAlloc(&p, chunk_bytes, cudaHostAllocDefault));
+      RT(rt_host_alloc(&p, chunk_bytes));
     }
     c->stage_bytes = chunk_bytes;
   }
@@ -3354,18 +3324,17 @@ static int cwt_batch_pipelined(cwtb_ctx *c, const void *X, int x_is_f32, int n_c
   rt_stream copy = c->copy_streams[0];
   RT(rt_memset(dpow, 0, (size_t)n_chan * n_scales * sizeof(double), c->stream));
   c->launches = 0;
-  bool timing = false;
   int k = 0;
   for (int ch0 = 0; ch0 < n_chan; ch0 += nb, ++k) {
     const int nc = std::min(nb, n_chan - ch0), slot = k & 1;
     // (re-plans only when the chunk geometry changes: first and a shorter last chunk)
     if ((e = prepare(c, n0, dt, scales, n_scales, family, param, precision, nullptr, nc))) return e;
-    if (!timing) { RT(cudaEventRecord(c->e0, c->stream)); timing = true; }
+    if (k == 0 && (e = time_begin(c))) return e;   // behind the first plan's synchronisation
     const char *src = (const char *)X + (size_t)ch0 * n0 * esz_in;
     const size_t cnt = (size_t)nc * n0;
     const void *from = src;
     if ((x_is_f32 != 0) != f32) {   // conversion: through the page-locked staging buffer
-      if (k >= 2) RT(cudaEventSynchronize(c->ev_h2d[slot]));   // the staging buffer is free again
+      if (k >= 2) RT(rt_event_sync(c->ev_h2d[slot]));   // the staging buffer is free again
       if (f32) for (size_t i = 0; i < cnt; ++i) ((float *)c->stage_host[slot])[i] = (float)((const double *)src)[i];
       else for (size_t i = 0; i < cnt; ++i) ((double *)c->stage_host[slot])[i] = (double)((const float *)src)[i];
       from = c->stage_host[slot];
@@ -3373,29 +3342,26 @@ static int cwt_batch_pipelined(cwtb_ctx *c, const void *X, int x_is_f32, int n_c
     // (input of the engine's type: straight from the caller's pageable array -- the driver's own staged
     // copy is faster than a host memcpy into page-locked memory plus a DMA, and while it blocks this
     // thread the kernels of the previous chunk keep running)
-    if (k >= 2) RT(cudaStreamWaitEvent(copy, c->ev_used[slot], 0));   // chunk k-2 has consumed this device buffer
-    RT(cudaMemcpyAsync(c->stage_dev[slot].p, from, cnt * esz, cudaMemcpyHostToDevice, copy));
-    RT(cudaEventRecord(c->ev_h2d[slot], copy));
-    RT(cudaStreamWaitEvent(c->stream, c->ev_h2d[slot], 0));
+    if (k >= 2) RT(rt_wait(copy, c->ev_used[slot]));   // chunk k-2 has consumed this device buffer
+    RT(rt_h2d(c->stage_dev[slot].p, from, cnt * esz, copy));
+    RT(rt_record(c->ev_h2d[slot], copy));
+    RT(rt_wait(c->stream, c->ev_h2d[slot]));
     c->job_dsig = c->stage_dev[slot].p;
     c->job.sig_is_f32 = f32;
     e = f32 ? run_job<float>(c, c->job, (const float *)c->stage_dev[slot].p)
             : run_job<double>(c, c->job, (const double *)c->stage_dev[slot].p);
     if (e) return e;
     if ((e = launch_row_power(c, dpow + (size_t)ch0 * n_scales))) return e;
-    RT(cudaEventRecord(c->ev_used[slot], c->stream));
+    RT(rt_record(c->ev_used[slot], c->stream));
   }
-  RT(cudaEventRecord(c->e1, c->stream));
+  if ((e = time_stop(c))) return e;
   RT(rt_d2h(power_out, dpow, (size_t)n_chan * n_scales * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   RT(rt_sync(copy));
-  float ms = 0;
-  RT(cudaEventElapsedTime(&ms, c->e0, c->e1));
-  c->last_ms = ms;
+  if ((e = time_read(c, &c->last_ms))) return e;
   for (size_t i = 0; i < (size_t)n_chan * n_scales; ++i) power_out[i] /= (double)n0;
   return 0;
 }
-#endif
 
 int cwtb_cwt_batch(cwtb_ctx *c, const void *X, int x_is_f32, int n_chan, int64_t n0, double dt,
                    const double *scales, int n_scales, int family, double param, int precision,
@@ -3409,10 +3375,8 @@ int cwtb_cwt_batch(cwtb_ctx *c, const void *X, int x_is_f32, int n_chan, int64_t
   size_t per_chan = wrow * n_scales;
   int nb = (int)std::max<size_t>(1, std::min<size_t>(c->batch_bytes / std::max<size_t>(per_chan, 1), 32768 / n_scales));
   nb = std::max(1, std::min(nb, n_chan));
-#ifndef CWTB_HOST_EMU
   if (c->batch_pipeline && power_out && !W_out && (c->pad_pow2 || (n0 & (n0 - 1)) == 0))
     return cwt_batch_pipelined(c, X, x_is_f32, n_chan, n0, dt, scales, n_scales, family, param, precision, power_out, nb);
-#endif
   std::vector<unsigned char> conv;
   for (int ch0 = 0; ch0 < n_chan; ch0 += nb) {
     const int nc = std::min(nb, n_chan - ch0);
@@ -3465,7 +3429,6 @@ int cwtb_cwt_batch_dev(cwtb_ctx *c, const void *d_X, int n_chan, int64_t n0, dou
 // (all-reduce), timings (max).  Buffers are host arrays staged through context-owned device
 // memory: sizes are O(channels x scales), a few MB.
 // ======================================================================================
-#ifndef CWTB_HOST_EMU
 namespace {
 typedef struct { char internal[128]; } nccl_uid;
 struct NcclApi {
@@ -3473,9 +3436,9 @@ struct NcclApi {
   int (*GetUniqueId)(nccl_uid *) = nullptr;
   int (*CommInitRank)(void **, int, nccl_uid, int) = nullptr;
   int (*CommDestroy)(void *) = nullptr;
-  int (*AllGather)(const void *, void *, size_t, int, void *, cudaStream_t) = nullptr;
-  int (*AllReduce)(const void *, void *, size_t, int, int, void *, cudaStream_t) = nullptr;
-  int (*Broadcast)(const void *, void *, size_t, int, int, void *, cudaStream_t) = nullptr;
+  int (*AllGather)(const void *, void *, size_t, int, void *, rt_stream) = nullptr;
+  int (*AllReduce)(const void *, void *, size_t, int, int, void *, rt_stream) = nullptr;
+  int (*Broadcast)(const void *, void *, size_t, int, int, void *, rt_stream) = nullptr;
   const char *(*GetErrorString)(int) = nullptr;
   bool ok = false;
 };
@@ -3484,17 +3447,19 @@ NcclApi &nccl_api() {
   static std::mutex m;   // contexts of several host threads may bind NCCL at the same time
   std::lock_guard<std::mutex> lock(m);
   if (a.h) return a;
+#ifndef CWTB_HOST_EMU   // the emulation binds nothing: it has no device buffers to hand NCCL
   for (const char *name : {"libnccl.so.2", "libnccl.so"}) {
     a.h = dlopen(name, RTLD_NOW | RTLD_GLOBAL);
     if (a.h) break;
   }
+#endif
   if (!a.h) return a;
   a.GetUniqueId = (int (*)(nccl_uid *))dlsym(a.h, "ncclGetUniqueId");
   a.CommInitRank = (int (*)(void **, int, nccl_uid, int))dlsym(a.h, "ncclCommInitRank");
   a.CommDestroy = (int (*)(void *))dlsym(a.h, "ncclCommDestroy");
-  a.AllGather = (int (*)(const void *, void *, size_t, int, void *, cudaStream_t))dlsym(a.h, "ncclAllGather");
-  a.AllReduce = (int (*)(const void *, void *, size_t, int, int, void *, cudaStream_t))dlsym(a.h, "ncclAllReduce");
-  a.Broadcast = (int (*)(const void *, void *, size_t, int, int, void *, cudaStream_t))dlsym(a.h, "ncclBroadcast");
+  a.AllGather = (int (*)(const void *, void *, size_t, int, void *, rt_stream))dlsym(a.h, "ncclAllGather");
+  a.AllReduce = (int (*)(const void *, void *, size_t, int, int, void *, rt_stream))dlsym(a.h, "ncclAllReduce");
+  a.Broadcast = (int (*)(const void *, void *, size_t, int, int, void *, rt_stream))dlsym(a.h, "ncclBroadcast");
   a.GetErrorString = (const char *(*)(int))dlsym(a.h, "ncclGetErrorString");
   a.ok = a.GetUniqueId && a.CommInitRank && a.CommDestroy && a.AllGather && a.AllReduce && a.Broadcast;
   return a;
@@ -3508,18 +3473,12 @@ enum { NCCL_CHAR = 0, NCCL_INT64 = 4, NCCL_FLOAT64 = 8, NCCL_SUM = 0, NCCL_MAX =
       return fail(c, CWTB_ERR_COMM, std::string(#call) + ": " +                                     \
                                         (nccl_api().GetErrorString ? nccl_api().GetErrorString(r_) : "NCCL error")); \
   } while (0)
-#endif
 
 int cwtb_comm_unique_id(void *id128) {
   if (!id128) return CWTB_ERR_ARG;
-#ifdef CWTB_HOST_EMU
-  memset(id128, 0, 128);
-  return 0;
-#else
   NcclApi &a = nccl_api();
   if (!a.ok) return CWTB_ERR_COMM;
   return a.GetUniqueId((nccl_uid *)id128) == 0 ? 0 : CWTB_ERR_COMM;
-#endif
 }
 
 int cwtb_comm_init(cwtb_ctx *c, int world, int rank, const void *id128) {
@@ -3527,30 +3486,24 @@ int cwtb_comm_init(cwtb_ctx *c, int world, int rank, const void *id128) {
   cwtb_comm_destroy(c);
   c->comm_world = world;
   c->comm_rank = rank;
-#ifndef CWTB_HOST_EMU
   if (world == 1) return 0;
   NcclApi &a = nccl_api();
   if (!a.ok) return fail(c, CWTB_ERR_COMM, "libnccl.so.2 could not be loaded");
-  RT(cudaSetDevice(c->device));
+  RT(rt_set_device(c->device));
   nccl_uid id;
   memcpy(&id, id128, sizeof id);
   NCCLCHK(a.CommInitRank(&c->comm, world, id, rank));
-#else
-  if (world != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "the emulation build has no communicator");
-#endif
   return 0;
 }
 
 int cwtb_comm_destroy(cwtb_ctx *c) {
   if (!c) return CWTB_ERR_ARG;
-#ifndef CWTB_HOST_EMU
   if (c->comm) {
-    cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->stream);
+    rt_set_device(c->device);
+    rt_sync(c->stream);
     nccl_api().CommDestroy(c->comm);
     c->comm = nullptr;
   }
-#endif
   c->comm_world = 1;
   c->comm_rank = 0;
   return 0;
@@ -3563,9 +3516,9 @@ int cwtb_comm_rank(cwtb_ctx *c) { return c ? c->comm_rank : -1; }
 int cwtb_comm_allgather(cwtb_ctx *c, const void *send, void *recv, size_t bytes) {
   if (!c || !send || !recv) return fail(c, CWTB_ERR_ARG, "allgather: null argument");
   if (c->comm_world == 1) { memmove(recv, send, bytes); return 0; }
-#ifndef CWTB_HOST_EMU
+  if (!c->comm) return fail(c, CWTB_ERR_COMM, "no communicator");
   int e;
-  RT(cudaSetDevice(c->device));
+  RT(rt_set_device(c->device));
   if ((e = ensure(c, c->comm_send, bytes))) return e;
   if ((e = ensure(c, c->comm_recv, bytes * c->comm_world))) return e;
   RT(rt_h2d(c->comm_send.p, send, bytes, c->stream));
@@ -3573,57 +3526,39 @@ int cwtb_comm_allgather(cwtb_ctx *c, const void *send, void *recv, size_t bytes)
   RT(rt_d2h(recv, c->comm_recv.p, bytes * c->comm_world, c->stream));
   RT(rt_sync(c->stream));
   return 0;
-#else
-  return fail(c, CWTB_ERR_UNSUPPORTED, "no communicator");
-#endif
 }
 
 static int comm_allreduce(cwtb_ctx *c, void *buf, size_t count, int dtype, int op) {
   if (!c || !buf) return fail(c, CWTB_ERR_ARG, "allreduce: null argument");
   if (c->comm_world == 1) return 0;
-#ifndef CWTB_HOST_EMU
+  if (!c->comm) return fail(c, CWTB_ERR_COMM, "no communicator");
   int e;
-  RT(cudaSetDevice(c->device));
+  RT(rt_set_device(c->device));
   if ((e = ensure(c, c->comm_send, count * 8))) return e;
   RT(rt_h2d(c->comm_send.p, buf, count * 8, c->stream));
   NCCLCHK(nccl_api().AllReduce(c->comm_send.p, c->comm_send.p, count, dtype, op, c->comm, c->stream));
   RT(rt_d2h(buf, c->comm_send.p, count * 8, c->stream));
   RT(rt_sync(c->stream));
   return 0;
-#else
-  (void)count; (void)dtype; (void)op;
-  return fail(c, CWTB_ERR_UNSUPPORTED, "no communicator");
-#endif
 }
 int cwtb_comm_allreduce_sum_i64(cwtb_ctx *c, int64_t *buf, size_t count) {
-#ifndef CWTB_HOST_EMU
   return comm_allreduce(c, buf, count, NCCL_INT64, NCCL_SUM);
-#else
-  return comm_allreduce(c, buf, count, 0, 0);
-#endif
 }
 int cwtb_comm_allreduce_max_f64(cwtb_ctx *c, double *buf, size_t count) {
-#ifndef CWTB_HOST_EMU
   return comm_allreduce(c, buf, count, NCCL_FLOAT64, NCCL_MAX);
-#else
-  return comm_allreduce(c, buf, count, 0, 0);
-#endif
 }
 int cwtb_comm_broadcast(cwtb_ctx *c, void *buf, size_t bytes, int root) {
   if (!c || !buf || root < 0 || root >= c->comm_world) return fail(c, CWTB_ERR_ARG, "broadcast: bad argument");
   if (c->comm_world == 1) return 0;
-#ifndef CWTB_HOST_EMU
+  if (!c->comm) return fail(c, CWTB_ERR_COMM, "no communicator");
   int e;
-  RT(cudaSetDevice(c->device));
+  RT(rt_set_device(c->device));
   if ((e = ensure(c, c->comm_send, bytes))) return e;
   if (c->comm_rank == root) RT(rt_h2d(c->comm_send.p, buf, bytes, c->stream));
   NCCLCHK(nccl_api().Broadcast(c->comm_send.p, c->comm_send.p, bytes, NCCL_CHAR, root, c->comm, c->stream));
   RT(rt_d2h(buf, c->comm_send.p, bytes, c->stream));
   RT(rt_sync(c->stream));
   return 0;
-#else
-  return fail(c, CWTB_ERR_UNSUPPORTED, "no communicator");
-#endif
 }
 
 }  // extern "C"
