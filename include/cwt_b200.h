@@ -253,12 +253,52 @@ int cwtb_cross_release(cwtb_ctx *ctx);
  * NULL.  No clamping: a denominator that is zero or rounds to <= 0 gives inf or NaN; both measures
  * are ill-conditioned where x1 and x2 are nearly coherent (|S_12|^2 -> S_1 S_2).  The smoothed fields
  * are combined in double in both precisions.  Precision: cwtb_set_coherence_precision; un-padded
- * transforms only in fp64, CWTB_TABLE unsupported.  Lifetime: the resident coherence and cross
- * spectrum are not written (their handles survive the call); afterwards no transform is resident
+ * transforms only in fp64, CWTB_TABLE unsupported.  Lifetime: the resident coherence, partial /
+ * multiple coherence and cross spectrum are not written (their handles survive the call); afterwards
+ * no transform is resident
  * (cwtb_get_w, cwtb_icwt_sum and the power calls return CWTB_ERR_STATE until the next transform). */
 int cwtb_wct3(cwtb_ctx *ctx, const double *y, const double *x1, const double *x2, int64_t n0,
               double dt, double dj, const double *scales, int n_scales, int family, double param,
               int boxcar_len, double *RP2_out, double *RM2_out);
+
+/* ---- resident partial and multiple coherence ---------------------------------------------------
+ * cwtb_wct3_resident computes what cwtb_wct3 computes (same arguments without the outputs, same
+ * precision switch and errors) and keeps three n_scales x n0 double fields in one device buffer of
+ * their own: RP2 at offset 0, the partial phase at offset a and RM2 at offset 2a (in doubles),
+ * a = (n_scales*n0 rounded up to a multiple of 32).  24 bytes per scale-point.  The partial phase is
+ *   phi = atan2(Im u, Re u),  u = S_y1 S_2 - S_y2 conj(S_12),
+ * the angle of the smoothed partial cross spectrum of y and x1 with x2 removed, in the sign convention
+ * of cwtb_wct's aWCT (angle of W_y conj(W_x1)); a zero u gives 0, a NaN one NaN.  aWCT is the angle
+ * of the unsmoothed cross spectrum, phi of a smoothed quantity, so the two differ even where x2
+ * plays no role.  RP2 and RM2 are bit-identical to cwtb_wct3's.  Lifetime:
+ *   - only cwtb_wct3_resident writes that buffer: it survives every other call (cwt*, xwt*, wct*,
+ *     wct3, the Monte-Carlo calls), and the resident coherence and cross spectrum survive it;
+ *   - it dies at the next cwtb_wct3_resident or cwtb_coherence3_release (which frees it; so does
+ *     cwtb_destroy).  cwtb_coherence3_serial changes at both, and is bumped before anything else,
+ *     so a cwtb_wct3_resident that fails part-way leaves nothing resident;
+ *   - afterwards no transform is resident, as after cwtb_wct3.
+ * The reading calls take a measure: CWTB_MEASURE_PARTIAL (RP2 with the partial phase) or
+ * CWTB_MEASURE_MULTIPLE (RM2, which has no phase: asking for its phase is CWTB_ERR_ARG).  They
+ * return CWTB_ERR_STATE when nothing is resident and CWTB_ERR_ARG for a bad measure or range; the
+ * reductions are deterministic, as those of cwtb_coherence_*. */
+enum cwtb_measure { CWTB_MEASURE_PARTIAL = 0, CWTB_MEASURE_MULTIPLE = 1 };
+int cwtb_wct3_resident(cwtb_ctx *ctx, const double *y, const double *x1, const double *x2, int64_t n0,
+                       double dt, double dj, const double *scales, int n_scales, int family, double param,
+                       int boxcar_len);
+int64_t cwtb_coherence3_serial(cwtb_ctx *ctx);
+int cwtb_coherence3_release(cwtb_ctx *ctx);
+/* Strided sub-grid of the measure (R_out) and of the partial phase (phase_out; PARTIAL only), either
+ * may be NULL, nrows x ncols doubles: the layout and checks of cwtb_coherence_window. */
+int cwtb_coherence3_window(cwtb_ctx *ctx, int measure, int row0, int nrows, int row_step, int64_t col0,
+                           int64_t ncols, int64_t col_step, double *R_out, double *phase_out);
+/* out[j] = [count, sum R, sum cos phi, sum sin phi] over the columns [lo[j], hi[j]) (NULL: the
+ * whole row) where thr is NULL or R > thr[j] (false for a NaN threshold), S x 4 doubles;
+ * want_phase != 0 (PARTIAL only) reads the phase, otherwise its sums are 0. */
+int cwtb_coherence3_row_stats(cwtb_ctx *ctx, int measure, const int64_t *lo, const int64_t *hi,
+                              const double *thr, int want_phase, double *out);
+/* out[3][n0]: sum_j weights[j]*R[j,n], sum_j weights[j]*cos phi[j,n], sum_j weights[j]*sin phi[j,n];
+ * for MULTIPLE the two phase planes are 0.  Rows with weight 0 are not read. */
+int cwtb_coherence3_scale_avg(cwtb_ctx *ctx, int measure, const double *weights, double *out);
 
 /* Reading calls on a resident complex field: CWTB_FIELD_W (the resident transform's W) or
  * CWTB_FIELD_CROSS (the cross spectrum).  They return CWTB_ERR_STATE when the field is not

@@ -14,7 +14,10 @@ MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
 F64, F32 = 0, 1
 FIELD_W, FIELD_CROSS = 0, 1      # complex fields of the cwtb_field_* calls
 FIELD_COH = -1                   # the resident coherence (calls of its own, not a cwtb_field)
-_NOT_RESIDENT = {FIELD_COH: "no coherence resident", FIELD_CROSS: "no cross spectrum resident"}
+FIELD_COH3 = -2                  # the resident partial and multiple coherence (cwtb_coherence3_*)
+MEASURE_PARTIAL, MEASURE_MULTIPLE = 0, 1   # the measures of the cwtb_coherence3_* calls
+_NOT_RESIDENT = {FIELD_COH: "no coherence resident", FIELD_CROSS: "no cross spectrum resident",
+                 FIELD_COH3: "no partial / multiple coherence resident"}
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -76,6 +79,12 @@ _SIGNATURES = {
     "cwtb_coherence_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P, _P]),
     "cwtb_coherence_row_stats": (_I, [_P, _P, _P, _P, _I, _P]),
     "cwtb_coherence_scale_avg": (_I, [_P, _P, _P]),
+    "cwtb_wct3_resident": (_I, [_P, _P, _P, _P, _I64, _D, _D, _P, _I, _I, _D, _I]),
+    "cwtb_coherence3_serial": (_I64, [_P]),
+    "cwtb_coherence3_release": (_I, [_P]),
+    "cwtb_coherence3_window": (_I, [_P, _I, _I, _I, _I, _I64, _I64, _I64, _P, _P]),
+    "cwtb_coherence3_row_stats": (_I, [_P, _I, _P, _P, _P, _I, _P]),
+    "cwtb_coherence3_scale_avg": (_I, [_P, _I, _P, _P]),
     "cwtb_xwt_resident": (_I, [_P, _P, _P, _I64, _D, _P, _I, _I, _D]),
     "cwtb_cross_serial": (_I64, [_P]),
     "cwtb_cross_release": (_I, [_P]),
@@ -184,7 +193,8 @@ class Engine(object):
         self._pool_bytes = 0
         self._dead = []          # retired pinned buffers waiting for _reap()
         self._outstanding = 0    # result arrays still alive that alias pinned memory
-        self._held = {}          # (rows, n0) of the resident coherence and cross spectrum, by field
+        self._held = {}          # (rows, n0) of the resident coherence, partial / multiple
+                                 # coherence and cross spectrum, by field
 
     def _reap(self):
         """Free the pinned buffers the finalizers retired.  Finalizers never call into the
@@ -630,6 +640,68 @@ class Engine(object):
         w = _weights("coherence_scale_avg", rows, weights)
         out = self.result_array((3, n0), np.float64)
         self._check(self.lib.cwtb_coherence_scale_avg(self.h, _ptr(w), _ptr(out)))
+        return out
+
+    @_locked
+    def wct3_resident(self, y, x1, x2, dt, dj, scales, family, param, boxcar_len, precision=F64):
+        """`wct3` with RP2, the partial phase and RM2 kept on the device; returns the serial
+        that identifies them.  No transform is resident afterwards."""
+        ys = [np.ascontiguousarray(v, dtype=np.float64) for v in (y, x1, x2)]
+        if any(v.ndim != 1 or v.shape != ys[0].shape for v in ys):
+            raise ValueError("wct3_resident: the three series must be 1-D and of equal length")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        self._held[FIELD_COH3] = None
+        self._resident = None
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_wct3_resident(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]),
+                                                ys[0].size, float(dt), float(dj), _ptr(sj), sj.size,
+                                                int(family), float(param), int(boxcar_len)))
+        self._held[FIELD_COH3] = (sj.size, ys[0].size)
+        return self.coherence3_serial()
+
+    @_locked
+    def coherence3_serial(self):
+        return int(self.lib.cwtb_coherence3_serial(self.h))
+
+    @_locked
+    def coherence3_release(self):
+        self._held[FIELD_COH3] = None
+        self._check(self.lib.cwtb_coherence3_release(self.h))
+
+    @_locked
+    def coherence3_window(self, measure, row0, nrows, row_step, col0, ncols, col_step,
+                          want_value=True, want_phase=False):
+        """(R, phase)[row0::row_step][:nrows, col0::col_step][:, :ncols] of the resident measure
+        (MEASURE_PARTIAL: RP2 and the partial phase; MEASURE_MULTIPLE: RM2, no phase); a field
+        not asked for is None."""
+        self._shape(FIELD_COH3)
+        R = self.result_array((nrows, ncols), np.float64) if want_value else None
+        ph = self.result_array((nrows, ncols), np.float64) if want_phase else None
+        self._check(self.lib.cwtb_coherence3_window(
+            self.h, int(measure), int(row0), int(nrows), int(row_step), int(col0), int(ncols),
+            int(col_step), _ptr(R) if want_value else None, _ptr(ph) if want_phase else None))
+        return R, ph
+
+    @_locked
+    def coherence3_row_stats(self, measure, lo, hi, thr=None, want_phase=False):
+        """[rows, 4]: count, sum R, sum cos phase, sum sin phase over the columns [lo[j], hi[j])
+        where thr is None or R > thr[j]."""
+        rows, _ = self._shape(FIELD_COH3)
+        lo, hi, thr = _row_args("coherence3_row_stats", rows, lo, hi, thr)
+        out = np.empty((rows, 4), dtype=np.float64)
+        self._check(self.lib.cwtb_coherence3_row_stats(self.h, int(measure), _ptr(lo), _ptr(hi),
+                                                       None if thr is None else _ptr(thr),
+                                                       1 if want_phase else 0, _ptr(out)))
+        return out
+
+    @_locked
+    def coherence3_scale_avg(self, measure, weights):
+        """[3, n0]: sum_j w_j R[j], sum_j w_j cos phase[j], sum_j w_j sin phase[j] (the last two
+        0 for MEASURE_MULTIPLE)."""
+        rows, n0 = self._shape(FIELD_COH3)
+        w = _weights("coherence3_scale_avg", rows, weights)
+        out = self.result_array((3, n0), np.float64)
+        self._check(self.lib.cwtb_coherence3_scale_avg(self.h, int(measure), _ptr(w), _ptr(out)))
         return out
 
     @_locked

@@ -291,6 +291,9 @@ struct cwtb_ctx {
   // cwtb_xwt_resident hands its transform's W over by swapping the two buffers, so W12 is never
   // copied and the old cross buffer becomes the next transform's W.  Nothing else writes it.
   ResidentSlot cross;
+  // resident partial and multiple coherence (cwtb_wct3_resident): RP2 [S][n0], the partial phase at
+  // coh_angle_offset(S*n0), RM2 at twice that offset, double.  Only cwtb_wct3_resident writes it.
+  ResidentSlot coh3;
   bool w_moved = false;          // W went to the cross spectrum, or cwtb_wct3 wrote a smoothed field
                                  // into it: no transform resident until the next one writes W
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
@@ -1637,7 +1640,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2231,14 +2234,16 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
 }
 
 // three transforms + partial / multiple coherence in the engine type T; outputs are device
-// pointers (either may be null) and double for every T.  With both outputs null (Monte-Carlo mode)
-// only the rows below maxscale are finished, into the histograms dhP / dhM (either may be null).
+// pointers (any may be null) and double for every T, dPP the partial phase.  With every output null
+// (Monte-Carlo mode) only the rows below maxscale are finished, into the histograms dhP / dhM
+// (either may be null).
 // Device memory per scale-point: the three transforms W, W2, W3 (the crosses are written over
 // them), the two auto fields C, A12 and the smoothing buffer F.
 template <typename T>
 static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, const T *dx2, int K,
                      double *dRP2, double *dRM2, const unsigned char *dmask = nullptr, int maxscale = 0,
-                     int nbins = 0, unsigned long long *dhP = nullptr, unsigned long long *dhM = nullptr) {
+                     int nbins = 0, unsigned long long *dhP = nullptr, unsigned long long *dhM = nullptr,
+                     double *dPP = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2258,7 +2263,7 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
   if ((e = launch<Wct3PrepBody<T>>(c, gx, S, pa))) return e;
   for (V *x : f)
     if ((e = smooth_time<T>(c, x, S, n0, job.N, d_g))) return e;
-  const int rows_out = dRP2 || dRM2 ? S : maxscale;
+  const int rows_out = dRP2 || dRM2 || dPP ? S : maxscale;
   if (rows_out <= 0) return 0;
   const double *win = (const double *)c->win.p;
   if (K > 64) {
@@ -2274,7 +2279,7 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
     win += K;
     K = 1;
   }
-  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dmask, dhP, dhM, n0, S, K, maxscale, nbins};
+  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dPP, dmask, dhP, dhM, n0, S, K, maxscale, nbins};
   using F16 = Wct3FinalBody<T, 16, 32, 16>;
   using F64K = Wct3FinalBody<T, 64, 64, 8>;
   if (K <= 16)
@@ -2591,14 +2596,16 @@ int cwtb_cross_release(cwtb_ctx *c) { return c ? slot_release(c, c->cross) : CWT
 static size_t coh_angle_offset(size_t cnt) { return (cnt + 31) & ~(size_t)31; }
 
 // A resident field of the reading calls: a cwtb_field (the transform's W or the cross spectrum),
-// or the coherence under an id of its own
-static constexpr int FIELD_COH = -1;
+// or a double field under an id of its own: the coherence (WCT with aWCT), the partial coherence
+// (RP2 with its phase) or the multiple coherence (RM2, no phase)
+static constexpr int FIELD_COH = -1, FIELD_COH3_P = -2, FIELD_COH3_M = -3;
+static bool double_field(int field) { return field < 0; }
 struct FieldRef {
   int field;
   const void *p;
-  int prec, S;      // prec: the complex field's element type (the coherence is double)
+  int prec, S;      // prec: the complex field's element type (the double fields are double)
   long long n0;
-  size_t angle;     // coherence: aWCT's offset from WCT, in doubles
+  size_t angle;     // coherence / partial coherence: the phase's offset from the value, in doubles
 };
 
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
@@ -2607,12 +2614,18 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
     if (!w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
     if (c->job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "field of a batched transform: fetch rows per channel");
     f = FieldRef{field, c->W.p, c->job.precision, c->job.S, c->job.n0, 0};
-  } else {
+  } else if (field == CWTB_FIELD_CROSS || field == FIELD_COH) {
     const bool coh = field == FIELD_COH;
     const ResidentSlot &s = coh ? c->coh : c->cross;
     if (s.S <= 0 || !s.buf.p)
       return fail(c, CWTB_ERR_STATE, coh ? "no coherence resident" : "no cross spectrum resident");
     f = FieldRef{field, s.buf.p, s.prec, s.S, s.n0, coh ? coh_angle_offset((size_t)s.S * s.n0) : 0};
+  } else {   // FIELD_COH3_P / _M: RP2, phase, RM2 at 0, off, 2 off
+    const ResidentSlot &s = c->coh3;
+    if (s.S <= 0 || !s.buf.p) return fail(c, CWTB_ERR_STATE, "no partial / multiple coherence resident");
+    const size_t off = coh_angle_offset((size_t)s.S * s.n0);
+    const bool part = field == FIELD_COH3_P;
+    f = FieldRef{field, (const double *)s.buf.p + (part ? 0 : 2 * off), s.prec, s.S, s.n0, part ? off : 0};
   }
   RT(rt_set_device(c->device));
   return 0;
@@ -2628,21 +2641,22 @@ extern "C++" {
 // fn(view) with the kernel view of a resident field (kernels.cuh)
 template <typename Fn>
 static int with_view(const FieldRef &f, int want_phase, Fn &&fn) {
-  if (f.field == FIELD_COH) {
+  if (f.field == FIELD_COH || f.field == FIELD_COH3_P) {
     const double *w = (const double *)f.p;
     return fn(CohView{w, w + f.angle, want_phase});
   }
+  if (f.field == FIELD_COH3_M) return fn(CohMagView{(const double *)f.p, nullptr, 0});
   if (f.prec == CWTB_F64) return fn(CxView<double>{(const cx<double> *)f.p});
   return fn(CxView<float>{(const cx<float> *)f.p});
 }
 
-// Strided sub-grid into out0 / out1: the coherence's WCT / aWCT (nothing asked for: nothing to
-// do), or a complex field as complex128 into out0
+// Strided sub-grid into out0 / out1: a double field's value / phase (nothing asked for: nothing to
+// do; a field without a phase takes out1 == null), or a complex field as complex128 into out0
 static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int row_step, int64_t col0,
                       int64_t ncols, int64_t col_step, void *out0, void *out1) {
   const int S = f.S;
   const long long n0 = f.n0;
-  const bool coh = f.field == FIELD_COH;
+  const bool coh = double_field(f.field);
   if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1)
     return fail(c, CWTB_ERR_ARG, "window: negative count or step < 1");
   if (nrows == 0 || ncols == 0 || (!out0 && !out1)) return 0;
@@ -2831,7 +2845,7 @@ extern "C++" {
 template <typename T>
 static int wct3_run(cwtb_ctx *c, const double *y, const double *x1, const double *x2, int64_t n0, double dt,
                     const double *scales, int n_scales, int family, double param, int boxcar_len,
-                    double *dRP2, double *dRM2) {
+                    double *dRP2, double *dRM2, double *dPP = nullptr) {
   int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_series<T>(c, c->sig, y, n0))) return e;
@@ -2842,7 +2856,7 @@ static int wct3_run(cwtb_ctx *c, const double *y, const double *x1, const double
   c->launches = 0;
   if ((e = time_begin(c))) return e;
   e = wct3_core<T>(c, c->job, (const T *)c->sig.p, (const T *)c->sig2.p, (const T *)c->sig3.p,
-                   boxcar_len, dRP2, dRM2);
+                   boxcar_len, dRP2, dRM2, nullptr, 0, 0, nullptr, nullptr, dPP);
   c->w_moved = true;   // W holds a smoothed field now, not a transform
   if (e) return e;
   if ((e = time_end(c, &c->last_ms))) return e;
@@ -2908,6 +2922,63 @@ int cwtb_coherence_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, 
 int cwtb_coherence_scale_avg(cwtb_ctx *c, const double *weights, double *out) {
   FieldRef f;
   int e = field_ref(c, FIELD_COH, f);
+  return e ? e : scale_avg_run(c, f, weights, out);
+}
+
+// ---- resident partial and multiple coherence ---------------------------------------------------
+int cwtb_wct3_resident(cwtb_ctx *c, const double *y, const double *x1, const double *x2, int64_t n0, double dt,
+                       double dj, const double *scales, int n_scales, int family, double param, int boxcar_len) {
+  (void)dj;
+  if (!c || !y || !x1 || !x2) return fail(c, CWTB_ERR_ARG, "null argument");
+  slot_begin(c->coh3);
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct3 needs an analytic wavelet family");
+  if (n0 < 1 || n_scales < 1) return fail(c, CWTB_ERR_ARG, "bad n0 / n_scales");
+  const size_t cnt = (size_t)n_scales * n0, off = coh_angle_offset(cnt);
+  RT(rt_set_device(c->device));
+  int e = ensure(c, c->coh3.buf, (2 * off + cnt) * sizeof(double));
+  if (e) return e;
+  double *d = (double *)c->coh3.buf.p;
+  e = c->coh_precision == CWTB_F32
+          ? wct3_run<float>(c, y, x1, x2, n0, dt, scales, n_scales, family, param, boxcar_len, d, d + 2 * off, d + off)
+          : wct3_run<double>(c, y, x1, x2, n0, dt, scales, n_scales, family, param, boxcar_len, d, d + 2 * off, d + off);
+  if (e) return e;
+  RT(rt_sync(c->stream));
+  c->coh3.S = n_scales;
+  c->coh3.n0 = n0;
+  c->coh3.prec = CWTB_F64;
+  return 0;
+}
+
+int64_t cwtb_coherence3_serial(cwtb_ctx *c) { return c ? c->coh3.serial : -1; }
+int cwtb_coherence3_release(cwtb_ctx *c) { return c ? slot_release(c, c->coh3) : CWTB_ERR_ARG; }
+
+// the field of a cwtb_coherence3_* call; the multiple coherence has no phase
+static int coh3_ref(cwtb_ctx *c, int measure, bool want_phase, FieldRef &f) {
+  if (!c) return CWTB_ERR_ARG;
+  if (measure != CWTB_MEASURE_PARTIAL && measure != CWTB_MEASURE_MULTIPLE)
+    return fail(c, CWTB_ERR_ARG, "unknown measure");
+  if (want_phase && measure == CWTB_MEASURE_MULTIPLE)
+    return fail(c, CWTB_ERR_ARG, "the multiple coherence has no phase");
+  return field_ref(c, measure == CWTB_MEASURE_PARTIAL ? FIELD_COH3_P : FIELD_COH3_M, f);
+}
+
+int cwtb_coherence3_window(cwtb_ctx *c, int measure, int row0, int nrows, int row_step, int64_t col0,
+                           int64_t ncols, int64_t col_step, double *R_out, double *phase_out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, phase_out != nullptr, f);
+  return e ? e : window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, R_out, phase_out);
+}
+
+int cwtb_coherence3_row_stats(cwtb_ctx *c, int measure, const int64_t *lo, const int64_t *hi, const double *thr,
+                              int want_phase, double *out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, want_phase != 0, f);
+  return e ? e : row_stats_run(c, f, lo, hi, thr, want_phase != 0, out);
+}
+
+int cwtb_coherence3_scale_avg(cwtb_ctx *c, int measure, const double *weights, double *out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, false, f);
   return e ? e : scale_avg_run(c, f, weights, out);
 }
 

@@ -1877,14 +1877,17 @@ template <typename T> struct Wct3PrepBody {
 // Tile: RS output rows x CW columns; phase 0 stages the RS + K - 1 input rows of the five fields
 // for these columns, phase 1 gives each of the NT = (RS / RG) CW threads RG consecutive rows of
 // one column.
-// Monte-Carlo mode (RP2 and RM2 both null): only the rows below maxscale and only the measures
+// PP, if given, receives the partial phase atan2(u.y, u.x): the angle of the smoothed partial cross
+// spectrum of y and x1 with x2 removed, in the sign convention of aWCT (angle of W_y conj(W_x1)).
+// A zero u gives 0 (np.angle(0)), a NaN gives NaN.
+// Monte-Carlo mode (RP2, RM2 and PP all null): only the rows below maxscale and only the measures
 // whose histogram is given; a measure's histogram counts floor(R2 nbins), clamped to
 // [0, nbins - 1], over the points with mask != 0.  A non-finite R2 (a zero denominator) is not
 // counted.
 template <typename T> struct Wct3FinalArgs {
   const cx<T> *A, *B, *Xy1, *Xy2, *X12;   // time-smoothed fields
   const double *win;
-  double *RP2, *RM2;                     // [rows][n], either may be null
+  double *RP2, *RM2, *PP;                // [rows][n], any may be null
   const unsigned char *mask;             // [rows][n], Monte-Carlo mode
   unsigned long long *histP, *histM;     // [rows][nbins], either may be null
   long long n;
@@ -1916,7 +1919,7 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
     double *sw = (double *)(st + NF * PLANE);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    const int rows_out = a.RP2 || a.RM2 ? a.rows : a.maxscale;
+    const int rows_out = a.RP2 || a.RM2 || a.PP ? a.rows : a.maxscale;
     if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
@@ -1978,11 +1981,14 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
         const double d12 = S1 * S2 - (S12.x * S12.x + S12.y * S12.y);
         const size_t o = (size_t)i * a.n + n;
         const bool binned = (a.histP || a.histM) && i < a.maxscale && a.mask[o];
-        if (a.RP2 || (a.histP && binned)) {
+        if (a.RP2 || a.PP || (a.histP && binned)) {
           const double2 u = csub(cscale(Sy1, S2), cmul(Sy2, cconj(S12)));
-          const double rp = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
-          if (a.RP2) a.RP2[o] = rp;
-          if (a.histP && binned) hist_count(a.histP, i, a.nbins, rp);
+          if (a.RP2 || (a.histP && binned)) {
+            const double rp = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
+            if (a.RP2) a.RP2[o] = rp;
+            if (a.histP && binned) hist_count(a.histP, i, a.nbins, rp);
+          }
+          if (a.PP) a.PP[o] = u.x == 0.0 && u.y == 0.0 ? 0.0 : atan2(u.y, u.x);
         }
         if (a.RM2 || (a.histM && binned)) {
           const double2 z = cmul(cmul(Sy1, S12), cconj(Sy2));
@@ -2116,21 +2122,26 @@ template <typename T> struct ScaleAvgBody {
 // Row stats [count, sum WCT, sum cos aWCT, sum sin aWCT] of the points with WCT > thr_j; aWCT is
 // not read when want_phase == 0.  Scale average [sum w_j WCT, sum w_j cos aWCT, sum w_j sin aWCT]
 // as three planes of n.  Window: WCT to o0, aWCT to o1, either may be null.
-struct CohView {
-  const double *WCT, *aWCT;
+// The same reads serve the resident partial coherence (RP2 and its phase, cwtb_wct3_resident).
+// CohMagView: a double field without a phase (the multiple coherence RM2): no phase field is read
+// whatever want_phase, the phase sums and planes stay 0 and o1 is not written.
+template <bool PHASE> struct CohViewT {
+  const double *WCT, *aWCT;   // aWCT: unused (may be null) without PHASE
   int want_phase;
   static constexpr int K = 4, E = 2, VPT = 16, NA = 3;   // VPT: two loads each, one per field
   struct Vec { double2 w, g; };
   HD Vec load(size_t q) const {
     Vec v{ld_stream((const double2 *)WCT + q), make_double2(0, 0)};
-    if (want_phase) v.g = ld_stream((const double2 *)aWCT + q);
+    if constexpr (PHASE) {
+      if (want_phase) v.g = ld_stream((const double2 *)aWCT + q);
+    }
     return v;
   }
   HD void add1(double (&s)[K], double w, double ang, bool has_thr, double t) const {
     if (has_thr && !(w > t)) return;
     s[0] += 1.0;
     s[1] += w;
-    if (want_phase) {
+    if (PHASE && want_phase) {
       double sn, cs;
       sincos_hd(ang, &sn, &cs);
       s[2] += cs;
@@ -2141,16 +2152,23 @@ struct CohView {
     add1(s, e ? v.w.y : v.w.x, e ? v.g.y : v.g.x, has_thr, t);
   }
   HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
-    add1(s, WCT[p], want_phase ? aWCT[p] : 0.0, has_thr, t);
+    add1(s, WCT[p], PHASE && want_phase ? aWCT[p] : 0.0, has_thr, t);
   }
   struct Pt { double w, a; };
-  HD Pt point(size_t p) const { return Pt{ld_stream(&WCT[p]), ld_stream(&aWCT[p])}; }
+  HD Pt point(size_t p) const {
+    if constexpr (PHASE) return Pt{ld_stream(&WCT[p]), ld_stream(&aWCT[p])};
+    else return Pt{ld_stream(&WCT[p]), 0.0};
+  }
   HD static void acc(double (&s)[NA], double wj, const Pt &v) {
-    double sn, cs;
-    sincos_hd(v.a, &sn, &cs);
-    s[0] += wj * v.w;
-    s[1] += wj * cs;
-    s[2] += wj * sn;
+    if constexpr (PHASE) {
+      double sn, cs;
+      sincos_hd(v.a, &sn, &cs);
+      s[0] += wj * v.w;
+      s[1] += wj * cs;
+      s[2] += wj * sn;
+    } else {
+      s[0] += wj * v.w;
+    }
   }
   HD static void put(double *out, long long n, long long N, const double (&s)[NA]) {
     st_stream(&out[n], s[0]);
@@ -2159,9 +2177,13 @@ struct CohView {
   }
   HD void copy(size_t src, double *o0, double *o1, size_t dst) const {
     if (o0) o0[dst] = WCT[src];
-    if (o1) o1[dst] = aWCT[src];
+    if constexpr (PHASE) {
+      if (o1) o1[dst] = aWCT[src];
+    }
   }
 };
+using CohView = CohViewT<true>;
+using CohMagView = CohViewT<false>;
 
 // 16 bytes of a complex field: one double2, or two float2
 template <typename T> struct CxVec16;

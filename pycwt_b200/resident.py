@@ -14,8 +14,9 @@ then do with W (pycwt/sample/simple_sample.py:64-96) are reductions of |W|^2:
 methods evaluate those products on the device, so only O(S) or O(N) numbers cross the bus.
 The handle is valid until the next transform on the same engine.
 
-`wct_resident` does the same for the wavelet coherence and `xwt_resident` for the cross-wavelet
-transform (see the second half of this module).
+`wct_resident` does the same for the wavelet coherence, `xwt_resident` for the cross-wavelet
+transform and `wct3_resident` for the partial and multiple coherence of three series (see the
+second half of this module).
 """
 import collections
 
@@ -25,10 +26,11 @@ from . import _engine
 from .helpers import ar1, fft, fft_kwargs
 from .wavelet import (_check_parameter_wavelet, _coi, _nan_rows, _precision, _resolve_scales,
                       _sync_padding, _wct_on_device, _wct_problem, _wct_significance,
-                      _xwt_on_device, _xwt_problem, _xwt_signif)
+                      _xwt_on_device, _xwt_problem, _xwt_signif, wct3_significance,
+                      wct3_surrogate_significance)
 
 __all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence',
-           'xwt_resident', 'ResidentCrossWavelet']
+           'xwt_resident', 'ResidentCrossWavelet', 'wct3_resident', 'ResidentCoherence3']
 
 
 def _coi_ranges(wavelet, dt, n0, period):
@@ -118,9 +120,9 @@ class _ResidentSlot(_Resident):
     """A product in a device buffer of its own, freed by the engine method `_RELEASE`."""
 
     def release(self):
-        """Free the device buffer (16 bytes per scale and time point for a coherence, 16 or 8
-        for a cross spectrum).  The handle is invalid afterwards; releasing an invalid handle
-        does nothing."""
+        """Free the device buffer (16 bytes per scale and time point for a coherence, 24 for a
+        partial and multiple coherence, 16 or 8 for a cross spectrum).  The handle is invalid
+        afterwards; releasing an invalid handle does nothing."""
         with self.engine.lock:
             if getattr(self.engine, self._SERIAL)() == self._serial:
                 getattr(self.engine, self._RELEASE)()
@@ -542,3 +544,178 @@ def xwt_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95, wave
     eng = engine or _engine.default_engine()
     serial = _xwt_on_device(eng, p, eng.xwt_resident)
     return ResidentCrossWavelet(eng, p, _xwt_signif(p, significance_level), precision, serial)
+
+
+# ---- resident partial and multiple coherence ---------------------------------------------------
+# `partial_wct` and `multiple_wct` each hand the caller one float64 [S, n0] field and run the whole
+# three-series pipeline for it; at config 4 that is two pipelines and 608 MB over PCIe.
+# `wct3_resident` runs the pipeline once and keeps RP2, the partial phase and RM2 on the device, in
+# a buffer of their own: the handle stays valid across later cwt / xwt / wct / wct_resident /
+# xwt_resident / partial_wct / Monte-Carlo calls, until the next `wct3_resident` on the same engine
+# or `release()`.
+
+_MEASURES = {'partial': _engine.MEASURE_PARTIAL, 'multiple': _engine.MEASURE_MULTIPLE}
+
+
+class ResidentCoherence3(_ResidentSlot):
+    """RP2, the partial phase and RM2 [S, n0] of one `wct3_resident` call, resident on the device.
+
+    The partial phase is the angle of the smoothed partial cross spectrum of y and x1 with x2
+    removed, u = S_y1 S_2 - S_y2 conj(S_12) (the numerator of RP2 = |u|^2 / (D_y D_12)), in the sign
+    convention of `wct`'s aWCT: the angle of W_y conj(W_x1).  aWCT is the angle of the *unsmoothed*
+    cross spectrum (reference wavelet.py:514); an unsmoothed partial spectrum does not exist, so the
+    partial phase is the angle of a smoothed quantity and differs from aWCT even where x2 plays no
+    role.  A zero u has phase 0.  RM2 has no phase.
+
+    `measure` arguments are 'partial' (RP2) or 'multiple' (RM2).  `sig` arguments take one entry
+    per scale in the units of the measure (as `wct3_significance` returns them); a point is
+    selected where R > sig[j], and a NaN entry selects no point of its scale."""
+
+    _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence3_serial', 'coherence3_release'
+    _GONE = ("this partial / multiple coherence is no longer resident: it was released or another "
+             "wct3_resident has run on the same engine")
+
+    def __init__(self, engine, problem, normalize, precision, serial):
+        p = problem
+        super(ResidentCoherence3, self).__init__(engine, p.wavelet, p.n0, p.dt, p.dj, p.sj,
+                                                 precision, serial)
+        self.s0 = p.s0
+        self.J = p.J
+        self.freq = p.freq
+        self.normalize = normalize
+        self._y = tuple(np.array(y, copy=True) for y in p.ys)   # raw series, for ar1 and surrogates
+
+    def _measure(self, measure):
+        try:
+            return _MEASURES[measure]
+        except (KeyError, TypeError):
+            raise ValueError("measure must be 'partial' or 'multiple', got %r" % (measure,))
+
+    def _threshold(self, sig):
+        if sig is None:
+            return None
+        thr = np.asarray(sig, dtype=float)
+        if thr.shape != (len(self.scales),):
+            raise ValueError("sig must have one entry per scale (%d), got shape %s"
+                             % (len(self.scales), thr.shape))
+        return thr
+
+    def _field(self, measure, want_value=True, want_phase=False):
+        S, n0 = self.shape
+        return self.engine.coherence3_window(measure, 0, S, 1, 0, n0, 1, want_value, want_phase)
+
+    # -- the products --------------------------------------------------------------------
+    @_live
+    def partial(self):
+        """RP2 (float64, S x n0), as returned by `partial_wct`: the expensive fetch."""
+        return self._field(_engine.MEASURE_PARTIAL)[0]
+
+    @_live
+    def multiple(self):
+        """RM2 (float64, S x n0), as returned by `multiple_wct`: the expensive fetch."""
+        return self._field(_engine.MEASURE_MULTIPLE)[0]
+
+    @_live
+    def phase(self):
+        """The partial phase (float64, S x n0, radians in [-pi, pi])."""
+        return self._field(_engine.MEASURE_PARTIAL, want_value=False, want_phase=True)[1]
+
+    @_live
+    def window(self, rows=slice(None), cols=slice(None)):
+        """(RP2[rows, cols], phase[rows, cols], RM2[rows, cols]) for two slices with steps >= 1,
+        gathered on the device: only the sub-grid crosses the bus (contour and phase-arrow plots)."""
+        S, n0 = self.shape
+        r0, nr, rs = _slice_range(rows, S, 'rows')
+        c0, nc, cs = _slice_range(cols, n0, 'cols')
+        if nr == 0 or nc == 0:
+            return np.empty((nr, nc)), np.empty((nr, nc)), np.empty((nr, nc))
+        rp, ph = self.engine.coherence3_window(_engine.MEASURE_PARTIAL, r0, nr, rs, c0, nc, cs,
+                                               want_phase=True)
+        rm = self.engine.coherence3_window(_engine.MEASURE_MULTIPLE, r0, nr, rs, c0, nc, cs)[0]
+        return rp, ph, rm
+
+    @_live
+    def global_coherence(self, measure='partial', inside_coi=False, sig=None):
+        """Mean of the measure per scale over the selected points: inside the cone of influence
+        (period_j <= coi[n]) if `inside_coi`, where R[j, n] > sig[j] if `sig` is given.  NaN for a
+        scale without points."""
+        m = self._measure(measure)
+        lo, hi = _column_ranges(self, inside_coi)
+        st = self.engine.coherence3_row_stats(m, lo, hi, self._threshold(sig))
+        return _ratio(st[:, 1], st[:, 0])
+
+    @_live
+    def significant_fraction(self, sig, measure='partial'):
+        """Per scale, the fraction of the points inside the cone of influence where R > sig[j];
+        NaN for a scale without points inside the cone."""
+        m = self._measure(measure)
+        lo, hi = self.coi_ranges()
+        st = self.engine.coherence3_row_stats(m, lo, hi, self._threshold(sig))
+        return _ratio(st[:, 0], hi - lo)
+
+    @_live
+    def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, sig=None,
+                   per_scale=False):
+        """Circular mean of the partial phase over the points of the scales with period_min <=
+        period < period_max, inside the cone of influence if `inside_coi`, where RP2 > sig if given:
+        MeanPhase(angle = atan2(sum sin, sum cos), strength = |sum e^{i phase}| / count, count), for
+        the whole band or, with `per_scale`, per scale (NaN angle and strength where the count
+        is 0)."""
+        sel = self._band(period_min, period_max)
+        lo, hi = _column_ranges(self, inside_coi)
+        lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
+        st = self.engine.coherence3_row_stats(_engine.MEASURE_PARTIAL, lo, hi, self._threshold(sig),
+                                              want_phase=True)
+        return _mean_phase(st[:, 0], st[:, 2], st[:, 3], per_scale)
+
+    @_live
+    def scale_avg(self, period_min, period_max):
+        """Three length-n0 series over the scales with period_min <= period < period_max: the mean
+        RP2, the circular mean partial phase atan2(sum sin, sum cos) and the mean RM2."""
+        sel = self._band(period_min, period_max)
+        if not sel.any():
+            raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
+        w = sel.astype(float)
+        k = float(sel.sum())
+        p = self.engine.coherence3_scale_avg(_engine.MEASURE_PARTIAL, w)
+        rp, ph = p[0] / k, np.arctan2(p[2], p[1])
+        rm = self.engine.coherence3_scale_avg(_engine.MEASURE_MULTIPLE, w)[0] / k
+        return rp, ph, rm
+
+    @_live
+    def significance(self, significance_level=0.95, mc_count=300, progress=True, seed=None):
+        """(sig_partial, sig_multiple) of `wct3_significance` with the lag-1 autocorrelations of the
+        raw series and this handle's dt, dj, s0, J, wavelet and precision.  The fields stay
+        resident."""
+        al = [ar1(y)[0] for y in self._y]
+        return wct3_significance(*al, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
+                                 significance_level=significance_level, wavelet=self.wavelet,
+                                 mc_count=mc_count, progress=progress, seed=seed,
+                                 precision=self.precision)
+
+    @_live
+    def surrogate_significance(self, significance_level=0.95, mc_count=300, seed=None,
+                               conditional=True):
+        """(sig_partial, sig_multiple) of `wct3_surrogate_significance` on this handle's series and
+        arguments.  The fields stay resident."""
+        return wct3_surrogate_significance(*self._y, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
+                                           significance_level=significance_level,
+                                           wavelet=self.wavelet, normalize=self.normalize,
+                                           mc_count=mc_count, seed=seed, precision=self.precision,
+                                           conditional=conditional)
+
+
+def wct3_resident(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
+                  precision='fp64', engine=None):
+    """Same partial and multiple coherence as `partial_wct(y, x1, x2, dt, dj, s0, J, wavelet,
+    normalize, precision)` and `multiple_wct(...)`, from one run of the pipeline, kept on the device
+    with the partial phase.
+
+    Returns a `ResidentCoherence3`.  Scales, boxcar, standardisation, the un-padded fallback to fp64,
+    the Paul / DOG smoothing filter and the errors are resolved by the same code as `partial_wct`'s.
+    No transform stays resident afterwards (handles of `cwt_resident` die); the handles of
+    `wct_resident` and `xwt_resident` survive."""
+    p = _wct_problem((y, x1, x2), dt, dj, s0, J, wavelet, normalize, precision)
+    eng = engine or _engine.default_engine()
+    serial = _wct_on_device(eng, p, eng.wct3_resident)
+    return ResidentCoherence3(eng, p, normalize, precision, serial)
