@@ -119,8 +119,8 @@ int cwtb_host_free(cwtb_ctx *ctx, void *p);
  * family/param  mother wavelet; for CWTB_TABLE `table` is a host [n_scales, Np]
  *             complex128 array holding sqrt(s*w1*Np)*conj(psi_ft) already
  * precision   arithmetic of the engine (fp64 or fp32)
- * The result stays resident on the device until the next cwtb_cwt* call on
- * this context; fetch it with cwtb_get_* or post-process it with cwtb_icwt...
+ * The result stays resident on the device (see "what stays resident" below);
+ * fetch it with cwtb_get_* or post-process it with cwtb_icwt...
  */
 int cwtb_cwt(cwtb_ctx *ctx, const void *signal, int signal_is_f32, int64_t n0,
              double dt, const double *scales, int n_scales, int family,
@@ -143,8 +143,35 @@ int64_t cwtb_padded_length(cwtb_ctx *ctx);
  * valid while this value is unchanged. */
 int64_t cwtb_job_serial(cwtb_ctx *ctx);
 /* Raw device pointer of the resident W (engine precision), for zero-copy
- * consumers (DLPack / __cuda_array_interface__ wrappers). */
+ * consumers (DLPack / __cuda_array_interface__ wrappers); NULL when none is resident. */
 void *cwtb_w_device_ptr(cwtb_ctx *ctx);
+
+/* ---- what stays resident --------------------------------------------------------------------
+ * A context holds at most one resident transform W, besides the resident coherence, partial /
+ * multiple coherence and cross spectrum of the calls below, which have lifetimes of their own.
+ *   - These calls leave a transform resident: cwtb_cwt, cwtb_cwt_dev, cwtb_cwt_to_host, cwtb_xwt
+ *     (W12), cwtb_cwt_batch and cwtb_cwt_batch_dev (the last chunk of channels: n_scales x its
+ *     channels rows), cwtb_bench_last and cwtb_profile_last (the transform they re-run).
+ *   - These leave none: cwtb_wct, cwtb_wct_resident, cwtb_wct3, cwtb_wct3_resident,
+ *     cwtb_xwt_resident, every Monte-Carlo call (cwtb_*_mc*), and any call of the first list that
+ *     fails once it has begun planning.
+ *   - Every other call leaves the resident transform as it is: cwtb_smooth, cwtb_fft_c2c,
+ *     cwtb_icwt_sum_host, the surrogate test hooks, the setters, every read and every release.
+ * cwtb_job_serial changes when a call of the first two lists begins planning (not at the re-runs).
+ * cwtb_get_w, cwtb_icwt_sum, the power calls, cwtb_field_* on CWTB_FIELD_W and cwtb_w_device_ptr
+ * read the resident transform: CWTB_ERR_STATE (NULL) when there is none.  cwtb_get_signal_fft,
+ * cwtb_padded_length and cwtb_last_plan describe the plan of the last call that planned, whether or
+ * not its transform is resident.
+ * cwtb_resident_shape reports what is resident, with the sizes every read of it copies: rows (0 when
+ * nothing is), n0 and precision (the element type of a complex product; CWTB_F64 for the coherence
+ * products, which are double).  Any output may be NULL.  CWTB_ERR_ARG for an unknown product. */
+enum cwtb_product {
+  CWTB_PRODUCT_W = 0,           /* the transform (CWTB_FIELD_W)                         */
+  CWTB_PRODUCT_CROSS = 1,       /* the cross spectrum (CWTB_FIELD_CROSS)               */
+  CWTB_PRODUCT_COHERENCE = 2,   /* WCT and aWCT of cwtb_wct_resident                   */
+  CWTB_PRODUCT_COHERENCE3 = 3   /* RP2, the partial phase and RM2 of cwtb_wct3_resident */
+};
+int cwtb_resident_shape(cwtb_ctx *ctx, int product, int *rows, int64_t *n0, int *precision);
 
 /* Whole call for host callers: H2D signal, transform, one D2H of W into `out`
  * (page-locked memory from cwtb_host_alloc makes the copy run at PCIe speed; the

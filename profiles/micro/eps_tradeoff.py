@@ -27,8 +27,6 @@ def main():
         eng.cwt_dev(dsig, 0, c["n"], c["dt"], sj, _engine.MORLET, c["f0"], _engine.F64)
         eng.bench_last(3)
         ms = eng.bench_last(20)
-        eng._resident = (len(sj), c["n"])
-        eng._resident_n0 = c["n"]
         return ms, eng.get_w(len(sj), c["n"])
 
     ms0, W0 = run(1e-16, 5e-13)

@@ -13,11 +13,10 @@ LIB_PATH = os.path.join(_HERE, "libcwtb200.so")
 MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
 F64, F32 = 0, 1
 FIELD_W, FIELD_CROSS = 0, 1      # complex fields of the cwtb_field_* calls
-FIELD_COH = -1                   # the resident coherence (calls of its own, not a cwtb_field)
-FIELD_COH3 = -2                  # the resident partial and multiple coherence (cwtb_coherence3_*)
 MEASURE_PARTIAL, MEASURE_MULTIPLE = 0, 1   # the measures of the cwtb_coherence3_* calls
-_NOT_RESIDENT = {FIELD_COH: "no coherence resident", FIELD_CROSS: "no cross spectrum resident",
-                 FIELD_COH3: "no partial / multiple coherence resident"}
+# the resident products of cwtb_resident_shape: the two fields, the coherence (cwtb_coherence_*) and
+# the partial and multiple coherence (cwtb_coherence3_*)
+PRODUCT_W, PRODUCT_CROSS, PRODUCT_COHERENCE, PRODUCT_COHERENCE3 = 0, 1, 2, 3
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -49,6 +48,7 @@ _SIGNATURES = {
     "cwtb_padded_length": (_I64, [_P]),
     "cwtb_job_serial": (_I64, [_P]),
     "cwtb_w_device_ptr": (_P, [_P]),
+    "cwtb_resident_shape": (_I, [_P, _I, ctypes.POINTER(_I), ctypes.POINTER(_I64), ctypes.POINTER(_I)]),
     "cwtb_last_kernel_ms": (_D, [_P]),
     "cwtb_last_launch_count": (_I, [_P]),
     "cwtb_last_plan": (_I, [_P, _P, _I]),
@@ -193,8 +193,6 @@ class Engine(object):
         self._pool_bytes = 0
         self._dead = []          # retired pinned buffers waiting for _reap()
         self._outstanding = 0    # result arrays still alive that alias pinned memory
-        self._held = {}          # (rows, n0) of the resident coherence, partial / multiple
-                                 # coherence and cross spectrum, by field
 
     def _reap(self):
         """Free the pinned buffers the finalizers retired.  Finalizers never call into the
@@ -242,18 +240,26 @@ class Engine(object):
     def version(self):
         return self.lib.cwtb_version().decode()
 
-    # (rows, n0) of the transform the device holds, when the last call left a single well-defined
-    # one there; the fetch/reduction methods check their arguments against it because the C side
-    # sizes its copies from the resident job, not from the caller's arrays
-    _resident = None
+    # ---- what is resident: the engine's record (cwtb_resident_shape) -------------------------
+    # The library sizes every copy from what is resident, not from the caller's arrays, so every
+    # method that hands it an output array sizes that array from the same record.
+    def _shape(self, product):
+        """(rows, n0, precision) of the resident product; EngineError when there is none."""
+        rows, n0, prec = _I(), _I64(), _I()
+        self._check(self.lib.cwtb_resident_shape(self.h, int(product), ctypes.byref(rows), ctypes.byref(n0),
+                                                 ctypes.byref(prec)))
+        if rows.value <= 0:
+            raise EngineError("no %s resident" % ("single transform", "cross spectrum", "coherence",
+                                                  "partial / multiple coherence")[product])
+        return rows.value, n0.value, prec.value
 
-    def _expect_resident(self, rows=None, n0=None):
-        if self._resident is None:
-            return
-        r, n = self._resident
+    def _transform(self, rows=None, n0=None):
+        """(rows, n0, precision) of the resident transform, which a caller's rows and n0 must match."""
+        r, n, prec = self._shape(PRODUCT_W)
         if (rows is not None and rows != r) or (n0 is not None and n0 != n):
             raise ValueError("the resident transform is %d x %d, the call asks for %s x %s"
                              % (r, n, "?" if rows is None else rows, "?" if n0 is None else n0))
+        return r, n, prec
 
     @_locked
     def set_band_eps(self, eps):
@@ -389,24 +395,23 @@ class Engine(object):
                 self._check(self.lib.cwtb_cwt_to_host(self.h, _ptr(sig), is32, sig.size, float(dt),
                                                       _ptr(sj), sj.size, int(family), float(param),
                                                       int(precision), _ptr(W), 1 if out_f64 else 0))
-                self._resident_n0 = sig.size
-                self._resident = (sj.size, sig.size)
                 return W
             self._check(self.lib.cwtb_cwt(self.h, _ptr(sig), is32, sig.size, float(dt),
                                           _ptr(sj), sj.size, int(family), float(param),
                                           int(precision), tptr))
-            self._resident_n0 = sig.size
-            self._resident = (sj.size, sig.size)
             if not fetch:
                 return None
             return self.get_w(sj.size, sig.size, precision, out_f64)
 
     @_locked
     def get_w(self, nrows, n0, precision=F64, out_f64=True):
-        dtype = np.complex128 if (precision == F64 or out_f64) else np.complex64
-        self._expect_resident(None, n0)
-        if self._resident is not None and nrows > self._resident[0]:
-            raise ValueError("get_w: %d rows requested, %d resident" % (nrows, self._resident[0]))
+        """The first `nrows` rows of the resident transform: complex128, or complex64 for an fp32
+        transform with out_f64 False.  The element type is the transform's; `precision` is not
+        read."""
+        rows, _, prec = self._transform(None, n0)
+        if nrows > rows:
+            raise ValueError("get_w: %d rows requested, %d resident" % (nrows, rows))
+        dtype = np.complex128 if (prec == F64 or out_f64) else np.complex64
         W = self.result_array((nrows, n0), dtype)
         self._check(self.lib.cwtb_get_w(self.h, _ptr(W), 1 if out_f64 else 0, 0, nrows))
         return W
@@ -458,7 +463,7 @@ class Engine(object):
         array W[S, n]."""
         with self.lock:
             if W is None:
-                n0 = self._resident_n0
+                _, n0, _ = self._shape(PRODUCT_W)
                 out = self.result_array((n0,), np.float64)     # pinned when large: D2H at PCIe speed
                 self._check(self.lib.cwtb_icwt_sum(self.h, _ptr(out)))
                 return out
@@ -471,7 +476,7 @@ class Engine(object):
 
     @_locked
     def global_power(self, nrows):
-        self._expect_resident(nrows)
+        self._transform(nrows)
         out = np.empty(nrows, dtype=np.float64)
         self._check(self.lib.cwtb_global_power(self.h, _ptr(out)))
         return out
@@ -483,7 +488,7 @@ class Engine(object):
         hi = np.ascontiguousarray(hi, dtype=np.int64)
         if lo.shape != hi.shape:
             raise ValueError("global_power_ranges: lo and hi must have one entry per row")
-        self._expect_resident(lo.size)
+        self._transform(lo.size)
         out = np.empty(lo.size, dtype=np.float64)
         with self.lock:
             self._check(self.lib.cwtb_global_power_ranges(self.h, _ptr(lo), _ptr(hi), _ptr(out)))
@@ -492,7 +497,7 @@ class Engine(object):
     @_locked
     def power(self, nrows, n0, row_scale=None):
         """|W|^2 of the resident transform, optionally times one factor per row."""
-        self._expect_resident(nrows, n0)
+        self._transform(nrows, n0)
         out = self.result_array((nrows, n0), np.float64)
         with self.lock:
             if row_scale is None:
@@ -508,8 +513,8 @@ class Engine(object):
     def scale_avg_power(self, weights):
         """sum_j weights[j] |W[j, :]|^2 of the resident transform (TC98 eq. 24)."""
         w = np.ascontiguousarray(weights, dtype=np.float64)
-        self._expect_resident(w.size)
-        out = self.result_array((self._resident_n0,), np.float64)
+        _, n0, _ = self._transform(w.size)
+        out = self.result_array((n0,), np.float64)
         with self.lock:
             self._check(self.lib.cwtb_scale_avg_power(self.h, _ptr(w), _ptr(out)))
         return out
@@ -528,8 +533,6 @@ class Engine(object):
             self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_xwt(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), _ptr(sj),
                                           sj.size, int(family), float(param), _ptr(out)))
-            self._resident_n0 = y1.size
-            self._resident = (sj.size, y1.size)     # W12 stays on the device
         return out
 
     @_locked
@@ -547,7 +550,6 @@ class Engine(object):
                                           _ptr(sj), sj.size, int(family), float(param),
                                           int(boxcar_len), _ptr(WCT),
                                           _ptr(aWCT) if want_angle else None))
-            self._resident = None                   # several intermediates, no single transform
         return WCT, aWCT
 
     @_locked
@@ -562,7 +564,6 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         RP2 = self.result_array((sj.size, ys[0].size), np.float64) if want_partial else None
         RM2 = self.result_array((sj.size, ys[0].size), np.float64) if want_multiple else None
-        self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]), ys[0].size,
                                        float(dt), float(dj), _ptr(sj), sj.size, int(family),
@@ -573,13 +574,6 @@ class Engine(object):
 
     # ---- resident coherence and cross spectrum (device buffers of their own, see
     # include/cwt_b200.h) and the reads of a resident field ------------------------------------
-    def _shape(self, field):
-        """(rows, n0) of the resident field: the coherence, the cross spectrum or, for any other
-        field, the transform."""
-        shape = self._held.get(field) if field in _NOT_RESIDENT else self._resident
-        if shape is None:
-            raise EngineError(_NOT_RESIDENT.get(field, "no single transform resident"))
-        return shape
 
     @_locked
     def wct_resident(self, y1, y2, dt, dj, scales, family, param, boxcar_len, precision=F64):
@@ -590,13 +584,10 @@ class Engine(object):
         if y1.shape != y2.shape or y1.ndim != 1:
             raise ValueError("wct_resident: the two series must be 1-D and of equal length")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
-        self._held[FIELD_COH] = None
-        self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
                                                _ptr(sj), sj.size, int(family), float(param),
                                                int(boxcar_len)))
-        self._held[FIELD_COH] = (sj.size, y1.size)
         return self.coherence_serial()
 
     @_locked
@@ -605,7 +596,6 @@ class Engine(object):
 
     @_locked
     def coherence_release(self):
-        self._held[FIELD_COH] = None
         self._check(self.lib.cwtb_coherence_release(self.h))
 
     @_locked
@@ -613,7 +603,7 @@ class Engine(object):
                          want_angle=True):
         """(WCT, aWCT)[row0::row_step][:nrows, col0::col_step][:, :ncols] of the resident
         coherence; a field not asked for is None."""
-        self._shape(FIELD_COH)
+        self._shape(PRODUCT_COHERENCE)
         WCT = self.result_array((nrows, ncols), np.float64) if want_wct else None
         aWCT = self.result_array((nrows, ncols), np.float64) if want_angle else None
         self._check(self.lib.cwtb_coherence_window(
@@ -625,7 +615,7 @@ class Engine(object):
     def coherence_row_stats(self, lo, hi, thr=None, want_phase=False):
         """[rows, 4]: count, sum WCT, sum cos aWCT, sum sin aWCT over the columns [lo[j], hi[j])
         where thr is None or WCT > thr[j]."""
-        rows, _ = self._shape(FIELD_COH)
+        rows, _, _ = self._shape(PRODUCT_COHERENCE)
         lo, hi, thr = _row_args("coherence_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 4), dtype=np.float64)
         self._check(self.lib.cwtb_coherence_row_stats(self.h, _ptr(lo), _ptr(hi),
@@ -636,7 +626,7 @@ class Engine(object):
     @_locked
     def coherence_scale_avg(self, weights):
         """[3, n0]: sum_j w_j WCT[j], sum_j w_j cos aWCT[j], sum_j w_j sin aWCT[j]."""
-        rows, n0 = self._shape(FIELD_COH)
+        rows, n0, _ = self._shape(PRODUCT_COHERENCE)
         w = _weights("coherence_scale_avg", rows, weights)
         out = self.result_array((3, n0), np.float64)
         self._check(self.lib.cwtb_coherence_scale_avg(self.h, _ptr(w), _ptr(out)))
@@ -650,13 +640,10 @@ class Engine(object):
         if any(v.ndim != 1 or v.shape != ys[0].shape for v in ys):
             raise ValueError("wct3_resident: the three series must be 1-D and of equal length")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
-        self._held[FIELD_COH3] = None
-        self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_resident(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]),
                                                 ys[0].size, float(dt), float(dj), _ptr(sj), sj.size,
                                                 int(family), float(param), int(boxcar_len)))
-        self._held[FIELD_COH3] = (sj.size, ys[0].size)
         return self.coherence3_serial()
 
     @_locked
@@ -665,7 +652,6 @@ class Engine(object):
 
     @_locked
     def coherence3_release(self):
-        self._held[FIELD_COH3] = None
         self._check(self.lib.cwtb_coherence3_release(self.h))
 
     @_locked
@@ -674,7 +660,7 @@ class Engine(object):
         """(R, phase)[row0::row_step][:nrows, col0::col_step][:, :ncols] of the resident measure
         (MEASURE_PARTIAL: RP2 and the partial phase; MEASURE_MULTIPLE: RM2, no phase); a field
         not asked for is None."""
-        self._shape(FIELD_COH3)
+        self._shape(PRODUCT_COHERENCE3)
         R = self.result_array((nrows, ncols), np.float64) if want_value else None
         ph = self.result_array((nrows, ncols), np.float64) if want_phase else None
         self._check(self.lib.cwtb_coherence3_window(
@@ -686,7 +672,7 @@ class Engine(object):
     def coherence3_row_stats(self, measure, lo, hi, thr=None, want_phase=False):
         """[rows, 4]: count, sum R, sum cos phase, sum sin phase over the columns [lo[j], hi[j])
         where thr is None or R > thr[j]."""
-        rows, _ = self._shape(FIELD_COH3)
+        rows, _, _ = self._shape(PRODUCT_COHERENCE3)
         lo, hi, thr = _row_args("coherence3_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 4), dtype=np.float64)
         self._check(self.lib.cwtb_coherence3_row_stats(self.h, int(measure), _ptr(lo), _ptr(hi),
@@ -698,7 +684,7 @@ class Engine(object):
     def coherence3_scale_avg(self, measure, weights):
         """[3, n0]: sum_j w_j R[j], sum_j w_j cos phase[j], sum_j w_j sin phase[j] (the last two
         0 for MEASURE_MULTIPLE)."""
-        rows, n0 = self._shape(FIELD_COH3)
+        rows, n0, _ = self._shape(PRODUCT_COHERENCE3)
         w = _weights("coherence3_scale_avg", rows, weights)
         out = self.result_array((3, n0), np.float64)
         self._check(self.lib.cwtb_coherence3_scale_avg(self.h, int(measure), _ptr(w), _ptr(out)))
@@ -713,12 +699,9 @@ class Engine(object):
         if y1.shape != y2.shape or y1.ndim != 1:
             raise ValueError("xwt_resident: the two series must be 1-D and of equal length")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
-        self._held[FIELD_CROSS] = None
-        self._resident = None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_xwt_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt),
                                                _ptr(sj), sj.size, int(family), float(param)))
-        self._held[FIELD_CROSS] = (sj.size, y1.size)
         return self.cross_serial()
 
     @_locked
@@ -727,13 +710,12 @@ class Engine(object):
 
     @_locked
     def cross_release(self):
-        self._held[FIELD_CROSS] = None
         self._check(self.lib.cwtb_cross_release(self.h))
 
     @_locked
     def field_get(self, field):
         """The whole field, complex128 [rows, n0]."""
-        rows, n0 = self._shape(field)
+        rows, n0, _ = self._shape(field)
         out = self.result_array((rows, n0), np.complex128)
         self._check(self.lib.cwtb_field_get(self.h, int(field), 0, rows, _ptr(out)))
         return out
@@ -751,7 +733,7 @@ class Engine(object):
     def field_row_stats(self, field, lo, hi, thr=None):
         """[rows, 5]: count, sum |F|^2, sum |F|, sum cos arg F, sum sin arg F over the columns
         [lo[j], hi[j]) where thr is None or |F|^2 > thr[j]."""
-        rows, _ = self._shape(field)
+        rows, _, _ = self._shape(field)
         lo, hi, thr = _row_args("field_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 5), dtype=np.float64)
         self._check(self.lib.cwtb_field_row_stats(self.h, int(field), _ptr(lo), _ptr(hi),
@@ -761,7 +743,7 @@ class Engine(object):
     @_locked
     def cross_scale_avg(self, weights):
         """sum_j w_j W12[j, :] (complex128, n0)."""
-        rows, n0 = self._shape(FIELD_CROSS)
+        rows, n0, _ = self._shape(PRODUCT_CROSS)
         w = _weights("cross_scale_avg", rows, weights)
         out = self.result_array((n0,), np.complex128)
         self._check(self.lib.cwtb_cross_scale_avg(self.h, _ptr(w), _ptr(out)))
@@ -787,18 +769,19 @@ class Engine(object):
     def wct_mc(self, noise, dt, dj, scales, family, param, boxcar_len, mask, maxscale, nbins,
                hist, precision=F64):
         noise = np.ascontiguousarray(noise, dtype=np.float64)
-        assert noise.ndim == 3 and noise.shape[1] == 2
+        if noise.ndim != 3 or noise.shape[1] != 2:
+            raise ValueError("wct_mc: surrogates must be [pairs, 2, n0]")
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
-        assert mask.shape == (sj.size, noise.shape[2])
-        assert hist.dtype == np.int64 and hist.flags.c_contiguous and hist.shape == (sj.size, nbins)
+        if mask.shape != (sj.size, noise.shape[2]):
+            raise ValueError("wct_mc: mask must be [scales, n0]")
+        h, _ = self._mc_hists("wct_mc", sj.size, nbins, hist, None)
         with self.lock:
             self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_wct_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2],
                                              float(dt), float(dj), _ptr(sj), sj.size, int(family),
                                              float(param), int(boxcar_len), _ptr(mask),
-                                             int(maxscale), int(nbins), _ptr(hist)))
-            self._resident = None
+                                             int(maxscale), int(nbins), h))
         return hist
 
     @_locked
@@ -808,14 +791,14 @@ class Engine(object):
         (Philox stream keyed by (seed, pair number)); accumulated into `hist`."""
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
-        assert mask.shape == (sj.size, int(n0))
-        assert hist.dtype == np.int64 and hist.flags.c_contiguous and hist.shape == (sj.size, nbins)
+        if mask.shape != (sj.size, int(n0)):
+            raise ValueError("wct_mc_seeded: mask must be [scales, n0]")
+        h, _ = self._mc_hists("wct_mc_seeded", sj.size, nbins, hist, None)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_pair), int(n_pairs),
                                                 int(n0), float(dt), _ptr(sj), sj.size, int(family),
                                                 float(param), int(boxcar_len), _ptr(mask), int(maxscale),
-                                                int(nbins), _ptr(hist)))
-        self._resident = None
+                                                int(nbins), h))
         return hist
 
     @_locked
@@ -826,14 +809,15 @@ class Engine(object):
         return out
 
     @staticmethod
-    def _mc3_hists(name, S, nbins, hist_partial, hist_multiple):
-        """The two histograms of a three-series Monte-Carlo call, checked; at least one given."""
-        if hist_partial is None and hist_multiple is None:
+    def _mc_hists(name, S, nbins, hist_a, hist_b):
+        """The histograms of a Monte-Carlo call (two series: hist_b None; three: the partial and
+        the multiple coherence), checked; at least one given."""
+        if hist_a is None and hist_b is None:
             raise ValueError("%s: no histogram given" % name)
-        for h in (hist_partial, hist_multiple):
+        for h in (hist_a, hist_b):
             if h is not None and not (h.dtype == np.int64 and h.flags.c_contiguous and h.shape == (S, nbins)):
                 raise ValueError("%s: histograms must be C-contiguous int64 [%d, %d]" % (name, S, nbins))
-        return [None if h is None else _ptr(h) for h in (hist_partial, hist_multiple)]
+        return [None if h is None else _ptr(h) for h in (hist_a, hist_b)]
 
     @_locked
     def wct3_mc(self, noise, dt, scales, family, param, boxcar_len, mask, maxscale, nbins,
@@ -848,8 +832,7 @@ class Engine(object):
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         if mask.shape != (sj.size, noise.shape[2]):
             raise ValueError("wct3_mc: mask must be [scales, n0]")
-        hp, hm = self._mc3_hists("wct3_mc", sj.size, nbins, hist_partial, hist_multiple)
-        self._resident = None
+        hp, hm = self._mc_hists("wct3_mc", sj.size, nbins, hist_partial, hist_multiple)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2], float(dt),
                                           _ptr(sj), sj.size, int(family), float(param), int(boxcar_len),
@@ -865,8 +848,7 @@ class Engine(object):
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
         if mask.shape != (sj.size, int(n0)):
             raise ValueError("wct3_mc_seeded: mask must be [scales, n0]")
-        hp, hm = self._mc3_hists("wct3_mc_seeded", sj.size, nbins, hist_partial, hist_multiple)
-        self._resident = None
+        hp, hm = self._mc_hists("wct3_mc_seeded", sj.size, nbins, hist_partial, hist_multiple)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_triple),
                                                  int(n_triples), int(n0), float(dt), _ptr(sj), sj.size,
@@ -909,8 +891,7 @@ class Engine(object):
             raise ValueError("wct_mc_phase: mask must be [scales, n0]")
         if nser == 2 and hist_b is not None:
             raise ValueError("wct_mc_phase: two series have one histogram")
-        ha, hb = self._mc3_hists("wct_mc_phase", sj.size, nbins, hist_a, hist_b)
-        self._resident = None
+        ha, hb = self._mc_hists("wct_mc_phase", sj.size, nbins, hist_a, hist_b)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_mc_phase(self.h, _ptr(series), nser, _ptr(groups), int(seed) & (2 ** 64 - 1),
                                                int(first_unit), int(n_units), n0, float(dt), _ptr(sj), sj.size,
@@ -946,7 +927,6 @@ class Engine(object):
                                                 float(param), int(precision),
                                                 _ptr(power) if want_power else None,
                                                 _ptr(W) if want_w else None))
-            self._resident = None                   # the last chunk of channels only
         return power, W
 
     # ---- device-resident benchmarking helpers -------------------------------------
@@ -971,8 +951,6 @@ class Engine(object):
         self._check(self.lib.cwtb_cwt_dev(self.h, dptr, int(is_f32), int(n0), float(dt),
                                           _ptr(sj), sj.size, int(family), float(param),
                                           int(precision)))
-        self._resident_n0 = int(n0)
-        self._resident = (sj.size, int(n0))
 
     @_locked
     def cwt_batch_dev(self, dptr, n_chan, n0, dt, scales, family, param, precision=F64,
@@ -982,8 +960,6 @@ class Engine(object):
         self._check(self.lib.cwtb_cwt_batch_dev(self.h, dptr, int(n_chan), int(n0), float(dt),
                                                 _ptr(sj), sj.size, int(family), float(param),
                                                 int(precision), _ptr(power) if want_power else None))
-        self._resident_n0 = int(n0)
-        self._resident = (int(n_chan) * sj.size, int(n0))
         return power
 
     @_locked

@@ -157,6 +157,7 @@ struct ClassRun {   // scales sharing one execution plan
 
 // A product that one call writes to a device buffer of its own and that later calls read in place
 // (cwtb_wct_resident, cwtb_xwt_resident).  serial is bumped before every write and on release.
+// The resident transform has the same record (cwtb_ctx::wt) without a buffer: W stays scratch.
 struct ResidentSlot {
   Buf buf;
   int S = 0;                     // rows resident (0: none)
@@ -164,6 +165,13 @@ struct ResidentSlot {
   int prec = 0;
   long long serial = 0;
 };
+
+// A call that writes a slot invalidates it first, so that one failing part-way leaves none resident
+static void slot_begin(ResidentSlot &s) {
+  ++s.serial;
+  s.S = 0;
+  s.n0 = 0;
+}
 
 // overlap-save plan of one input scale (os_plan): group + 1 (0: not overlap-save), kept taps
 // [t1 - M + 1, t1] of its impulse response, offset of its H in the context's H buffer
@@ -221,7 +229,6 @@ struct cwtb_ctx {
   int coh_precision = 0;         // arithmetic of xwt / wct / wct_mc: CWTB_F64 or CWTB_F32
                                  // (cwtb_set_coherence_precision)
   std::map<unsigned, BluePlan> blue;
-  long long serial = 0;          // counts transforms: identifies what is resident (cwtb_job_serial)
   rt_stream copy_streams[2]{};   // device->host copies that overlap the kernels or each other
   std::string err;
   double band_eps = 1e-16;
@@ -294,8 +301,10 @@ struct cwtb_ctx {
   // resident partial and multiple coherence (cwtb_wct3_resident): RP2 [S][n0], the partial phase at
   // coh_angle_offset(S*n0), RM2 at twice that offset, double.  Only cwtb_wct3_resident writes it.
   ResidentSlot coh3;
-  bool w_moved = false;          // W went to the cross spectrum, or cwtb_wct3 wrote a smoothed field
-                                 // into it: no transform resident until the next one writes W
+  // resident transform: rows = scales x channels of the complete W in the scratch buffer W, of
+  // precision prec.  prepare opens it (serial: cwtb_job_serial); only a transform entry point that
+  // completes fills it (w_fill), so while it is filled `job` is the plan it was filled from.
+  ResidentSlot wt;
   const void *job_dsig = nullptr;  // device signal of the last cwt_dev call (not owned)
   double last_ms = 0;
   int launches = 0;
@@ -1057,7 +1066,6 @@ static int run_job_exact(cwtb_ctx *c, const Job &job, const double *dsig, double
   if (!Wout) {
     if ((e = ensure(c, c->W, (size_t)S * job.n0 * sizeof(double2)))) return e;
     Wout = (double2 *)c->W.p;
-    c->w_moved = false;
   }
   if ((e = blue_rows(c, dsig, 1, n, (double2 *)c->spec.p, n, n, 1, -1, 1.0, n))) return e;
   const BluePlan *pl;
@@ -1232,7 +1240,6 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
   if (!Wout) {
     if ((e = ensure(c, c->W, (size_t)S * job.n0 * sizeof(V)))) return e;
     Wout = (V *)c->W.p;
-    c->w_moved = false;
   }
   V *spec = (V *)c->spec.p;
   V *W = Wout;
@@ -1535,6 +1542,20 @@ static int time_end(cwtb_ctx *c, double *ms) {
   return time_read(c, ms);
 }
 
+// The record of the resident transform, filled from the plan by a transform entry point once W is
+// complete.  A read that the entry point makes afterwards and that fails empties it again (w_kept):
+// a call that fails leaves no transform resident.
+static void w_fill(cwtb_ctx *c) {
+  c->wt.S = c->job.S * c->job.nbatch;
+  c->wt.n0 = c->job.n0;
+  c->wt.prec = c->job.precision;
+}
+static int w_kept(cwtb_ctx *c, int e) {
+  if (e) c->wt.S = 0;
+  return e;
+}
+
+// iters runs of the plan on the device signal dsig; W is complete, and resident, afterwards
 static int timed_run(cwtb_ctx *c, const void *dsig, int iters, double *ms_out) {
   const Job &job = c->job;
   c->launches = 0;
@@ -1549,6 +1570,7 @@ static int timed_run(cwtb_ctx *c, const void *dsig, int iters, double *ms_out) {
   if ((e = time_end(c, &ms))) return e;
   if (ms_out) *ms_out = ms / iters;
   c->launches /= std::max(1, iters);
+  w_fill(c);
   return 0;
 }
 
@@ -1886,7 +1908,10 @@ static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, i
   if (!scales) return fail(c, CWTB_ERR_ARG, "null scales");
   RT(rt_set_device(c->device));
   if (nbatch < 1 || (long long)nbatch * S > 60000) return fail(c, CWTB_ERR_ARG, "batch too large for one launch");
-  ++c->serial;   // whatever was resident is about to be replaced
+  // whatever transform was resident is about to be replaced, and the re-runs of cwtb_bench_last /
+  // cwtb_profile_last wait for a signal of the new plan
+  slot_begin(c->wt);
+  c->job_dsig = nullptr;
   cwtb_ctx::PlanKey key;
   key.n0 = n0; key.dt = dt; key.param = param; key.band_eps = c->band_eps; key.band_eps32 = c->band_eps32;
   key.expand_eps = c->expand_eps; key.expand_eps32 = c->expand_eps32; key.S = S; key.family = family;
@@ -1979,13 +2004,12 @@ int cwtb_bench_last(cwtb_ctx *c, int iters, double *ms_out) {
   return timed_run(c, c->job_dsig, iters, ms_out);
 }
 
-// a transform's W is on the device (cwtb_xwt_resident moves it to the cross spectrum)
-static bool w_resident(const cwtb_ctx *c) { return c->job.valid && !c->w_moved; }
+static bool w_resident(const cwtb_ctx *c) { return c->wt.S > 0; }
 
 double cwtb_last_kernel_ms(cwtb_ctx *c) { return c ? c->last_ms : -1; }
 int cwtb_last_launch_count(cwtb_ctx *c) { return c ? c->launches : -1; }
 int64_t cwtb_padded_length(cwtb_ctx *c) { return (c && c->job.valid) ? (int64_t)c->job.N : -1; }
-int64_t cwtb_job_serial(cwtb_ctx *c) { return c ? c->serial : -1; }
+int64_t cwtb_job_serial(cwtb_ctx *c) { return c ? c->wt.serial : -1; }
 void *cwtb_w_device_ptr(cwtb_ctx *c) { return (c && w_resident(c)) ? c->W.p : nullptr; }
 
 int cwtb_last_plan(cwtb_ctx *c, int *out, int n) {
@@ -2033,9 +2057,9 @@ static int field_to_host(cwtb_ctx *c, const void *field, int prec, size_t first,
 
 int cwtb_get_w(cwtb_ctx *c, void *out, int out_f64, int row0, int nrows) {
   if (!c || !w_resident(c) || !out) return fail(c, CWTB_ERR_STATE, "no transform resident");
-  const Job &job = c->job;
-  if (row0 < 0 || nrows < 0 || row0 + nrows > job.S * job.nbatch) return fail(c, CWTB_ERR_ARG, "row range");
-  return field_to_host(c, c->W.p, job.precision, (size_t)row0 * job.n0, (size_t)nrows * job.n0, out, out_f64);
+  const ResidentSlot &w = c->wt;
+  if (row0 < 0 || nrows < 0 || row0 + nrows > w.S) return fail(c, CWTB_ERR_ARG, "row range");
+  return field_to_host(c, c->W.p, w.prec, (size_t)row0 * w.n0, (size_t)nrows * w.n0, out, out_f64);
 }
 
 int cwtb_get_signal_fft(cwtb_ctx *c, void *out) {
@@ -2195,7 +2219,6 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   const size_t cnt = (size_t)S * n0;
   int e;
   if ((e = ensure(c, c->W, cnt * sizeof(V)))) return e;
-  c->w_moved = false;
   if ((e = ensure(c, c->W2, cnt * sizeof(V)))) return e;
   if ((e = ensure(c, c->C, cnt * sizeof(V)))) return e;
   if ((e = ensure(c, c->A12, cnt * sizeof(V)))) return e;
@@ -2251,7 +2274,6 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
   int e;
   for (Buf *b : {&c->W, &c->W2, &c->W3, &c->C, &c->A12})
     if ((e = ensure(c, *b, cnt * sizeof(V)))) return e;
-  c->w_moved = false;
   if ((e = run_job<T>(c, job, dy, (V *)c->W.p, EPI_STORE))) return e;
   if ((e = run_job<T>(c, job, dx1, (V *)c->W2.p, EPI_STORE))) return e;
   if ((e = run_job<T>(c, job, dx2, (V *)c->W3.p, EPI_STORE))) return e;
@@ -2369,13 +2391,15 @@ int cwtb_cwt_to_host(cwtb_ctx *c, const void *signal, int signal_is_f32, int64_t
       RT(rt_d2h(out, W, (size_t)r0 * rowb, c->stream));               // after every chain has joined
       RT(rt_sync(c->copy_streams[0]));
       RT(rt_sync(c->stream));
-      return time_read(c, &c->last_ms);
+      if ((e = time_read(c, &c->last_ms))) return e;
+      w_fill(c);
+      return 0;
     }
     // not eligible: fall through to the plain sequence (prepare runs again, cheap)
   }
   int e = cwtb_cwt(c, signal, signal_is_f32, n0, dt, scales, n_scales, family, param, precision, nullptr);
   if (e) return e;
-  return cwtb_get_w(c, out, out_f64, 0, n_scales);
+  return w_kept(c, cwtb_get_w(c, out, out_f64, 0, n_scales));
 }
 
 // rows per block of the column reductions: enough blocks to fill the machine, few enough that the
@@ -2520,11 +2544,11 @@ int cwtb_scale_avg_power(cwtb_ctx *c, const double *weights, double *out) {
   return 0;
 }
 
-// the resident job is a job of type T afterwards: cwtb_get_w widens an fp32 W12 on the device
+// W12 in W; the plan is a job of type T afterwards: cwtb_get_w widens an fp32 W12 on the device
 extern "C++" {
 template <typename T>
 static int xwt_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double dt, const double *scales,
-                   int n_scales, int family, double param, void *W12_out) {
+                   int n_scales, int family, double param) {
   int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_series<T>(c, c->sig, y1, n0))) return e;
@@ -2535,7 +2559,6 @@ static int xwt_run(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, 
   if ((e = run_job<T>(c, c->job, (const T *)c->sig2.p, nullptr, EPI_MULCONJ))) return e;
   if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
-  if (W12_out) return cwtb_get_w(c, W12_out, 1, 0, n_scales);
   RT(rt_sync(c->stream));
   return 0;
 }
@@ -2545,19 +2568,14 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
              int n_scales, int family, double param, void *W12_out) {
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
   if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
-  return c->coh_precision == CWTB_F32
-             ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out)
-             : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, W12_out);
+  int e = c->coh_precision == CWTB_F32 ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param)
+                                       : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param);
+  if (e) return e;
+  w_fill(c);   // W12 is the resident transform
+  return W12_out ? w_kept(c, cwtb_get_w(c, W12_out, 1, 0, n_scales)) : 0;
 }
 
 // ---- resident products and the reading calls ------------------------------------------------
-// A call that writes a slot invalidates it first, so that one failing part-way leaves none resident
-static void slot_begin(ResidentSlot &s) {
-  ++s.serial;
-  s.S = 0;
-  s.n0 = 0;
-}
-
 static int slot_release(cwtb_ctx *c, ResidentSlot &s) {
   slot_begin(s);
   if (s.buf.p) {
@@ -2574,14 +2592,12 @@ int cwtb_xwt_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n
   if (!c || !y1 || !y2) return fail(c, CWTB_ERR_ARG, "null argument");
   if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "xwt needs an analytic wavelet family");
   slot_begin(c->cross);
-  int e = c->coh_precision == CWTB_F32
-              ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr)
-              : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param, nullptr);
+  int e = c->coh_precision == CWTB_F32 ? xwt_run<float>(c, y1, y2, n0, dt, scales, n_scales, family, param)
+                                       : xwt_run<double>(c, y1, y2, n0, dt, scales, n_scales, family, param);
   if (e) return e;
   // W12 is the transform's W: take the buffer over.  No kernel or plan keeps W's address (every
   // run takes it afresh from c->W), so the old cross buffer can serve as the next W.
   std::swap(c->W, c->cross.buf);
-  c->w_moved = true;
   c->cross.S = n_scales;
   c->cross.n0 = n0;
   c->cross.prec = c->job.precision;
@@ -2611,9 +2627,10 @@ struct FieldRef {
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   if (!c) return CWTB_ERR_ARG;
   if (field == CWTB_FIELD_W) {
-    if (!w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
+    const ResidentSlot &s = c->wt;
+    if (s.S <= 0) return fail(c, CWTB_ERR_STATE, "no transform resident");
     if (c->job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "field of a batched transform: fetch rows per channel");
-    f = FieldRef{field, c->W.p, c->job.precision, c->job.S, c->job.n0, 0};
+    f = FieldRef{field, c->W.p, s.prec, s.S, s.n0, 0};
   } else if (field == CWTB_FIELD_CROSS || field == FIELD_COH) {
     const bool coh = field == FIELD_COH;
     const ResidentSlot &s = coh ? c->coh : c->cross;
@@ -2857,7 +2874,6 @@ static int wct3_run(cwtb_ctx *c, const double *y, const double *x1, const double
   if ((e = time_begin(c))) return e;
   e = wct3_core<T>(c, c->job, (const T *)c->sig.p, (const T *)c->sig2.p, (const T *)c->sig3.p,
                    boxcar_len, dRP2, dRM2, nullptr, 0, 0, nullptr, nullptr, dPP);
-  c->w_moved = true;   // W holds a smoothed field now, not a transform
   if (e) return e;
   if ((e = time_end(c, &c->last_ms))) return e;
   c->job_dsig = nullptr;
@@ -2980,6 +2996,20 @@ int cwtb_coherence3_scale_avg(cwtb_ctx *c, int measure, const double *weights, d
   FieldRef f;
   int e = coh3_ref(c, measure, false, f);
   return e ? e : scale_avg_run(c, f, weights, out);
+}
+
+int cwtb_resident_shape(cwtb_ctx *c, int product, int *rows, int64_t *n0, int *precision) {
+  if (!c) return CWTB_ERR_ARG;
+  const ResidentSlot *s = product == CWTB_PRODUCT_W           ? &c->wt
+                        : product == CWTB_PRODUCT_CROSS       ? &c->cross
+                        : product == CWTB_PRODUCT_COHERENCE   ? &c->coh
+                        : product == CWTB_PRODUCT_COHERENCE3  ? &c->coh3 : nullptr;
+  if (!s) return fail(c, CWTB_ERR_ARG, "unknown product");
+  const bool on = s->S > 0;
+  if (rows) *rows = on ? s->S : 0;
+  if (n0) *n0 = on ? s->n0 : 0;
+  if (precision) *precision = on ? s->prec : CWTB_F64;
+  return 0;
 }
 
 int cwtb_set_coherence_precision(cwtb_ctx *c, int precision) {
@@ -3141,7 +3171,6 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
       e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0])
                     : wct3_core<T>(c, c->job, a, a + n0, a + 2 * n0, boxcar_len, nullptr, nullptr, dmask, maxscale,
                                    nbins, dh[0], dh[1]);
-      if (nser == 3) c->w_moved = true;   // W holds a smoothed field now, not a transform
       if (e) return e;
     }
   }
@@ -3431,6 +3460,7 @@ static int cwt_batch_pipelined(cwtb_ctx *c, const void *X, int x_is_f32, int n_c
   RT(rt_sync(copy));
   if ((e = time_read(c, &c->last_ms))) return e;
   for (size_t i = 0; i < (size_t)n_chan * n_scales; ++i) power_out[i] /= (double)n0;
+  w_fill(c);   // the last chunk
   return 0;
 }
 
@@ -3468,8 +3498,8 @@ int cwtb_cwt_batch(cwtb_ctx *c, const void *X, int x_is_f32, int n_chan, int64_t
     c->job_dsig = c->sig.p;
     c->job.sig_is_f32 = f32;
     if ((e = timed_run(c, c->sig.p, 1, &c->last_ms))) return e;
-    if (power_out && (e = cwtb_global_power(c, power_out + (size_t)ch0 * n_scales))) return e;
-    if (W_out && (e = cwtb_get_w(c, (char *)W_out + (size_t)ch0 * per_chan, 0, 0, nc * n_scales))) return e;
+    if (power_out && (e = cwtb_global_power(c, power_out + (size_t)ch0 * n_scales))) return w_kept(c, e);
+    if (W_out && (e = cwtb_get_w(c, (char *)W_out + (size_t)ch0 * per_chan, 0, 0, nc * n_scales))) return w_kept(c, e);
   }
   return 0;
 }
@@ -3486,8 +3516,7 @@ int cwtb_cwt_batch_dev(cwtb_ctx *c, const void *d_X, int n_chan, int64_t n0, dou
   c->job_dsig = d_X;
   c->job.sig_is_f32 = (precision == CWTB_F32);
   if ((e = timed_run(c, d_X, 1, &c->last_ms))) return e;
-  if (power_out) return cwtb_global_power(c, power_out);
-  return 0;
+  return power_out ? w_kept(c, cwtb_global_power(c, power_out)) : 0;
 }
 
 

@@ -296,26 +296,45 @@ def test_unpadded_mode_public_api(emu, monkeypatch):
 
 
 def test_python_side_shape_guards(emu):
-    """The C side sizes its copies from the resident job; the ctypes layer refuses calls whose
-    array shapes disagree with it instead of letting them overrun."""
+    """The C side sizes its copies from the resident transform; the ctypes layer sizes its arrays
+    from the engine's record of it and refuses calls whose array shapes disagree with it instead
+    of letting them overrun, whichever call left the transform."""
     x = np.random.RandomState(0).randn(100)
     sj = np.array([2.0, 4.0, 8.0])
-    emu.cwt(x, 1.0, sj, 0, 6.0, fetch=False)
-    with pytest.raises(ValueError):
-        emu.get_w(3, 64)                 # wrong column count
-    with pytest.raises(ValueError):
-        emu.get_w(4, 100)                # more rows than resident
-    with pytest.raises(ValueError):
-        emu.global_power(5)
-    with pytest.raises(ValueError):
-        emu.power(3, 99)
-    with pytest.raises(ValueError):
-        emu.scale_avg_power(np.ones(2))
-    with pytest.raises(ValueError):
-        emu.global_power_ranges(np.zeros(3), np.ones(4))
-    with pytest.raises(ValueError):
-        emu.smooth(np.ones((4, 100)), 1.0, sj, 5)
-    assert emu.get_w(2, 100).shape == (2, 100) and emu.global_power(3).shape == (3,)
+
+    def cwt_dev(precision):
+        xd = x.astype(np.float32 if precision else np.float64)
+        d = emu.dev_alloc(xd.nbytes)
+        emu.h2d(d, xd)
+        emu.cwt_dev(d, precision, 100, 1.0, sj, 0, 6.0, precision)
+        emu.dev_free(d)
+
+    for setup in (lambda: emu.cwt(x, 1.0, sj, 0, 6.0, fetch=False),
+                  lambda: emu.cwt(x, 1.0, sj, 0, 6.0),
+                  lambda: emu.cwt(x, 1.0, sj, 0, 6.0, precision=1, fetch=False),
+                  lambda: cwt_dev(0), lambda: cwt_dev(1),
+                  lambda: emu.xwt(x, x[::-1], 1.0, sj, 0, 6.0),
+                  lambda: emu.cwt_batch(x[None, :], 1.0, sj, 0, 6.0),
+                  lambda: emu.cwt_batch(x[None, :], 1.0, sj, 0, 6.0, want_w=True)):
+        setup()
+        with pytest.raises(ValueError):
+            emu.get_w(3, 64)                 # wrong column count
+        with pytest.raises(ValueError):
+            emu.get_w(4, 100)                # more rows than resident
+        with pytest.raises(ValueError):
+            emu.global_power(5)
+        with pytest.raises(ValueError):
+            emu.power(3, 99)
+        with pytest.raises(ValueError):
+            emu.scale_avg_power(np.ones(2))
+        with pytest.raises(ValueError):
+            emu.global_power_ranges(np.zeros(3), np.ones(4))
+        with pytest.raises(ValueError):
+            emu.global_power_ranges(np.zeros(2), np.ones(2))
+        with pytest.raises(ValueError):
+            emu.smooth(np.ones((4, 100)), 1.0, sj, 5)
+        assert emu.get_w(2, 100).shape == (2, 100) and emu.global_power(3).shape == (3,)
+        assert emu.icwt_sum().shape == (100,) and emu.scale_avg_power(np.ones(3)).shape == (100,)
 
 
 def check_seeded_monte_carlo(eng):
