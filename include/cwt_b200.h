@@ -431,6 +431,57 @@ int cwtb_wct_mc_phase(cwtb_ctx *ctx, const double *series, int nser, const int *
 int cwtb_mc_phase_surrogates(cwtb_ctx *ctx, const double *series, int nser, const int *group,
                              uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out);
 
+/* ---- point-wise tests of the resident coherence against phase-randomised surrogates ----------
+ * cwtb_coherence_surrogate_counts (two series: the resident coherence of cwtb_wct_resident) and
+ * cwtb_coherence3_surrogate_counts (three: the resident RP2 and RM2 of cwtb_wct3_resident) run the
+ * units first_unit .. first_unit + n_units - 1 of cwtb_wct_mc_phase (same arguments, same surrogates,
+ * same histograms accumulated into hist / hist_partial, hist_multiple) and also count, for every
+ * point of every row (the cone of influence and the rows from maxscale on included),
+ *   k[s, n] += 1  where  R2_unit[s, n] >= R2_obs[s, n]  or R2_unit[s, n] is not finite,
+ * into uint32 counters [n_scales][n0] per measure that live with the resident product (4 bytes per
+ * scale-point for the coherence, 8 for the partial and multiple coherence), allocated at the first
+ * call.  reset != 0 zeroes them first; otherwise the units are added to the ones already counted, so
+ * units [0, a) then [a, M) give the counts of [0, M).  CWTB_ERR_STATE: `serial` is not the product's
+ * current serial (cwtb_coherence_serial / cwtb_coherence3_serial), or n_scales / n0 differ from the
+ * resident product's.  CWTB_ERR_ARG: the arguments of cwtb_wct_mc_phase, or a total of units above
+ * 2^32 - 1.  The counts compare like with like only when the call runs the plan the product was
+ * computed with (the same scales, precision, padding mode and smoothing filter).  Lifetime: the
+ * counts die with their product (a new cwtb_wct_resident / cwtb_wct3_resident, the release calls,
+ * cwtb_destroy); a counting call that fails leaves none readable. */
+int cwtb_coherence_surrogate_counts(cwtb_ctx *ctx, const double *series, const int *group, uint64_t seed,
+                                    int64_t first_unit, int n_units, int64_t n0, double dt,
+                                    const double *scales, int n_scales, int family, double param,
+                                    int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                                    int64_t *hist, int64_t serial, int reset);
+int cwtb_coherence3_surrogate_counts(cwtb_ctx *ctx, const double *series, const int *group, uint64_t seed,
+                                     int64_t first_unit, int n_units, int64_t n0, double dt,
+                                     const double *scales, int n_scales, int family, double param,
+                                     int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                                     int64_t *hist_partial, int64_t *hist_multiple, int64_t serial,
+                                     int reset);
+/* Reading the counts of M units.  They return CWTB_ERR_STATE when the product or its counts are not
+ * resident, and the errors of the corresponding cwtb_coherence*_window / _row_stats calls.
+ * p-value window: p = (1 + k) / (1 + M) in double, NaN where the observed value is not finite, with
+ * the layout and checks of cwtb_coherence_window. */
+int cwtb_coherence_pvalue_window(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0,
+                                 int64_t ncols, int64_t col_step, double *p_out);
+int cwtb_coherence3_pvalue_window(cwtb_ctx *ctx, int measure, int row0, int nrows, int row_step,
+                                  int64_t col0, int64_t ncols, int64_t col_step, double *p_out);
+/* The row stats of cwtb_coherence_row_stats / cwtb_coherence3_row_stats over the points whose
+ * observed value is finite and whose count k <= kmax (and R > thr[j] where thr is given).  A
+ * selection p <= alpha is the cut kmax = the largest k with (1 + k) / (1 + M) <= alpha. */
+int cwtb_coherence_pvalue_row_stats(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, const double *thr,
+                                    int64_t kmax, int want_phase, double *out);
+int cwtb_coherence3_pvalue_row_stats(cwtb_ctx *ctx, int measure, const int64_t *lo, const int64_t *hi,
+                                     const double *thr, int64_t kmax, int want_phase, double *out);
+/* out[k] (nbins = M + 1 int64, else CWTB_ERR_ARG) = the number of points with count k over the
+ * columns [lo[j], hi[j]) of every row j whose observed value is finite: the histogram that decides
+ * a Benjamini-Hochberg / -Yekutieli step-up test on the host.  Integer sums: bit-identical. */
+int cwtb_coherence_count_hist(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, int64_t nbins,
+                              int64_t *out);
+int cwtb_coherence3_count_hist(cwtb_ctx *ctx, int measure, const int64_t *lo, const int64_t *hi,
+                               int64_t nbins, int64_t *out);
+
 /* ---- batched transform of independent channels (SURVEY 8d config 5) ------- */
 /* X: host [n_chan, n0] (float or double).  The per-channel transforms stay on
  * the device; `power_out` (may be NULL) receives the per-channel global wavelet

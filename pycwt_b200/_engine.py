@@ -103,6 +103,16 @@ _SIGNATURES = {
     "cwtb_wct_mc_phase": (_I, [_P, _P, _I, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _I, _I,
                                 _P, _P]),
     "cwtb_mc_phase_surrogates": (_I, [_P, _P, _I, _P, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_coherence_surrogate_counts": (_I, [_P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I,
+                                             _P, _I, _I, _P, _I64, _I]),
+    "cwtb_coherence3_surrogate_counts": (_I, [_P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I,
+                                              _P, _I, _I, _P, _P, _I64, _I]),
+    "cwtb_coherence_pvalue_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_coherence3_pvalue_window": (_I, [_P, _I, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_coherence_pvalue_row_stats": (_I, [_P, _P, _P, _P, _I64, _I, _P]),
+    "cwtb_coherence3_pvalue_row_stats": (_I, [_P, _I, _P, _P, _P, _I64, _I, _P]),
+    "cwtb_coherence_count_hist": (_I, [_P, _P, _P, _I64, _P]),
+    "cwtb_coherence3_count_hist": (_I, [_P, _I, _P, _P, _I64, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -907,6 +917,77 @@ class Engine(object):
         self._check(self.lib.cwtb_mc_phase_surrogates(self.h, _ptr(series), series.shape[0], _ptr(groups),
                                                       int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
                                                       series.shape[1], _ptr(out)))
+        return out
+
+    # ---- point-wise tests of a resident coherence against phase-randomised surrogates ----------
+    # `measure` None: the resident coherence (cwtb_coherence_*); MEASURE_PARTIAL / _MULTIPLE: the
+    # resident partial / multiple coherence (cwtb_coherence3_*).
+    @_locked
+    def surrogate_counts(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+                         mask, maxscale, nbins, hist_a, hist_b=None, serial=None, reset=True, precision=F64):
+        """`wct_mc_phase` that also counts, per point, the units whose coherence (two series) or
+        partial and multiple coherence (three) reach the resident product's, into that product's
+        counters (cwtb_coherence*_surrogate_counts); `serial` is the product's serial.  `reset`
+        zeroes the counters first, otherwise the units are added."""
+        series, groups = self._phase_inputs("surrogate_counts", series, groups)
+        nser, n0 = series.shape
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        if mask.shape != (sj.size, n0):
+            raise ValueError("surrogate_counts: mask must be [scales, n0]")
+        if nser == 2 and hist_b is not None:
+            raise ValueError("surrogate_counts: two series have one histogram")
+        ha, hb = self._mc_hists("surrogate_counts", sj.size, nbins, hist_a, hist_b)
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        args = (self.h, _ptr(series), _ptr(groups), int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
+                float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
+                int(nbins))
+        if nser == 2:
+            self._check(self.lib.cwtb_coherence_surrogate_counts(*args, ha, int(serial), 1 if reset else 0))
+        else:
+            self._check(self.lib.cwtb_coherence3_surrogate_counts(*args, ha, hb, int(serial), 1 if reset else 0))
+        return hist_a, hist_b
+
+    @_locked
+    def pvalue_window(self, measure, row0, nrows, row_step, col0, ncols, col_step):
+        """p = (1 + k) / (1 + M) [row0::row_step][:nrows, col0::col_step][:, :ncols] of the counts
+        of the resident product, NaN where its value is not finite."""
+        P = self.result_array((nrows, ncols), np.float64)
+        w = (int(row0), int(nrows), int(row_step), int(col0), int(ncols), int(col_step), _ptr(P))
+        if measure is None:
+            self._shape(PRODUCT_COHERENCE)
+            self._check(self.lib.cwtb_coherence_pvalue_window(self.h, *w))
+        else:
+            self._shape(PRODUCT_COHERENCE3)
+            self._check(self.lib.cwtb_coherence3_pvalue_window(self.h, int(measure), *w))
+        return P
+
+    @_locked
+    def pvalue_row_stats(self, measure, lo, hi, kmax, thr=None, want_phase=False):
+        """[rows, 4] of `coherence_row_stats` / `coherence3_row_stats` over the points with a finite
+        value and a count k <= kmax."""
+        rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else PRODUCT_COHERENCE3)
+        lo, hi, thr = _row_args("pvalue_row_stats", rows, lo, hi, thr)
+        out = np.empty((rows, 4), dtype=np.float64)
+        a = (_ptr(lo), _ptr(hi), None if thr is None else _ptr(thr), int(kmax), 1 if want_phase else 0, _ptr(out))
+        if measure is None:
+            self._check(self.lib.cwtb_coherence_pvalue_row_stats(self.h, *a))
+        else:
+            self._check(self.lib.cwtb_coherence3_pvalue_row_stats(self.h, int(measure), *a))
+        return out
+
+    @_locked
+    def count_hist(self, measure, lo, hi, nbins):
+        """int64 [nbins]: the number of points with count k over the columns [lo[j], hi[j]) whose
+        value is finite; nbins must be M + 1."""
+        rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else PRODUCT_COHERENCE3)
+        lo, hi, _ = _row_args("count_hist", rows, lo, hi, None)
+        out = np.empty(int(nbins), dtype=np.int64)
+        if measure is None:
+            self._check(self.lib.cwtb_coherence_count_hist(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
+        else:
+            self._check(self.lib.cwtb_coherence3_count_hist(self.h, int(measure), _ptr(lo), _ptr(hi), int(nbins),
+                                                            _ptr(out)))
         return out
 
     @_locked

@@ -164,13 +164,19 @@ struct ResidentSlot {
   long long n0 = 0;
   int prec = 0;
   long long serial = 0;
+  // the coherence slots: surrogate exceedance counts of the resident fields, uint32 [S][n0] per
+  // measure (cwtb_coherence*_surrogate_counts), and the units they hold (-1: none readable)
+  Buf counts;
+  long long units = -1;
 };
 
 // A call that writes a slot invalidates it first, so that one failing part-way leaves none resident
+// (and no counts of an earlier product readable)
 static void slot_begin(ResidentSlot &s) {
   ++s.serial;
   s.S = 0;
   s.n0 = 0;
+  s.units = -1;
 }
 
 // overlap-save plan of one input scale (os_plan): group + 1 (0: not overlap-save), kept taps
@@ -1662,7 +1668,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2212,7 +2218,7 @@ static int smooth_time(cwtb_ctx *c, cx<T> *X, int S, long long n0, unsigned N, c
 template <typename T>
 static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2, int K,
                     double *dWCT, double *daWCT, const unsigned char *dmask, int maxscale, int nbins,
-                    unsigned long long *dhist) {
+                    unsigned long long *dhist, const double *dobs = nullptr, unsigned *dcnt = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2236,10 +2242,10 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   }
   if ((e = smooth_time<T>(c, (V *)c->C.p, S, n0, job.N, d_g))) return e;
   if ((e = smooth_time<T>(c, (V *)c->A12.p, S, n0, job.N, d_g))) return e;
-  const int rows_out = dWCT ? S : maxscale;
+  const int rows_out = dWCT || dcnt ? S : maxscale;   // counting: every row
   if (rows_out <= 0) return 0;
   WctFinalArgs<T> fa{(const V *)c->C.p, (const V *)c->A12.p, (const double *)c->win.p, dWCT,
-                     dmask, dhist, n0, S, K, maxscale, nbins};
+                     dmask, dhist, n0, S, K, maxscale, nbins, dobs, dcnt};
   if (K > 64) {
     // longer than the fused kernel stages: the scale boxcar of both fields into W and W2 (dead
     // since WctPrepBody), then the ratio through the fused kernel with the unit tap at win + K
@@ -2259,14 +2265,15 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
 // three transforms + partial / multiple coherence in the engine type T; outputs are device
 // pointers (any may be null) and double for every T, dPP the partial phase.  With every output null
 // (Monte-Carlo mode) only the rows below maxscale are finished, into the histograms dhP / dhM
-// (either may be null).
+// (either may be null); with counters (cP / cM, against the observed oP / oM) every row is finished.
 // Device memory per scale-point: the three transforms W, W2, W3 (the crosses are written over
 // them), the two auto fields C, A12 and the smoothing buffer F.
 template <typename T>
 static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, const T *dx2, int K,
                      double *dRP2, double *dRM2, const unsigned char *dmask = nullptr, int maxscale = 0,
                      int nbins = 0, unsigned long long *dhP = nullptr, unsigned long long *dhM = nullptr,
-                     double *dPP = nullptr) {
+                     double *dPP = nullptr, const double *oP = nullptr, const double *oM = nullptr,
+                     unsigned *cP = nullptr, unsigned *cM = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2285,7 +2292,7 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
   if ((e = launch<Wct3PrepBody<T>>(c, gx, S, pa))) return e;
   for (V *x : f)
     if ((e = smooth_time<T>(c, x, S, n0, job.N, d_g))) return e;
-  const int rows_out = dRP2 || dRM2 || dPP ? S : maxscale;
+  const int rows_out = dRP2 || dRM2 || dPP || cP || cM ? S : maxscale;
   if (rows_out <= 0) return 0;
   const double *win = (const double *)c->win.p;
   if (K > 64) {
@@ -2301,7 +2308,8 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
     win += K;
     K = 1;
   }
-  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dPP, dmask, dhP, dhM, n0, S, K, maxscale, nbins};
+  Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dPP, dmask, dhP, dhM, n0, S, K, maxscale, nbins,
+                      oP, oM, cP, cM};
   using F16 = Wct3FinalBody<T, 16, 32, 16>;
   using F64K = Wct3FinalBody<T, 64, 64, 8>;
   if (K <= 16)
@@ -2578,11 +2586,13 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
 // ---- resident products and the reading calls ------------------------------------------------
 static int slot_release(cwtb_ctx *c, ResidentSlot &s) {
   slot_begin(s);
-  if (s.buf.p) {
+  if (s.buf.p || s.counts.p) {
     RT(rt_set_device(c->device));
     RT(rt_sync(c->stream));
-    rt_free(s.buf.p);
-    s.buf = Buf{};
+    for (Buf *b : {&s.buf, &s.counts}) {
+      if (b->p) rt_free(b->p);
+      *b = Buf{};
+    }
   }
   return 0;
 }
@@ -2622,6 +2632,10 @@ struct FieldRef {
   int prec, S;      // prec: the complex field's element type (the double fields are double)
   long long n0;
   size_t angle;     // coherence / partial coherence: the phase's offset from the value, in doubles
+  // a double field read with its surrogate exceedance counts (count_ref): the counts, the units M
+  // they hold and the row stats' cut k <= kmax; cnt null: the field alone
+  const unsigned *cnt = nullptr;
+  long long m = 0, kmax = 0;
 };
 
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
@@ -2648,6 +2662,17 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   return 0;
 }
 
+// The counts of a coherence field f (field_ref of FIELD_COH, FIELD_COH3_P or FIELD_COH3_M) added
+// to it, with the row stats' cut kmax
+static int count_ref(cwtb_ctx *c, long long kmax, FieldRef &f) {
+  const ResidentSlot &s = f.field == FIELD_COH ? c->coh : c->coh3;
+  if (s.units < 0 || !s.counts.p) return fail(c, CWTB_ERR_STATE, "no surrogate counts resident for this product");
+  f.cnt = (const unsigned *)s.counts.p + (f.field == FIELD_COH3_M ? coh_angle_offset((size_t)s.S * s.n0) : 0);
+  f.m = s.units;
+  f.kmax = kmax;
+  return 0;
+}
+
 // the field of a cwtb_field_* call
 static int cx_field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   if (c && field != CWTB_FIELD_W && field != CWTB_FIELD_CROSS) return fail(c, CWTB_ERR_ARG, "unknown field");
@@ -2667,8 +2692,19 @@ static int with_view(const FieldRef &f, int want_phase, Fn &&fn) {
   return fn(CxView<float>{(const cx<float> *)f.p});
 }
 
+// the reads of the window and the row stats: with_view's view, or the counting view of a field
+// that carries counts
+template <typename Fn>
+static int with_read_view(const FieldRef &f, int want_phase, Fn &&fn) {
+  if (!f.cnt) return with_view(f, want_phase, fn);
+  const double *w = (const double *)f.p;
+  if (f.field == FIELD_COH3_M) return fn(CohCountViewT<false>{w, nullptr, f.cnt, f.kmax, f.m, 0});
+  return fn(CohCountViewT<true>{w, w + f.angle, f.cnt, f.kmax, f.m, want_phase});
+}
+
 // Strided sub-grid into out0 / out1: a double field's value / phase (nothing asked for: nothing to
-// do; a field without a phase takes out1 == null), or a complex field as complex128 into out0
+// do; a field without a phase takes out1 == null), a field with counts its p-values into out0, or a
+// complex field as complex128 into out0
 static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int row_step, int64_t col0,
                       int64_t ncols, int64_t col_step, void *out0, void *out1) {
   const int S = f.S;
@@ -2680,7 +2716,7 @@ static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int r
   if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
       col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
     return fail(c, CWTB_ERR_ARG, "window outside the resident field");
-  if (row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
+  if (!f.cnt && row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
     const size_t off = (size_t)row0 * n0, cnt = (size_t)nrows * n0;
     if (!coh) return field_to_host(c, f.p, f.prec, off, cnt, out0, 1);
     const double *dW = (const double *)f.p;
@@ -2693,7 +2729,7 @@ static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int r
   int e = ensure(c, c->aux, m * sizeof(double2));
   if (e) return e;
   double *o0 = (double *)c->aux.p, *o1 = o0 + m;   // a complex128 output takes both halves
-  e = with_view(f, 0, [&](auto v) {
+  e = with_read_view(f, 0, [&](auto v) {
     WindowArgs<decltype(v)> a{v, out0 ? o0 : nullptr, out1 ? o1 : nullptr, n0, row0, row_step, col0, col_step, ncols};
     return launch<WindowBody<decltype(v)>>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a);
   });
@@ -2719,7 +2755,7 @@ static int row_stats_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, cons
       return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
   }
   if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
-  return with_view(f, want_phase, [&](auto v) {
+  return with_read_view(f, want_phase, [&](auto v) {
     using B = RowStatsBody<decltype(v)>;
     constexpr int K = B::K;
     const int nchunk = (int)((n0 + B::CHUNK - 1) / B::CHUNK);
@@ -2768,6 +2804,40 @@ static int scale_avg_run(cwtb_ctx *c, const FieldRef &f, const double *weights, 
     RT(rt_sync(c->stream));
     return 0;
   });
+}
+
+// Histogram [M + 1] of the counts of a field with counts over the columns [lo_j, hi_j) of every
+// row, of the points whose value is finite
+static int count_hist_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, const int64_t *hi, int64_t nbins,
+                          int64_t *out) {
+  if (!lo || !hi || !out) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (nbins != f.m + 1) return fail(c, CWTB_ERR_ARG, "count_hist: the histogram has M + 1 bins (M: the units counted)");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  std::vector<long long> h(2 * (size_t)S);
+  long long span = 0;
+  for (int j = 0; j < S; ++j) {
+    h[j] = lo[j];
+    h[S + j] = hi[j];
+    if (lo[j] < 0 || hi[j] > n0 || lo[j] > hi[j])
+      return fail(c, CWTB_ERR_ARG, "count_hist: column range outside [0, n0) or lo > hi");
+    span = std::max(span, (long long)(hi[j] - lo[j]));
+  }
+  // aux: [lo S][hi S][hist nbins], 8 bytes each
+  int e = ensure(c, c->aux, (2 * (size_t)S + (size_t)nbins) * sizeof(long long));
+  if (e) return e;
+  long long *dlo = (long long *)c->aux.p, *dhi = dlo + S;
+  unsigned long long *dh = (unsigned long long *)(dhi + S);
+  RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
+  RT(rt_memset(dh, 0, (size_t)nbins * sizeof(long long), c->stream));
+  CountHistArgs a{(const double *)f.p, f.cnt, dlo, dhi, dh, n0, nbins};
+  using Sh = CountHistBody<true>;
+  const unsigned gx = (unsigned)((span + Sh::CHUNK - 1) / Sh::CHUNK);
+  e = nbins <= Sh::SMEM_BINS ? launch<Sh>(c, gx, (unsigned)S, a) : launch<CountHistBody<false>>(c, gx, (unsigned)S, a);
+  if (e) return e;
+  RT(rt_d2h(out, dh, (size_t)nbins * sizeof(long long), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
 }
 }  // extern "C++"
 
@@ -2998,6 +3068,56 @@ int cwtb_coherence3_scale_avg(cwtb_ctx *c, int measure, const double *weights, d
   return e ? e : scale_avg_run(c, f, weights, out);
 }
 
+// ---- point-wise tests against surrogates: reading the counts ----------------------------------
+int cwtb_coherence_pvalue_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                                 int64_t col_step, double *p_out) {
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  if (!p_out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, p_out, nullptr);
+}
+
+int cwtb_coherence_pvalue_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, const double *thr,
+                                    int64_t kmax, int want_phase, double *out) {
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  if (e || (e = count_ref(c, kmax, f))) return e;
+  return row_stats_run(c, f, lo, hi, thr, want_phase != 0, out);
+}
+
+int cwtb_coherence_count_hist(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, int64_t nbins, int64_t *out) {
+  FieldRef f;
+  int e = field_ref(c, FIELD_COH, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  return count_hist_run(c, f, lo, hi, nbins, out);
+}
+
+int cwtb_coherence3_pvalue_window(cwtb_ctx *c, int measure, int row0, int nrows, int row_step, int64_t col0,
+                                  int64_t ncols, int64_t col_step, double *p_out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, false, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  if (!p_out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, p_out, nullptr);
+}
+
+int cwtb_coherence3_pvalue_row_stats(cwtb_ctx *c, int measure, const int64_t *lo, const int64_t *hi,
+                                     const double *thr, int64_t kmax, int want_phase, double *out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, want_phase != 0, f);
+  if (e || (e = count_ref(c, kmax, f))) return e;
+  return row_stats_run(c, f, lo, hi, thr, want_phase != 0, out);
+}
+
+int cwtb_coherence3_count_hist(cwtb_ctx *c, int measure, const int64_t *lo, const int64_t *hi, int64_t nbins,
+                               int64_t *out) {
+  FieldRef f;
+  int e = coh3_ref(c, measure, false, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  return count_hist_run(c, f, lo, hi, nbins, out);
+}
+
 int cwtb_resident_shape(cwtb_ctx *c, int product, int *rows, int64_t *n0, int *precision) {
   if (!c) return CWTB_ERR_ARG;
   const ResidentSlot *s = product == CWTB_PRODUCT_W           ? &c->wt
@@ -3090,6 +3210,10 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
 // the data whose spectra are in c->pspec, drawn on the device from (seed, unit0 + i); or neither ->
 // white noise drawn on the device from (seed, unit0 + i); coherence in the engine type T
 struct PhaseSrc { int group[3]; };
+// the exceedance counters of a counting run (cwtb_coherence*_surrogate_counts) and the observed
+// fields they compare against, per measure: the coherence in [0]; the partial and the multiple
+// coherence in [0] and [1] (either counter may be null)
+struct CountDst { const double *obs[2]; unsigned *cnt[2]; };
 
 extern "C++" {
 // nb surrogate units of the data spectra c->pspec [nser][n0] into out [nb][nser][n0]: rotation,
@@ -3117,7 +3241,7 @@ template <typename T>
 static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed, long long unit0,
                   int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                   double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
-                  int64_t *const hist[2]) {
+                  int64_t *const hist[2], const CountDst *cd = nullptr) {
   int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
   if (e) return e;
   if ((e = upload_window(c, boxcar_len))) return e;
@@ -3168,9 +3292,15 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
         a = (const T *)c->noise.p + (size_t)i * usz;
       }
       const unsigned char *dmask = (const unsigned char *)c->mask.p;
-      e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0])
+      // The counters are read and written without atomics by the final kernel of every unit.  That
+      // kernel runs on c->stream (run_job forks its transforms onto other streams but joins them
+      // back and leaves c->cur = c->stream; the smoothing and final launches follow on it), so the
+      // final launches of successive units and batches are ordered and never overlap.
+      const CountDst k = cd ? *cd : CountDst{};
+      e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0],
+                                  k.obs[0], k.cnt[0])
                     : wct3_core<T>(c, c->job, a, a + n0, a + 2 * n0, boxcar_len, nullptr, nullptr, dmask, maxscale,
-                                   nbins, dh[0], dh[1]);
+                                   nbins, dh[0], dh[1], nullptr, k.obs[0], k.obs[1], k.cnt[0], k.cnt[1]);
       if (e) return e;
     }
   }
@@ -3190,7 +3320,7 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
 static int mc_core(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed,
                    long long unit0, int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                    double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
-                   int64_t *const hist[2]) {
+                   int64_t *const hist[2], const CountDst *cd = nullptr) {
   if (!c || !mask || !(hist[0] || hist[1]) || n_units < 0 || nbins < 1 || maxscale < 0 || maxscale > n_scales)
     return fail(c, CWTB_ERR_ARG, nser == 2 ? "wct_mc: bad argument" : "wct3_mc: bad argument");
   if (family == CWTB_TABLE)
@@ -3198,9 +3328,9 @@ static int mc_core(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *p
                                                    : "wct3_mc needs an analytic wavelet family");
   return c->coh_precision == CWTB_F32
              ? mc_run<float>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
-                             boxcar_len, mask, maxscale, nbins, hist)
+                             boxcar_len, mask, maxscale, nbins, hist, cd)
              : mc_run<double>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
-                              boxcar_len, mask, maxscale, nbins, hist);
+                              boxcar_len, mask, maxscale, nbins, hist, cd);
 }
 
 int cwtb_wct_mc(cwtb_ctx *c, const double *noise, int n_pairs, int64_t n0, double dt, double dj,
@@ -3329,6 +3459,60 @@ int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const 
   RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;
+}
+
+// ---- point-wise tests against surrogates: counting -------------------------------------------
+// The units' exceedance counts of the resident coherence (nser 2) or partial and multiple
+// coherence (nser 3) added to the slot's counters, with the histograms of cwtb_wct_mc_phase
+static int surrogate_counts(cwtb_ctx *c, int nser, const double *series, const int *group, uint64_t seed,
+                            int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                            int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                            int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b, int64_t serial, int reset) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = nser == 2 ? "coherence_surrogate_counts" : "coherence3_surrogate_counts";
+  ResidentSlot &s = nser == 2 ? c->coh : c->coh3;
+  if (s.S <= 0 || !s.buf.p || serial != s.serial)
+    return fail(c, CWTB_ERR_STATE, nm + ": the serial is not that of the resident product");
+  if (n_scales != s.S || n0 != s.n0)
+    return fail(c, CWTB_ERR_STATE, nm + ": scales or length differ from the resident product's");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, nm + " needs an analytic wavelet family");
+  if (!mask || !(hist_a || hist_b)) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  const long long base = reset || s.units < 0 ? 0 : s.units;
+  if (n_units < 0 || n_units > 0xFFFFFFFFll - base)
+    return fail(c, CWTB_ERR_ARG, nm + ": more units than a 32-bit counter holds");
+  PhaseSrc ph{};
+  int e = phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &ph);
+  if (e) return e;
+  const size_t cnt = (size_t)s.S * s.n0, off = coh_angle_offset(cnt);
+  if ((e = ensure(c, s.counts, (nser == 2 ? cnt : off + cnt) * sizeof(unsigned)))) return e;
+  s.units = -1;   // nothing readable until this call completes
+  if (base == 0) RT(rt_memset(s.counts.p, 0, s.counts.bytes, c->stream));
+  const double *obs = (const double *)s.buf.p;   // WCT; RP2 at 0 and RM2 at 2 off
+  unsigned *k = (unsigned *)s.counts.p;           // one field; RP2's at 0 and RM2's at off
+  const CountDst cd = nser == 2 ? CountDst{{obs, nullptr}, {k, nullptr}} : CountDst{{obs, obs + 2 * off}, {k, k + off}};
+  int64_t *const h[2] = {hist_a, hist_b};
+  if ((e = mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                   boxcar_len, mask, maxscale, nbins, h, &cd)))
+    return e;
+  s.units = base + n_units;
+  return 0;
+}
+
+int cwtb_coherence_surrogate_counts(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
+                                    int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                    int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                    int maxscale, int nbins, int64_t *hist, int64_t serial, int reset) {
+  return surrogate_counts(c, 2, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                          boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, reset);
+}
+
+int cwtb_coherence3_surrogate_counts(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
+                                     int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                     int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                     int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
+                                     int64_t serial, int reset) {
+  return surrogate_counts(c, 3, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                          boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial, reset);
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

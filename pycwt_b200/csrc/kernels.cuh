@@ -1751,6 +1751,9 @@ template <typename T> struct BoxcarBody {
 // ---- Body: coherence  WCT = |S12|^2 / (S1 S2)  after the scale boxcar; optional histogram
 // of floor(WCT * nbins) over masked points (wavelet.py:513, 624-630) ---------------------
 // Fields, staging and sums in the engine type T; WCT is written (and binned) as double.
+// Counting (cnt given, Monte-Carlo mode): every row is finished, not only those below maxscale,
+// and each point's counter goes up by one where the surrogate's value reaches the observed one
+// (count_exceed).  The histogram is binned as without counting.
 template <typename T> struct WctFinalArgs {
   const cx<T> *C, *A12;     // time-smoothed fields
   const double *win;
@@ -1759,7 +1762,15 @@ template <typename T> struct WctFinalArgs {
   unsigned long long *hist;    // [rows][nbins], may be null
   long long n;
   int rows, K, maxscale, nbins;
+  const double *obs;        // observed WCT [rows][n] (the resident coherence), with cnt
+  unsigned *cnt;            // exceedance counters [rows][n], or null
 };
+// One surrogate value r2 against the observed value at point o: an exceedance where r2 >= obs or
+// r2 is not finite (the conservative choice).  No atomics: within a launch every point belongs to
+// one thread, and the final launches of successive surrogate units run in order on one stream.
+HD void count_exceed(unsigned *cnt, const double *obs, size_t o, double r2) {
+  if (!isfinite(r2) || r2 >= obs[o]) cnt[o] += 1u;
+}
 // Tile: RS = 32 output rows x CW = 32 columns.  Phase 0 stages the RS + K - 1 input rows of both
 // time-smoothed fields for these columns in shared memory (each input element is read from global
 // memory (RS + K - 1) / RS times instead of K times); in phase 1 a thread produces 4 consecutive
@@ -1778,7 +1789,8 @@ template <typename T, int KMAX_> struct WctFinalBody {
     T *sw = (T *)(sx + (size_t)(RS + KMAX - 1) * CW);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    const int rows_out = a.WCT ? a.rows : a.maxscale;  // Monte-Carlo mode: rows below maxscale only
+    // Monte-Carlo mode without counting: rows below maxscale only
+    const int rows_out = a.WCT || a.cnt ? a.rows : a.maxscale;
     if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
@@ -1822,6 +1834,7 @@ template <typename T, int KMAX_> struct WctFinalBody {
           const double r2 = (double)((xr[e] * xr[e] + xi[e] * xi[e]) / (cr[e] * ci[e]));
           const size_t o = (size_t)i * a.n + n;
           if (a.WCT) a.WCT[o] = r2;
+          if (a.cnt) count_exceed(a.cnt, a.obs, o, r2);
           if (a.hist && i < a.maxscale && a.mask[o] && r2 == r2) {
             int bin = (int)floor(r2 * a.nbins);
             bin = bin < 0 ? 0 : (bin >= a.nbins ? a.nbins - 1 : bin);
@@ -1883,7 +1896,8 @@ template <typename T> struct Wct3PrepBody {
 // Monte-Carlo mode (RP2, RM2 and PP all null): only the rows below maxscale and only the measures
 // whose histogram is given; a measure's histogram counts floor(R2 nbins), clamped to
 // [0, nbins - 1], over the points with mask != 0.  A non-finite R2 (a zero denominator) is not
-// counted.
+// counted.  Counting (cntP or cntM given, Monte-Carlo mode): every row is finished, and each
+// measure with counters counts its exceedances of the observed field (count_exceed).
 template <typename T> struct Wct3FinalArgs {
   const cx<T> *A, *B, *Xy1, *Xy2, *X12;   // time-smoothed fields
   const double *win;
@@ -1892,6 +1906,8 @@ template <typename T> struct Wct3FinalArgs {
   unsigned long long *histP, *histM;     // [rows][nbins], either may be null
   long long n;
   int rows, K, maxscale, nbins;
+  const double *obsP, *obsM;             // observed RP2 / RM2 [rows][n], with the counters
+  unsigned *cntP, *cntM;                 // exceedance counters [rows][n], either may be null
 };
 // one count for R2 in its row's histogram; non-finite R2 is skipped before any conversion to int
 HD void hist_count(unsigned long long *hist, int row, int nbins, double r2) {
@@ -1919,7 +1935,7 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
     double *sw = (double *)(st + NF * PLANE);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    const int rows_out = a.RP2 || a.RM2 || a.PP ? a.rows : a.maxscale;
+    const int rows_out = a.RP2 || a.RM2 || a.PP || a.cntP || a.cntM ? a.rows : a.maxscale;
     if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
@@ -1981,20 +1997,22 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
         const double d12 = S1 * S2 - (S12.x * S12.x + S12.y * S12.y);
         const size_t o = (size_t)i * a.n + n;
         const bool binned = (a.histP || a.histM) && i < a.maxscale && a.mask[o];
-        if (a.RP2 || a.PP || (a.histP && binned)) {
+        if (a.RP2 || a.PP || (a.histP && binned) || a.cntP) {
           const double2 u = csub(cscale(Sy1, S2), cmul(Sy2, cconj(S12)));
-          if (a.RP2 || (a.histP && binned)) {
+          if (a.RP2 || (a.histP && binned) || a.cntP) {
             const double rp = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
             if (a.RP2) a.RP2[o] = rp;
             if (a.histP && binned) hist_count(a.histP, i, a.nbins, rp);
+            if (a.cntP) count_exceed(a.cntP, a.obsP, o, rp);
           }
           if (a.PP) a.PP[o] = u.x == 0.0 && u.y == 0.0 ? 0.0 : atan2(u.y, u.x);
         }
-        if (a.RM2 || (a.histM && binned)) {
+        if (a.RM2 || (a.histM && binned) || a.cntM) {
           const double2 z = cmul(cmul(Sy1, S12), cconj(Sy2));
           const double rm = (S2 * ny1 + S1 * ny2 - 2.0 * z.x) / (Sy * d12);
           if (a.RM2) a.RM2[o] = rm;
           if (a.histM && binned) hist_count(a.histM, i, a.nbins, rm);
+          if (a.cntM) count_exceed(a.cntM, a.obsM, o, rm);
         }
       }
     }
@@ -2184,6 +2202,48 @@ template <bool PHASE> struct CohViewT {
 };
 using CohView = CohViewT<true>;
 using CohMagView = CohViewT<false>;
+
+// The same double fields with their surrogate exceedance counts k (uint32 [rows][n], the same flat
+// index; cwtb_coherence*_surrogate_counts) from M units.  Row stats: CohViewT's four sums over the
+// points whose value is finite, whose k <= kmax and, with a threshold, whose value > thr_j.
+// Window: the p-value (1 + k) / (1 + M) to o0, NaN where the value is not finite.
+template <bool PHASE> struct CohCountViewT {
+  const double *WCT, *aWCT;   // aWCT: unused (may be null) without PHASE
+  const unsigned *cnt;
+  long long kmax, m;          // m: the units M the counts hold
+  int want_phase;
+  static constexpr int K = 4, E = 2, VPT = 16;
+  struct Vec { double2 w, g; uint2 k; };
+  HD Vec load(size_t q) const {
+    Vec v{ld_stream((const double2 *)WCT + q), make_double2(0, 0), ld_stream((const uint2 *)cnt + q)};
+    if constexpr (PHASE) {
+      if (want_phase) v.g = ld_stream((const double2 *)aWCT + q);
+    }
+    return v;
+  }
+  HD void add1(double (&s)[K], double w, double ang, unsigned k, bool has_thr, double t) const {
+    if (!isfinite(w) || (long long)k > kmax) return;
+    if (has_thr && !(w > t)) return;
+    s[0] += 1.0;
+    s[1] += w;
+    if (PHASE && want_phase) {
+      double sn, cs;
+      sincos_hd(ang, &sn, &cs);
+      s[2] += cs;
+      s[3] += sn;
+    }
+  }
+  HD void add(double (&s)[K], const Vec &v, int e, bool has_thr, double t) const {
+    add1(s, e ? v.w.y : v.w.x, e ? v.g.y : v.g.x, e ? v.k.y : v.k.x, has_thr, t);
+  }
+  HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
+    add1(s, WCT[p], PHASE && want_phase ? aWCT[p] : 0.0, cnt[p], has_thr, t);
+  }
+  HD void copy(size_t src, double *o0, double *, size_t dst) const {
+    const double w = WCT[src];
+    o0[dst] = isfinite(w) ? (double)(1 + (long long)cnt[src]) / (double)(1 + m) : w - w;   // inf - inf: NaN
+  }
+};
 
 // 16 bytes of a complex field: one double2, or two float2
 template <typename T> struct CxVec16;
@@ -2389,6 +2449,57 @@ template <typename View> struct WindowBody {
     if (c >= a.ncols) return;
     const size_t src = (size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + c * a.col_step;
     a.f.copy(src, a.o0, a.o1, (size_t)by * a.ncols + c);
+  }
+};
+
+// ---- Body: histogram of the exceedance counts k in [0, nb) over the columns [lo_j, hi_j) of every
+// row, of the points whose observed value is finite (cwtb_coherence*_count_hist) -------------------
+// CTA (bx, j) covers the chunk [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j.  SHARED: the CTA
+// counts into a uint32 histogram in shared memory (nb <= SMEM_BINS) and adds its non-zero bins to
+// the 64-bit global histogram at the end; otherwise every point is one 64-bit atomic in global
+// memory.  Integer sums: the result does not depend on the order, repeated calls are bit-identical.
+struct CountHistArgs {
+  const double *obs;
+  const unsigned *cnt;
+  const long long *lo, *hi;   // per row
+  unsigned long long *hist;   // [nb], zeroed by the caller
+  long long n, nb;
+};
+template <bool SHARED> struct CountHistBody {
+  using Args = CountHistArgs;
+  static constexpr int NPHASE = SHARED ? 3 : 1;
+  static constexpr int SMEM_BINS = 12288;                  // 48 KiB: four CTAs per SM
+  static constexpr long long CHUNK = 32LL * NT;
+  static constexpr size_t SMEM = SHARED ? SMEM_BINS * sizeof(unsigned) : 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    unsigned *sh = (unsigned *)smraw;
+    if constexpr (SHARED && PH == 0) {
+      for (long long b = tid; b < a.nb; b += NT) sh[b] = 0u;
+    } else if constexpr (PH == (SHARED ? 1 : 0)) {
+      const long long c0 = a.lo[by] + (long long)bx * CHUNK;
+      const long long c1 = c0 + CHUNK < a.hi[by] ? c0 + CHUNK : a.hi[by];
+      for (long long n = c0 + tid; n < c1; n += NT) {
+        const size_t o = (size_t)by * a.n + n;
+        if (!isfinite(ld_stream(&a.obs[o]))) continue;
+        const unsigned k = ld_stream(&a.cnt[o]);
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+        if constexpr (SHARED) atomicAdd(&sh[k], 1u);
+        else atomicAdd(&a.hist[k], 1ull);
+#else
+        if constexpr (SHARED) sh[k] += 1u;
+        else a.hist[k] += 1ull;
+#endif
+      }
+    } else {
+      for (long long b = tid; b < a.nb; b += NT)
+        if (sh[b]) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+          atomicAdd(&a.hist[b], (unsigned long long)sh[b]);
+#else
+          a.hist[b] += sh[b];
+#endif
+        }
+    }
   }
 };
 

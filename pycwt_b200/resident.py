@@ -23,14 +23,17 @@ import collections
 import numpy as np
 
 from . import _engine
+from . import helpers as _helpers
 from .helpers import ar1, fft, fft_kwargs
-from .wavelet import (_check_parameter_wavelet, _coi, _nan_rows, _precision, _resolve_scales,
+from .wavelet import (_check_parameter_wavelet, _coi, _mc_levels, _nan_rows, _precision,
+                      _resolve_scales, _surrogate_histogram, _surrogate_problem, _surrogate_seed,
                       _sync_padding, _wct_on_device, _wct_problem, _wct_significance,
                       _xwt_on_device, _xwt_problem, _xwt_signif, wct3_significance,
-                      wct3_surrogate_significance)
+                      wct3_surrogate_significance, wct_surrogate_significance)
 
 __all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence',
-           'xwt_resident', 'ResidentCrossWavelet', 'wct3_resident', 'ResidentCoherence3']
+           'xwt_resident', 'ResidentCrossWavelet', 'wct3_resident', 'ResidentCoherence3',
+           'FdrResult']
 
 
 def _coi_ranges(wavelet, dt, n0, period):
@@ -330,21 +333,139 @@ def _ratio(num, den):
         return np.where(den > 0, num / np.where(den > 0, den, 1.0), np.nan)
 
 
-class ResidentCoherence(_ResidentSlot):
-    """WCT and aWCT [S, n0] of one `wct_resident` call, resident on the device."""
+# ---- point-wise tests against phase-randomised surrogates --------------------------------------
+# `surrogate_test` runs the M surrogate units 0 .. M - 1 of `wct_surrogate_significance` /
+# `wct3_surrogate_significance` (same seed, same units) and, in the same device run, counts per
+# point k[s, n] = #{i : R2_i[s, n] >= R2_obs[s, n]} (a non-finite R2_i counts) into counters that
+# live with the resident product.  p = (1 + k) / (1 + M); NaN where R2_obs is not finite.
+
+FdrResult = collections.namedtuple('FdrResult', 'alpha rejected tested')
+
+_MAX_UNITS = 2 ** 31 - 1    # units of one counting call (a C int); the counters are uint32
+
+
+def _kmax(alpha, M):
+    """The largest k with (1 + k) / (1 + M) <= alpha (-1: none), evaluated in double."""
+    if isinstance(alpha, bool) or not np.isscalar(alpha) or not 0 < alpha <= 1:
+        raise ValueError("alpha must lie in (0, 1], got %r" % (alpha,))
+    k = min(M, max(-1, int(np.floor(alpha * (1 + M))) - 1))
+    while k < M and (1 + (k + 1)) / (1 + M) <= alpha:
+        k += 1
+    while k >= 0 and (1 + k) / (1 + M) > alpha:
+        k -= 1
+    return k
+
+
+def _fdr(hist, M, q, method):
+    """Benjamini-Hochberg / -Yekutieli step-up test of the p-values (1 + k) / (1 + M) from their
+    histogram over k.  At the value of k the rank is the cumulative count H(k) (ties), and the
+    adjusted p-values are formed as scipy.stats.false_discovery_control forms them."""
+    m = int(hist.sum())
+    if m == 0:
+        return FdrResult(0.0, 0, 0)
+    k = np.flatnonzero(hist)
+    rank = np.cumsum(hist)[k].astype(float)
+    p = (1 + k) / (1 + M)
+    adj = p * (m / rank)
+    if method == 'by':
+        adj = adj * np.sum(1 / np.arange(1, m + 1, dtype=float))
+    ok = np.flatnonzero(adj <= q)
+    if ok.size == 0:
+        return FdrResult(0.0, 0, m)
+    top = ok[-1]
+    return FdrResult(float(p[top]), int(rank[top]), m)
+
+
+class _SurrogateTest(object):
+    """The point-wise test of a resident coherence product: the counts of its last
+    `surrogate_test` and what is read from them.  A subclass names its measures (`_MEASURE_OF`:
+    None for the coherence)."""
+
+    _UNTESTED = ("no surrogate test has counted for this product: call surrogate_test first")
+    surrogate_seed = None     # seed and M of the last surrogate_test
+    surrogate_units = None
+
+    def _count(self, mc_count, seed, groups):
+        """(prob, hist) of a counting run of units 0 .. mc_count - 1 (the caller holds the lock)."""
+        if isinstance(mc_count, bool) or not isinstance(mc_count, (int, np.integer)) \
+                or not 1 <= mc_count <= _MAX_UNITS:
+            raise ValueError("mc_count must be an integer in [1, %d], got %r" % (_MAX_UNITS, mc_count))
+        if bool(_helpers._FFT_NEXT_POW2) != self._padding:
+            raise ValueError("the FFT padding mode has changed since this product was computed: its "
+                             "counts would not compare like with like")
+        seed = _surrogate_seed(seed)
+        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
+                                     self.normalize, self.precision)
+        self.surrogate_seed = self.surrogate_units = None
+        hist = _surrogate_histogram(p, prob, groups, seed, 0, int(mc_count), engine=self.engine,
+                                    serial=self._serial)
+        self.surrogate_seed, self.surrogate_units = seed, int(mc_count)
+        return prob, hist
+
+    def _units(self):
+        if self.surrogate_units is None:
+            raise _engine.EngineError(self._UNTESTED)
+        return self.surrogate_units
+
+    def _pvalues(self, measure, rows, cols):
+        self._units()
+        S, n0 = self.shape
+        r0, nr, rs = _slice_range(rows, S, 'rows')
+        c0, nc, cs = _slice_range(cols, n0, 'cols')
+        if nr == 0 or nc == 0:
+            return np.empty((nr, nc))
+        return self.engine.pvalue_window(measure, r0, nr, rs, c0, nc, cs)
+
+    def _cut_stats(self, measure, lo, hi, thr, alpha, want_phase=False):
+        """Row stats over the points with p <= alpha (and R > thr where given)."""
+        kmax = _kmax(alpha, self._units())
+        return self.engine.pvalue_row_stats(measure, lo, hi, kmax, thr, want_phase)
+
+    def _pvalue_fraction(self, measure, alpha):
+        M = self._units()
+        lo, hi = self.coi_ranges()
+        sel = self.engine.pvalue_row_stats(measure, lo, hi, _kmax(alpha, M))[:, 0]
+        tested = self.engine.pvalue_row_stats(measure, lo, hi, M)[:, 0]
+        return _ratio(sel, tested)
+
+    def _fdr_threshold(self, measure, q, method, inside_coi):
+        if isinstance(q, bool) or not np.isscalar(q) or not 0 < q < 1:
+            raise ValueError("q must lie in (0, 1), got %r" % (q,))
+        if method not in ('bh', 'by'):
+            raise ValueError("method must be 'bh' or 'by', got %r" % (method,))
+        M = self._units()
+        lo, hi = _column_ranges(self, inside_coi)
+        return _fdr(self.engine.count_hist(measure, lo, hi, M + 1), M, q, method)
+
+
+class ResidentCoherence(_SurrogateTest, _ResidentSlot):
+    """WCT and aWCT [S, n0] of one `wct_resident` call, resident on the device.
+
+    Point-wise test: `surrogate_test(mc_count=M, seed=seed)` runs the surrogate pairs 0 .. M - 1 of
+    `wct_surrogate_significance(..., mc_count=M, seed=seed)` and counts, per point, the pairs whose
+    coherence reaches the observed one, k[s, n] = #{i : WCT_i[s, n] >= WCT[s, n]} (a non-finite
+    WCT_i counts: the conservative choice), on every row and column, the cone of influence included
+    (the surrogates have the data's length and the same edge effects).  p = (1 + k) / (1 + M)
+    (Davison & Hinkley 1997; North et al. 2002), so the smallest p is 1 / (M + 1); NaN where WCT is
+    not finite, and such points are left out of every fraction and count.  A selection p <= alpha is
+    the integer cut k <= kmax, kmax the largest k with (1 + k) / (1 + M) <= alpha in double.  The
+    counts take 4 bytes per scale-point on the device and live until the next `surrogate_test`,
+    `release()` or `wct_resident` on the same engine."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence_serial', 'coherence_release'
     _GONE = ("this coherence is no longer resident: it was released or another wct_resident has "
              "run on the same engine")
 
-    def __init__(self, engine, problem, precision, serial):
+    def __init__(self, engine, problem, normalize, precision, serial):
         p = problem
         super(ResidentCoherence, self).__init__(engine, p.wavelet, p.n0, p.dt, p.dj, p.sj,
                                                 precision, serial)
         self.s0 = p.s0
         self.J = p.J
         self.freq = p.freq
-        self._y = tuple(np.array(y, copy=True) for y in p.ys)   # raw series, for ar1
+        self.normalize = normalize
+        self._y = tuple(np.array(y, copy=True) for y in p.ys)   # raw series, for ar1 and surrogates
+        self._padding = bool(_helpers._FFT_NEXT_POW2)
 
     def _threshold(self, sig95):
         if sig95 is None:
@@ -393,12 +514,16 @@ class ResidentCoherence(_ResidentSlot):
                                  precision=self.precision)
 
     @_live
-    def global_coherence(self, inside_coi=False, sig95=None):
+    def global_coherence(self, inside_coi=False, sig95=None, alpha=None):
         """Mean WCT per scale over the selected points: inside the cone of influence
         (period_j <= coi[n]) if `inside_coi`, where WCT[j, n] > sig95[j] if `sig95` is given
-        (false where sig95[j] is NaN).  NaN for a scale without points."""
+        (false where sig95[j] is NaN), where the p-value of the last `surrogate_test` is <= alpha if
+        `alpha` is given (both: logical AND).  NaN for a scale without points."""
         lo, hi = _column_ranges(self, inside_coi)
-        st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95))
+        if alpha is not None:
+            st = self._cut_stats(None, lo, hi, self._threshold(sig95), alpha)
+        else:
+            st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95))
         return _ratio(st[:, 1], st[:, 0])
 
     @_live
@@ -411,16 +536,20 @@ class ResidentCoherence(_ResidentSlot):
 
     @_live
     def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, sig95=None,
-                   per_scale=False):
+                   per_scale=False, alpha=None):
         """Circular mean of aWCT over the points of the scales with period_min <= period <
-        period_max, inside the cone of influence if `inside_coi`, where WCT > sig95 if given
-        (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
-        |sum e^{i aWCT}| / count, count), for the whole band or, with `per_scale`, per scale
-        (arrays; NaN angle and strength where the count is 0)."""
+        period_max, inside the cone of influence if `inside_coi`, where WCT > sig95 if given and
+        where the p-value of the last `surrogate_test` is <= alpha if given (Grinsted et al. 2004):
+        MeanPhase(angle = atan2(sum sin, sum cos), strength = |sum e^{i aWCT}| / count, count), for
+        the whole band or, with `per_scale`, per scale (arrays; NaN angle and strength where the
+        count is 0)."""
         sel = self._band(period_min, period_max)
         lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
-        st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95), want_phase=True)
+        if alpha is not None:
+            st = self._cut_stats(None, lo, hi, self._threshold(sig95), alpha, want_phase=True)
+        else:
+            st = self.engine.coherence_row_stats(lo, hi, self._threshold(sig95), want_phase=True)
         return _mean_phase(st[:, 0], st[:, 2], st[:, 3], per_scale)
 
     @_live
@@ -433,6 +562,52 @@ class ResidentCoherence(_ResidentSlot):
         out = self.engine.coherence_scale_avg(sel.astype(float))
         return out[0] / float(sel.sum()), np.arctan2(out[2], out[1])
 
+    @_live
+    def surrogate_significance(self, significance_level=0.95, mc_count=300, seed=None):
+        """`wct_surrogate_significance` on this handle's series and arguments.  The coherence stays
+        resident."""
+        return wct_surrogate_significance(*self._y, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
+                                          significance_level=significance_level,
+                                          wavelet=self.wavelet, normalize=self.normalize,
+                                          mc_count=mc_count, seed=seed, precision=self.precision)
+
+    @_live
+    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95):
+        """Run the surrogate pairs 0 .. mc_count - 1 once: count per point the pairs whose coherence
+        reaches this one (kept on the device, replacing the counts of an earlier test) and return
+        the per-scale levels, bit-identical to `surrogate_significance` with the same `seed` and
+        `mc_count`.  `seed=None` draws the seed from numpy's global RNG; the seed and M are kept as
+        `surrogate_seed` and `surrogate_units`.  ValueError for mc_count outside [1, 2^31 - 1] or
+        when the FFT padding mode differs from the one this coherence was computed with."""
+        prob, hist = self._count(mc_count, seed, (0, 1))
+        return _mc_levels(prob, hist[0], significance_level)
+
+    @_live
+    def pvalues(self, rows=slice(None), cols=slice(None)):
+        """p[rows, cols] = (1 + k) / (1 + M) (float64) of the last `surrogate_test`, with the slicing
+        of `window`; NaN where WCT is not finite."""
+        return self._pvalues(None, rows, cols)
+
+    @_live
+    def pvalue_fraction(self, alpha):
+        """Per scale, the fraction of the points inside the cone of influence (with a finite p) whose
+        p <= alpha; NaN for a scale without such points."""
+        return self._pvalue_fraction(None, alpha)
+
+    @_live
+    def fdr_threshold(self, q=0.05, method='bh', inside_coi=True):
+        """False-discovery-rate control of the p-values of the last `surrogate_test`, over the points
+        with a finite p inside the cone of influence (every such point with `inside_coi=False`):
+        Benjamini & Hochberg (1995), `method='bh'`, or Benjamini & Yekutieli (2001), `'by'`.
+        Returns FdrResult(alpha, rejected, tested): the largest p-value the step-up procedure rejects
+        (0.0 if none; select with `pvalues() <= alpha`), the points rejected and the points tested.
+        p takes only the values (1 + k) / (1 + M), so the procedure is decided exactly from a
+        histogram of k (tied p-values take the rank of the last of them) and equals
+        scipy.stats.false_discovery_control on the same p-values.  The points of a map are strongly
+        dependent: BH controls the FDR under positive regression dependence (Benjamini &
+        Yekutieli 2001), BY under any dependence, at the price of power."""
+        return self._fdr_threshold(None, q, method, inside_coi)
+
 
 def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
                  precision='fp64', engine=None):
@@ -444,7 +619,7 @@ def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=T
     p = _wct_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
     eng = engine or _engine.default_engine()
     serial = _wct_on_device(eng, p, eng.wct_resident)
-    return ResidentCoherence(eng, p, precision, serial)
+    return ResidentCoherence(eng, p, normalize, precision, serial)
 
 
 # ---- resident cross spectrum -------------------------------------------------------------------
@@ -557,7 +732,7 @@ def xwt_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95, wave
 _MEASURES = {'partial': _engine.MEASURE_PARTIAL, 'multiple': _engine.MEASURE_MULTIPLE}
 
 
-class ResidentCoherence3(_ResidentSlot):
+class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
     """RP2, the partial phase and RM2 [S, n0] of one `wct3_resident` call, resident on the device.
 
     The partial phase is the angle of the smoothed partial cross spectrum of y and x1 with x2
@@ -569,7 +744,11 @@ class ResidentCoherence3(_ResidentSlot):
 
     `measure` arguments are 'partial' (RP2) or 'multiple' (RM2).  `sig` arguments take one entry
     per scale in the units of the measure (as `wct3_significance` returns them); a point is
-    selected where R > sig[j], and a NaN entry selects no point of its scale."""
+    selected where R > sig[j], and a NaN entry selects no point of its scale.
+
+    Point-wise test: `surrogate_test` counts, per point and measure, the surrogate triples of
+    `wct3_surrogate_significance` that reach the observed RP2 / RM2, with the definitions of
+    `ResidentCoherence` (8 bytes per scale-point on the device for the two measures)."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence3_serial', 'coherence3_release'
     _GONE = ("this partial / multiple coherence is no longer resident: it was released or another "
@@ -584,6 +763,7 @@ class ResidentCoherence3(_ResidentSlot):
         self.freq = p.freq
         self.normalize = normalize
         self._y = tuple(np.array(y, copy=True) for y in p.ys)   # raw series, for ar1 and surrogates
+        self._padding = bool(_helpers._FFT_NEXT_POW2)
 
     def _measure(self, measure):
         try:
@@ -635,13 +815,17 @@ class ResidentCoherence3(_ResidentSlot):
         return rp, ph, rm
 
     @_live
-    def global_coherence(self, measure='partial', inside_coi=False, sig=None):
+    def global_coherence(self, measure='partial', inside_coi=False, sig=None, alpha=None):
         """Mean of the measure per scale over the selected points: inside the cone of influence
-        (period_j <= coi[n]) if `inside_coi`, where R[j, n] > sig[j] if `sig` is given.  NaN for a
+        (period_j <= coi[n]) if `inside_coi`, where R[j, n] > sig[j] if `sig` is given, where the
+        measure's p-value of the last `surrogate_test` is <= alpha if `alpha` is given.  NaN for a
         scale without points."""
         m = self._measure(measure)
         lo, hi = _column_ranges(self, inside_coi)
-        st = self.engine.coherence3_row_stats(m, lo, hi, self._threshold(sig))
+        if alpha is not None:
+            st = self._cut_stats(m, lo, hi, self._threshold(sig), alpha)
+        else:
+            st = self.engine.coherence3_row_stats(m, lo, hi, self._threshold(sig))
         return _ratio(st[:, 1], st[:, 0])
 
     @_live
@@ -655,17 +839,21 @@ class ResidentCoherence3(_ResidentSlot):
 
     @_live
     def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, sig=None,
-                   per_scale=False):
+                   per_scale=False, alpha=None):
         """Circular mean of the partial phase over the points of the scales with period_min <=
-        period < period_max, inside the cone of influence if `inside_coi`, where RP2 > sig if given:
-        MeanPhase(angle = atan2(sum sin, sum cos), strength = |sum e^{i phase}| / count, count), for
-        the whole band or, with `per_scale`, per scale (NaN angle and strength where the count
-        is 0)."""
+        period < period_max, inside the cone of influence if `inside_coi`, where RP2 > sig if given
+        and where RP2's p-value of the last `surrogate_test` is <= alpha if given: MeanPhase(angle =
+        atan2(sum sin, sum cos), strength = |sum e^{i phase}| / count, count), for the whole band
+        or, with `per_scale`, per scale (NaN angle and strength where the count is 0)."""
         sel = self._band(period_min, period_max)
         lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
-        st = self.engine.coherence3_row_stats(_engine.MEASURE_PARTIAL, lo, hi, self._threshold(sig),
-                                              want_phase=True)
+        if alpha is not None:
+            st = self._cut_stats(_engine.MEASURE_PARTIAL, lo, hi, self._threshold(sig), alpha,
+                                 want_phase=True)
+        else:
+            st = self.engine.coherence3_row_stats(_engine.MEASURE_PARTIAL, lo, hi,
+                                                  self._threshold(sig), want_phase=True)
         return _mean_phase(st[:, 0], st[:, 2], st[:, 3], per_scale)
 
     @_live
@@ -703,6 +891,33 @@ class ResidentCoherence3(_ResidentSlot):
                                            wavelet=self.wavelet, normalize=self.normalize,
                                            mc_count=mc_count, seed=seed, precision=self.precision,
                                            conditional=conditional)
+
+    @_live
+    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95, conditional=True):
+        """Run the surrogate triples 0 .. mc_count - 1 once: count per point the triples whose RP2
+        and RM2 reach this handle's (one count field per measure, kept on the device, replacing the
+        counts of an earlier test) and return (sig_partial, sig_multiple), bit-identical to
+        `surrogate_significance` with the same `seed`, `mc_count` and `conditional`.  Seed, errors
+        and records as `ResidentCoherence.surrogate_test`."""
+        prob, hist = self._count(mc_count, seed, (0, 1, 1) if conditional else (0, 1, 2))
+        return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
+
+    @_live
+    def pvalues(self, rows=slice(None), cols=slice(None), measure='partial'):
+        """The measure's p[rows, cols] = (1 + k) / (1 + M) (float64) of the last `surrogate_test`,
+        with the slicing of `window`; NaN where the measure is not finite."""
+        return self._pvalues(self._measure(measure), rows, cols)
+
+    @_live
+    def pvalue_fraction(self, alpha, measure='partial'):
+        """Per scale, the fraction of the points inside the cone of influence (with a finite p) whose
+        p <= alpha; NaN for a scale without such points."""
+        return self._pvalue_fraction(self._measure(measure), alpha)
+
+    @_live
+    def fdr_threshold(self, q=0.05, method='bh', inside_coi=True, measure='partial'):
+        """`ResidentCoherence.fdr_threshold` over the measure's p-values."""
+        return self._fdr_threshold(self._measure(measure), q, method, inside_coi)
 
 
 def wct3_resident(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,

@@ -708,18 +708,24 @@ def _surrogate_problem(series, dt, dj, s0, J, wavelet, normalize, precision):
     return p, _mc_problem(dt, dj, p.s0, p.J, p.wavelet, N=p.n0)
 
 
-def _surrogate_histogram(p, prob, groups, seed, first, count, engine=None):
+def _surrogate_histogram(p, prob, groups, seed, first, count, engine=None, serial=None):
     """Histograms int64 [nser - 1, S, nbins] of the coherence (two series) or of the partial and
     multiple coherence (three) of the surrogate units first .. first + count - 1 of the
-    standardised data `p.yns`, drawn and accumulated on the device in one transaction."""
+    standardised data `p.yns`, drawn and accumulated on the device in one transaction.  With the
+    `serial` of the resident product of the same data, the same run also counts, per point, the
+    units that reach the product's value (`Engine.surrogate_counts`, counters reset first)."""
     nser = len(p.yns)
     hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
     eng = engine or _engine.default_engine()
 
     def call(*a, boxcar_len, precision):
         dt, _, sj, family, param = a[nser:]
-        eng.wct_mc_phase(np.stack(a[:nser]), groups, seed, first, count, dt, sj, family, param, boxcar_len,
-                         prob['mask'], prob['maxscale'], prob['nbins'], *hist, precision=precision)
+        args = (np.stack(a[:nser]), groups, seed, first, count, dt, sj, family, param, boxcar_len,
+                prob['mask'], prob['maxscale'], prob['nbins'], *hist)
+        if serial is None:
+            eng.wct_mc_phase(*args, precision=precision)
+        else:
+            eng.surrogate_counts(*args, serial=serial, reset=True, precision=precision)
 
     _wct_on_device(eng, p, call)
     return hist
