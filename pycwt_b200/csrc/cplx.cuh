@@ -8,8 +8,12 @@
 #ifndef HD
 #ifdef CWTB_HOST_EMU
 #define HD inline  // tests-only CPU emulation build: no device code at all
+#define HD_NOINLINE inline
 #else
 #define HD __host__ __device__ __forceinline__
+// a function whose code one kernel runs from several call sites: kept out of line so the kernel's
+// code stays small enough for the instruction cache
+#define HD_NOINLINE __host__ __device__ __noinline__
 #endif
 #endif
 

@@ -1754,12 +1754,13 @@ int cwtb_sync(cwtb_ctx *c) {
 // ---- overlap-save planning (kernels.cuh: OsBody) ----------------------------------------------
 // Cost model, us per row of 2^20 outputs on H100 (see DESIGN.md §4): the overlap-save kernel at
 // hop = L scaled by L / hop, against the two-kernel pair the row would otherwise take.  Measured at
-// config 2 (H100 80GB HBM3, 700 W): OsBody<4> 0.337 ms for rows j = 20..47 (83..263 taps, L / hop
-// 1.09..1.35), 12.0 us per row; the dense pair 22.3-23.2 us per row.  Rows that expand by R = 4 are
-// not candidates: their expansion kernel (7.3-7.8 us per row with 16-20 taps, plus a share of the
-// coarse transform) costs less than the overlap-save kernel even at hop = L.
-static const double kOsUs = 9.5;
-static const double kTwoKernelUs = 23.2;   // dense first + second kernel (PassABody<1024> + PassBBody<1024>)
+// config 2 (H100 80GB HBM3, 700 W) with the register-resident tile core: OsBody<4> 0.245 ms for rows
+// j = 20..47 (83..263 taps, L / hop 1.09..1.35), 8.75 us per row; the dense pair 11.7 + 11.8 us per
+// row.  Rows that expand by R = 4 are not candidates: their expansion kernel (7.3-7.8 us per row with
+// 16-20 taps, plus a share of the coarse transform) costs less than the overlap-save kernel even at
+// hop = L.
+static const double kOsUs = 7.0;
+static const double kTwoKernelUs = 23.5;   // dense first + second kernel (PassABody<1024> + PassBBody<1024>)
 
 struct DevTmp {   // device scratch of the planner, freed on every path out
   void *p = nullptr;

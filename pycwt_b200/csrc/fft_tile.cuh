@@ -444,4 +444,99 @@ HD void tile_second(cx<T> *sm, const cx<T> *tw, int tid) {  // only for 3-pass p
   pass_mid<T, K, K / Plan<K>::R1, Plan<K>::R2, SIGN, SmemLoader<T, K, ROWS>, ROWS>(sm, tw, ld, tid);
 }
 
+// ---- register-resident 1024-point fp64 core: 1024 = 32 x 32, one shared-memory exchange ---------
+// The CTA (NT = 128 threads) owns the P = 4 transforms of a 4096-element fp64 tile, one column of one
+// transform per thread in each of two phases (n = n1 + 32 n2, q = k1 + 32 k2):
+//   phase A, thread (b, n1):  x[n2] = in_b[n1 + 32 n2] from the loader, DFT_32 over n2 in registers,
+//                             output k1 times w_1024^{n1 k1}, written to the exchange as Y_b[n1][k1];
+//   CTA barrier;
+//   phase B, thread (b, k1):  y[n1] = Y_b[n1][k1], DFT_32 over n1 in registers: X_b[k1 + 32 k2] = y[k2].
+// Each element crosses shared memory once (one write, one read) instead of the three read-write passes
+// of the (8, 8, 16) plan, with one barrier instead of three.  Nothing stays in registers across the
+// barrier, so the emulation's phase-by-phase loop over threads runs the same code.
+// Phase B hands its outputs to the storer in two halves, q = (k1 + 512 h) + 32 c for c < 16, so the
+// storers see whole-sector runs exactly as after pass_last (digit reversal in the store address), and
+// those that walk a twiddle recurrence over c take the same 15 steps as after the radix-16 last pass.
+// Lane maps: X32_BMAJOR  b = tid % 4, column = tid / 4 (lanes over b first: outputs contiguous in b
+//                        leave as 64-byte runs, as from pass_last);
+//            X32_WARP    b = tid / 32, column = tid % 32 (one warp per transform: inputs and outputs
+//                        contiguous in the position).
+enum { X32_BMAJOR = 0, X32_WARP = 1 };
+struct X32 {
+  static constexpr int K = 1024, C = 32, P = 4;
+  static_assert(TileCfg<double>::NT == P * C && TileCfg<double>::TILE == P * K,
+                "the register-resident core assumes a 4096-element fp64 tile in 128 threads");
+  template <int MAP> HD static void map(int tid, int &b, int &col) {
+    if (MAP == X32_BMAJOR) { b = tid % P; col = tid / P; } else { b = tid / C; col = tid % C; }
+  }
+};
+// Exchange buffer of its own: [b][n1][k1], rows of 33 and a transform pitch of 1058 elements (2 mod 8
+// sixteen-byte bank groups): a quarter-warp touches 8 distinct groups in both phases and both maps.
+struct X32Ex {
+  static constexpr int ROW = 33, BP = 32 * ROW + 2;
+  static constexpr size_t BYTES = (size_t)X32::P * BP * sizeof(double2);
+  HD static int at(int b, int n1, int k1) { return b * BP + n1 * ROW + k1; }
+};
+// Exchange in place in the tile the loader reads (Lay<double, 1024, ROWS>): Y_b[n1][k1] goes to position
+// n1 + 32 k1, one of the positions thread (b, n1) has just read, so no thread overwrites another's input.
+template <bool ROWS> struct X32InTile {
+  HD static int at(int b, int n1, int k1) { return Lay<double, X32::K, ROWS>::phys(b, n1 + 32 * k1); }
+};
+
+// DFT_32 of a loaded column, the twiddles w_1024^{n1 k1} and the write to the exchange.  With
+// k1 = 8 a + c the twiddle is tw_1024(n1, c) * tw_256(2 n1, a): two correctly rounded table entries
+// (fft_tile.cuh: tw_offset), ten loads per column.
+template <int SIGN, class EX>
+HD void x32_exchange_out(double2 *ex, const double2 *__restrict__ tw, int b, int n1, double2 (&x)[32]) {
+  dftR<32, SIGN, double>(x);
+  double2 wa[4];
+#pragma unroll
+  for (int a = 1; a < 4; ++a) {
+    wa[a] = ldg(&tw[tw_offset(256) + (a - 1) * 64 + 2 * n1]);
+    if (SIGN < 0) wa[a].y = -wa[a].y;
+  }
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    double2 wc = mk<double>(1.0, 0.0);
+    if (c > 0) {
+      wc = ldg(&tw[tw_offset(1024) + (c - 1) * 128 + n1]);
+      if (SIGN < 0) wc.y = -wc.y;
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const int k1 = 8 * a + c;
+      if (k1 > 0) {
+        const double2 w = a == 0 ? wc : (c == 0 ? wa[a] : cmul(wc, wa[a]));
+        x[k1] = cmul(x[k1], w);
+      }
+      ex[EX::at(b, n1, k1)] = x[k1];
+    }
+  }
+}
+// phase A: the loader fills the thread's column (positions n1 + 32 i), then the exchange is written
+template <int SIGN, int MAP, class EX, class Loader>
+HD void x32_first(double2 *ex, const double2 *tw, Loader &ld, int tid) {
+  int b, n1;
+  X32::map<MAP>(tid, b, n1);
+  double2 x[32];
+  ld.begin(n1, 32, b, X32::P);
+  ld.load(b, x);
+  x32_exchange_out<SIGN, EX>(ex, tw, b, n1, x);
+}
+// phase B: the second DFT_32 and the store (storer interface of pass_last)
+template <int SIGN, int MAP, class EX, class Storer>
+HD void x32_last(const double2 *ex, Storer &st, int tid) {
+  int b, k1;
+  X32::map<MAP>(tid, b, k1);
+  double2 y[32];
+#pragma unroll
+  for (int n1 = 0; n1 < 32; ++n1) y[n1] = ex[EX::at(b, n1, k1)];
+  dftR<32, SIGN, double>(y);
+  double2 lo[16], hi[16];
+#pragma unroll
+  for (int c = 0; c < 16; ++c) { lo[c] = y[c]; hi[c] = y[c + 16]; }
+  st.store(b, k1, 32, lo);
+  st.store(b, k1 + 512, 32, hi);
+}
+
 }  // namespace cwtb

@@ -400,7 +400,10 @@ template <typename T> struct PassBArgs {
 // K2 = 1024 leaves P = TILE/K2 = Q/2 transforms per tile (64-byte output runs, 2-way bank
 // conflict on the last pass of the unskewed row layout); K2 = 512 has P = Q: 128-byte output
 // runs, conflict-free.  The pruned (band) scales use 512, the dense ones need 1024 (K1 <= 1024).
-template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
+// REG: fp64 K2 = 1024 runs the register-resident core (fft_tile.cuh: x32_first / x32_last) with the
+// exchange in place in the row tile; the coarse transforms of the expansion rows (CoarseBBody) keep
+// the three-pass core.
+template <typename T, int SIGN, int K2 = K2C, bool REG = (sizeof(T) == 8 && K2 == X32::K)> struct PassBBody {
   static constexpr int NTB = TileCfg<T>::NT;   // threads per CTA of this kernel
   static constexpr int NT = NTB;
   using V = cx<T>;
@@ -410,7 +413,7 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
   static constexpr int NP = Plan<K>::NP;
   // phase 0: one thread issues the bulk-async (TMA) copies of the tile's rows -- the rows
   // Z[u0 .. u0+P) are contiguous in global memory -- then the FFT passes run from shared memory
-  static constexpr int NPHASE = NP + 1;
+  static constexpr int NPHASE = REG ? 3 : NP + 1;
   static constexpr size_t SMEM = LY::TILE_BYTES + 16;
   // bulk-async copies need 16-byte aligned shared-memory destinations: every row start
   static constexpr bool ROWS_ALIGNED = (LY::PITCH * sizeof(V)) % 16 == 0;
@@ -452,8 +455,11 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
       tb.wait(0);
       SmemLoader<T, K, true> ld;
       ld.sm = sm;
-      tile_first<T, K, SIGN, SmemLoader<T, K, true>, true>(sm, a.tw, ld, tid);
-    } else if constexpr (PH == 2 && NP == 3) {
+      if constexpr (REG)
+        x32_first<SIGN, X32_WARP, X32InTile<true>>(sm, a.tw, ld, tid);
+      else
+        tile_first<T, K, SIGN, SmemLoader<T, K, true>, true>(sm, a.tw, ld, tid);
+    } else if constexpr (PH == 2 && NP == 3 && !REG) {
       tile_second<T, K, SIGN, true>(sm, a.tw, tid);
     } else {
       const int il = a.ileave > 1 ? a.ileave : 1;
@@ -473,8 +479,11 @@ template <typename T, int SIGN, int K2 = K2C> struct PassBBody {
         st.epi.post = a.post;
         st.epi.nfreq = (long long)a.N * il;
       }
-      pass_last<T, K, SIGN, OutStorer<T>, true>(sm, st, tid);
-      if (tid == 0) tb.inval();   // every thread passed wait() two barriers ago
+      if constexpr (REG)
+        x32_last<SIGN, X32_BMAJOR, X32InTile<true>>(sm, st, tid);
+      else
+        pass_last<T, K, SIGN, OutStorer<T>, true>(sm, st, tid);
+      if (tid == 0) tb.inval();   // every thread passed wait() at least one barrier ago
     }
   }
 };
@@ -567,47 +576,49 @@ struct OsStorer {
   }
 };
 
+// Transforms: the register-resident core (fft_tile.cuh: x32_first / x32_last), one warp per block,
+// with an exchange buffer of its own next to the half spectrum.
 template <int G> struct OsBody {
-  static constexpr int L = 1024;
+  static constexpr int L = X32::K;
   static constexpr int NTB = TileCfg<double>::NT;
   static constexpr int NT = NTB;
   using Args = OsArgs;
-  using LY = Lay<double, L>;
-  static constexpr int P = LY::P;
-  static_assert(Plan<L>::NP == 3, "overlap-save phases assume a three-pass tile plan");
-  static constexpr int NPHASE = 3 + 3 * G;
-  static constexpr size_t SMEM = LY::TILE_BYTES + (size_t)P * (L / 2 + 1) * sizeof(double2);
+  static constexpr int P = X32::P;
+  static constexpr int NPHASE = 2 + 2 * G;
+  static constexpr size_t SMEM = X32Ex::BYTES + (size_t)P * (L / 2 + 1) * sizeof(double2);
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
-    double2 *sm = (double2 *)smraw;
-    double2 *xs = (double2 *)((char *)smraw + LY::TILE_BYTES);
+    double2 *ex = (double2 *)smraw;
+    double2 *xs = (double2 *)((char *)smraw + X32Ex::BYTES);
     const OsGroup g = a.groups[by];
     const long long n_first = (long long)bx * P * g.hop;
     if (n_first >= a.n0) return;   // whole CTA: no block of this tile holds outputs
     if constexpr (PH == 0) {
-      OsSigLoader<L, Plan<L>::R1> ld;
+      OsSigLoader<L, X32::C> ld;
       ld.x = a.sig + (size_t)a.descs[g.first].chan * a.n0; ld.start = n_first - g.t1; ld.n0 = a.n0; ld.nmask = a.N - 1; ld.hop = g.hop;
-      tile_first<double, L, -1>(sm, a.tw, ld, tid);
+      x32_first<-1, X32_WARP, X32Ex>(ex, a.tw, ld, tid);
     } else if constexpr (PH == 1) {
-      tile_second<double, L, -1>(sm, a.tw, tid);
-    } else if constexpr (PH == 2) {
       OsHalfStorer<L> st{xs};
-      pass_last<double, L, -1, OsHalfStorer<L>, false, true>(sm, st, tid);
+      x32_last<-1, X32_WARP, X32Ex>(ex, st, tid);
     } else {
-      constexpr int r = (PH - 3) / 3, step = (PH - 3) % 3;
+      constexpr int r = (PH - 2) / 2;
       if (r >= g.count) return;
-      if constexpr (step == 0) {
-        OsSpecLoader<L, Plan<L>::R1> ld;
-        ld.xs = xs; ld.H = a.H + g.hoff + (long long)r * L;
-        tile_first<double, L, +1>(sm, a.tw, ld, tid);
-      } else if constexpr (step == 1) {
-        tile_second<double, L, +1>(sm, a.tw, tid);
-      } else {
-        OsStorer st;
-        st.row = a.W + (size_t)a.descs[g.first + r].row * a.n0;
-        st.nb0 = n_first - g.t1; st.n0 = a.n0; st.t1 = g.t1; st.hop = g.hop; st.epi = a.epi;
-        pass_last<double, L, +1, OsStorer, false, true>(sm, st, tid);
-      }
+      if constexpr (PH % 2 == 0) inv_first(a, g, r, n_first, ex, xs, tid);
+      else inv_last(a, g, r, n_first, ex, tid);
     }
+  }
+  // the inverse transform of row r of the group: one copy of the code for all G rows
+  HD_NOINLINE static void inv_first(const Args &a, const OsGroup &g, int r, long long n_first, double2 *ex,
+                                    const double2 *xs, int tid) {
+    OsSpecLoader<L, X32::C> ld;
+    ld.xs = xs; ld.H = a.H + g.hoff + (long long)r * L;
+    x32_first<+1, X32_WARP, X32Ex>(ex, a.tw, ld, tid);
+  }
+  HD_NOINLINE static void inv_last(const Args &a, const OsGroup &g, int r, long long n_first, const double2 *ex,
+                                   int tid) {
+    OsStorer st;
+    st.row = a.W + (size_t)a.descs[g.first + r].row * a.n0;
+    st.nb0 = n_first - g.t1; st.n0 = a.n0; st.t1 = g.t1; st.hop = g.hop; st.epi = a.epi;
+    x32_last<+1, X32_WARP, X32Ex>(ex, st, tid);
   }
 };
 
@@ -681,6 +692,10 @@ template <typename T> struct PassAArgs {
   unsigned Nx;         // MODE_COARSE: length of the signal's spectrum (N is the coarse length)
 };
 
+// REG: the fp64 dense rows of K1 = 1024 fill the register-resident core (fft_tile.cuh:
+// x32_exchange_out / x32_last) straight from their spectrum loads: a thread's share of the tile is one
+// column (b = tid % 4, positions tid / 4 + 32 i) of the three-pass core's fill as well, so phase 0
+// loads, transforms and writes the exchange, and phase 1 finishes and stores.  No tile in shared memory.
 template <typename T, int K1, int MODE, int SIGN> struct PassABody {
   static constexpr int NTB = TileCfg<T>::NT;   // threads per CTA of this kernel
   static constexpr int NT = NTB;
@@ -690,8 +705,74 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
   static constexpr int NP = Plan<K1>::NP;
   static constexpr int P = LY::P;
   static constexpr int T2 = P < K2C ? P : K2C;  // r2 values per tile (a.K2 is a multiple of it)
-  static constexpr int NPHASE = NP == 1 ? 1 : NP + 1;
-  static constexpr size_t SMEM = LY::BYTES;
+  static constexpr bool REG = sizeof(T) == 8 && K1 == X32::K && MODE == MODE_DENSE;
+  static constexpr int NPHASE = REG ? 2 : (NP == 1 ? 1 : NP + 1);
+  static constexpr size_t SMEM = REG ? X32Ex::BYTES : LY::BYTES;
+
+  // Morlet, dense scale: a thread's bins are k0, k0 + D, k0 + 2D, ... (D = (NT/T2)*K2), so
+  //   g(k + D) = g(k) * rho(k),  rho(k + D) = rho(k) * exp(-a^2),  a = s * w_D,
+  // replaces the exp per bin by two multiplies.  Re-seeded with exact exp() when the
+  // band is entered, at the signed-bin wrap and every 16 steps (error <= ~1e-14 relative).
+  // Batches of UB bins: the spectrum loads of a batch are issued together (independent of the
+  // recurrence), then the Gaussian values follow one another.  One load per iteration, as the
+  // plain loop compiles, leaves every thread waiting a full L2 round trip 32 times per tile.
+  static constexpr int DPOS = NT / T2 > 0 ? NT / T2 : 1;
+  static constexpr int UB = CWTB_PASSA_BATCH;
+  struct GaussWalk {
+    const Args &a;
+    const ScaleDesc &d;
+    unsigned rb;   // r2 of the thread's bins: r20 + b
+    const V *sp;   // the thread's bin of position 0
+    long long D;
+    double aa, q, g = 0, rho = 0;
+    long long kprev = 0;
+    int since = 1 << 30;
+    HD GaussWalk(const Args &a_, const ScaleDesc &d_, int r20, int b) : a(a_), d(d_), rb((unsigned)(r20 + b)) {
+      sp = a.spec + (size_t)d.chan * a.N + rb;
+      D = (long long)DPOS * a.K2;
+      const double wd = 6.283185307179586 * ((double)D * a.fam.dw);
+      aa = d.s * wd;
+      q = exp(-aa * aa);
+    }
+    // spectrum values of positions pos0 + u*DPOS (kk[u] = INT_MAX: outside the band or past K1)
+    HD void load(int pos0, V (&raw)[UB], int (&kk)[UB]) const {
+#pragma unroll
+      for (int u = 0; u < UB; ++u) {
+        const int pos = pos0 + u * DPOS;
+        const unsigned r = (unsigned)pos * a.K2 + rb;
+        const int k = (int)r - (r >= a.N / 2 ? (int)a.N : 0);
+        const bool in = pos < K1 && k >= d.k_lo && k <= d.k_hi;
+        kk[u] = in ? k : (int)0x7fffffff;
+        raw[u] = in ? ldg(&sp[(size_t)pos * a.K2]) : mk<T>(0, 0);
+      }
+    }
+    // exact g(k) and rho(k), out of line: the register-resident fill unrolls 32 steps of the walk
+    HD_NOINLINE static double2 seed(double s, double dw, double f0, double aa, int k) {
+      const double f = s * (6.283185307179586 * ((double)k * dw));
+      const double dd = f - f0;
+      return make_double2(exp(-0.5 * dd * dd), exp(-aa * dd - 0.5 * aa * aa));
+    }
+    // the next value of the walk: raw * Gaussian * amp, or zero outside the band
+    HD V next(V raw, int kk) {
+      if (kk == (int)0x7fffffff) { since = 1 << 30; return mk<T>(0, 0); }
+      const int k = kk;
+      // (a value in the subnormal range has lost its relative precision: with band_eps = 0 the
+      // band reaches bins where exp() is below 1e-308, and the recurrence would carry that
+      // error up to the peak -- re-seed until the value is a normal number again)
+      if (since >= 16 || (long long)k != kprev + D || g < 1e-290) {
+        const double2 gr = seed(d.s, a.fam.dw, a.fam.f0, aa, k);
+        g = gr.x;
+        rho = gr.y;
+        since = 0;
+      } else {
+        g *= rho;
+        rho *= q;
+        ++since;
+      }
+      kprev = k;
+      return cscale(raw, (T)(g * d.amp));
+    }
+  };
 
   struct Src {
     const Args &a;
@@ -729,6 +810,9 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
     }
   };
 
+  // the register-resident fill unrolls its 32 positions: one copy of the families' evaluation
+  HD_NOINLINE static V get_out_of_line(const Args &a, int by, int p, int pos, int r2) { return Src(a, by, p).get(pos, r2); }
+
   template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
     V *sm = (V *)smraw;
     const int NTILE2 = (int)(a.K2 / T2);
@@ -751,6 +835,30 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
         for (int i = 0; i < K1; ++i) x[i] = src.get(i, r20 + b);
         dftR<K1, SIGN, T>(x);
         st.store(b, 0, 1, x);
+      }
+    } else if constexpr (REG) {
+      if constexpr (PH == 0) {
+        static_assert(T2 == X32::P && DPOS == X32::C && X32::K % (DPOS * UB) == 0, "dense fill vs core columns");
+        Src src(a, by, p);
+        const int b = tid % T2, n1 = tid / T2;   // X32_BMAJOR
+        V x[X32::C];
+        if (a.fam.family == 0) {
+          GaussWalk gw(a, src.d, r20, b);
+#pragma unroll
+          for (int it = 0; it < X32::C / UB; ++it) {
+            V raw[UB];
+            int kk[UB];
+            gw.load(n1 + it * UB * DPOS, raw, kk);
+#pragma unroll
+            for (int u = 0; u < UB; ++u) x[it * UB + u] = gw.next(raw[u], kk[u]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < X32::C; ++i) x[i] = get_out_of_line(a, by, p, n1 + DPOS * i, r20 + b);
+        }
+        x32_exchange_out<SIGN, X32Ex>(sm, a.tw, b, n1, x);
+      } else {
+        x32_last<SIGN, X32_BMAJOR, X32Ex>(sm, st, tid);
       }
     } else if constexpr (PH == 0) {
       Src src(a, by, p);
@@ -777,64 +885,17 @@ template <typename T, int K1, int MODE, int SIGN> struct PassABody {
         }
       }
       if (MODE == MODE_DENSE && a.fam.family == 0 && T2 <= NT) {
-        // Morlet, dense scale: a thread's bins are k0, k0 + D, k0 + 2D, ... (D = (NT/T2)*K2), so
-        //   g(k + D) = g(k) * rho(k),  rho(k + D) = rho(k) * exp(-a^2),  a = s * w_D,
-        // replaces the exp per bin by two multiplies.  Re-seeded with exact exp() when the
-        // band is entered, at the signed-bin wrap and every 16 steps (error <= ~1e-14 relative).
-        constexpr int DPOS = NT / T2;
-        const ScaleDesc &d = src.d;
         const int b = tid % T2;
-        const long long D = (long long)DPOS * a.K2;
-        const double wd = 6.283185307179586 * ((double)D * a.fam.dw);
-        const double aa = d.s * wd;
-        const double q = exp(-aa * aa);
-        double g = 0, rho = 0;
-        long long kprev = 0;
-        int since = 1 << 30;
-        // Batches of UB bins: the spectrum loads of a batch are issued together (independent of the
-        // recurrence), then the Gaussian values follow one another.  One load per iteration, as the
-        // plain loop compiles, leaves every thread waiting a full L2 round trip 32 times per tile.
-        constexpr int UB = CWTB_PASSA_BATCH;
-        const V *sp = a.spec + (size_t)d.chan * a.N + (unsigned)(r20 + b);
+        GaussWalk gw(a, src.d, r20, b);
         for (int pos0 = tid / T2; pos0 < K1; pos0 += DPOS * UB) {
           V raw[UB];
           int kk[UB];
-#pragma unroll
-          for (int u = 0; u < UB; ++u) {
-            const int pos = pos0 + u * DPOS;
-            const unsigned r = (unsigned)pos * a.K2 + (unsigned)(r20 + b);
-            const int k = (int)r - (r >= a.N / 2 ? (int)a.N : 0);
-            const bool in = pos < K1 && k >= d.k_lo && k <= d.k_hi;
-            kk[u] = in ? k : (int)0x7fffffff;
-            raw[u] = in ? ldg(&sp[(size_t)pos * a.K2]) : mk<T>(0, 0);
-          }
+          gw.load(pos0, raw, kk);
 #pragma unroll
           for (int u = 0; u < UB; ++u) {
             const int pos = pos0 + u * DPOS;
             if (pos >= K1) break;
-            V v = mk<T>(0, 0);
-            if (kk[u] != (int)0x7fffffff) {
-              const int k = kk[u];
-              // (a value in the subnormal range has lost its relative precision: with band_eps = 0 the
-              // band reaches bins where exp() is below 1e-308, and the recurrence would carry that
-              // error up to the peak -- re-seed until the value is a normal number again)
-              if (since >= 16 || (long long)k != kprev + D || g < 1e-290) {
-                const double f = d.s * (6.283185307179586 * ((double)k * a.fam.dw));
-                const double dd = f - a.fam.f0;
-                g = exp(-0.5 * dd * dd);
-                rho = exp(-aa * dd - 0.5 * aa * aa);
-                since = 0;
-              } else {
-                g *= rho;
-                rho *= q;
-                ++since;
-              }
-              kprev = k;
-              v = cscale(raw[u], (T)(g * d.amp));
-            } else {
-              since = 1 << 30;
-            }
-            sm[LY::phys(b, pos)] = v;
+            sm[LY::phys(b, pos)] = gw.next(raw[u], kk[u]);
           }
         }
       } else {
@@ -1032,7 +1093,7 @@ template <typename T> struct CoarseABody {
 
 // second kernel of the same rows: PassBBody from Z into C
 template <typename T> struct CoarseBBody {
-  using B = PassBBody<T, +1>;
+  using B = PassBBody<T, +1, K2C, false>;
   static constexpr int NTB = B::NTB;
   static constexpr int NT = NTB;
   using Args = CoarseArgs<T>;
