@@ -482,6 +482,58 @@ int cwtb_coherence_count_hist(cwtb_ctx *ctx, const int64_t *lo, const int64_t *h
 int cwtb_coherence3_count_hist(cwtb_ctx *ctx, int measure, const int64_t *lo, const int64_t *hi,
                                int64_t nbins, int64_t *out);
 
+/* ---- cluster tests of the resident coherence against phase-randomised surrogates -------------
+ * cwtb_coherence_cluster_test (the resident coherence) and cwtb_coherence3_cluster_test (the
+ * resident RP2 or RM2, by `measure`) take the arguments of cwtb_coherence*_surrogate_counts (same
+ * units, surrogates and histograms) and, per row j of the map, a threshold thr[j], a column range
+ * [lo[j], hi[j]) and a weight q[j] <= 2^32.  In the resident map and in the map of every unit, point
+ * (j, n) is selected where the value is finite, > thr[j] (a NaN selects nothing) and
+ * lo[j] <= n < hi[j].  Clusters are the 8-connected components of the selection in the
+ * (row, column) grid; column 0 and column n0 - 1 are not neighbours.  A cluster's Q is the sum of
+ * q[j] over its points, in uint64.  qmax_out[i] (n_units uint64) receives the largest Q of unit
+ * first_unit + i, 0 without clusters; the clusters of the resident map are kept with the product
+ * (the label image takes 4 bytes per scale-point).  The counts of an earlier surrogate-count call
+ * are neither read nor changed.  CWTB_ERR_UNSUPPORTED: n_scales * n0 >= 2^32.  CWTB_ERR_ARG: a
+ * weight above 2^32, a column range outside [0, n0) or lo > hi, an unknown measure, and the
+ * errors of cwtb_coherence*_surrogate_counts, whose CWTB_ERR_STATE cases apply too.  Lifetime:
+ * the clusters die with their product (a new cwtb_wct_resident / cwtb_wct3_resident, the release
+ * calls, cwtb_destroy) and with the next cluster test of it; a call that fails leaves none
+ * readable. */
+int cwtb_coherence_cluster_test(cwtb_ctx *ctx, const double *series, const int *group, uint64_t seed,
+                                int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                int maxscale, int nbins, int64_t *hist, int64_t serial, const double *thr,
+                                const int64_t *lo, const int64_t *hi, const uint64_t *q, uint64_t *qmax_out);
+int cwtb_coherence3_cluster_test(cwtb_ctx *ctx, const double *series, const int *group, uint64_t seed,
+                                 int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                 int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                 int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
+                                 int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
+                                 const uint64_t *q, int measure, uint64_t *qmax_out);
+/* The clusters of the resident map of the last cluster test, ordered by Q descending, ties by the
+ * row-major index of the cluster's first point: *count = their number, and the first
+ * min(cap, count) rows into Q[cap], points[cap] (point count) and box[cap][4] = first row, last
+ * row + 1, first column, last column + 1.  CWTB_ERR_STATE: no product resident, or no cluster test
+ * has completed for it. */
+int cwtb_coherence_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                                 int64_t *box);
+int cwtb_coherence3_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                                  int64_t *box);
+/* Window of the label image: 0 off the clusters, c + 1 on the cluster of table row c, int32, with
+ * the layout and checks of cwtb_coherence_window and the errors of the table calls. */
+int cwtb_coherence_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0,
+                                  int64_t ncols, int64_t col_step, int32_t *out);
+int cwtb_coherence3_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0,
+                                   int64_t ncols, int64_t col_step, int32_t *out);
+/* Test hook: labels a host bitmask bits [n_scales][ceil(n0 / 32)] (column n: bit n % 32 of word
+ * n / 32; no bit set past column n0 - 1) with the weights q[n_scales] through the cluster tests'
+ * labeller: the table as cwtb_coherence_cluster_table returns it, the label image labels
+ * [n_scales][n0] (may be NULL) and the largest Q into *qmax.  The shape is checked before anything
+ * is read or allocated: CWTB_ERR_UNSUPPORTED for n_scales * n0 >= 2^32. */
+int cwtb_cluster_label_bits(cwtb_ctx *ctx, const uint32_t *bits, int n_scales, int64_t n0, const uint64_t *q,
+                            int64_t cap, int64_t *count, uint64_t *Q, int64_t *points, int64_t *box,
+                            int32_t *labels, uint64_t *qmax);
+
 /* ---- batched transform of independent channels (SURVEY 8d config 5) ------- */
 /* X: host [n_chan, n0] (float or double).  The per-channel transforms stay on
  * the device; `power_out` (may be NULL) receives the per-channel global wavelet

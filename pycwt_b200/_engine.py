@@ -113,6 +113,15 @@ _SIGNATURES = {
     "cwtb_coherence3_pvalue_row_stats": (_I, [_P, _I, _P, _P, _P, _I64, _I, _P]),
     "cwtb_coherence_count_hist": (_I, [_P, _P, _P, _I64, _P]),
     "cwtb_coherence3_count_hist": (_I, [_P, _I, _P, _P, _I64, _P]),
+    "cwtb_coherence_cluster_test": (_I, [_P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I,
+                                         _P, _I, _I, _P, _I64, _P, _P, _P, _P, _P]),
+    "cwtb_coherence3_cluster_test": (_I, [_P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D, _I,
+                                          _P, _I, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P]),
+    "cwtb_coherence_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
+    "cwtb_coherence3_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
+    "cwtb_coherence_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_coherence3_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_cluster_label_bits": (_I, [_P, _P, _I, _I64, _P, _I64, _P, _P, _P, _P, _P, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -989,6 +998,95 @@ class Engine(object):
             self._check(self.lib.cwtb_coherence3_count_hist(self.h, int(measure), _ptr(lo), _ptr(hi), int(nbins),
                                                             _ptr(out)))
         return out
+
+    # ---- cluster tests of a resident coherence against phase-randomised surrogates ------------
+    # `measure` None: the resident coherence; MEASURE_PARTIAL / _MULTIPLE: the resident partial /
+    # multiple coherence.
+    @_locked
+    def cluster_test(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+                     mask, maxscale, nbins, hist_a, hist_b=None, serial=None, thr=None, lo=None, hi=None, q=None,
+                     measure=None, precision=F64):
+        """`wct_mc_phase` that also labels the clusters of the resident product's map and of every
+        unit's (cwtb_coherence*_cluster_test): uint64 [n_units], the largest cluster sum Q of each
+        unit.  The resident map's clusters stay with the product (`cluster_table`,
+        `cluster_labels`)."""
+        series, groups = self._phase_inputs("cluster_test", series, groups)
+        nser, n0 = series.shape
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        mask = np.ascontiguousarray(mask, dtype=np.uint8)
+        if mask.shape != (sj.size, n0):
+            raise ValueError("cluster_test: mask must be [scales, n0]")
+        if nser == 2 and (hist_b is not None or measure is not None):
+            raise ValueError("cluster_test: two series have one histogram and one measure")
+        ha, hb = self._mc_hists("cluster_test", sj.size, nbins, hist_a, hist_b)
+        lo, hi, thr = _row_args("cluster_test", sj.size, lo, hi, thr)
+        q = np.ascontiguousarray(q, dtype=np.uint64)
+        if q.shape != (sj.size,):
+            raise ValueError("cluster_test: q must have one entry per scale")
+        qmax = np.zeros(int(n_units), dtype=np.uint64)
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        args = (self.h, _ptr(series), _ptr(groups), int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
+                float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
+                int(nbins))
+        rows = (_ptr(thr), _ptr(lo), _ptr(hi), _ptr(q))
+        if nser == 2:
+            self._check(self.lib.cwtb_coherence_cluster_test(*args, ha, int(serial), *rows, _ptr(qmax)))
+        else:
+            self._check(self.lib.cwtb_coherence3_cluster_test(*args, ha, hb, int(serial), *rows, int(measure),
+                                                              _ptr(qmax)))
+        return qmax
+
+    @staticmethod
+    def _table(call):
+        """(Q uint64, points int64, box int64 [count, 4]) of a table call(cap, count, Q, points, box)."""
+        count = _I64()
+        call(0, ctypes.byref(count), None, None, None)
+        m = count.value
+        Q = np.empty(m, dtype=np.uint64)
+        pts = np.empty(m, dtype=np.int64)
+        box = np.empty((m, 4), dtype=np.int64)
+        call(m, ctypes.byref(count), _ptr(Q), _ptr(pts), _ptr(box))
+        return Q, pts, box
+
+    @_locked
+    def cluster_table(self, triple=False):
+        """The resident map's clusters of the last cluster test of the coherence (`triple` False) or
+        of the partial / multiple coherence (True): (Q, points, box [:, 4] = first row, last row + 1,
+        first column, last column + 1), in table order."""
+        fn = self.lib.cwtb_coherence3_cluster_table if triple else self.lib.cwtb_coherence_cluster_table
+        return self._table(lambda *a: self._check(fn(self.h, *a)))
+
+    @_locked
+    def cluster_labels(self, triple, row0, nrows, row_step, col0, ncols, col_step):
+        """int32 labels [row0::row_step][:nrows, col0::col_step][:, :ncols] of the last cluster
+        test of the coherence (`triple` False) or of the partial / multiple coherence (True): 0 off
+        the clusters, c + 1 on table row c."""
+        out = np.empty((int(nrows), int(ncols)), dtype=np.int32)
+        w = (int(row0), int(nrows), int(row_step), int(col0), int(ncols), int(col_step), _ptr(out))
+        fn = self.lib.cwtb_coherence3_cluster_labels if triple else self.lib.cwtb_coherence_cluster_labels
+        self._check(fn(self.h, *w))
+        return out
+
+    @_locked
+    def cluster_label_bits(self, bits, n0, q, want_labels=True):
+        """Test hook: the cluster tests' labeller on a host bitmask uint32 [S, ceil(n0 / 32)] with the
+        weights q [S]: (Q, points, box, labels int32 [S, n0] or None, qmax)."""
+        bits = np.ascontiguousarray(bits, dtype=np.uint32)
+        q = np.ascontiguousarray(q, dtype=np.uint64)
+        if bits.ndim != 2 or bits.shape[1] != (int(n0) + 31) // 32:
+            raise ValueError("cluster_label_bits: bits must be [scales, ceil(n0 / 32)]")
+        S = int(bits.shape[0])
+        if q.shape != (S,):
+            raise ValueError("cluster_label_bits: q must have one entry per scale")
+        labels = np.empty((S, int(n0)), dtype=np.int32) if want_labels else None
+        qmax = np.zeros(1, dtype=np.uint64)
+        lab = None if labels is None else _ptr(labels)
+
+        def call(cap, count, Q, pts, box):
+            self._check(self.lib.cwtb_cluster_label_bits(self.h, _ptr(bits), S, int(n0), _ptr(q), cap, count,
+                                                         Q, pts, box, lab, _ptr(qmax)))
+        Q, pts, box = self._table(call)
+        return Q, pts, box, labels, int(qmax[0])
 
     @_locked
     def cwt_batch(self, X, dt, scales, family, param, precision=F64, want_power=True,

@@ -155,6 +155,13 @@ struct ClassRun {   // scales sharing one execution plan
   int os = 0;           // overlap-save group + 1 (0: another path)
 };
 
+// The clusters of a map, in table order (Q descending, ties by the flat index of the first point):
+// Q = sum of q_j over the points, the point count, and the box [row0, row1) x [col0, col1)
+struct ClusterTable {
+  std::vector<unsigned long long> Q, pts;
+  std::vector<long long> box;   // [clusters][4]
+};
+
 // A product that one call writes to a device buffer of its own and that later calls read in place
 // (cwtb_wct_resident, cwtb_xwt_resident).  serial is bumped before every write and on release.
 // The resident transform has the same record (cwtb_ctx::wt) without a buffer: W stays scratch.
@@ -168,15 +175,23 @@ struct ResidentSlot {
   // measure (cwtb_coherence*_surrogate_counts), and the units they hold (-1: none readable)
   Buf counts;
   long long units = -1;
+  // the coherence slots: the observed clusters of the last cwtb_coherence*_cluster_test, the label
+  // image int32 [S][n0] (0: no cluster, c + 1: row c of the table) and the table, valid with
+  // `clusters`
+  Buf labels;
+  ClusterTable table;
+  bool clusters = false;
 };
 
 // A call that writes a slot invalidates it first, so that one failing part-way leaves none resident
-// (and no counts of an earlier product readable)
+// (and no counts or clusters of an earlier product readable)
 static void slot_begin(ResidentSlot &s) {
   ++s.serial;
   s.S = 0;
   s.n0 = 0;
   s.units = -1;
+  s.clusters = false;
+  s.table = ClusterTable{};
 }
 
 // overlap-save plan of one input scale (os_plan): group + 1 (0: not overlap-save), kept taps
@@ -272,6 +287,9 @@ struct cwtb_ctx {
   size_t wtab_uploaded = 0;      // elements already on the device
   size_t wtab_max_bytes = (size_t)256 << 20;   // CWTB_WTAB_MB: host mirror size above which the cache starts over
   Buf sig, sig2, sig3, spec, Z, Zc[3], Y, B, W, W2, W3, descs, table, scratch, C, A12, F, aux, rowd, win, mask, hist, noise, wide, blueA, blueX, blueY, pspec, prot;
+  // cluster tests: the selection bitmask, its per-row arguments (thr, lo, hi, q), the chunk and row
+  // tables of the labeller, its run tables (sized from the run count of each map), the units' maxima
+  Buf cl_bits, cl_rows, cl_hdr, cl_runs, cl_qmax;
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
   // geometry and settings reuses it (planning + descriptor upload: ~0.3 ms for 256 scales, several ms
@@ -1668,7 +1686,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts, &c->coh.labels, &c->coh3.labels, &c->cl_bits, &c->cl_rows, &c->cl_hdr, &c->cl_runs, &c->cl_qmax})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2219,7 +2237,8 @@ static int smooth_time(cwtb_ctx *c, cx<T> *X, int S, long long n0, unsigned N, c
 template <typename T>
 static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2, int K,
                     double *dWCT, double *daWCT, const unsigned char *dmask, int maxscale, int nbins,
-                    unsigned long long *dhist, const double *dobs = nullptr, unsigned *dcnt = nullptr) {
+                    unsigned long long *dhist, const double *dobs = nullptr, unsigned *dcnt = nullptr,
+                    const SelArgs *sel = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2243,10 +2262,10 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   }
   if ((e = smooth_time<T>(c, (V *)c->C.p, S, n0, job.N, d_g))) return e;
   if ((e = smooth_time<T>(c, (V *)c->A12.p, S, n0, job.N, d_g))) return e;
-  const int rows_out = dWCT || dcnt ? S : maxscale;   // counting: every row
+  const int rows_out = dWCT || dcnt || sel ? S : maxscale;   // counting or selection bits: every row
   if (rows_out <= 0) return 0;
   WctFinalArgs<T> fa{(const V *)c->C.p, (const V *)c->A12.p, (const double *)c->win.p, dWCT,
-                     dmask, dhist, n0, S, K, maxscale, nbins, dobs, dcnt};
+                     dmask, dhist, n0, S, K, maxscale, nbins, dobs, dcnt, sel ? *sel : SelArgs{}};
   if (K > 64) {
     // longer than the fused kernel stages: the scale boxcar of both fields into W and W2 (dead
     // since WctPrepBody), then the ratio through the fused kernel with the unit tap at win + K
@@ -2260,13 +2279,24 @@ static int wct_core(cwtb_ctx *c, const Job &job, const T *dsig1, const T *dsig2,
   }
   using F16 = WctFinalBody<T, 16>;
   const unsigned fx = (unsigned)((n0 + F16::CW - 1) / F16::CW), fy = (unsigned)((rows_out + F16::RS - 1) / F16::RS);
+  if (sel)
+    return K <= 16 ? launch<WctFinalBody<T, 16, true>>(c, fx, fy, fa) : launch<WctFinalBody<T, 64, true>>(c, fx, fy, fa);
   return K <= 16 ? launch<F16>(c, fx, fy, fa) : launch<WctFinalBody<T, 64>>(c, fx, fy, fa);
+}
+
+// the launch of Wct3FinalBody: F16 for boxcars of up to 16 taps, else F64K
+template <class F16, class F64K>
+static int wct3_final(cwtb_ctx *c, const typename F16::Args &fa, int K, long long n0, int rows_out) {
+  if (K <= 16)
+    return launch<F16>(c, (unsigned)((n0 + F16::CW - 1) / F16::CW), (unsigned)((rows_out + F16::RS - 1) / F16::RS), fa);
+  return launch<F64K>(c, (unsigned)((n0 + F64K::CW - 1) / F64K::CW), (unsigned)((rows_out + F64K::RS - 1) / F64K::RS), fa);
 }
 
 // three transforms + partial / multiple coherence in the engine type T; outputs are device
 // pointers (any may be null) and double for every T, dPP the partial phase.  With every output null
 // (Monte-Carlo mode) only the rows below maxscale are finished, into the histograms dhP / dhM
-// (either may be null); with counters (cP / cM, against the observed oP / oM) every row is finished.
+// (either may be null); with counters (cP / cM, against the observed oP / oM) or selection bits
+// (sel) every row is finished.
 // Device memory per scale-point: the three transforms W, W2, W3 (the crosses are written over
 // them), the two auto fields C, A12 and the smoothing buffer F.
 template <typename T>
@@ -2274,7 +2304,7 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
                      double *dRP2, double *dRM2, const unsigned char *dmask = nullptr, int maxscale = 0,
                      int nbins = 0, unsigned long long *dhP = nullptr, unsigned long long *dhM = nullptr,
                      double *dPP = nullptr, const double *oP = nullptr, const double *oM = nullptr,
-                     unsigned *cP = nullptr, unsigned *cM = nullptr) {
+                     unsigned *cP = nullptr, unsigned *cM = nullptr, const SelArgs *sel = nullptr) {
   using V = cx<T>;
   const int S = job.S;
   const long long n0 = job.n0;
@@ -2293,7 +2323,7 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
   if ((e = launch<Wct3PrepBody<T>>(c, gx, S, pa))) return e;
   for (V *x : f)
     if ((e = smooth_time<T>(c, x, S, n0, job.N, d_g))) return e;
-  const int rows_out = dRP2 || dRM2 || dPP || cP || cM ? S : maxscale;
+  const int rows_out = dRP2 || dRM2 || dPP || cP || cM || sel ? S : maxscale;
   if (rows_out <= 0) return 0;
   const double *win = (const double *)c->win.p;
   if (K > 64) {
@@ -2310,12 +2340,9 @@ static int wct3_core(cwtb_ctx *c, const Job &job, const T *dy, const T *dx1, con
     K = 1;
   }
   Wct3FinalArgs<T> fa{f[0], f[1], f[2], f[3], f[4], win, dRP2, dRM2, dPP, dmask, dhP, dhM, n0, S, K, maxscale, nbins,
-                      oP, oM, cP, cM};
-  using F16 = Wct3FinalBody<T, 16, 32, 16>;
-  using F64K = Wct3FinalBody<T, 64, 64, 8>;
-  if (K <= 16)
-    return launch<F16>(c, (unsigned)((n0 + F16::CW - 1) / F16::CW), (unsigned)((rows_out + F16::RS - 1) / F16::RS), fa);
-  return launch<F64K>(c, (unsigned)((n0 + F64K::CW - 1) / F64K::CW), (unsigned)((rows_out + F64K::RS - 1) / F64K::RS), fa);
+                      oP, oM, cP, cM, sel ? *sel : SelArgs{}};
+  if (sel) return wct3_final<Wct3FinalBody<T, 16, 32, 16, true>, Wct3FinalBody<T, 64, 64, 8, true>>(c, fa, K, n0, rows_out);
+  return wct3_final<Wct3FinalBody<T, 16, 32, 16>, Wct3FinalBody<T, 64, 64, 8>>(c, fa, K, n0, rows_out);
 }
 
 // the engine precision of T, and host series (double) as device series of type T: the fp32
@@ -2587,10 +2614,10 @@ int cwtb_xwt(cwtb_ctx *c, const double *y1, const double *y2, int64_t n0, double
 // ---- resident products and the reading calls ------------------------------------------------
 static int slot_release(cwtb_ctx *c, ResidentSlot &s) {
   slot_begin(s);
-  if (s.buf.p || s.counts.p) {
+  if (s.buf.p || s.counts.p || s.labels.p) {
     RT(rt_set_device(c->device));
     RT(rt_sync(c->stream));
-    for (Buf *b : {&s.buf, &s.counts}) {
+    for (Buf *b : {&s.buf, &s.counts, &s.labels}) {
       if (b->p) rt_free(b->p);
       *b = Buf{};
     }
@@ -3205,6 +3232,93 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
   return 0;
 }
 
+// ---- cluster labelling ---------------------------------------------------------------------------
+extern "C++" {
+// Labels the selection bitmask c->cl_bits [S][ceil(n0 / 32)] with the per-row weights dq (device,
+// [S]) through ClusterCountBody .. ClusterMaxBody: the largest cluster sum goes to *dqmax (device,
+// zeroed by the caller).  With `tab`, also the table of every cluster and the label image dlabels
+// [S][n0].  The run count is read back to size the run tables: one synchronisation per map.
+static int label_bits(cwtb_ctx *c, int S, long long n0, const unsigned long long *dq, unsigned long long *dqmax,
+                      ClusterTable *tab, int *dlabels) {
+  using CB = ClusterCountBody;
+  ClusterArgs a{};
+  a.bits = (const unsigned *)c->cl_bits.p;
+  a.n = n0;
+  a.words = (n0 + 31) / 32;
+  a.rows = S;
+  a.cpr = (int)((a.words + CB::CHW - 1) / CB::CHW);
+  a.q = dq;
+  a.qmax = dqmax;
+  const size_t nch = (size_t)S * a.cpr;
+  int e = ensure(c, c->cl_hdr, (2 * nch + S + 3) * sizeof(unsigned));
+  if (e) return e;
+  a.chunk = (unsigned *)c->cl_hdr.p;
+  a.chunk_end = a.chunk + nch;
+  a.rowbeg = a.chunk_end + nch;
+  a.total = a.rowbeg + S + 1;
+  if ((e = launch<CB>(c, (unsigned)a.cpr, (unsigned)S, a))) return e;
+  if ((e = launch<ClusterScanBody>(c, 1, 1, a))) return e;
+  unsigned tot[2];
+  RT(rt_d2h(tot, a.total, sizeof tot, c->stream));
+  RT(rt_sync(c->stream));
+  if (tot[0] != tot[1]) return fail(c, CWTB_ERR_STATE, "cluster labelling: the runs' starts and ends differ");
+  const size_t R = tot[0];
+  a.runs = tot[0];
+  // 8-byte sums first: qsum [R] (and pts [R]); then start, end, parent [R] (and rmax, cmin, cmax,
+  // cid [R]) of 4 bytes
+  // grown with half again as much room, so that the units of a Monte-Carlo run, whose run counts
+  // scatter around one value, rarely free and allocate inside the loop
+  const size_t per = tab ? 2 * 8 + 7 * 4 : 8 + 3 * 4, need = std::max<size_t>(R, 1) * per;
+  if (c->cl_runs.bytes < need && (e = ensure(c, c->cl_runs, need + need / 2))) return e;
+  unsigned long long *q64 = (unsigned long long *)c->cl_runs.p;
+  unsigned *u32 = (unsigned *)(q64 + (tab ? 2 : 1) * R);
+  a.qsum = q64;
+  a.start = u32;
+  a.end = u32 + R;
+  a.parent = u32 + 2 * R;
+  if (tab) a.st = ClusterStats{q64 + R, u32 + 3 * R, u32 + 4 * R, u32 + 5 * R};
+  const unsigned gr = (unsigned)((R + NT - 1) / NT);
+  if ((e = launch<ClusterExtractBody>(c, (unsigned)a.cpr, (unsigned)S, a))) return e;
+  if ((e = launch<ClusterUnionBody>(c, gr, 1, a))) return e;
+  if ((e = launch<ClusterSumBody>(c, gr, 1, a))) return e;
+  if ((e = launch<ClusterMaxBody>(c, gr, 1, a))) return e;
+  if (!tab) return 0;
+  // the table: the roots (parent[k] == k) in table order
+  std::vector<unsigned long long> hq(R), hpts(R);
+  std::vector<unsigned> hu(6 * R);
+  if (R) {
+    RT(rt_d2h(hq.data(), a.qsum, R * 8, c->stream));
+    RT(rt_d2h(hpts.data(), a.st.pts, R * 8, c->stream));
+    RT(rt_d2h(hu.data(), u32, 6 * R * 4, c->stream));
+    RT(rt_sync(c->stream));
+  }
+  const unsigned *hs = hu.data(), *hp = hs + 2 * R, *hrm = hs + 3 * R, *hc0 = hs + 4 * R, *hc1 = hs + 5 * R;
+  std::vector<unsigned> roots;
+  for (size_t k = 0; k < R; ++k)
+    if (hp[k] == (unsigned)k) roots.push_back((unsigned)k);
+  std::sort(roots.begin(), roots.end(), [&](unsigned x, unsigned y) {
+    return hq[x] != hq[y] ? hq[x] > hq[y] : hs[x] < hs[y];
+  });
+  ClusterTable t;
+  std::vector<int> cid(std::max<size_t>(R, 1), 0);
+  for (size_t i = 0; i < roots.size(); ++i) {
+    const unsigned r = roots[i];
+    cid[r] = (int)i + 1;
+    t.Q.push_back(hq[r]);
+    t.pts.push_back(hpts[r]);
+    for (long long v : {(long long)(hs[r] / (unsigned long long)n0), (long long)hrm[r] + 1, (long long)hc0[r], (long long)hc1[r]})
+      t.box.push_back(v);
+  }
+  int *dcid = (int *)(u32 + 6 * R);
+  if (R) RT(rt_h2d(dcid, cid.data(), R * sizeof(int), c->stream));
+  ClusterPaintArgs pa{a, dcid, dlabels};
+  if ((e = launch<ClusterPaintBody>(c, (unsigned)((n0 + NT - 1) / NT), (unsigned)S, pa))) return e;
+  RT(rt_sync(c->stream));
+  *tab = std::move(t);
+  return 0;
+}
+}  // extern "C++"
+
 // common part of the Monte-Carlo entry points, for surrogate units of nser = 2 series (coherence,
 // one histogram) or 3 (partial and multiple coherence, hist[0] and hist[1], either may be null):
 // `noise` host surrogates [n_units][nser][n0]; or `phase` groups -> phase-randomised surrogates of
@@ -3214,7 +3328,16 @@ struct PhaseSrc { int group[3]; };
 // the exceedance counters of a counting run (cwtb_coherence*_surrogate_counts) and the observed
 // fields they compare against, per measure: the coherence in [0]; the partial and the multiple
 // coherence in [0] and [1] (either counter may be null)
-struct CountDst { const double *obs[2]; unsigned *cnt[2]; };
+// A cluster test (cwtb_coherence*_cluster_test) adds the selection bits of every unit's map (sel),
+// labelled after the unit's final launch with the per-row weights q; the unit's largest cluster sum
+// goes to qmax[unit - unit0].
+struct CountDst {
+  const double *obs[2];
+  unsigned *cnt[2];
+  SelArgs sel;
+  const unsigned long long *q;
+  unsigned long long *qmax;
+};
 
 extern "C++" {
 // nb surrogate units of the data spectra c->pspec [nser][n0] into out [nb][nser][n0]: rotation,
@@ -3297,12 +3420,16 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
       // kernel runs on c->stream (run_job forks its transforms onto other streams but joins them
       // back and leaves c->cur = c->stream; the smoothing and final launches follow on it), so the
       // final launches of successive units and batches are ordered and never overlap.
+      // The selection bits are written the same way, and labelled on c->stream before the next
+      // unit's final launch writes them again.
       const CountDst k = cd ? *cd : CountDst{};
+      const SelArgs *sel = k.sel.bits ? &k.sel : nullptr;
       e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0],
-                                  k.obs[0], k.cnt[0])
+                                  k.obs[0], k.cnt[0], sel)
                     : wct3_core<T>(c, c->job, a, a + n0, a + 2 * n0, boxcar_len, nullptr, nullptr, dmask, maxscale,
-                                   nbins, dh[0], dh[1], nullptr, k.obs[0], k.obs[1], k.cnt[0], k.cnt[1]);
+                                   nbins, dh[0], dh[1], nullptr, k.obs[0], k.obs[1], k.cnt[0], k.cnt[1], sel);
       if (e) return e;
+      if (sel && (e = label_bits(c, n_scales, n0, k.q, k.qmax + i0 + i, nullptr, nullptr))) return e;
     }
   }
   if ((e = time_end(c, &c->last_ms))) return e;
@@ -3514,6 +3641,214 @@ int cwtb_coherence3_surrogate_counts(cwtb_ctx *c, const double *series, const in
                                      int64_t serial, int reset) {
   return surrogate_counts(c, 3, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
                           boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial, reset);
+}
+
+// ---- cluster tests against surrogates ----------------------------------------------------------
+// The per-row arguments of a cluster test into c->cl_rows: thr [S] double, lo, hi [S] int64, q [S]
+// uint64 (thr, lo, hi null: the test hook, which needs q alone)
+static int cluster_rows(cwtb_ctx *c, const std::string &nm, int S, long long n0, const double *thr, const int64_t *lo,
+                        const int64_t *hi, const uint64_t *q, SelArgs &sel, const unsigned long long *&dq) {
+  if (!q || (!thr && (lo || hi)) || (thr && (!lo || !hi))) return fail(c, CWTB_ERR_ARG, nm + ": null argument");
+  for (int j = 0; j < S; ++j) {
+    if (q[j] > (1ull << 32)) return fail(c, CWTB_ERR_ARG, nm + ": a weight q above 2^32");
+    if (lo && (lo[j] < 0 || hi[j] > n0 || lo[j] > hi[j]))
+      return fail(c, CWTB_ERR_ARG, nm + ": column range outside [0, n0) or lo > hi");
+  }
+  int e = ensure(c, c->cl_rows, (size_t)S * 32);
+  if (e) return e;
+  double *dthr = (double *)c->cl_rows.p;
+  long long *dlo = (long long *)(dthr + S), *dhi = dlo + S;
+  unsigned long long *dq64 = (unsigned long long *)(dhi + S);
+  if (thr) {
+    RT(rt_h2d(dthr, thr, (size_t)S * 8, c->stream));
+    RT(rt_h2d(dlo, lo, (size_t)S * 8, c->stream));
+    RT(rt_h2d(dhi, hi, (size_t)S * 8, c->stream));
+  }
+  RT(rt_h2d(dq64, q, (size_t)S * 8, c->stream));
+  const long long words = (n0 + 31) / 32;
+  if ((e = ensure(c, c->cl_bits, (size_t)S * words * sizeof(unsigned)))) return e;
+  sel = SelArgs{(unsigned *)c->cl_bits.p, dthr, dlo, dhi, words, 0};
+  dq = dq64;
+  return 0;
+}
+
+// a map of S x n0 points labels with 32-bit flat indices, and its sums of q <= 2^32 fit 64 bits
+static int cluster_shape(cwtb_ctx *c, const std::string &nm, long long S, long long n0) {
+  if (S < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, nm + ": bad n_scales / n0");
+  if ((unsigned long long)S * (unsigned long long)n0 >= (1ull << 32))
+    return fail(c, CWTB_ERR_UNSUPPORTED, nm + ": n_scales * n0 must stay below 2^32");
+  return 0;
+}
+
+static int cluster_test(cwtb_ctx *c, int nser, const double *series, const int *group, uint64_t seed,
+                        int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales, int n_scales,
+                        int family, double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                        int64_t *hist_a, int64_t *hist_b, int64_t serial, const double *thr, const int64_t *lo,
+                        const int64_t *hi, const uint64_t *q, int measure, uint64_t *qmax_out) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = nser == 2 ? "coherence_cluster_test" : "coherence3_cluster_test";
+  ResidentSlot &s = nser == 2 ? c->coh : c->coh3;
+  s.clusters = false;   // nothing readable until this call completes
+  s.table = ClusterTable{};
+  if (s.S <= 0 || !s.buf.p || serial != s.serial)
+    return fail(c, CWTB_ERR_STATE, nm + ": the serial is not that of the resident product");
+  if (n_scales != s.S || n0 != s.n0)
+    return fail(c, CWTB_ERR_STATE, nm + ": scales or length differ from the resident product's");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, nm + " needs an analytic wavelet family");
+  if (!mask || !(hist_a || hist_b) || !thr || (n_units > 0 && !qmax_out))
+    return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  int e = cluster_shape(c, nm, n_scales, n0);
+  if (e) return e;
+  FieldRef f;
+  if ((e = nser == 2 ? field_ref(c, FIELD_COH, f) : coh3_ref(c, measure, false, f))) return e;
+  PhaseSrc ph{};
+  if ((e = phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &ph))) return e;
+  SelArgs sel;
+  const unsigned long long *dq;
+  if ((e = cluster_rows(c, nm, n_scales, n0, thr, lo, hi, q, sel, dq))) return e;
+  sel.measure = measure == CWTB_MEASURE_MULTIPLE ? 1 : 0;
+  if ((e = ensure(c, c->cl_qmax, (size_t)(n_units + 1) * sizeof(unsigned long long)))) return e;
+  if ((e = ensure(c, s.labels, (size_t)n_scales * n0 * sizeof(int)))) return e;
+  unsigned long long *dqmax = (unsigned long long *)c->cl_qmax.p;
+  RT(rt_memset(dqmax, 0, (size_t)(n_units + 1) * sizeof(unsigned long long), c->stream));
+  // the observed map: its bits through the field layer, then the same labelling as the units'
+  ThreshBitsArgs ta{(const double *)f.p, sel, n0};
+  if ((e = launch<ThreshBitsBody>(c, (unsigned)((n0 + NT - 1) / NT), (unsigned)n_scales, ta))) return e;
+  ClusterTable tab;
+  if ((e = label_bits(c, n_scales, n0, dq, dqmax + n_units, &tab, (int *)s.labels.p))) return e;
+  // the units: the final kernels write whole chunks of columns, so the bits past the last column
+  // stay as zeroed here
+  RT(rt_memset(sel.bits, 0, (size_t)n_scales * sel.words * sizeof(unsigned), c->stream));
+  CountDst cd{};
+  cd.sel = sel;
+  cd.q = dq;
+  cd.qmax = dqmax;
+  int64_t *const h[2] = {hist_a, hist_b};
+  if ((e = mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                   boxcar_len, mask, maxscale, nbins, h, &cd)))
+    return e;
+  if (n_units > 0) RT(rt_d2h(qmax_out, dqmax, (size_t)n_units * sizeof(unsigned long long), c->stream));
+  RT(rt_sync(c->stream));
+  s.table = std::move(tab);
+  s.clusters = true;
+  return 0;
+}
+
+int cwtb_coherence_cluster_test(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
+                                int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                int maxscale, int nbins, int64_t *hist, int64_t serial, const double *thr,
+                                const int64_t *lo, const int64_t *hi, const uint64_t *q, uint64_t *qmax_out) {
+  return cluster_test(c, 2, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                      boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, thr, lo, hi, q, 0, qmax_out);
+}
+
+int cwtb_coherence3_cluster_test(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
+                                 int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                 int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                 int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
+                                 int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
+                                 const uint64_t *q, int measure, uint64_t *qmax_out) {
+  return cluster_test(c, 3, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                      boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial, thr, lo, hi, q,
+                      measure, qmax_out);
+}
+
+// the first min(cap, count) rows of a table
+static int table_out(cwtb_ctx *c, const ClusterTable &t, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                     int64_t *box) {
+  if (!count || cap < 0) return fail(c, CWTB_ERR_ARG, "cluster table: bad argument");
+  const size_t m = std::min<size_t>((size_t)cap, t.Q.size());
+  if (m && (!Q || !points || !box)) return fail(c, CWTB_ERR_ARG, "cluster table: null argument");
+  *count = (int64_t)t.Q.size();
+  for (size_t i = 0; i < m; ++i) {
+    Q[i] = t.Q[i];
+    points[i] = (int64_t)t.pts[i];
+  }
+  if (m) memcpy(box, t.box.data(), m * 4 * sizeof(int64_t));
+  return 0;
+}
+
+static int clusters_of(cwtb_ctx *c, ResidentSlot &s, const char *what) {
+  if (!c) return CWTB_ERR_ARG;
+  if (s.S <= 0 || !s.buf.p) return fail(c, CWTB_ERR_STATE, std::string("no ") + what + " resident");
+  if (!s.clusters) return fail(c, CWTB_ERR_STATE, "no cluster test has run for this product");
+  RT(rt_set_device(c->device));
+  return 0;
+}
+
+int cwtb_coherence_cluster_table(cwtb_ctx *c, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                                 int64_t *box) {
+  int e = c ? clusters_of(c, c->coh, "coherence") : CWTB_ERR_ARG;
+  return e ? e : table_out(c, c->coh.table, cap, count, Q, points, box);
+}
+
+int cwtb_coherence3_cluster_table(cwtb_ctx *c, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                                  int64_t *box) {
+  int e = c ? clusters_of(c, c->coh3, "partial / multiple coherence") : CWTB_ERR_ARG;
+  return e ? e : table_out(c, c->coh3.table, cap, count, Q, points, box);
+}
+
+// labels[row0 + r row_step][col0 + k col_step] into out [nrows][ncols], with window_run's checks
+static int labels_window(cwtb_ctx *c, const ResidentSlot &s, int row0, int nrows, int row_step, int64_t col0,
+                         int64_t ncols, int64_t col_step, int32_t *out) {
+  const int S = s.S;
+  const long long n0 = s.n0;
+  if (nrows < 0 || ncols < 0 || row_step < 1 || col_step < 1) return fail(c, CWTB_ERR_ARG, "bad window");
+  if (nrows == 0 || ncols == 0) return 0;
+  if (!out) return fail(c, CWTB_ERR_ARG, "null argument");
+  if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
+      col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
+    return fail(c, CWTB_ERR_ARG, "window outside the resident field");
+  const size_t m = (size_t)nrows * ncols;
+  int e = ensure(c, c->aux, m * sizeof(int));
+  if (e) return e;
+  LabelWindowArgs a{(const int *)s.labels.p, (int *)c->aux.p, n0, row0, row_step, col0, col_step, ncols};
+  if ((e = launch<LabelWindowBody>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a))) return e;
+  RT(rt_d2h(out, c->aux.p, m * sizeof(int), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+int cwtb_coherence_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                                  int64_t col_step, int32_t *out) {
+  int e = c ? clusters_of(c, c->coh, "coherence") : CWTB_ERR_ARG;
+  return e ? e : labels_window(c, c->coh, row0, nrows, row_step, col0, ncols, col_step, out);
+}
+
+int cwtb_coherence3_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                                   int64_t col_step, int32_t *out) {
+  int e = c ? clusters_of(c, c->coh3, "partial / multiple coherence") : CWTB_ERR_ARG;
+  return e ? e : labels_window(c, c->coh3, row0, nrows, row_step, col0, ncols, col_step, out);
+}
+
+int cwtb_cluster_label_bits(cwtb_ctx *c, const uint32_t *bits, int n_scales, int64_t n0, const uint64_t *q,
+                            int64_t cap, int64_t *count, uint64_t *Q, int64_t *points, int64_t *box,
+                            int32_t *labels, uint64_t *qmax) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = "cluster_label_bits";
+  int e = cluster_shape(c, nm, n_scales, n0);
+  if (e) return e;
+  if (!bits || !qmax || !count) return fail(c, CWTB_ERR_ARG, nm + ": null argument");
+  const long long words = (n0 + 31) / 32;
+  if (n0 % 32)
+    for (int j = 0; j < n_scales; ++j)
+      if (bits[(size_t)j * words + words - 1] >> (n0 % 32))
+        return fail(c, CWTB_ERR_ARG, nm + ": bits set past the last column");
+  RT(rt_set_device(c->device));
+  SelArgs sel;
+  const unsigned long long *dq;
+  if ((e = cluster_rows(c, nm, n_scales, n0, nullptr, nullptr, nullptr, q, sel, dq))) return e;
+  RT(rt_h2d(sel.bits, bits, (size_t)n_scales * words * sizeof(unsigned), c->stream));
+  if ((e = ensure(c, c->cl_qmax, sizeof(unsigned long long)))) return e;
+  if ((e = ensure(c, c->scratch, (size_t)n_scales * n0 * sizeof(int)))) return e;
+  RT(rt_memset(c->cl_qmax.p, 0, sizeof(unsigned long long), c->stream));
+  ClusterTable t;
+  if ((e = label_bits(c, n_scales, n0, dq, (unsigned long long *)c->cl_qmax.p, &t, (int *)c->scratch.p))) return e;
+  RT(rt_d2h(qmax, c->cl_qmax.p, sizeof(unsigned long long), c->stream));
+  if (labels) RT(rt_d2h(labels, c->scratch.p, (size_t)n_scales * n0 * sizeof(int), c->stream));
+  RT(rt_sync(c->stream));
+  return table_out(c, t, cap, count, Q, points, box);
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

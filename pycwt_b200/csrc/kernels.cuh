@@ -1809,6 +1809,67 @@ template <typename T> struct BoxcarBody {
   }
 };
 
+// ---- selection bits of the cluster test (cwtb_coherence*_cluster_test) -------------------------
+// Point (j, n) of a map R is selected where R[j, n] is finite, R[j, n] > thr[j] (a NaN thr selects
+// nothing) and lo[j] <= n < hi[j].  The selection of a map is a bitmask [rows][words] of uint32,
+// words = ceil(n / 32): column n is bit n % 32 of word n / 32, the bits past the last column are 0.
+struct SelArgs {
+  unsigned *bits;           // [rows][words], or null: no selection wanted
+  const double *thr;        // [rows]
+  const long long *lo, *hi; // [rows]
+  long long words;
+  int measure;              // Wct3FinalBody: the measure selected (0 partial, 1 multiple)
+};
+HD bool cluster_sel(const SelArgs &s, int row, long long n, double r) {
+  return isfinite(r) && r > s.thr[row] && n >= s.lo[row] && n < s.hi[row];
+}
+// The lanes of a warp whose column lies below n_valid, for warps whose lanes hold chunks of cw
+// consecutive columns (lane l: column c0 + l % cw, c0 a multiple of cw), cw in {8, 16, 32}
+HD unsigned sel_lanes(int cw, long long n_valid) {
+  const unsigned c = n_valid >= cw ? (cw == 32 ? ~0u : (1u << cw) - 1u) : (1u << n_valid) - 1u;
+  unsigned m = 0;
+  for (int h = 0; h < 32; h += cw) m |= c << h;
+  return m;
+}
+// Selection bit p of (row, n) into s.bits.  On the device the lanes `lanes` (sel_lanes) vote and
+// the first lane of each chunk stores its cw bits as one 8-, 16- or 32-bit word at byte n / 8: one
+// writer per chunk, no atomics.  The emulation build sets or clears the bit itself.  A lane of a
+// row < 0 votes and stores nothing.
+HD void sel_store(const SelArgs &s, int row, long long n, int cw, bool p, unsigned lanes) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  const unsigned b = __ballot_sync(lanes, p);
+  if (row >= 0 && (n & (cw - 1)) == 0) {
+    const unsigned v = b >> ((threadIdx.x & 31) & ~(unsigned)(cw - 1));
+    unsigned char *dst = (unsigned char *)(s.bits + (size_t)row * s.words) + (n >> 3);
+    if (cw == 32) *(unsigned *)dst = v;
+    else if (cw == 16) *(unsigned short *)dst = (unsigned short)v;
+    else *dst = (unsigned char)v;
+  }
+#else
+  (void)cw;
+  (void)lanes;
+  if (row < 0) return;
+  unsigned &w = s.bits[(size_t)row * s.words + (n >> 5)];
+  const unsigned bit = 1u << (n & 31);
+  w = p ? (w | bit) : (w & ~bit);
+#endif
+}
+
+// ---- Body: selection bits of a resident double field (the observed map of a cluster test) -------
+// One thread per column of row by; a warp's lanes are 32 aligned columns.
+struct ThreshBitsArgs { const double *R; SelArgs sel; long long n; };
+struct ThreshBitsBody {
+  using Args = ThreshBitsArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long n0 = (long long)bx * NT + (tid & ~31), n = n0 + (tid & 31);
+    if (n0 >= a.n) return;   // the whole warp
+    const bool p = n < a.n && cluster_sel(a.sel, by, n, ld_stream(&a.R[(size_t)by * a.n + n]));
+    sel_store(a.sel, by, n, 32, p, ~0u);
+  }
+};
+
 // ---- Body: coherence  WCT = |S12|^2 / (S1 S2)  after the scale boxcar; optional histogram
 // of floor(WCT * nbins) over masked points (wavelet.py:513, 624-630) ---------------------
 // Fields, staging and sums in the engine type T; WCT is written (and binned) as double.
@@ -1825,6 +1886,7 @@ template <typename T> struct WctFinalArgs {
   int rows, K, maxscale, nbins;
   const double *obs;        // observed WCT [rows][n] (the resident coherence), with cnt
   unsigned *cnt;            // exceedance counters [rows][n], or null
+  SelArgs sel;              // selection bits of every row (the SEL instantiation)
 };
 // One surrogate value r2 against the observed value at point o: an exceedance where r2 >= obs or
 // r2 is not finite (the conservative choice).  No atomics: within a launch every point belongs to
@@ -1836,7 +1898,9 @@ HD void count_exceed(unsigned *cnt, const double *obs, size_t o, double r2) {
 // time-smoothed fields for these columns in shared memory (each input element is read from global
 // memory (RS + K - 1) / RS times instead of K times); in phase 1 a thread produces 4 consecutive
 // rows of one column, so every staged value feeds up to four accumulators.
-template <typename T, int KMAX_> struct WctFinalBody {
+// SEL: the instantiation that writes selection bits (a.sel); the others ignore a.sel, so their code
+// is that of a kernel without them.
+template <typename T, int KMAX_, bool SEL = false> struct WctFinalBody {
   using Args = WctFinalArgs<T>;
   using V = cx<T>;
   static constexpr int NPHASE = 2;
@@ -1850,8 +1914,8 @@ template <typename T, int KMAX_> struct WctFinalBody {
     T *sw = (T *)(sx + (size_t)(RS + KMAX - 1) * CW);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    // Monte-Carlo mode without counting: rows below maxscale only
-    const int rows_out = a.WCT || a.cnt ? a.rows : a.maxscale;
+    // Monte-Carlo mode without counting or selection bits: rows below maxscale only
+    const int rows_out = SEL || a.WCT || a.cnt ? a.rows : a.maxscale;
     if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
@@ -1896,6 +1960,8 @@ template <typename T, int KMAX_> struct WctFinalBody {
           const size_t o = (size_t)i * a.n + n;
           if (a.WCT) a.WCT[o] = r2;
           if (a.cnt) count_exceed(a.cnt, a.obs, o, r2);
+          // a warp's lanes are the CW = 32 columns of one row here (rows_out = rows: no lane breaks)
+          if constexpr (SEL) sel_store(a.sel, i, n, CW, cluster_sel(a.sel, i, n, r2), sel_lanes(CW, a.n - n0));
           if (a.hist && i < a.maxscale && a.mask[o] && r2 == r2) {
             int bin = (int)floor(r2 * a.nbins);
             bin = bin < 0 ? 0 : (bin >= a.nbins ? a.nbins - 1 : bin);
@@ -1969,6 +2035,7 @@ template <typename T> struct Wct3FinalArgs {
   int rows, K, maxscale, nbins;
   const double *obsP, *obsM;             // observed RP2 / RM2 [rows][n], with the counters
   unsigned *cntP, *cntM;                 // exceedance counters [rows][n], either may be null
+  SelArgs sel;                           // selection bits of sel.measure, every row (SEL)
 };
 // one count for R2 in its row's histogram; non-finite R2 is skipped before any conversion to int
 HD void hist_count(unsigned long long *hist, int row, int nbins, double r2) {
@@ -1981,7 +2048,8 @@ HD void hist_count(unsigned long long *hist, int row, int nbins, double r2) {
   hist[(size_t)row * nbins + bin] += 1ull;
 #endif
 }
-template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
+// SEL: as WctFinalBody's, for the measure a.sel.measure
+template <typename T, int KMAX_, int RS_, int CW_, bool SEL = false> struct Wct3FinalBody {
   using Args = Wct3FinalArgs<T>;
   using V = cx<T>;
   static constexpr int NPHASE = 2;
@@ -1996,7 +2064,7 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
     double *sw = (double *)(st + NF * PLANE);
     const int i0 = by * RS;
     const long long n0 = (long long)bx * CW;
-    const int rows_out = a.RP2 || a.RM2 || a.PP || a.cntP || a.cntM ? a.rows : a.maxscale;
+    const int rows_out = SEL || a.RP2 || a.RM2 || a.PP || a.cntP || a.cntM ? a.rows : a.maxscale;
     if (i0 >= rows_out) return;
     const int qlo = i0 + off - K + 1;
     if constexpr (PH == 0) {
@@ -2046,6 +2114,7 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
           }
         }
       }
+      unsigned selp = 0;   // bit e: row i0 + RG grp + e selected
 #pragma unroll
       for (int e = 0; e < RG; ++e) {
         const int i = i0 + RG * grp + e;
@@ -2058,22 +2127,35 @@ template <typename T, int KMAX_, int RS_, int CW_> struct Wct3FinalBody {
         const double d12 = S1 * S2 - (S12.x * S12.x + S12.y * S12.y);
         const size_t o = (size_t)i * a.n + n;
         const bool binned = (a.histP || a.histM) && i < a.maxscale && a.mask[o];
-        if (a.RP2 || a.PP || (a.histP && binned) || a.cntP) {
+        const bool selP = SEL && a.sel.measure == 0, selM = SEL && a.sel.measure != 0;
+        if (a.RP2 || a.PP || (a.histP && binned) || a.cntP || selP) {
           const double2 u = csub(cscale(Sy1, S2), cmul(Sy2, cconj(S12)));
-          if (a.RP2 || (a.histP && binned) || a.cntP) {
+          if (a.RP2 || (a.histP && binned) || a.cntP || selP) {
             const double rp = (u.x * u.x + u.y * u.y) / ((Sy * S2 - ny2) * d12);
             if (a.RP2) a.RP2[o] = rp;
             if (a.histP && binned) hist_count(a.histP, i, a.nbins, rp);
             if (a.cntP) count_exceed(a.cntP, a.obsP, o, rp);
+            if (selP && cluster_sel(a.sel, i, n, rp)) selp |= 1u << e;
           }
           if (a.PP) a.PP[o] = u.x == 0.0 && u.y == 0.0 ? 0.0 : atan2(u.y, u.x);
         }
-        if (a.RM2 || (a.histM && binned) || a.cntM) {
+        if (a.RM2 || (a.histM && binned) || a.cntM || selM) {
           const double2 z = cmul(cmul(Sy1, S12), cconj(Sy2));
           const double rm = (S2 * ny1 + S1 * ny2 - 2.0 * z.x) / (Sy * d12);
           if (a.RM2) a.RM2[o] = rm;
           if (a.histM && binned) hist_count(a.histM, i, a.nbins, rm);
           if (a.cntM) count_exceed(a.cntM, a.obsM, o, rm);
+          if (selM && cluster_sel(a.sel, i, n, rm)) selp |= 1u << e;
+        }
+      }
+      // The selection bits after the row loop: a warp holds 32 / CW groups, and a group past the
+      // last row has left that loop early.  Every lane with a column votes for every e.
+      if constexpr (SEL) {
+        const unsigned lanes = sel_lanes(CW, a.n - n0);
+#pragma unroll
+        for (int e = 0; e < RG; ++e) {
+          const int i = i0 + RG * grp + e;
+          sel_store(a.sel, i < a.rows ? i : -1, n, CW, (selp >> e) & 1u, lanes);
         }
       }
     }
@@ -2561,6 +2643,360 @@ template <bool SHARED> struct CountHistBody {
 #endif
         }
     }
+  }
+};
+
+// ---- cluster labelling of a selection bitmask (cwtb_coherence*_cluster_test) --------------------
+// Clusters are the 8-connected components of the set bits of a bitmask [rows][words] (SelArgs'
+// layout, n columns, rows * n < 2^32 so that a point's flat index j n + col fits 32 bits).  The
+// labelling works on runs, the maximal horizontal stretches of set bits of a row:
+//   ClusterCountBody    CTA (chunk, j): the runs that start and end in a chunk of CHW words of row j
+//   ClusterScanBody     one CTA: exclusive offsets of the chunks, the runs of every row, the total
+//   (the host reads the total and sizes the run tables from it)
+//   ClusterExtractBody  CTA (chunk, j): run k's first point start[k] and end[k] (one past its last),
+//                       flat indices in row-major order, its parent k and its sums zeroed
+//   ClusterUnionBody    thread per run: unions with every run of the row above whose columns reach
+//                       [start - 1, end] (8-connectivity; time is not circular)
+//   ClusterSumBody      thread per run: q_j * length (and, for a table, the point count and the box)
+//                       into its root's sums
+//   ClusterMaxBody      the largest root sum into qmax[unit]
+// Union-find: a union links the larger of two roots to the smaller with a compare-and-swap, so the
+// root of a cluster is its smallest run, the run of its first point in row-major order, whatever
+// order the unions run in.  find() halves paths with plain stores: a non-root is never the target
+// of a link, and every value stored is an ancestor of the node.
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+HD unsigned uf_find(unsigned *parent, unsigned x) {
+  volatile unsigned *p = parent;
+  unsigned y = p[x];
+  while (y != x) {
+    const unsigned z = p[y];
+    if (z != y) p[x] = z;
+    x = y;
+    y = z;
+  }
+  return x;
+}
+#else
+HD unsigned uf_find(unsigned *p, unsigned x) {
+  while (p[x] != x) {
+    if (p[p[x]] != p[x]) p[x] = p[p[x]];
+    x = p[x];
+  }
+  return x;
+}
+#endif
+HD void uf_union(unsigned *parent, unsigned a, unsigned b) {
+  for (;;) {
+    a = uf_find(parent, a);
+    b = uf_find(parent, b);
+    if (a == b) return;
+    if (a < b) { const unsigned t = a; a = b; b = t; }
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+    if (atomicCAS(&parent[a], a, b) == a) return;
+#else
+    parent[a] = b;
+    return;
+#endif
+  }
+}
+HD void atomic_add_u64(unsigned long long *p, unsigned long long v) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  atomicAdd(p, v);
+#else
+  *p += v;
+#endif
+}
+HD void atomic_max_u64(unsigned long long *p, unsigned long long v) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  atomicMax(p, v);
+#else
+  if (v > *p) *p = v;
+#endif
+}
+HD void atomic_max_u32(unsigned *p, unsigned v) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  atomicMax(p, v);
+#else
+  if (v > *p) *p = v;
+#endif
+}
+HD void atomic_min_u32(unsigned *p, unsigned v) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  atomicMin(p, v);
+#else
+  if (v < *p) *p = v;
+#endif
+}
+HD int popc32(unsigned x) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  return __popc(x);
+#else
+  return __builtin_popcount(x);
+#endif
+}
+HD int ffs32(unsigned x) {   // index of the lowest set bit, x != 0
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  return __ffs(x) - 1;
+#else
+  return __builtin_ctz(x);
+#endif
+}
+
+// The per-cluster sums of a table (the observed map and the test hook): point count, last row,
+// first column and one past the last column; the first row is the root's.
+struct ClusterStats {
+  unsigned long long *pts;
+  unsigned *rmax, *cmin, *cmax;
+};
+struct ClusterArgs {
+  const unsigned *bits;       // [rows][words]
+  long long n, words;
+  int rows, cpr;              // cpr: chunks per row
+  unsigned *chunk;            // [rows cpr]: packed counts (starts << 16 | ends), then start offsets
+  unsigned *chunk_end;        // [rows cpr]: end offsets
+  unsigned *rowbeg;           // [rows + 1]: first run of each row; rowbeg[rows] = runs
+  unsigned *total;            // [2]: runs counted by starts and by ends
+  unsigned *start, *end, *parent;   // [runs]
+  unsigned long long *qsum;         // [runs]: root sums of q_j * length
+  const unsigned long long *q;      // [rows]: the weight of a point of each row
+  ClusterStats st;                  // pts null: no table
+  unsigned long long *qmax;         // the unit's maximum
+  unsigned runs;
+};
+// The run starts and ends of word w of row j, as bit sets (bits past the row's end are 0)
+HD void run_bits(const ClusterArgs &a, int j, long long w, unsigned &st, unsigned &en) {
+  const unsigned *r = a.bits + (size_t)j * a.words;
+  const unsigned m = r[w];
+  const unsigned prev = w > 0 ? r[w - 1] >> 31 : 0u;
+  const unsigned next = w + 1 < a.words ? r[w + 1] & 1u : 0u;
+  st = m & ~((m << 1) | prev);
+  en = m & ~((m >> 1) | (next << 31));
+}
+struct ClusterCountBody {
+  using Args = ClusterArgs;
+  static constexpr int NPHASE = 2, WPT = 8;
+  static constexpr long long CHW = (long long)WPT * NT;   // words per chunk
+  // a chunk holds at most 16 CHW run starts (an alternating mask) and as many ends: each count has 16 bits
+  static_assert(16 * CHW < 65536, "ClusterCountBody: the packed run counts of a chunk need 16 * CHW < 2^16");
+  static constexpr size_t SMEM = NT * sizeof(unsigned);
+  // the packed start / end counts of this thread's words of chunk bx of row by
+  HD static unsigned count(const Args &a, int bx, int by, int tid) {
+    const long long w0 = (long long)bx * CHW + (long long)tid * WPT;
+    unsigned c = 0;
+    for (long long w = w0; w < w0 + WPT && w < a.words; ++w) {
+      unsigned st, en;
+      run_bits(a, by, w, st, en);
+      c += ((unsigned)popc32(st) << 16) | (unsigned)popc32(en);
+    }
+    return c;
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    unsigned *sh = (unsigned *)smraw;
+    if constexpr (PH == 0) {
+      sh[tid] = count(a, bx, by, tid);
+    } else if (tid == 0) {
+      unsigned c = 0;
+      for (int t = 0; t < NT; ++t) c += sh[t];
+      a.chunk[(size_t)by * a.cpr + bx] = c;
+    }
+  }
+};
+// One CTA.  Thread t scans the chunks [t G, (t + 1) G), G = ceil(chunks / NT).
+struct ClusterScanBody {
+  using Args = ClusterArgs;
+  static constexpr int NPHASE = 3;
+  static constexpr size_t SMEM = 2 * NT * sizeof(unsigned);
+  template <int PH> HD static void phase(const Args &a, int, int, int tid, void *smraw) {
+    unsigned *ss = (unsigned *)smraw, *se = ss + NT;
+    const long long nch = (long long)a.rows * a.cpr, G = (nch + NT - 1) / NT;
+    const long long c0 = tid * G, c1 = c0 + G < nch ? c0 + G : nch;
+    if constexpr (PH == 0) {
+      unsigned s = 0, e = 0;
+      for (long long c = c0; c < c1; ++c) {
+        s += a.chunk[c] >> 16;
+        e += a.chunk[c] & 0xFFFFu;
+      }
+      ss[tid] = s;
+      se[tid] = e;
+    } else if constexpr (PH == 1) {
+      if (tid == 0) {
+        unsigned s = 0, e = 0;
+        for (int t = 0; t < NT; ++t) {
+          const unsigned ts = ss[t], te = se[t];
+          ss[t] = s;
+          se[t] = e;
+          s += ts;
+          e += te;
+        }
+        a.total[0] = s;
+        a.total[1] = e;
+        a.rowbeg[a.rows] = s;
+      }
+    } else {
+      unsigned s = ss[tid], e = se[tid];
+      for (long long c = c0; c < c1; ++c) {
+        const unsigned v = a.chunk[c];
+        if (c % a.cpr == 0) a.rowbeg[c / a.cpr] = s;
+        a.chunk[c] = s;
+        a.chunk_end[c] = e;
+        s += v >> 16;
+        e += v & 0xFFFFu;
+      }
+    }
+  }
+};
+struct ClusterExtractBody {
+  using Args = ClusterArgs;
+  using CB = ClusterCountBody;
+  static constexpr int NPHASE = 3;
+  static constexpr size_t SMEM = NT * sizeof(unsigned);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    unsigned *sh = (unsigned *)smraw;
+    if constexpr (PH == 0) {
+      sh[tid] = CB::count(a, bx, by, tid);
+    } else if constexpr (PH == 1) {
+      if (tid == 0) {
+        unsigned c = 0;
+        for (int t = 0; t < NT; ++t) {
+          const unsigned v = sh[t];
+          sh[t] = c;
+          c += v;
+        }
+      }
+    } else {
+      const size_t ci = (size_t)by * a.cpr + bx;
+      unsigned ks = a.chunk[ci] + (sh[tid] >> 16), ke = a.chunk_end[ci] + (sh[tid] & 0xFFFFu);
+      const long long w0 = (long long)bx * CB::CHW + (long long)tid * CB::WPT;
+      const unsigned base = (unsigned)((unsigned long long)by * (unsigned long long)a.n);
+      for (long long w = w0; w < w0 + CB::WPT && w < a.words; ++w) {
+        unsigned st, en;
+        run_bits(a, by, w, st, en);
+        for (; st; st &= st - 1, ++ks) {
+          a.start[ks] = base + (unsigned)(32 * w + ffs32(st));
+          a.parent[ks] = ks;
+          a.qsum[ks] = 0ull;
+          if (a.st.pts) {
+            a.st.pts[ks] = 0ull;
+            a.st.rmax[ks] = 0u;
+            a.st.cmin[ks] = 0xFFFFFFFFu;
+            a.st.cmax[ks] = 0u;
+          }
+        }
+        for (; en; en &= en - 1, ++ke) a.end[ke] = base + (unsigned)(32 * w + ffs32(en)) + 1u;
+      }
+    }
+  }
+};
+// the row of run k (rowbeg is sorted: the last row whose first run is <= k)
+HD int run_row(const ClusterArgs &a, unsigned k) {
+  int lo = 0, hi = a.rows - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (a.rowbeg[mid] <= k) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+struct ClusterUnionBody {
+  using Args = ClusterArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const unsigned long long k = (unsigned long long)bx * NT + tid;
+    if (k >= a.runs) return;
+    const int j = run_row(a, (unsigned)k);
+    if (j == 0) return;
+    const unsigned n = (unsigned)a.n;
+    // in row j - 1: the runs p with end[p] >= s and start[p] <= e, s = start - 1 col, e = end col
+    const unsigned s = a.start[k] - n, e = a.end[k] - n;
+    unsigned lo = a.rowbeg[j - 1], hi = a.rowbeg[j];
+    while (lo < hi) {   // the first run of row j - 1 with end >= s
+      const unsigned mid = lo + (hi - lo) / 2;
+      if (a.end[mid] < s) lo = mid + 1;
+      else hi = mid;
+    }
+    for (unsigned p = lo; p < a.rowbeg[j] && a.start[p] <= e; ++p) uf_union(a.parent, (unsigned)k, p);
+  }
+};
+struct ClusterSumBody {
+  using Args = ClusterArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const unsigned long long k = (unsigned long long)bx * NT + tid;
+    if (k >= a.runs) return;
+    const unsigned r = uf_find(a.parent, (unsigned)k);
+    const int j = run_row(a, (unsigned)k);
+    const unsigned len = a.end[k] - a.start[k];
+    atomic_add_u64(&a.qsum[r], a.q[j] * len);
+    if (a.st.pts) {
+      const unsigned c0 = a.start[k] - (unsigned)j * (unsigned)a.n;
+      atomic_add_u64(&a.st.pts[r], len);
+      atomic_max_u32(&a.st.rmax[r], (unsigned)j);
+      atomic_min_u32(&a.st.cmin[r], c0);
+      atomic_max_u32(&a.st.cmax[r], c0 + len);
+      a.parent[k] = r;   // a find of another thread may store an ancestor over r: not a flat forest
+    }
+  }
+};
+struct ClusterMaxBody {
+  using Args = ClusterArgs;
+  static constexpr int NPHASE = 2;
+  static constexpr size_t SMEM = NT * sizeof(unsigned long long);
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *smraw) {
+    unsigned long long *sh = (unsigned long long *)smraw;
+    if constexpr (PH == 0) {
+      const unsigned long long k = (unsigned long long)bx * NT + tid;
+      sh[tid] = k < a.runs && a.parent[k] == (unsigned)k ? a.qsum[k] : 0ull;
+    } else if (tid == 0) {
+      unsigned long long m = 0;
+      for (int t = 0; t < NT; ++t) m = sh[t] > m ? sh[t] : m;
+      if (m) atomic_max_u64(a.qmax, m);
+    }
+  }
+};
+// ---- Body: the label image [rows][n] int32 of a labelled bitmask: 0 off the clusters, else
+// cid[root of the point's run] (the table rank + 1) ----------------------------------------------
+struct ClusterPaintArgs { ClusterArgs c; const int *cid; int *labels; };
+struct ClusterPaintBody {
+  using Args = ClusterPaintArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const ClusterArgs &c = a.c;
+    const long long n = (long long)bx * NT + tid;
+    if (n >= c.n) return;
+    const size_t o = (size_t)by * c.n + n;
+    int lab = 0;
+    if ((c.bits[(size_t)by * c.words + (n >> 5)] >> (n & 31)) & 1u) {
+      unsigned lo = c.rowbeg[by], hi = c.rowbeg[by + 1] - 1;   // the last run of the row starting <= o
+      while (lo < hi) {
+        const unsigned mid = lo + (hi - lo + 1) / 2;
+        if (c.start[mid] <= (unsigned)o) lo = mid;
+        else hi = mid - 1;
+      }
+      lab = a.cid[uf_find(c.parent, lo)];
+    }
+    a.labels[o] = lab;
+  }
+};
+
+// ---- Body: strided window of an int32 image [rows][n] (the cluster labels) -------------------------
+struct LabelWindowArgs {
+  const int *in;
+  int *out;            // [nrows][ncols]
+  long long n;
+  int row0, row_step;
+  long long col0, col_step, ncols;
+};
+struct LabelWindowBody {
+  using Args = LabelWindowArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long k = (long long)bx * NT + tid;
+    if (k >= a.ncols) return;
+    a.out[(size_t)by * a.ncols + k] = a.in[(size_t)(a.row0 + (long long)by * a.row_step) * a.n + a.col0 + k * a.col_step];
   }
 };
 

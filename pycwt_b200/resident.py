@@ -33,7 +33,7 @@ from .wavelet import (_check_parameter_wavelet, _coi, _mc_levels, _nan_rows, _pr
 
 __all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence',
            'xwt_resident', 'ResidentCrossWavelet', 'wct3_resident', 'ResidentCoherence3',
-           'FdrResult']
+           'FdrResult', 'ClusterResult']
 
 
 def _coi_ranges(wavelet, dt, n0, period):
@@ -376,24 +376,88 @@ def _fdr(hist, M, q, method):
     return FdrResult(float(p[top]), int(rank[top]), m)
 
 
+# ---- cluster tests against phase-randomised surrogates -------------------------------------------
+# `cluster_test(sig, mc_count=M, seed=s)` selects the points with a finite R > sig[j] (inside the
+# cone of influence by default) in the resident map and in the map of each surrogate unit 0 .. M - 1
+# of `surrogate_significance(mc_count=M, seed=s)`, labels the 8-connected clusters of each on the
+# device and weighs a cluster by its area normalised by the reproducing kernel's width,
+# A = sum dj dt / s_j over its points.  Exactly: a point of row j weighs the integer
+# q_j = floor(2^32 s_min / s_j + 1/2) (double arithmetic), Q = sum q_j in uint64, and
+# A = (dj dt / s_min) Q / 2^32.  p_c = (1 + #{u : Qmax_u >= Q_c}) / (1 + M), Qmax_u the largest Q of
+# unit u (0 without clusters): the max-statistic test, which controls the family-wise error over
+# the clusters (Nichols & Holmes 2002; Maris & Oostenveld 2007).
+
+ClusterResult = collections.namedtuple('ClusterResult', 'area points rows cols pvalue null_max')
+
+
+def _cluster_weights(h):
+    """(q uint64 [S], the area of one unit of Q)."""
+    sj = np.asarray(h.scales, dtype=float)
+    smin = sj.min()
+    q = np.floor(2.0 ** 32 * smin / sj + 0.5).astype(np.uint64)
+    return q, h.dj * h.dt / smin / 2.0 ** 32
+
+
 class _SurrogateTest(object):
-    """The point-wise test of a resident coherence product: the counts of its last
-    `surrogate_test` and what is read from them.  A subclass names its measures (`_MEASURE_OF`:
-    None for the coherence)."""
+    """The point-wise and cluster tests of a resident coherence product: the counts of its last
+    `surrogate_test`, the clusters of its last `cluster_test`, and what is read from them.  A
+    subclass names its measures (`_MEASURE_OF`: None for the coherence) and whether its product is
+    the engine's partial and multiple coherence (`_TRIPLE`), whose clusters the engine keeps apart
+    from the coherence's."""
 
     _UNTESTED = ("no surrogate test has counted for this product: call surrogate_test first")
     surrogate_seed = None     # seed and M of the last surrogate_test
     surrogate_units = None
 
-    def _count(self, mc_count, seed, groups):
-        """(prob, hist) of a counting run of units 0 .. mc_count - 1 (the caller holds the lock)."""
+    def _seed_of_run(self, mc_count, seed):
+        """The checks of a surrogate run of units 0 .. mc_count - 1, and its seed."""
         if isinstance(mc_count, bool) or not isinstance(mc_count, (int, np.integer)) \
                 or not 1 <= mc_count <= _MAX_UNITS:
             raise ValueError("mc_count must be an integer in [1, %d], got %r" % (_MAX_UNITS, mc_count))
         if bool(_helpers._FFT_NEXT_POW2) != self._padding:
             raise ValueError("the FFT padding mode has changed since this product was computed: its "
                              "counts would not compare like with like")
-        seed = _surrogate_seed(seed)
+        return _surrogate_seed(seed)
+
+    def _cluster(self, sig, mc_count, seed, groups, inside_coi, measure):
+        """ClusterResult of a cluster test of units 0 .. mc_count - 1 (the caller holds the lock)."""
+        thr = self._threshold(sig)
+        if thr is None:
+            raise ValueError("cluster_test needs a per-scale threshold sig")
+        seed = self._seed_of_run(mc_count, seed)
+        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
+                                     self.normalize, self.precision)
+        lo, hi = _column_ranges(self, inside_coi)
+        q, unit_area = _cluster_weights(self)
+        nser = len(p.yns)
+        hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
+        eng = self.engine
+
+        def call(*a, boxcar_len, precision):
+            dt, _, sj, family, param = a[nser:]
+            return eng.cluster_test(np.stack(a[:nser]), groups, seed, 0, int(mc_count), dt, sj, family,
+                                    param, boxcar_len, prob['mask'], prob['maxscale'], prob['nbins'],
+                                    *hist, serial=self._serial, thr=thr, lo=lo, hi=hi, q=q,
+                                    measure=measure, precision=precision)
+
+        qmax = _wct_on_device(eng, p, call)
+        Q, pts, box = eng.cluster_table(self._TRIPLE)
+        M = int(mc_count)
+        reached = M - np.searchsorted(np.sort(qmax), Q, side='left')
+        return ClusterResult(Q.astype(float) * unit_area, pts, box[:, 0:2], box[:, 2:4],
+                             (1.0 + reached) / (1.0 + M), qmax.astype(float) * unit_area)
+
+    def _cluster_labels(self, rows, cols):
+        S, n0 = self.shape
+        r0, nr, rs = _slice_range(rows, S, 'rows')
+        c0, nc, cs = _slice_range(cols, n0, 'cols')
+        if nr == 0 or nc == 0:
+            return np.empty((nr, nc), dtype=np.int32)
+        return self.engine.cluster_labels(self._TRIPLE, r0, nr, rs, c0, nc, cs)
+
+    def _count(self, mc_count, seed, groups):
+        """(prob, hist) of a counting run of units 0 .. mc_count - 1 (the caller holds the lock)."""
+        seed = self._seed_of_run(mc_count, seed)
         p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
                                      self.normalize, self.precision)
         self.surrogate_seed = self.surrogate_units = None
@@ -453,6 +517,7 @@ class ResidentCoherence(_SurrogateTest, _ResidentSlot):
     `release()` or `wct_resident` on the same engine."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence_serial', 'coherence_release'
+    _TRIPLE = False
     _GONE = ("this coherence is no longer resident: it was released or another wct_resident has "
              "run on the same engine")
 
@@ -608,6 +673,34 @@ class ResidentCoherence(_SurrogateTest, _ResidentSlot):
         Yekutieli 2001), BY under any dependence, at the price of power."""
         return self._fdr_threshold(None, q, method, inside_coi)
 
+    @_live
+    def cluster_test(self, sig, mc_count=300, seed=None, inside_coi=True):
+        """Cluster (areawise) test of this coherence against the surrogate pairs 0 .. mc_count - 1 of
+        `surrogate_significance(mc_count=mc_count, seed=seed)` (Maraun et al. 2007; Schulte et
+        al. 2015).  A point is selected where WCT is finite and > sig[j] (a NaN selects nothing),
+        inside the cone of influence if `inside_coi`; clusters are the 8-connected patches of the
+        selection, in this map and in every surrogate pair's, labelled on the device.  A cluster's
+        area is A = sum dj dt / s_j over its points (the module notes give the exact integer
+        weights), and its p-value is (1 + #{pairs whose largest cluster is at least as large}) /
+        (1 + M): rejecting p <= alpha controls the family-wise error over clusters at alpha.
+
+        `sig` should not come from the same surrogates as the null: take
+        `surrogate_significance(mc_count=M, seed=s1)` and test with a seed s2 != s1, or take the
+        white-noise levels of `significance()`.  Returns ClusterResult(area, points, rows, cols,
+        pvalue, null_max): per cluster of this map, ordered by area descending (ties by the
+        row-major index of the first point), its area, point count, row range [first, last + 1),
+        column range and p-value, and the M pairs' largest areas in pair order.  The labels stay on
+        the device (`cluster_labels`, 4 bytes per scale-point) until the next `cluster_test`,
+        `release()` or `wct_resident`.  ValueError for a `sig` without one entry per scale and for
+        the checks of `surrogate_test`; the counts of an earlier `surrogate_test` are kept."""
+        return self._cluster(sig, mc_count, seed, (0, 1), inside_coi, None)
+
+    @_live
+    def cluster_labels(self, rows=slice(None), cols=slice(None)):
+        """int32 labels[rows, cols] of the last `cluster_test`, with the slicing of `window`: 0 off
+        the clusters, c + 1 on cluster c of its result."""
+        return self._cluster_labels(rows, cols)
+
 
 def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
                  precision='fp64', engine=None):
@@ -751,6 +844,7 @@ class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
     `ResidentCoherence` (8 bytes per scale-point on the device for the two measures)."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence3_serial', 'coherence3_release'
+    _TRIPLE = True
     _GONE = ("this partial / multiple coherence is no longer resident: it was released or another "
              "wct3_resident has run on the same engine")
 
@@ -918,6 +1012,20 @@ class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
     def fdr_threshold(self, q=0.05, method='bh', inside_coi=True, measure='partial'):
         """`ResidentCoherence.fdr_threshold` over the measure's p-values."""
         return self._fdr_threshold(self._measure(measure), q, method, inside_coi)
+
+    @_live
+    def cluster_test(self, sig, mc_count=300, seed=None, inside_coi=True, measure='partial',
+                     conditional=True):
+        """`ResidentCoherence.cluster_test` of the measure against the surrogate triples
+        0 .. mc_count - 1 of `surrogate_significance(mc_count=mc_count, seed=seed,
+        conditional=conditional)`; `sig` in the units of the measure."""
+        m = self._measure(measure)
+        return self._cluster(sig, mc_count, seed, (0, 1, 1) if conditional else (0, 1, 2), inside_coi, m)
+
+    @_live
+    def cluster_labels(self, rows=slice(None), cols=slice(None)):
+        """`ResidentCoherence.cluster_labels` of the last `cluster_test`."""
+        return self._cluster_labels(rows, cols)
 
 
 def wct3_resident(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=True,
