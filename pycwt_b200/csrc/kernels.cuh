@@ -1956,7 +1956,9 @@ template <typename T, int KMAX_, bool SEL = false> struct WctFinalBody {
         for (int e = 0; e < RG; ++e) {
           const int i = i0 + RG * g + e;
           if (i >= rows_out) break;
-          const double r2 = (double)((xr[e] * xr[e] + xi[e] * xi[e]) / (cr[e] * ci[e]));
+          // the ratio in double: numerator and denominator go as amplitude^4 and would leave
+          // float's range near 2^+-31 times a unit series, the fields (amplitude^2) do not
+          const double r2 = ((double)xr[e] * xr[e] + (double)xi[e] * xi[e]) / ((double)cr[e] * ci[e]);
           const size_t o = (size_t)i * a.n + n;
           if (a.WCT) a.WCT[o] = r2;
           if (a.cnt) count_exceed(a.cnt, a.obs, o, r2);

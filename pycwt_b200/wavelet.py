@@ -288,6 +288,19 @@ def _standardise(y, normalize):
     return y, ((y - y.mean()) / std if normalize else y), std
 
 
+def _unit_binade(y):
+    """y times the power of two that brings max|y| into [1/2, 1): exact, so the coherence of the
+    result is that of y.  The coherence pipeline smooths the auto-spectra of two series as the real
+    and imaginary parts of one complex field, and an FFT's twiddle products mix the rounding of the
+    two parts: a series whose amplitude is 2^d times the other's would see the rounding of the
+    larger enlarged by about 2^(2d) in its own field.  y is returned as is when it is all zero or
+    not finite."""
+    m = np.max(np.abs(y)) if y.size else 0.0
+    if not (np.isfinite(m) and m > 0):
+        return y
+    return np.ldexp(y, -int(np.frexp(m)[1]))
+
+
 def xwt(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
         wavelet='morlet', normalize=True, precision='fp64'):
     """Cross wavelet transform W1 * conj(W2) (reference wavelet.py:316-419).
@@ -410,6 +423,10 @@ def _wct_problem(series, dt, dj, s0, J, wavelet, normalize, precision):
     if J == -1:
         J = int(np.round(np.log2(series[0].size * dt / s0) / dj))  # .size: ndarray required, as in the reference
     ys, yns = zip(*[_standardise(y, normalize)[:2] for y in series])
+    if not normalize:
+        # series in their own units: the same binade for all, so that none drowns in the rounding of
+        # another (`_unit_binade`).  WCT, aWCT, RP2, RM2 and their significance do not depend on it
+        yns = tuple(_unit_binade(y) for y in yns)
     n0 = yns[0].size
     sj, freq = _resolve_scales(n0, dt, dj, s0, J, wavelet, None)
     klen = _boxcar_len(wavelet, dj)
@@ -442,7 +459,10 @@ def wct(y1, y2, dt, dj=1/12, s0=-1, J=-1, sig=True,
     on the GPU; `sig` comes from wct_significance (GPU Monte-Carlo) when sig=True.
     `precision` (an extension of the reference signature): 'fp64' (default) or 'fp32', the
     arithmetic of the device pipeline, also that of the significance test; WCT and aWCT are
-    float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6)."""
+    float64 either way and fp32 WCT is within 1e-3 of fp64 (DESIGN.md section 6).  With
+    `normalize=False` each series is first scaled by the power of two that brings its largest
+    magnitude into [1/2, 1): exact, so WCT and aWCT are those of the series as given, whatever
+    their amplitudes and units."""
     p = _wct_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
     (y1, y2), wavelet, s0, J, freq = p.ys, p.wavelet, p.s0, p.J, p.freq
     eng = _engine.default_engine()
