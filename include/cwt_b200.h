@@ -169,7 +169,8 @@ enum cwtb_product {
   CWTB_PRODUCT_W = 0,           /* the transform (CWTB_FIELD_W)                         */
   CWTB_PRODUCT_CROSS = 1,       /* the cross spectrum (CWTB_FIELD_CROSS)               */
   CWTB_PRODUCT_COHERENCE = 2,   /* WCT and aWCT of cwtb_wct_resident                   */
-  CWTB_PRODUCT_COHERENCE3 = 3   /* RP2, the partial phase and RM2 of cwtb_wct3_resident */
+  CWTB_PRODUCT_COHERENCE3 = 3,  /* RP2, the partial phase and RM2 of cwtb_wct3_resident */
+  CWTB_PRODUCT_POWER = 5        /* the kept W of cwtb_power_resident (CWTB_FIELD_POWER)     */
 };
 int cwtb_resident_shape(cwtb_ctx *ctx, int product, int *rows, int64_t *n0, int *precision);
 
@@ -269,6 +270,76 @@ int cwtb_xwt_resident(cwtb_ctx *ctx, const double *y1, const double *y2, int64_t
 int64_t cwtb_cross_serial(cwtb_ctx *ctx);
 int cwtb_cross_release(cwtb_ctx *ctx);
 
+/* ---- resident wavelet power and its tests against surrogates ----------------------------------
+ * cwtb_power_resident runs what cwtb_cwt runs on one real series (same arguments, in the precision
+ * of cwtb_set_coherence_precision; un-padded transforms only in fp64, CWTB_TABLE unsupported) and
+ * keeps its W (n_scales x n0, complex of that precision) in a device buffer of its own, the
+ * transform's W buffer handed over without a copy, as cwtb_xwt_resident does.  The power
+ * P = re^2 + im^2 of a coefficient is formed in double (exact products for an fp32 W), by one
+ * function for the kept W and for every surrogate.  Lifetime:
+ *   - only cwtb_power_resident writes that buffer: it survives every other call (cwt*, xwt*, wct*,
+ *     the Monte-Carlo calls, the power tests below) byte for byte;
+ *   - it dies at the next cwtb_power_resident or cwtb_power_release (which frees it; so does
+ *     cwtb_destroy).  cwtb_power_serial changes at both, and is bumped before the buffer is
+ *     written, so a cwtb_power_resident that fails part-way changes it too;
+ *   - afterwards no transform is resident, as after cwtb_xwt_resident.
+ * The cwtb_field_* calls read it as CWTB_FIELD_POWER. */
+int cwtb_power_resident(cwtb_ctx *ctx, const double *signal, int64_t n0, double dt, const double *scales,
+                        int n_scales, int family, double param);
+int64_t cwtb_power_serial(cwtb_ctx *ctx);
+int cwtb_power_release(cwtb_ctx *ctx);
+/* cwtb_scale_avg_power on the kept W */
+int cwtb_power_scale_avg(cwtb_ctx *ctx, const double *weights, double *out);
+/* The nulls of the power tests.  CWTB_NULL_AR1: unit u is x = m + sigma z, z[0] = e[0],
+ * z[i] = g z[i-1] + sqrt(1 - g^2) e[i], e standard normals that are a pure function of (seed, u, i)
+ * (the Philox4x32-10 stream of cwtb_wct_mc_seeded under a counter tag of its own: no counter of
+ * the white-noise pairs or triples or of the phase-randomised surrogates recurs for
+ * 0 <= u < 2^61), drawn on the device by a parallel scan in double (fp32: rounded).
+ * CWTB_NULL_PHASE: the phase-randomised surrogates of the series (cwtb_wct_mc_phase, one series in
+ * phase group 0): the periodogram is kept exactly. */
+enum cwtb_null { CWTB_NULL_AR1 = 0, CWTB_NULL_PHASE = 1 };
+/* Test hook: the AR(1) units first_unit .. first_unit + n_units - 1, out[n_units][n0] doubles.
+ * CWTB_ERR_ARG: |g| >= 1, a non-finite g, m or sigma, n0 < 1, a negative unit number. */
+int cwtb_mc_ar1_surrogates(cwtb_ctx *ctx, double g, double m, double sigma, uint64_t seed,
+                           int64_t first_unit, int n_units, int64_t n0, double *out);
+/* Point-wise test: for each unit, draw it (`null`; `series` [n0] is the data of the phase null, g,
+ * m, sigma the AR(1) null's parameters), transform it with the kept W's plan, exactly as one
+ * cwtb_cwt of it in the kept W's precision would, and count on every point
+ *   k[s, n] += 1  where  P_unit[s, n] >= P_obs[s, n]  or P_unit[s, n] is not finite
+ * into uint32 counters [n_scales][n0] that live with the kept W (4 bytes per scale-point).  Reset,
+ * accumulation, CWTB_ERR_STATE (serial, n_scales, n0) and the 2^32 - 1 limit as
+ * cwtb_coherence_surrogate_counts; CWTB_ERR_ARG also for an unknown null and the errors of
+ * cwtb_mc_ar1_surrogates / cwtb_mc_phase_surrogates.  The units are transformed one at a time. */
+int cwtb_power_surrogate_counts(cwtb_ctx *ctx, const double *series, int null, double g, double m, double sigma,
+                                uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                const double *scales, int n_scales, int family, double param, int64_t serial,
+                                int reset);
+/* Cluster test: the units of cwtb_power_surrogate_counts, and the selection, clusters, weights,
+ * qmax_out, checks and lifetime of cwtb_coherence_cluster_test with P in place of the coherence
+ * (finite P > thr[j] on [lo[j], hi[j])).  The counts are neither read nor changed. */
+int cwtb_power_cluster_test(cwtb_ctx *ctx, const double *series, int null, double g, double m, double sigma,
+                            uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                            const double *scales, int n_scales, int family, double param, int64_t serial,
+                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
+                            uint64_t *qmax_out);
+/* Strided sub-grid of P = re^2 + im^2 of the kept W (the tests' P, in double), nrows x ncols doubles,
+ * with the layout and checks of cwtb_field_window: 8 bytes per point cross the bus, not 16. */
+int cwtb_power_window(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                      int64_t col_step, double *out);
+/* Reading the counts and clusters, as the cwtb_coherence_* calls of the same names read the
+ * coherence's: the p-value window (NaN where P is not finite), the row stats of
+ * cwtb_field_row_stats (S x 5) over the points with a finite P and k <= kmax, the histogram of k,
+ * the cluster table and the label window. */
+int cwtb_power_pvalue_window(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                             int64_t col_step, double *p_out);
+int cwtb_power_pvalue_row_stats(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, const double *thr,
+                                int64_t kmax, double *out);
+int cwtb_power_count_hist(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, int64_t nbins, int64_t *out);
+int cwtb_power_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                             int64_t *box);
+int cwtb_power_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                              int64_t col_step, int32_t *out);
+
 /* ---- partial and multiple wavelet coherence of three series (Mihanovic et al. 2009; Ng & Chan
  * 2012) -------------------------------------------------------------------------------------------
  * y, x1, x2: three signals of n0 samples (standardised by the caller as for cwtb_wct).  With S the
@@ -327,13 +398,16 @@ int cwtb_coherence3_row_stats(cwtb_ctx *ctx, int measure, const int64_t *lo, con
  * for MULTIPLE the two phase planes are 0.  Rows with weight 0 are not read. */
 int cwtb_coherence3_scale_avg(cwtb_ctx *ctx, int measure, const double *weights, double *out);
 
-/* Reading calls on a resident complex field: CWTB_FIELD_W (the resident transform's W) or
- * CWTB_FIELD_CROSS (the cross spectrum).  They return CWTB_ERR_STATE when the field is not
- * resident, CWTB_ERR_UNSUPPORTED for the W of a batched transform and CWTB_ERR_ARG for bad
+/* Reading calls on a resident complex field: CWTB_FIELD_W (the resident transform's W),
+ * CWTB_FIELD_CROSS (the cross spectrum) or CWTB_FIELD_POWER (the kept W of cwtb_power_resident).
+ * They return CWTB_ERR_STATE when the field is not resident, CWTB_ERR_UNSUPPORTED for the W of a batched transform and CWTB_ERR_ARG for bad
  * ranges.  Outputs are complex128 / double whatever the field's precision (fp32 fields are widened
  * on the device); the reductions are deterministic (fixed partition and summation order, no
  * atomics: repeated calls are bit-identical). */
-enum cwtb_field { CWTB_FIELD_W = 0, CWTB_FIELD_CROSS = 1 };
+/* A complex field has the id of its product (cwtb_resident_shape), so that one id sizes every read of
+ * it.  Ids 2 and 3 are the double products, and 4 is no product: it was an unknown product before
+ * the power came, and callers that probe for one keep getting CWTB_ERR_ARG from it. */
+enum cwtb_field { CWTB_FIELD_W = 0, CWTB_FIELD_CROSS = 1, CWTB_FIELD_POWER = 5 };
 /* rows [row0, row0 + nrows), nrows x n0 complex128 */
 int cwtb_field_get(cwtb_ctx *ctx, int field, int row0, int nrows, void *out);
 /* strided sub-grid, nrows x ncols complex128: out[r][c] = F[row0 + r*row_step][col0 + c*col_step],

@@ -15,6 +15,7 @@ from .wavelet import partial_wct, multiple_wct, wct3_significance  # noqa: F401 
 from .wavelet import wct_surrogate_significance, wct3_surrogate_significance  # noqa: F401  (extension)
 from .resident import xwt_resident, ResidentCrossWavelet  # noqa: F401  (extension)
 from .resident import wct3_resident, ResidentCoherence3  # noqa: F401  (extension)
+from .resident import power_resident, ResidentPower  # noqa: F401  (extension)
 from .resident import ClusterResult  # noqa: F401  (extension)
 
 __all__ = ['cwt', 'icwt', 'significance', 'xwt', 'wct', 'wct_significance',

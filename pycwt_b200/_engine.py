@@ -12,11 +12,15 @@ LIB_PATH = os.path.join(_HERE, "libcwtb200.so")
 
 MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
 F64, F32 = 0, 1
-FIELD_W, FIELD_CROSS = 0, 1      # complex fields of the cwtb_field_* calls
+# complex fields of the cwtb_field_* calls, each with the id of its product below
+FIELD_W, FIELD_CROSS, FIELD_POWER = 0, 1, 5
 MEASURE_PARTIAL, MEASURE_MULTIPLE = 0, 1   # the measures of the cwtb_coherence3_* calls
-# the resident products of cwtb_resident_shape: the two fields, the coherence (cwtb_coherence_*) and
-# the partial and multiple coherence (cwtb_coherence3_*)
-PRODUCT_W, PRODUCT_CROSS, PRODUCT_COHERENCE, PRODUCT_COHERENCE3 = 0, 1, 2, 3
+# the resident products of cwtb_resident_shape: the two fields, the coherence (cwtb_coherence_*), the
+# partial and multiple coherence (cwtb_coherence3_*) and the power (cwtb_power_*)
+PRODUCT_W, PRODUCT_CROSS, PRODUCT_COHERENCE, PRODUCT_COHERENCE3, PRODUCT_POWER = 0, 1, 2, 3, 5   # 4: none
+NULL_AR1, NULL_PHASE = 0, 1      # the nulls of the power tests (cwtb_power_surrogate_counts)
+# the `measure` of the surrogate-test readers below that names the resident power
+POWER = 'power'
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -122,6 +126,21 @@ _SIGNATURES = {
     "cwtb_coherence_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_coherence3_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_cluster_label_bits": (_I, [_P, _P, _I, _I64, _P, _I64, _P, _P, _P, _P, _P, _P]),
+    "cwtb_power_resident": (_I, [_P, _P, _I64, _D, _P, _I, _I, _D]),
+    "cwtb_power_serial": (_I64, [_P]),
+    "cwtb_power_release": (_I, [_P]),
+    "cwtb_power_scale_avg": (_I, [_P, _P, _P]),
+    "cwtb_mc_ar1_surrogates": (_I, [_P, _D, _D, _D, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_power_surrogate_counts": (_I, [_P, _P, _I, _D, _D, _D, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I,
+                                         _D, _I64, _I]),
+    "cwtb_power_cluster_test": (_I, [_P, _P, _I, _D, _D, _D, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D,
+                                     _I64, _P, _P, _P, _P, _P]),
+    "cwtb_power_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_power_pvalue_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_power_pvalue_row_stats": (_I, [_P, _P, _P, _P, _I64, _P]),
+    "cwtb_power_count_hist": (_I, [_P, _P, _P, _I64, _P]),
+    "cwtb_power_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
+    "cwtb_power_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -268,8 +287,10 @@ class Engine(object):
         self._check(self.lib.cwtb_resident_shape(self.h, int(product), ctypes.byref(rows), ctypes.byref(n0),
                                                  ctypes.byref(prec)))
         if rows.value <= 0:
-            raise EngineError("no %s resident" % ("single transform", "cross spectrum", "coherence",
-                                                  "partial / multiple coherence")[product])
+            raise EngineError("no %s resident" % {PRODUCT_W: "single transform", PRODUCT_CROSS: "cross spectrum",
+                                                  PRODUCT_COHERENCE: "coherence",
+                                                  PRODUCT_COHERENCE3: "partial / multiple coherence",
+                                                  PRODUCT_POWER: "power"}[product])
         return rows.value, n0.value, prec.value
 
     def _transform(self, rows=None, n0=None):
@@ -966,6 +987,9 @@ class Engine(object):
         if measure is None:
             self._shape(PRODUCT_COHERENCE)
             self._check(self.lib.cwtb_coherence_pvalue_window(self.h, *w))
+        elif measure == POWER:
+            self._shape(PRODUCT_POWER)
+            self._check(self.lib.cwtb_power_pvalue_window(self.h, *w))
         else:
             self._shape(PRODUCT_COHERENCE3)
             self._check(self.lib.cwtb_coherence3_pvalue_window(self.h, int(measure), *w))
@@ -973,8 +997,16 @@ class Engine(object):
 
     @_locked
     def pvalue_row_stats(self, measure, lo, hi, kmax, thr=None, want_phase=False):
-        """[rows, 4] of `coherence_row_stats` / `coherence3_row_stats` over the points with a finite
-        value and a count k <= kmax."""
+        """[rows, 4] of `coherence_row_stats` / `coherence3_row_stats` ([rows, 5] of
+        `field_row_stats` for the power) over the points with a finite value and a count k <= kmax."""
+        if measure == POWER:
+            rows, _, _ = self._shape(PRODUCT_POWER)
+            lo, hi, thr = _row_args("pvalue_row_stats", rows, lo, hi, thr)
+            out = np.empty((rows, 5), dtype=np.float64)
+            self._check(self.lib.cwtb_power_pvalue_row_stats(self.h, _ptr(lo), _ptr(hi),
+                                                             None if thr is None else _ptr(thr), int(kmax),
+                                                             _ptr(out)))
+            return out
         rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else PRODUCT_COHERENCE3)
         lo, hi, thr = _row_args("pvalue_row_stats", rows, lo, hi, thr)
         out = np.empty((rows, 4), dtype=np.float64)
@@ -989,10 +1021,13 @@ class Engine(object):
     def count_hist(self, measure, lo, hi, nbins):
         """int64 [nbins]: the number of points with count k over the columns [lo[j], hi[j]) whose
         value is finite; nbins must be M + 1."""
-        rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else PRODUCT_COHERENCE3)
+        rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else
+                                 PRODUCT_POWER if measure == POWER else PRODUCT_COHERENCE3)
         lo, hi, _ = _row_args("count_hist", rows, lo, hi, None)
         out = np.empty(int(nbins), dtype=np.int64)
-        if measure is None:
+        if measure == POWER:
+            self._check(self.lib.cwtb_power_count_hist(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
+        elif measure is None:
             self._check(self.lib.cwtb_coherence_count_hist(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
         else:
             self._check(self.lib.cwtb_coherence3_count_hist(self.h, int(measure), _ptr(lo), _ptr(hi), int(nbins),
@@ -1048,24 +1083,120 @@ class Engine(object):
         call(m, ctypes.byref(count), _ptr(Q), _ptr(pts), _ptr(box))
         return Q, pts, box
 
+    def _cluster_call(self, triple, what):
+        """cwtb_{coherence, coherence3, power}_cluster_<what> for `triple` False, True or POWER."""
+        name = "power" if triple == POWER else "coherence3" if triple else "coherence"
+        return getattr(self.lib, "cwtb_%s_cluster_%s" % (name, what))
+
     @_locked
     def cluster_table(self, triple=False):
-        """The resident map's clusters of the last cluster test of the coherence (`triple` False) or
-        of the partial / multiple coherence (True): (Q, points, box [:, 4] = first row, last row + 1,
-        first column, last column + 1), in table order."""
-        fn = self.lib.cwtb_coherence3_cluster_table if triple else self.lib.cwtb_coherence_cluster_table
+        """The resident map's clusters of the last cluster test of the coherence (`triple` False),
+        of the partial / multiple coherence (True) or of the power (POWER): (Q, points, box [:, 4] =
+        first row, last row + 1, first column, last column + 1), in table order."""
+        fn = self._cluster_call(triple, "table")
         return self._table(lambda *a: self._check(fn(self.h, *a)))
 
     @_locked
     def cluster_labels(self, triple, row0, nrows, row_step, col0, ncols, col_step):
         """int32 labels [row0::row_step][:nrows, col0::col_step][:, :ncols] of the last cluster
-        test of the coherence (`triple` False) or of the partial / multiple coherence (True): 0 off
-        the clusters, c + 1 on table row c."""
+        test of the coherence (`triple` False), of the partial / multiple coherence (True) or of the
+        power (POWER): 0 off the clusters, c + 1 on table row c."""
         out = np.empty((int(nrows), int(ncols)), dtype=np.int32)
         w = (int(row0), int(nrows), int(row_step), int(col0), int(ncols), int(col_step), _ptr(out))
-        fn = self.lib.cwtb_coherence3_cluster_labels if triple else self.lib.cwtb_coherence_cluster_labels
-        self._check(fn(self.h, *w))
+        self._check(self._cluster_call(triple, "labels")(self.h, *w))
         return out
+
+    # ---- the resident power and its tests against AR(1) or phase-randomised surrogates ---------
+    @_locked
+    def power_resident(self, y, dt, scales, family, param, precision=F64):
+        """`cwt` of `y` in `precision` with W kept on the device as the resident power; returns the
+        power serial that identifies it.  No transform is resident afterwards."""
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        if y.ndim != 1:
+            raise ValueError("power_resident: the series must be 1-D")
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
+        self._check(self.lib.cwtb_power_resident(self.h, _ptr(y), y.size, float(dt), _ptr(sj), sj.size,
+                                                 int(family), float(param)))
+        return self.power_serial()
+
+    @_locked
+    def power_serial(self):
+        return int(self.lib.cwtb_power_serial(self.h))
+
+    @_locked
+    def power_release(self):
+        self._check(self.lib.cwtb_power_release(self.h))
+
+    @_locked
+    def power_window(self, row0, nrows, row_step, col0, ncols, col_step):
+        """P = |W|^2 [row0::row_step][:nrows, col0::col_step][:, :ncols] (float64) of the resident
+        power, formed on the device as its tests form it."""
+        self._shape(PRODUCT_POWER)
+        out = self.result_array((nrows, ncols), np.float64)
+        self._check(self.lib.cwtb_power_window(self.h, int(row0), int(nrows), int(row_step), int(col0), int(ncols),
+                                               int(col_step), _ptr(out)))
+        return out
+
+    @_locked
+    def power_scale_avg(self, weights):
+        """sum_j w_j |W[j, :]|^2 (float64, n0) of the resident power."""
+        rows, n0, _ = self._shape(PRODUCT_POWER)
+        w = _weights("power_scale_avg", rows, weights)
+        out = self.result_array((n0,), np.float64)
+        self._check(self.lib.cwtb_power_scale_avg(self.h, _ptr(w), _ptr(out)))
+        return out
+
+    @_locked
+    def mc_ar1_surrogates(self, g, m, sigma, seed, first_unit, n_units, n0):
+        """The AR(1) units of the power tests, float64 [n_units, n0]."""
+        out = np.empty((int(n_units), int(n0)), dtype=np.float64)
+        self._check(self.lib.cwtb_mc_ar1_surrogates(self.h, float(g), float(m), float(sigma),
+                                                    int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
+                                                    int(n0), _ptr(out)))
+        return out
+
+    @staticmethod
+    def _power_args(name, series, null, g, m, sigma, seed, first_unit, n_units, dt, sj, family, param, serial):
+        """The arguments of a power test up to `serial` (the series: the phase null's data, 1-D).  The
+        caller keeps `series` and `sj` alive across the call."""
+        if series.ndim != 1:
+            raise ValueError("%s: the series must be 1-D" % name)
+        if null == NULL_PHASE and not np.isfinite(series).all():
+            raise ValueError("%s: non-finite sample" % name)
+        return (_ptr(series), int(null), float(g), float(m), float(sigma), int(seed) & (2 ** 64 - 1),
+                int(first_unit), int(n_units), series.size, float(dt), _ptr(sj), sj.size, int(family),
+                float(param), int(serial))
+
+    @_locked
+    def power_surrogate_counts(self, series, null, g, m, sigma, seed, first_unit, n_units, dt, scales, family,
+                               param, serial, reset=True):
+        """Count, per point, the units of the null whose power reaches the resident power's, into its
+        counters (cwtb_power_surrogate_counts); `serial` is the power's serial.  `reset` zeroes the
+        counters first, otherwise the units are added."""
+        series = np.ascontiguousarray(series, dtype=np.float64)
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        a = self._power_args("power_surrogate_counts", series, null, g, m, sigma, seed, first_unit, n_units, dt, sj,
+                             family, param, serial)
+        self._check(self.lib.cwtb_power_surrogate_counts(self.h, *a, 1 if reset else 0))
+
+    @_locked
+    def power_cluster_test(self, series, null, g, m, sigma, seed, first_unit, n_units, dt, scales, family, param,
+                           serial, thr, lo, hi, q):
+        """Label the clusters of the resident power's map and of every unit's
+        (cwtb_power_cluster_test): uint64 [n_units], the largest cluster sum Q of each unit."""
+        series = np.ascontiguousarray(series, dtype=np.float64)
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        a = self._power_args("power_cluster_test", series, null, g, m, sigma, seed, first_unit, n_units, dt, sj,
+                             family, param, serial)
+        lo, hi, thr = _row_args("power_cluster_test", sj.size, lo, hi, thr)
+        q = np.ascontiguousarray(q, dtype=np.uint64)
+        if q.shape != (sj.size,):
+            raise ValueError("power_cluster_test: q must have one entry per scale")
+        qmax = np.zeros(int(n_units), dtype=np.uint64)
+        self._check(self.lib.cwtb_power_cluster_test(self.h, *a, _ptr(thr), _ptr(lo), _ptr(hi), _ptr(q),
+                                                     _ptr(qmax)))
+        return qmax
 
     @_locked
     def cluster_label_bits(self, bits, n0, q, want_labels=True):

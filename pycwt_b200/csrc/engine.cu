@@ -290,6 +290,7 @@ struct cwtb_ctx {
   // cluster tests: the selection bitmask, its per-row arguments (thr, lo, hi, q), the chunk and row
   // tables of the labeller, its run tables (sized from the run count of each map), the units' maxima
   Buf cl_bits, cl_rows, cl_hdr, cl_runs, cl_qmax;
+  Buf arc;                       // AR(1) surrogates: the CTAs' (g^L, b) pairs and carry-ins (Ar1Args::blk)
   Job job;
   // what the resident plan (job + uploaded descriptors) was built from: a call with the same
   // geometry and settings reuses it (planning + descriptor upload: ~0.3 ms for 256 scales, several ms
@@ -325,6 +326,10 @@ struct cwtb_ctx {
   // resident partial and multiple coherence (cwtb_wct3_resident): RP2 [S][n0], the partial phase at
   // coh_angle_offset(S*n0), RM2 at twice that offset, double.  Only cwtb_wct3_resident writes it.
   ResidentSlot coh3;
+  // resident wavelet power (cwtb_power_resident): its transform's W [S][n0] of precision prec, handed
+  // over by swapping buffers as cwtb_xwt_resident does, with the power tests' counts and clusters.
+  // Only cwtb_power_resident writes it.
+  ResidentSlot pw;
   // resident transform: rows = scales x channels of the complete W in the scratch buffer W, of
   // precision prec.  prepare opens it (serial: cwtb_job_serial); only a transform entry point that
   // completes fills it (w_fill), so while it is filled `job` is the plan it was filled from.
@@ -1686,7 +1691,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts, &c->coh.labels, &c->coh3.labels, &c->cl_bits, &c->cl_rows, &c->cl_hdr, &c->cl_runs, &c->cl_qmax})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts, &c->coh.labels, &c->coh3.labels, &c->pw.buf, &c->pw.counts, &c->pw.labels, &c->arc, &c->cl_bits, &c->cl_rows, &c->cl_hdr, &c->cl_runs, &c->cl_qmax})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2546,38 +2551,44 @@ int cwtb_global_power_ranges(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, 
   return power_common(c, nullptr, out, nullptr, lo, hi);
 }
 
-int cwtb_scale_avg_power(cwtb_ctx *c, const double *weights, double *out) {
-  if (!c || !w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
+// scale-averaged power of the S x n0 complex field W of precision prec (cwtb_scale_avg_power)
+static int scale_avg_power_run(cwtb_ctx *c, const void *W, int prec, int S, long long n0, const double *weights,
+                               double *out) {
   if (!weights || !out) return fail(c, CWTB_ERR_ARG, "null argument");
-  const Job &job = c->job;
-  if (job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "scale average of a batched transform: fetch rows per channel");
   // [weights S doubles][selected rows S ints]: rows with a zero weight are not read at all
-  std::vector<double> w(weights, weights + job.S);
+  std::vector<double> w(weights, weights + S);
   std::vector<int> sel;
-  for (int j = 0; j < job.S; ++j)
+  for (int j = 0; j < S; ++j)
     if (w[j] != 0.0) sel.push_back(j);
   const int nsel = (int)sel.size();
-  w.resize((size_t)job.S + ((size_t)job.S + 1) / 2);
-  if (nsel) memcpy(w.data() + job.S, sel.data(), sizeof(int) * nsel);
+  w.resize((size_t)S + ((size_t)S + 1) / 2);
+  if (nsel) memcpy(w.data() + S, sel.data(), sizeof(int) * nsel);
   int e = upload_doubles(c, c->rowd, w);
   if (e) return e;
-  if ((e = ensure(c, c->aux, (size_t)job.n0 * sizeof(double)))) return e;
-  const unsigned gx = (unsigned)((job.n0 + NT - 1) / NT);
+  if ((e = ensure(c, c->aux, (size_t)n0 * sizeof(double)))) return e;
+  const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
   const int spb = nsel <= 32 ? std::max(nsel, 1) : 32;
   const unsigned gy = (unsigned)std::max(1, (nsel + spb - 1) / spb);
-  if (gy > 1) RT(rt_memset(c->aux.p, 0, (size_t)job.n0 * sizeof(double), c->stream));
-  const int *dsel = (const int *)((const double *)c->rowd.p + job.S);
-  if (job.precision == CWTB_F64) {
-    ScaleAvgArgs<double> a{(const double2 *)c->W.p, (const double *)c->rowd.p, (double *)c->aux.p, job.n0, job.S, dsel, nsel, spb};
+  if (gy > 1) RT(rt_memset(c->aux.p, 0, (size_t)n0 * sizeof(double), c->stream));
+  const int *dsel = (const int *)((const double *)c->rowd.p + S);
+  if (prec == CWTB_F64) {
+    ScaleAvgArgs<double> a{(const double2 *)W, (const double *)c->rowd.p, (double *)c->aux.p, n0, S, dsel, nsel, spb};
     e = launch<ScaleAvgBody<double>>(c, gx, gy, a);
   } else {
-    ScaleAvgArgs<float> a{(const float2 *)c->W.p, (const double *)c->rowd.p, (double *)c->aux.p, job.n0, job.S, dsel, nsel, spb};
+    ScaleAvgArgs<float> a{(const float2 *)W, (const double *)c->rowd.p, (double *)c->aux.p, n0, S, dsel, nsel, spb};
     e = launch<ScaleAvgBody<float>>(c, gx, gy, a);
   }
   if (e) return e;
-  RT(rt_d2h(out, c->aux.p, (size_t)job.n0 * sizeof(double), c->stream));
+  RT(rt_d2h(out, c->aux.p, (size_t)n0 * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;
+}
+
+int cwtb_scale_avg_power(cwtb_ctx *c, const double *weights, double *out) {
+  if (!c || !w_resident(c)) return fail(c, CWTB_ERR_STATE, "no transform resident");
+  const Job &job = c->job;
+  if (job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "scale average of a batched transform: fetch rows per channel");
+  return scale_avg_power_run(c, c->W.p, job.precision, job.S, job.n0, weights, out);
 }
 
 // W12 in W; the plan is a job of type T afterwards: cwtb_get_w widens an fp32 W12 on the device
@@ -2645,11 +2656,57 @@ int cwtb_xwt_resident(cwtb_ctx *c, const double *y1, const double *y2, int64_t n
 int64_t cwtb_cross_serial(cwtb_ctx *c) { return c ? c->cross.serial : -1; }
 int cwtb_cross_release(cwtb_ctx *c) { return c ? slot_release(c, c->cross) : CWTB_ERR_ARG; }
 
+// W of one series in W: what cwtb_cwt runs on it in the engine type T (the series rounded on the
+// device for fp32, as cwtb_cwt rounds it on the host)
+extern "C++" {
+template <typename T>
+static int power_run(cwtb_ctx *c, const double *y, int64_t n0, double dt, const double *scales, int n_scales,
+                     int family, double param) {
+  int e = prepare(c, n0, dt, scales, n_scales, family, param, prec_of<T>(), nullptr);
+  if (e) return e;
+  if ((e = upload_series<T>(c, c->sig, y, n0))) return e;
+  c->launches = 0;
+  if ((e = time_begin(c))) return e;
+  if ((e = run_job<T>(c, c->job, (const T *)c->sig.p, nullptr, EPI_STORE))) return e;
+  if ((e = time_end(c, &c->last_ms))) return e;
+  c->job_dsig = nullptr;
+  RT(rt_sync(c->stream));
+  return 0;
+}
+}  // extern "C++"
+
+int cwtb_power_resident(cwtb_ctx *c, const double *y, int64_t n0, double dt, const double *scales, int n_scales,
+                        int family, double param) {
+  if (!c || !y) return fail(c, CWTB_ERR_ARG, "null argument");
+  slot_begin(c->pw);
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "power_resident needs an analytic wavelet family");
+  int e = c->coh_precision == CWTB_F32 ? power_run<float>(c, y, n0, dt, scales, n_scales, family, param)
+                                       : power_run<double>(c, y, n0, dt, scales, n_scales, family, param);
+  if (e) return e;
+  std::swap(c->W, c->pw.buf);   // as cwtb_xwt_resident: the transform's W becomes the slot's buffer
+  c->pw.S = n_scales;
+  c->pw.n0 = n0;
+  c->pw.prec = c->job.precision;
+  return 0;
+}
+
+int64_t cwtb_power_serial(cwtb_ctx *c) { return c ? c->pw.serial : -1; }
+int cwtb_power_release(cwtb_ctx *c) { return c ? slot_release(c, c->pw) : CWTB_ERR_ARG; }
+
+int cwtb_power_scale_avg(cwtb_ctx *c, const double *weights, double *out) {
+  if (!c) return CWTB_ERR_ARG;
+  const ResidentSlot &s = c->pw;
+  if (s.S <= 0 || !s.buf.p) return fail(c, CWTB_ERR_STATE, "no power resident");
+  RT(rt_set_device(c->device));
+  return scale_avg_power_run(c, s.buf.p, s.prec, s.S, s.n0, weights, out);
+}
+
 // WCT and aWCT of a coherence share one device buffer; aWCT starts on a 256-byte boundary, so that
 // a flat index has the same alignment in both fields (the 16-byte loads of RowStatsBody<CohView>)
 static size_t coh_angle_offset(size_t cnt) { return (cnt + 31) & ~(size_t)31; }
 
-// A resident field of the reading calls: a cwtb_field (the transform's W or the cross spectrum),
+// A resident field of the reading calls: a cwtb_field (the transform's W, the cross spectrum or the
+// kept W of the power),
 // or a double field under an id of its own: the coherence (WCT with aWCT), the partial coherence
 // (RP2 with its phase) or the multiple coherence (RM2, no phase)
 static constexpr int FIELD_COH = -1, FIELD_COH3_P = -2, FIELD_COH3_M = -3;
@@ -2664,6 +2721,7 @@ struct FieldRef {
   // they hold and the row stats' cut k <= kmax; cnt null: the field alone
   const unsigned *cnt = nullptr;
   long long m = 0, kmax = 0;
+  bool power = false;   // a complex field's window as its power P (CxPowerView)
 };
 
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
@@ -2673,11 +2731,12 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
     if (s.S <= 0) return fail(c, CWTB_ERR_STATE, "no transform resident");
     if (c->job.nbatch != 1) return fail(c, CWTB_ERR_UNSUPPORTED, "field of a batched transform: fetch rows per channel");
     f = FieldRef{field, c->W.p, s.prec, s.S, s.n0, 0};
-  } else if (field == CWTB_FIELD_CROSS || field == FIELD_COH) {
+  } else if (field == CWTB_FIELD_CROSS || field == CWTB_FIELD_POWER || field == FIELD_COH) {
     const bool coh = field == FIELD_COH;
-    const ResidentSlot &s = coh ? c->coh : c->cross;
+    const ResidentSlot &s = coh ? c->coh : field == CWTB_FIELD_POWER ? c->pw : c->cross;
     if (s.S <= 0 || !s.buf.p)
-      return fail(c, CWTB_ERR_STATE, coh ? "no coherence resident" : "no cross spectrum resident");
+      return fail(c, CWTB_ERR_STATE, coh ? "no coherence resident"
+                                     : field == CWTB_FIELD_POWER ? "no power resident" : "no cross spectrum resident");
     f = FieldRef{field, s.buf.p, s.prec, s.S, s.n0, coh ? coh_angle_offset((size_t)s.S * s.n0) : 0};
   } else {   // FIELD_COH3_P / _M: RP2, phase, RM2 at 0, off, 2 off
     const ResidentSlot &s = c->coh3;
@@ -2690,10 +2749,10 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   return 0;
 }
 
-// The counts of a coherence field f (field_ref of FIELD_COH, FIELD_COH3_P or FIELD_COH3_M) added
-// to it, with the row stats' cut kmax
+// The counts of a tested field f (field_ref of FIELD_COH, FIELD_COH3_P, FIELD_COH3_M or
+// CWTB_FIELD_POWER) added to it, with the row stats' cut kmax
 static int count_ref(cwtb_ctx *c, long long kmax, FieldRef &f) {
-  const ResidentSlot &s = f.field == FIELD_COH ? c->coh : c->coh3;
+  const ResidentSlot &s = f.field == FIELD_COH ? c->coh : f.field == CWTB_FIELD_POWER ? c->pw : c->coh3;
   if (s.units < 0 || !s.counts.p) return fail(c, CWTB_ERR_STATE, "no surrogate counts resident for this product");
   f.cnt = (const unsigned *)s.counts.p + (f.field == FIELD_COH3_M ? coh_angle_offset((size_t)s.S * s.n0) : 0);
   f.m = s.units;
@@ -2703,7 +2762,8 @@ static int count_ref(cwtb_ctx *c, long long kmax, FieldRef &f) {
 
 // the field of a cwtb_field_* call
 static int cx_field_ref(cwtb_ctx *c, int field, FieldRef &f) {
-  if (c && field != CWTB_FIELD_W && field != CWTB_FIELD_CROSS) return fail(c, CWTB_ERR_ARG, "unknown field");
+  if (c && field != CWTB_FIELD_W && field != CWTB_FIELD_CROSS && field != CWTB_FIELD_POWER)
+    return fail(c, CWTB_ERR_ARG, "unknown field");
   return field_ref(c, field, f);
 }
 
@@ -2720,19 +2780,28 @@ static int with_view(const FieldRef &f, int want_phase, Fn &&fn) {
   return fn(CxView<float>{(const cx<float> *)f.p});
 }
 
-// the reads of the window and the row stats: with_view's view, or the counting view of a field
-// that carries counts
+// fn(view) with the counting view of a field that carries counts (count_ref)
 template <typename Fn>
-static int with_read_view(const FieldRef &f, int want_phase, Fn &&fn) {
-  if (!f.cnt) return with_view(f, want_phase, fn);
+static int with_count_view(const FieldRef &f, int want_phase, Fn &&fn) {
+  if (!double_field(f.field)) {   // the power
+    if (f.prec == CWTB_F64) return fn(CxCountView<double>{(const cx<double> *)f.p, f.cnt, f.kmax, f.m});
+    return fn(CxCountView<float>{(const cx<float> *)f.p, f.cnt, f.kmax, f.m});
+  }
   const double *w = (const double *)f.p;
   if (f.field == FIELD_COH3_M) return fn(CohCountViewT<false>{w, nullptr, f.cnt, f.kmax, f.m, 0});
   return fn(CohCountViewT<true>{w, w + f.angle, f.cnt, f.kmax, f.m, want_phase});
 }
 
+// the reads of the window and the row stats: with_view's view, or the counting view of a field
+// that carries counts
+template <typename Fn>
+static int with_read_view(const FieldRef &f, int want_phase, Fn &&fn) {
+  return f.cnt ? with_count_view(f, want_phase, fn) : with_view(f, want_phase, fn);
+}
+
 // Strided sub-grid into out0 / out1: a double field's value / phase (nothing asked for: nothing to
-// do; a field without a phase takes out1 == null), a field with counts its p-values into out0, or a
-// complex field as complex128 into out0
+// do; a field without a phase takes out1 == null), a field with counts its p-values into out0, a
+// complex field read as power its P into out0 (double), or a complex field as complex128 into out0
 static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int row_step, int64_t col0,
                       int64_t ncols, int64_t col_step, void *out0, void *out1) {
   const int S = f.S;
@@ -2744,7 +2813,7 @@ static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int r
   if (row0 < 0 || row0 >= S || (long long)(nrows - 1) > (long long)(S - 1 - row0) / row_step ||
       col0 < 0 || col0 >= n0 || (ncols - 1) > (n0 - 1 - col0) / col_step)
     return fail(c, CWTB_ERR_ARG, "window outside the resident field");
-  if (!f.cnt && row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
+  if (!f.cnt && !f.power && row_step == 1 && col_step == 1 && col0 == 0 && ncols == n0) {   // whole rows: plain copies
     const size_t off = (size_t)row0 * n0, cnt = (size_t)nrows * n0;
     if (!coh) return field_to_host(c, f.p, f.prec, off, cnt, out0, 1);
     const double *dW = (const double *)f.p;
@@ -2757,12 +2826,15 @@ static int window_run(cwtb_ctx *c, const FieldRef &f, int row0, int nrows, int r
   int e = ensure(c, c->aux, m * sizeof(double2));
   if (e) return e;
   double *o0 = (double *)c->aux.p, *o1 = o0 + m;   // a complex128 output takes both halves
-  e = with_read_view(f, 0, [&](auto v) {
+  auto run = [&](auto v) {
     WindowArgs<decltype(v)> a{v, out0 ? o0 : nullptr, out1 ? o1 : nullptr, n0, row0, row_step, col0, col_step, ncols};
     return launch<WindowBody<decltype(v)>>(c, (unsigned)((ncols + NT - 1) / NT), (unsigned)nrows, a);
-  });
+  };
+  if (!f.power) e = with_read_view(f, 0, run);
+  else if (f.prec == CWTB_F64) e = run(CxPowerView<double>{(const cx<double> *)f.p});
+  else e = run(CxPowerView<float>{(const cx<float> *)f.p});
   if (e) return e;
-  const size_t bytes = m * (coh ? sizeof(double) : sizeof(double2));
+  const size_t bytes = m * (coh || f.cnt || f.power ? sizeof(double) : sizeof(double2));
   if (out0) RT(rt_d2h(out0, o0, bytes, c->stream));
   if (out1) RT(rt_d2h(out1, o1, bytes, c->stream));
   RT(rt_sync(c->stream));
@@ -2858,10 +2930,13 @@ static int count_hist_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, con
   unsigned long long *dh = (unsigned long long *)(dhi + S);
   RT(rt_h2d(dlo, h.data(), h.size() * sizeof(long long), c->stream));
   RT(rt_memset(dh, 0, (size_t)nbins * sizeof(long long), c->stream));
-  CountHistArgs a{(const double *)f.p, f.cnt, dlo, dhi, dh, n0, nbins};
-  using Sh = CountHistBody<true>;
-  const unsigned gx = (unsigned)((span + Sh::CHUNK - 1) / Sh::CHUNK);
-  e = nbins <= Sh::SMEM_BINS ? launch<Sh>(c, gx, (unsigned)S, a) : launch<CountHistBody<false>>(c, gx, (unsigned)S, a);
+  e = with_count_view(f, 0, [&](auto v) {
+    CountHistArgs<decltype(v)> a{v, dlo, dhi, dh, n0, nbins};
+    using Sh = CountHistBody<decltype(v), true>;
+    const unsigned gx = (unsigned)((span + Sh::CHUNK - 1) / Sh::CHUNK);
+    return nbins <= Sh::SMEM_BINS ? launch<Sh>(c, gx, (unsigned)S, a)
+                                  : launch<CountHistBody<decltype(v), false>>(c, gx, (unsigned)S, a);
+  });
   if (e) return e;
   RT(rt_d2h(out, dh, (size_t)nbins * sizeof(long long), c->stream));
   RT(rt_sync(c->stream));
@@ -3151,7 +3226,8 @@ int cwtb_resident_shape(cwtb_ctx *c, int product, int *rows, int64_t *n0, int *p
   const ResidentSlot *s = product == CWTB_PRODUCT_W           ? &c->wt
                         : product == CWTB_PRODUCT_CROSS       ? &c->cross
                         : product == CWTB_PRODUCT_COHERENCE   ? &c->coh
-                        : product == CWTB_PRODUCT_COHERENCE3  ? &c->coh3 : nullptr;
+                        : product == CWTB_PRODUCT_COHERENCE3  ? &c->coh3
+                        : product == CWTB_PRODUCT_POWER       ? &c->pw : nullptr;
   if (!s) return fail(c, CWTB_ERR_ARG, "unknown product");
   const bool on = s->S > 0;
   if (rows) *rows = on ? s->S : 0;
@@ -3529,7 +3605,7 @@ int cwtb_mc_surrogates3(cwtb_ctx *c, uint64_t seed, int64_t first_triple, int n_
 static int phase_spectra(cwtb_ctx *c, const char *name, const double *series, int nser, const int *group,
                          int64_t first_unit, int n_units, int64_t n0, PhaseSrc *ph) {
   const std::string nm(name);
-  if (!c || !series || !group || (nser != 2 && nser != 3) || n0 < 4 || n_units < 0 || first_unit < 0 ||
+  if (!c || !series || !group || nser < 1 || nser > 3 || n0 < 4 || n_units < 0 || first_unit < 0 ||
       first_unit > (1ll << 61) - n_units)
     return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
   for (int r = 0; r < nser; ++r) {
@@ -3560,7 +3636,7 @@ int cwtb_wct_mc_phase(cwtb_ctx *c, const double *series, int nser, const int *gr
                       int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b) {
   if (nser == 2 && hist_b) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: two series have one histogram");
   if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc_phase needs an analytic wavelet family");
-  if (!mask || !(hist_a || hist_b)) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: bad argument");
+  if (!mask || !(hist_a || hist_b) || (nser != 2 && nser != 3)) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: bad argument");
   PhaseSrc ph{};
   int e = phase_spectra(c, "wct_mc_phase", series, nser, group, first_unit, n_units, n0, &ph);
   if (e) return e;
@@ -3571,7 +3647,7 @@ int cwtb_wct_mc_phase(cwtb_ctx *c, const double *series, int nser, const int *gr
 
 int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const int *group, uint64_t seed,
                              int64_t first_unit, int n_units, int64_t n0, double *out) {
-  if (!out || n_units < 1) return fail(c, CWTB_ERR_ARG, "mc_phase_surrogates: bad argument");
+  if (!out || n_units < 1 || (nser != 2 && nser != 3)) return fail(c, CWTB_ERR_ARG, "mc_phase_surrogates: bad argument");
   PhaseSrc ph{};
   int e = phase_spectra(c, "mc_phase_surrogates", series, nser, group, first_unit, n_units, n0, &ph);
   if (e) return e;
@@ -3849,6 +3925,250 @@ int cwtb_cluster_label_bits(cwtb_ctx *c, const uint32_t *bits, int n_scales, int
   if (labels) RT(rt_d2h(labels, c->scratch.p, (size_t)n_scales * n0 * sizeof(int), c->stream));
   RT(rt_sync(c->stream));
   return table_out(c, t, cap, count, Q, points, box);
+}
+
+// ---- AR(1) red-noise surrogates (Ar1BlockBody, Ar1CarryBody, Ar1WriteBody) ------------------------
+struct Ar1Src { double g, m, sigma; };
+
+static int ar1_check(cwtb_ctx *c, const std::string &nm, const Ar1Src &ar) {
+  if (!std::isfinite(ar.g) || !(std::fabs(ar.g) < 1.0) || !std::isfinite(ar.m) || !std::isfinite(ar.sigma))
+    return fail(c, CWTB_ERR_ARG, nm + ": the AR(1) parameters must be finite, with |g| < 1");
+  return 0;
+}
+
+extern "C++" {
+// nb AR(1) units from unit0 into out [nb][n0] (nb <= MAX_ROWS); c->arc holds the CTAs' carries
+template <typename T>
+static int ar1_units(cwtb_ctx *c, const Ar1Src &ar, unsigned long long seed, long long unit0, int nb, int64_t n0,
+                     T *out) {
+  const long long per = (long long)NT * AR1_CH;   // samples per CTA
+  const int nblk = (int)((n0 + per - 1) / per);
+  int e = ensure(c, c->arc, (size_t)nb * nblk * 2 * sizeof(double));
+  if (e) return e;
+  struct Tag { cwtb_ctx *c; ~Tag() { c->prof_tag = ""; } } tag{c};
+  c->prof_tag = "ar1:";
+  Ar1Args<T> a{out, (double *)c->arc.p, seed, unit0, (long long)n0, ar.g, std::sqrt((1.0 - ar.g) * (1.0 + ar.g)),
+               ar.m, ar.sigma, nblk, nb};
+  if ((e = launch<Ar1BlockBody<T>>(c, (unsigned)nblk, (unsigned)nb, a))) return e;
+  Ar1CarryArgs ca{(double *)c->arc.p, nblk, nb};
+  if ((e = launch<Ar1CarryBody>(c, (unsigned)((nb + NT - 1) / NT), 1, ca))) return e;
+  return launch<Ar1WriteBody<T>>(c, (unsigned)nblk, (unsigned)nb, a);
+}
+}  // extern "C++"
+
+int cwtb_mc_ar1_surrogates(cwtb_ctx *c, double g, double m, double sigma, uint64_t seed, int64_t first_unit,
+                           int n_units, int64_t n0, double *out) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = "mc_ar1_surrogates";
+  if (!out || n_units < 1 || n0 < 1 || first_unit < 0 || first_unit > (1ll << 61) - n_units)
+    return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  const Ar1Src ar{g, m, sigma};
+  int e = ar1_check(c, nm, ar);
+  if (e) return e;
+  RT(rt_set_device(c->device));
+  const size_t cnt = (size_t)n_units * n0;
+  if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
+  for (int i0 = 0; i0 < n_units; i0 += (int)MAX_ROWS) {
+    const int nb = std::min((int)MAX_ROWS, n_units - i0);
+    if ((e = ar1_units<double>(c, ar, seed, first_unit + i0, nb, n0, (double *)c->noise.p + (size_t)i0 * n0))) return e;
+  }
+  RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+// ---- tests of the resident power against surrogates -------------------------------------------
+// The null of a power test: AR(1) units, or phase-randomised units of the series (its spectrum in
+// c->pspec, phase group 0)
+struct PowerNull { int kind; Ar1Src ar; PhaseSrc ph; };
+
+static int power_null(cwtb_ctx *c, const std::string &nm, const double *series, int null, double g, double m,
+                      double sigma, int64_t first_unit, int n_units, int64_t n0, PowerNull &pn) {
+  pn = PowerNull{null, Ar1Src{g, m, sigma}, PhaseSrc{}};
+  if (null == CWTB_NULL_PHASE) {
+    const int group = 0;
+    return phase_spectra(c, nm.c_str(), series, 1, &group, first_unit, n_units, n0, &pn.ph);
+  }
+  if (null != CWTB_NULL_AR1) return fail(c, CWTB_ERR_ARG, nm + ": unknown null");
+  if (n_units < 0 || first_unit < 0 || first_unit > (1ll << 61) - n_units)
+    return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  int e = ar1_check(c, nm, pn.ar);
+  if (e) return e;
+  RT(rt_set_device(c->device));
+  return 0;
+}
+
+// the checks of the power tests against the resident power
+static int power_slot(cwtb_ctx *c, const std::string &nm, int64_t serial, int n_scales, int64_t n0, int family) {
+  const ResidentSlot &s = c->pw;
+  if (s.S <= 0 || !s.buf.p || serial != s.serial)
+    return fail(c, CWTB_ERR_STATE, nm + ": the serial is not that of the resident product");
+  if (n_scales != s.S || n0 != s.n0)
+    return fail(c, CWTB_ERR_STATE, nm + ": scales or length differ from the resident product's");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, nm + " needs an analytic wavelet family");
+  return 0;
+}
+
+extern "C++" {
+// PowerCountBody over the S x n0 field W: counts against obs into cnt (may be null), selection bits
+// (sel may be null)
+template <typename T>
+static int power_compare(cwtb_ctx *c, const void *W, const void *obs, unsigned *cnt, const SelArgs *sel, int S,
+                         int64_t n0) {
+  PowerCountArgs<T> a{(const cx<T> *)W, (const cx<T> *)obs, cnt, sel ? *sel : SelArgs{}, (long long)n0};
+  const unsigned gx = (unsigned)((n0 + NT - 1) / NT);
+  return sel ? launch<PowerCountBody<T, true>>(c, gx, (unsigned)S, a)
+             : launch<PowerCountBody<T, false>>(c, gx, (unsigned)S, a);
+}
+
+// The units [unit0, unit0 + n_units) of the null: each drawn, transformed with the resident power's
+// plan (one cwtb_cwt of it: one unit at a time, W in c->W) and compared with the resident W: counts
+// into cnt, or selection bits (sel) labelled right away, the unit's largest cluster into dqmax[i]
+template <typename T>
+static int power_units(cwtb_ctx *c, const PowerNull &pn, unsigned long long seed, long long unit0, int n_units,
+                       int64_t n0, double dt, const double *scales, int S, int family, double param, unsigned *cnt,
+                       const SelArgs *sel, const unsigned long long *dq, unsigned long long *dqmax) {
+  int e = prepare(c, n0, dt, scales, S, family, param, prec_of<T>(), nullptr);
+  if (e) return e;
+  const bool phase = pn.kind == CWTB_NULL_PHASE;
+  // the units of one draw: the rotated spectra of phase-randomised units take 16 B per sample
+  const size_t per = (size_t)n0 * (phase ? sizeof(double2) : sizeof(T));
+  const int batch = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_units, ((size_t)256 << 20) / per, (size_t)MAX_ROWS}));
+  if ((e = ensure(c, c->noise, (size_t)batch * n0 * sizeof(T)))) return e;
+  if (phase && (e = ensure(c, c->prot, (size_t)batch * n0 * sizeof(double2)))) return e;
+  c->launches = 0;
+  if ((e = time_begin(c))) return e;
+  for (int i0 = 0; i0 < n_units; i0 += batch) {
+    const int nb = std::min(batch, n_units - i0);
+    T *x = (T *)c->noise.p;
+    e = phase ? phase_units<T>(c, pn.ph, 1, seed, unit0 + i0, nb, n0, x) : ar1_units<T>(c, pn.ar, seed, unit0 + i0, nb, n0, x);
+    if (e) return e;
+    for (int i = 0; i < nb; ++i) {
+      // run_job joins its streams back into c->stream, where the comparisons of successive units
+      // follow each other: the counters and the selection bits have one writer at a time
+      if ((e = run_job<T>(c, c->job, x + (size_t)i * n0, nullptr, EPI_STORE))) return e;
+      if ((e = power_compare<T>(c, c->W.p, c->pw.buf.p, cnt, sel, S, n0))) return e;
+      if (sel && (e = label_bits(c, S, n0, dq, dqmax + i0 + i, nullptr, nullptr))) return e;
+    }
+  }
+  if ((e = time_end(c, &c->last_ms))) return e;
+  c->job_dsig = nullptr;
+  return 0;
+}
+}  // extern "C++"
+
+int cwtb_power_surrogate_counts(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
+                                uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                const double *scales, int n_scales, int family, double param, int64_t serial,
+                                int reset) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = "power_surrogate_counts";
+  ResidentSlot &s = c->pw;
+  int e = power_slot(c, nm, serial, n_scales, n0, family);
+  if (e) return e;
+  const long long base = reset || s.units < 0 ? 0 : s.units;
+  if (n_units < 0 || n_units > 0xFFFFFFFFll - base)
+    return fail(c, CWTB_ERR_ARG, nm + ": more units than a 32-bit counter holds");
+  PowerNull pn;
+  if ((e = power_null(c, nm, series, null, g, m, sigma, first_unit, n_units, n0, pn))) return e;
+  if ((e = ensure(c, s.counts, (size_t)s.S * s.n0 * sizeof(unsigned)))) return e;
+  s.units = -1;   // nothing readable until this call completes
+  if (base == 0) RT(rt_memset(s.counts.p, 0, s.counts.bytes, c->stream));
+  e = s.prec == CWTB_F32 ? power_units<float>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                                              (unsigned *)s.counts.p, nullptr, nullptr, nullptr)
+                         : power_units<double>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                                               (unsigned *)s.counts.p, nullptr, nullptr, nullptr);
+  if (e) return e;
+  RT(rt_sync(c->stream));
+  s.units = base + n_units;
+  return 0;
+}
+
+int cwtb_power_cluster_test(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
+                            uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                            const double *scales, int n_scales, int family, double param, int64_t serial,
+                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
+                            uint64_t *qmax_out) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = "power_cluster_test";
+  ResidentSlot &s = c->pw;
+  s.clusters = false;   // nothing readable until this call completes
+  s.table = ClusterTable{};
+  int e = power_slot(c, nm, serial, n_scales, n0, family);
+  if (e) return e;
+  if (!thr || n_units < 0 || (n_units > 0 && !qmax_out)) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  if ((e = cluster_shape(c, nm, n_scales, n0))) return e;
+  PowerNull pn;
+  if ((e = power_null(c, nm, series, null, g, m, sigma, first_unit, n_units, n0, pn))) return e;
+  SelArgs sel;
+  const unsigned long long *dq;
+  if ((e = cluster_rows(c, nm, n_scales, n0, thr, lo, hi, q, sel, dq))) return e;
+  if ((e = ensure(c, c->cl_qmax, (size_t)(n_units + 1) * sizeof(unsigned long long)))) return e;
+  if ((e = ensure(c, s.labels, (size_t)n_scales * n0 * sizeof(int)))) return e;
+  unsigned long long *dqmax = (unsigned long long *)c->cl_qmax.p;
+  RT(rt_memset(dqmax, 0, (size_t)(n_units + 1) * sizeof(unsigned long long), c->stream));
+  // the observed map: the comparison kernel's bits of the resident W, labelled as the units' are
+  // (every launch writes whole words: no bit past the last column is ever set)
+  e = s.prec == CWTB_F32 ? power_compare<float>(c, s.buf.p, nullptr, nullptr, &sel, n_scales, n0)
+                         : power_compare<double>(c, s.buf.p, nullptr, nullptr, &sel, n_scales, n0);
+  if (e) return e;
+  ClusterTable tab;
+  if ((e = label_bits(c, n_scales, n0, dq, dqmax + n_units, &tab, (int *)s.labels.p))) return e;
+  e = s.prec == CWTB_F32 ? power_units<float>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                                              nullptr, &sel, dq, dqmax)
+                         : power_units<double>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                                               nullptr, &sel, dq, dqmax);
+  if (e) return e;
+  if (n_units > 0) RT(rt_d2h(qmax_out, dqmax, (size_t)n_units * sizeof(unsigned long long), c->stream));
+  RT(rt_sync(c->stream));
+  s.table = std::move(tab);
+  s.clusters = true;
+  return 0;
+}
+
+int cwtb_power_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols, int64_t col_step,
+                      double *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_POWER, f);
+  if (e) return e;
+  if (!out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  f.power = true;
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, out, nullptr);
+}
+
+int cwtb_power_pvalue_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                             int64_t col_step, double *p_out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_POWER, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  if (!p_out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, p_out, nullptr);
+}
+
+int cwtb_power_pvalue_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, const double *thr, int64_t kmax,
+                                double *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_POWER, f);
+  if (e || (e = count_ref(c, kmax, f))) return e;
+  return row_stats_run(c, f, lo, hi, thr, 0, out);
+}
+
+int cwtb_power_count_hist(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, int64_t nbins, int64_t *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_POWER, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  return count_hist_run(c, f, lo, hi, nbins, out);
+}
+
+int cwtb_power_cluster_table(cwtb_ctx *c, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points, int64_t *box) {
+  int e = c ? clusters_of(c, c->pw, "power") : CWTB_ERR_ARG;
+  return e ? e : table_out(c, c->pw.table, cap, count, Q, points, box);
+}
+
+int cwtb_power_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                              int64_t col_step, int32_t *out) {
+  int e = c ? clusters_of(c, c->pw, "power") : CWTB_ERR_ARG;
+  return e ? e : labels_window(c, c->pw, row0, nrows, row_step, col0, ncols, col_step, out);
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

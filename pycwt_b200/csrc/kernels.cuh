@@ -1688,6 +1688,17 @@ HD void philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsign
   }
   o[0] = c0; o[1] = c1; o[2] = c2; o[3] = c3;
 }
+// Two standard normals (Box-Muller) from one Philox4x32-10 block: two 53-bit uniforms in (0, 1),
+// offset by half an ulp so that log() is finite
+HD void philox_normals(const unsigned (&o)[4], double &e0, double &e1) {
+  const double u1 = ((double)(o[0] >> 5) * 67108864.0 + (double)(o[1] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
+  const double u2 = ((double)(o[2] >> 5) * 67108864.0 + (double)(o[3] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
+  const double r = sqrt(-2.0 * log(u1));
+  double sn, cs;
+  sincospi_hd(2.0 * u2, &sn, &cs);
+  e0 = r * cs;
+  e1 = r * sn;
+}
 template <typename T> struct NoiseBody {
   using Args = NoiseArgs<T>;
   static constexpr int NPHASE = 1;
@@ -1702,15 +1713,11 @@ template <typename T> struct NoiseBody {
     unsigned o[4];
     philox4x32_10((unsigned)j, (unsigned)((unsigned long long)j >> 32), (unsigned)unit, c3,
                   (unsigned)a.seed, (unsigned)(a.seed >> 32), o);
-    // uniforms in (0, 1): 53 bits from two words, offset by half an ulp so that log() is finite
-    const double u1 = ((double)(o[0] >> 5) * 67108864.0 + (double)(o[1] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
-    const double u2 = ((double)(o[2] >> 5) * 67108864.0 + (double)(o[3] >> 6) + 0.5) * (1.0 / 9007199254740992.0);
-    const double r = sqrt(-2.0 * log(u1));
-    double sn, cs;
-    sincospi_hd(2.0 * u2, &sn, &cs);
+    double e0, e1;
+    philox_normals(o, e0, e1);
     T *dst = a.out + (size_t)by * a.n + 2 * j;
-    dst[0] = (T)(r * cs);
-    if (2 * j + 1 < a.n) dst[1] = (T)(r * sn);
+    dst[0] = (T)e0;
+    if (2 * j + 1 < a.n) dst[1] = (T)e1;
   }
 };
 
@@ -1763,6 +1770,125 @@ struct PhaseRotBody {
     const double2 r = make_double2(x.x * cs - x.y * sn, x.x * sn + x.y * cs);
     dst[k] = r;
     dst[a.n - k] = make_double2(r.x, -r.y);
+  }
+};
+
+// ---- Bodies: AR(1) red-noise surrogates on the device (the power test's red-noise null) ----------
+// Unit u of length n is x = m + sigma z with z[0] = e[0], z[i] = g z[i-1] + sqrt(1 - g^2) e[i] (the
+// background of Torrence & Compo 1998, section 4), |g| < 1.  e[2j], e[2j+1] are the two normals of
+// one Philox4x32-10 block (philox_normals, NoiseBody's conversion), a pure function of (seed, u, j):
+// counter words (j, 2^31, u lo, 2^31 | (u hi << 2) | 3).  PhaseRotBody's second word is a phase
+// group below 2^31 and NoiseBody's a sample index below 2^26, so bit 31 of the second word keeps this
+// stream apart from both for 0 <= u < 2^61 (j < 2^31).
+// The recurrence is a linear scan over the whole series: z_end = g^L z_start + b over a stretch of L
+// samples, b its end state from a zero start.  A thread owns AR1_CH consecutive samples (whole
+// normal pairs), a CTA NT of those stretches.  Ar1BlockBody forms every CTA's (g^L, b), Ar1CarryBody
+// chains them per unit into each CTA's carry-in, Ar1WriteBody redraws the normals from the thread's
+// carry-in and writes x once.  The carries are in double and |g| < 1, so a rounding error decays
+// along the series instead of growing.  The draw is in double for every T (fp32: the fp64 surrogate
+// rounded).  The stretches depend on NT, the draws (seed, u, j) do not.
+constexpr int AR1_CH = 32;   // samples per thread (even)
+template <typename T> struct Ar1Args {
+  T *out;                   // [n_units][n]
+  double *blk;              // [n_units][nblk][2]: (g^L, b) of each CTA, then (., carry-in)
+  unsigned long long seed;
+  long long unit0;          // global index of the first unit
+  long long n;
+  double g, s, m, sigma;    // s = sqrt(1 - g^2)
+  int nblk, n_units;
+};
+// Samples [i0, i1) of unit `unit` from the state z before i0: the state after i1 - 1, and x into dst
+// (null: nothing written)
+template <typename T>
+HD double ar1_run(const Ar1Args<T> &a, unsigned long long unit, long long i0, long long i1, double z, T *dst) {
+  for (long long i = i0; i < i1; i += 2) {
+    unsigned o[4];
+    philox4x32_10((unsigned)(i >> 1), 0x80000000u, (unsigned)unit, 0x80000000u | ((unsigned)(unit >> 32) << 2) | 3u,
+                  (unsigned)a.seed, (unsigned)(a.seed >> 32), o);
+    double e0, e1;
+    philox_normals(o, e0, e1);
+    z = i == 0 ? e0 : fma(a.g, z, a.s * e0);
+    if (dst) dst[i] = (T)(a.m + a.sigma * z);
+    if (i + 1 < i1) {
+      z = fma(a.g, z, a.s * e1);
+      if (dst) dst[i + 1] = (T)(a.m + a.sigma * z);
+    }
+  }
+  return z;
+}
+// the samples [i0, i1) of thread tid of CTA bx, and g^(i1 - i0)
+template <typename T> HD double ar1_span(const Ar1Args<T> &a, int bx, int tid, long long &i0, long long &i1) {
+  i0 = ((long long)bx * NT + tid) * AR1_CH;
+  i1 = i0 + AR1_CH < a.n ? i0 + AR1_CH : a.n;
+  double p = 1.0;
+  for (long long i = i0; i < i1; ++i) p *= a.g;
+  return p;
+}
+// (g^L, b) of the thread's stretch into sm [2][NT]
+template <typename T> HD void ar1_local(const Ar1Args<T> &a, int bx, int by, int tid, double *sm) {
+  long long i0, i1;
+  sm[tid] = ar1_span(a, bx, tid, i0, i1);
+  sm[NT + tid] = ar1_run<T>(a, (unsigned long long)(a.unit0 + by), i0, i1, 0.0, nullptr);
+}
+template <typename T> struct Ar1BlockBody {   // grid (nblk, n_units)
+  using Args = Ar1Args<T>;
+  static constexpr int NPHASE = 2;
+  static constexpr size_t SMEM = 2 * NT * sizeof(double);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double *sm = (double *)smraw;
+    if constexpr (PH == 0) {
+      ar1_local(a, bx, by, tid, sm);
+    } else if (tid == 0) {
+      double A = 1.0, B = 0.0;
+      for (int t = 0; t < NT; ++t) {
+        B = fma(sm[t], B, sm[NT + t]);
+        A *= sm[t];
+      }
+      double *d = a.blk + 2 * ((size_t)by * a.nblk + bx);
+      d[0] = A;
+      d[1] = B;
+    }
+  }
+};
+struct Ar1CarryArgs { double *blk; int nblk, n_units; };
+struct Ar1CarryBody {   // one thread per unit
+  using Args = Ar1CarryArgs;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int, int tid, void *) {
+    const int u = bx * NT + tid;
+    if (u >= a.n_units) return;
+    double *d = a.blk + 2 * (size_t)u * a.nblk;
+    double z = 0.0;
+    for (int b = 0; b < a.nblk; ++b) {
+      const double A = d[2 * b], B = d[2 * b + 1];
+      d[2 * b + 1] = z;
+      z = fma(A, z, B);
+    }
+  }
+};
+template <typename T> struct Ar1WriteBody {   // grid (nblk, n_units)
+  using Args = Ar1Args<T>;
+  static constexpr int NPHASE = 3;
+  static constexpr size_t SMEM = 2 * NT * sizeof(double);
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *smraw) {
+    double *sm = (double *)smraw;
+    if constexpr (PH == 0) {
+      ar1_local(a, bx, by, tid, sm);
+    } else if constexpr (PH == 1) {
+      if (tid == 0) {   // each thread's carry-in into sm[NT + t]
+        double z = a.blk[2 * ((size_t)by * a.nblk + bx) + 1];
+        for (int t = 0; t < NT; ++t) {
+          const double A = sm[t], B = sm[NT + t];
+          sm[NT + t] = z;
+          z = fma(A, z, B);
+        }
+      }
+    } else {
+      long long i0, i1;
+      ar1_span(a, bx, tid, i0, i1);
+      ar1_run<T>(a, (unsigned long long)(a.unit0 + by), i0, i1, sm[NT + tid], a.out + (size_t)by * a.n);
+    }
   }
 };
 
@@ -1867,6 +1993,43 @@ struct ThreshBitsBody {
     if (n0 >= a.n) return;   // the whole warp
     const bool p = n < a.n && cluster_sel(a.sel, by, n, ld_stream(&a.R[(size_t)by * a.n + n]));
     sel_store(a.sel, by, n, 32, p, ~0u);
+  }
+};
+
+// ---- the wavelet power |W|^2 of a coefficient, as the power test compares and selects it ---------
+// Every read of the resident power's tests forms P through this one function, the observed and the
+// surrogate power alike, so their comparison is bit-consistent: double products rounded on their own
+// (no contraction), exact for the widened parts of an fp32 W.  The same arithmetic as CxView's |F|^2.
+template <typename T> HD double power_of(const cx<T> &v) { return norm2_rn((double)v.x, (double)v.y); }
+
+// ---- Body: a surrogate unit's power against the resident power (cwtb_power_surrogate_counts /
+// _cluster_test) ---------------------------------------------------------------------------------
+// One thread per column of row by, a warp's lanes 32 aligned columns.  With cnt: k += 1 where the
+// unit's P_i >= P_obs or P_i is not finite (count_exceed's rule; no atomics: the count launches of
+// successive units run in order on one stream).  SEL: the selection bits of P (cluster_sel).  The
+// observed map's bits are this kernel on the resident W without counters.
+template <typename T> struct PowerCountArgs {
+  const cx<T> *W;           // [rows][n] the unit's transform
+  const cx<T> *obs;         // [rows][n] the resident W (with cnt)
+  unsigned *cnt;            // [rows][n] exceedance counters, or null
+  SelArgs sel;
+  long long n;
+};
+template <typename T, bool SEL> struct PowerCountBody {
+  using Args = PowerCountArgs<T>;
+  static constexpr int NPHASE = 1;
+  static constexpr size_t SMEM = 0;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    const long long n0 = (long long)bx * NT + (tid & ~31), n = n0 + (tid & 31);
+    if (n0 >= a.n) return;   // the whole warp
+    bool p = false;
+    if (n < a.n) {
+      const size_t o = (size_t)by * a.n + n;
+      const double P = power_of<T>(ld_stream(&a.W[o]));
+      if (a.cnt && (!isfinite(P) || P >= power_of<T>(ld_stream(&a.obs[o])))) a.cnt[o] += 1u;
+      p = SEL && cluster_sel(a.sel, by, n, P);
+    }
+    if constexpr (SEL) sel_store(a.sel, by, n, 32, p, ~0u);
   }
 };
 
@@ -2388,6 +2551,7 @@ template <bool PHASE> struct CohCountViewT {
     const double w = WCT[src];
     o0[dst] = isfinite(w) ? (double)(1 + (long long)cnt[src]) / (double)(1 + m) : w - w;   // inf - inf: NaN
   }
+  HD bool finite(size_t o) const { return isfinite(ld_stream(&WCT[o])); }   // CountHistBody
 };
 
 // 16 bytes of a complex field: one double2, or two float2
@@ -2447,6 +2611,47 @@ template <typename T> struct CxView {
     const cx<T> v = F[src];
     ((double2 *)o0)[dst] = make_double2((double)v.x, (double)v.y);
   }
+};
+
+// The power P = power_of(F) of a complex field, as the power tests form it.  Window: P to o0.
+template <typename T> struct CxPowerView {
+  const cx<T> *F;
+  HD void copy(size_t src, double *o0, double *, size_t dst) const { o0[dst] = power_of<T>(F[src]); }
+};
+
+// A complex field with the surrogate exceedance counts of its power P = power_of(F) (the resident
+// power, cwtb_power_surrogate_counts), CohCountViewT's counterpart.  Row stats: CxView's five sums
+// over the points whose P is finite, whose k <= kmax and, with a threshold, whose P > thr_j.  Window:
+// the p-value (1 + k) / (1 + M) to o0, NaN where P is not finite.
+template <typename T> struct CxCountView {
+  const cx<T> *F;
+  const unsigned *cnt;
+  long long kmax, m;
+  using V16 = CxVec16<T>;
+  static constexpr int K = CxView<T>::K, E = V16::E, VPT = 32;
+  struct Vec { typename V16::V w; unsigned k[E]; };
+  HD Vec load(size_t q) const {
+    Vec v;
+    v.w = ld_stream((const typename V16::V *)F + q);
+#pragma unroll
+    for (int e = 0; e < E; ++e) v.k[e] = ld_stream(&cnt[q * E + e]);
+    return v;
+  }
+  HD void add1(double (&s)[K], double re, double im, unsigned k, bool has_thr, double t) const {
+    if (!isfinite(norm2_rn(re, im)) || (long long)k > kmax) return;
+    CxView<T>::add1(s, re, im, has_thr, t);
+  }
+  HD void add(double (&s)[K], const Vec &v, int e, bool has_thr, double t) const {
+    add1(s, V16::re(v.w, e), V16::im(v.w, e), v.k[e], has_thr, t);
+  }
+  HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
+    add1(s, F[p].x, F[p].y, cnt[p], has_thr, t);
+  }
+  HD void copy(size_t src, double *o0, double *, size_t dst) const {
+    const double P = power_of<T>(F[src]);
+    o0[dst] = isfinite(P) ? (double)(1 + (long long)cnt[src]) / (double)(1 + m) : P - P;   // inf - inf: NaN
+  }
+  HD bool finite(size_t o) const { return isfinite(power_of<T>(ld_stream(&F[o]))); }   // CountHistBody
 };
 
 // Per-row sums of a view over the columns [lo_j, hi_j) where thr is null or the view's point
@@ -2598,20 +2803,20 @@ template <typename View> struct WindowBody {
 };
 
 // ---- Body: histogram of the exceedance counts k in [0, nb) over the columns [lo_j, hi_j) of every
-// row, of the points whose observed value is finite (cwtb_coherence*_count_hist) -------------------
+// row, of the points whose observed value is finite (cwtb_coherence*_count_hist, cwtb_power_count_hist)
 // CTA (bx, j) covers the chunk [lo_j + bx CHUNK, lo_j + (bx + 1) CHUNK) of row j.  SHARED: the CTA
 // counts into a uint32 histogram in shared memory (nb <= SMEM_BINS) and adds its non-zero bins to
 // the 64-bit global histogram at the end; otherwise every point is one 64-bit atomic in global
 // memory.  Integer sums: the result does not depend on the order, repeated calls are bit-identical.
-struct CountHistArgs {
-  const double *obs;
-  const unsigned *cnt;
+// View: a counting view (CohCountViewT, CxCountView): its counts and finite().
+template <typename View> struct CountHistArgs {
+  View f;
   const long long *lo, *hi;   // per row
   unsigned long long *hist;   // [nb], zeroed by the caller
   long long n, nb;
 };
-template <bool SHARED> struct CountHistBody {
-  using Args = CountHistArgs;
+template <typename View, bool SHARED> struct CountHistBody {
+  using Args = CountHistArgs<View>;
   static constexpr int NPHASE = SHARED ? 3 : 1;
   static constexpr int SMEM_BINS = 12288;                  // 48 KiB: four CTAs per SM
   static constexpr long long CHUNK = 32LL * NT;
@@ -2625,8 +2830,8 @@ template <bool SHARED> struct CountHistBody {
       const long long c1 = c0 + CHUNK < a.hi[by] ? c0 + CHUNK : a.hi[by];
       for (long long n = c0 + tid; n < c1; n += NT) {
         const size_t o = (size_t)by * a.n + n;
-        if (!isfinite(ld_stream(&a.obs[o]))) continue;
-        const unsigned k = ld_stream(&a.cnt[o]);
+        if (!a.f.finite(o)) continue;
+        const unsigned k = ld_stream(&a.f.cnt[o]);
 #if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
         if constexpr (SHARED) atomicAdd(&sh[k], 1u);
         else atomicAdd(&a.hist[k], 1ull);

@@ -15,7 +15,8 @@ methods evaluate those products on the device, so only O(S) or O(N) numbers cros
 The handle is valid until the next transform on the same engine.
 
 `wct_resident` does the same for the wavelet coherence, `xwt_resident` for the cross-wavelet
-transform and `wct3_resident` for the partial and multiple coherence of three series (see the
+transform, `wct3_resident` for the partial and multiple coherence of three series and
+`power_resident` for the wavelet power of one series with its tests against surrogates (see the
 second half of this module).
 """
 import collections
@@ -25,15 +26,15 @@ import numpy as np
 from . import _engine
 from . import helpers as _helpers
 from .helpers import ar1, fft, fft_kwargs
-from .wavelet import (_check_parameter_wavelet, _coi, _mc_levels, _nan_rows, _precision,
-                      _resolve_scales, _surrogate_histogram, _surrogate_problem, _surrogate_seed,
+from .wavelet import (_check_parameter_wavelet, _coherence_precision, _coi, _mc_levels, _nan_rows,
+                      _precision, _resolve_scales, _standardise, _surrogate_histogram, _surrogate_problem, _surrogate_seed,
                       _sync_padding, _wct_on_device, _wct_problem, _wct_significance,
                       _xwt_on_device, _xwt_problem, _xwt_signif, wct3_significance,
                       wct3_surrogate_significance, wct_surrogate_significance)
 
 __all__ = ['cwt_resident', 'ResidentTransform', 'wct_resident', 'ResidentCoherence',
            'xwt_resident', 'ResidentCrossWavelet', 'wct3_resident', 'ResidentCoherence3',
-           'FdrResult', 'ClusterResult']
+           'power_resident', 'ResidentPower', 'FdrResult', 'ClusterResult']
 
 
 def _coi_ranges(wavelet, dt, n0, period):
@@ -124,8 +125,9 @@ class _ResidentSlot(_Resident):
 
     def release(self):
         """Free the device buffer (16 bytes per scale and time point for a coherence, 24 for a
-        partial and multiple coherence, 16 or 8 for a cross spectrum).  The handle is invalid
-        afterwards; releasing an invalid handle does nothing."""
+        partial and multiple coherence, 16 or 8 for a cross spectrum or a power, whose tests add 4
+        for the counts and 4 for the cluster labels).  The handle is invalid afterwards; releasing
+        an invalid handle does nothing."""
         with self.engine.lock:
             if getattr(self.engine, self._SERIAL)() == self._serial:
                 getattr(self.engine, self._RELEASE)()
@@ -224,27 +226,39 @@ class ResidentTransform(_Resident):
         return out
 
 
+def _engine_wavelet(wavelet, name):
+    """(wavelet, (family, param)) of a resident transform: TypeError for a wavelet the engine does
+    not evaluate itself."""
+    wavelet = _check_parameter_wavelet(wavelet)
+    spec = wavelet._engine_spec() if hasattr(wavelet, '_engine_spec') else None
+    if spec is None:
+        # duck-typed objects, subclasses that override psi_ft, non-integer or out-of-range orders
+        raise TypeError("%s needs one of the analytic families the engine evaluates "
+                        "itself: Morlet(f0), Paul(m) or DOG(m) with an integer order in [1, 64] "
+                        "and the stock psi_ft" % name)
+    return wavelet, spec
+
+
+def _kept_scales(n0, dt, dj, s0, J, wavelet, freqs):
+    """(scales, freqs) of `cwt` for an n0-point series: without the rows the reference drops as
+    all-NaN (Paul at very large scales)."""
+    sj, freqs = _resolve_scales(n0, dt, dj, s0, J, wavelet, freqs)
+    npad = fft_kwargs(range(n0))['n']
+    keep = ~_nan_rows(wavelet, np.asarray(sj, dtype=float), npad, dt)
+    if not keep.any():
+        raise ValueError("every scale of this transform is NaN in the reference")
+    return sj[keep], freqs[keep]
+
+
 def cwt_resident(signal, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', freqs=None, engine=None):
     """Same transform as `cwt` (reference wavelet.py:13-124), W kept on the device.
 
     Returns a `ResidentTransform`.  Scales whose row the reference would drop as all-NaN
     (Paul at very large scales) are dropped here as well, so `.scales` / `.freqs` equal the
     ones `cwt` returns."""
-    wavelet = _check_parameter_wavelet(wavelet)
-    spec = wavelet._engine_spec() if hasattr(wavelet, '_engine_spec') else None
-    if spec is None:
-        # duck-typed objects, subclasses that override psi_ft, non-integer or out-of-range orders
-        raise TypeError("cwt_resident needs one of the analytic families the engine evaluates "
-                        "itself: Morlet(f0), Paul(m) or DOG(m) with an integer order in [1, 64] "
-                        "and the stock psi_ft")
+    wavelet, spec = _engine_wavelet(wavelet, "cwt_resident")
     n0 = len(signal)
-    sj, freqs = _resolve_scales(n0, dt, dj, s0, J, wavelet, freqs)
-    npad = fft_kwargs(signal)['n']
-    keep = ~_nan_rows(wavelet, np.asarray(sj, dtype=float), npad, dt)
-    if keep.any():
-        sj, freqs = sj[keep], freqs[keep]
-    else:
-        raise ValueError("every scale of this transform is NaN in the reference")
+    sj, freqs = _kept_scales(n0, dt, dj, s0, J, wavelet, freqs)
     eng = engine or _engine.default_engine()
     sig = np.asarray(signal)
     if sig.dtype != np.float32:
@@ -399,11 +413,12 @@ def _cluster_weights(h):
 
 
 class _SurrogateTest(object):
-    """The point-wise and cluster tests of a resident coherence product: the counts of its last
+    """The point-wise and cluster tests of a resident product: the counts of its last
     `surrogate_test`, the clusters of its last `cluster_test`, and what is read from them.  A
-    subclass names its measures (`_MEASURE_OF`: None for the coherence) and whether its product is
-    the engine's partial and multiple coherence (`_TRIPLE`), whose clusters the engine keeps apart
-    from the coherence's."""
+    subclass names the engine's clusters of its product (`_CLUSTERS`: False for the coherence, True
+    for the partial and multiple coherence, `_engine.POWER` for the power), passes its measure to
+    the readers (None for the coherence, `_engine.POWER` for the power) and runs its units on the
+    device (`_count_units`, `_cluster_units`)."""
 
     _UNTESTED = ("no surrogate test has counted for this product: call surrogate_test first")
     surrogate_seed = None     # seed and M of the last surrogate_test
@@ -419,29 +434,17 @@ class _SurrogateTest(object):
                              "counts would not compare like with like")
         return _surrogate_seed(seed)
 
-    def _cluster(self, sig, mc_count, seed, groups, inside_coi, measure):
-        """ClusterResult of a cluster test of units 0 .. mc_count - 1 (the caller holds the lock)."""
+    def _cluster(self, sig, mc_count, seed, inside_coi, *args):
+        """ClusterResult of a cluster test of units 0 .. mc_count - 1 (the caller holds the lock);
+        `args` go to `_cluster_units`."""
         thr = self._threshold(sig)
         if thr is None:
             raise ValueError("cluster_test needs a per-scale threshold sig")
         seed = self._seed_of_run(mc_count, seed)
-        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
-                                     self.normalize, self.precision)
         lo, hi = _column_ranges(self, inside_coi)
         q, unit_area = _cluster_weights(self)
-        nser = len(p.yns)
-        hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
-        eng = self.engine
-
-        def call(*a, boxcar_len, precision):
-            dt, _, sj, family, param = a[nser:]
-            return eng.cluster_test(np.stack(a[:nser]), groups, seed, 0, int(mc_count), dt, sj, family,
-                                    param, boxcar_len, prob['mask'], prob['maxscale'], prob['nbins'],
-                                    *hist, serial=self._serial, thr=thr, lo=lo, hi=hi, q=q,
-                                    measure=measure, precision=precision)
-
-        qmax = _wct_on_device(eng, p, call)
-        Q, pts, box = eng.cluster_table(self._TRIPLE)
+        qmax = self._cluster_units(seed, int(mc_count), thr, lo, hi, q, *args)
+        Q, pts, box = self.engine.cluster_table(self._CLUSTERS)
         M = int(mc_count)
         reached = M - np.searchsorted(np.sort(qmax), Q, side='left')
         return ClusterResult(Q.astype(float) * unit_area, pts, box[:, 0:2], box[:, 2:4],
@@ -453,18 +456,16 @@ class _SurrogateTest(object):
         c0, nc, cs = _slice_range(cols, n0, 'cols')
         if nr == 0 or nc == 0:
             return np.empty((nr, nc), dtype=np.int32)
-        return self.engine.cluster_labels(self._TRIPLE, r0, nr, rs, c0, nc, cs)
+        return self.engine.cluster_labels(self._CLUSTERS, r0, nr, rs, c0, nc, cs)
 
-    def _count(self, mc_count, seed, groups):
-        """(prob, hist) of a counting run of units 0 .. mc_count - 1 (the caller holds the lock)."""
+    def _count(self, mc_count, seed, *args):
+        """What `_count_units` returns for a counting run of units 0 .. mc_count - 1 (the caller
+        holds the lock)."""
         seed = self._seed_of_run(mc_count, seed)
-        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
-                                     self.normalize, self.precision)
         self.surrogate_seed = self.surrogate_units = None
-        hist = _surrogate_histogram(p, prob, groups, seed, 0, int(mc_count), engine=self.engine,
-                                    serial=self._serial)
+        out = self._count_units(seed, int(mc_count), *args)
         self.surrogate_seed, self.surrogate_units = seed, int(mc_count)
-        return prob, hist
+        return out
 
     def _units(self):
         if self.surrogate_units is None:
@@ -502,7 +503,37 @@ class _SurrogateTest(object):
         return _fdr(self.engine.count_hist(measure, lo, hi, M + 1), M, q, method)
 
 
-class ResidentCoherence(_SurrogateTest, _ResidentSlot):
+class _CoherenceTest(_SurrogateTest):
+    """The units of the coherence products' tests: the phase-randomised surrogates of their series
+    through the whole coherence pipeline, with the Monte-Carlo histograms of `_surrogate_problem`."""
+
+    def _count_units(self, seed, M, groups):
+        """(prob, hist) of a counting run."""
+        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
+                                     self.normalize, self.precision)
+        hist = _surrogate_histogram(p, prob, groups, seed, 0, M, engine=self.engine,
+                                    serial=self._serial)
+        return prob, hist
+
+    def _cluster_units(self, seed, M, thr, lo, hi, q, groups, measure):
+        """The units' largest cluster sums, uint64 [M]."""
+        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
+                                     self.normalize, self.precision)
+        nser = len(p.yns)
+        hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
+        eng = self.engine
+
+        def call(*a, boxcar_len, precision):
+            dt, _, sj, family, param = a[nser:]
+            return eng.cluster_test(np.stack(a[:nser]), groups, seed, 0, M, dt, sj, family,
+                                    param, boxcar_len, prob['mask'], prob['maxscale'], prob['nbins'],
+                                    *hist, serial=self._serial, thr=thr, lo=lo, hi=hi, q=q,
+                                    measure=measure, precision=precision)
+
+        return _wct_on_device(eng, p, call)
+
+
+class ResidentCoherence(_CoherenceTest, _ResidentSlot):
     """WCT and aWCT [S, n0] of one `wct_resident` call, resident on the device.
 
     Point-wise test: `surrogate_test(mc_count=M, seed=seed)` runs the surrogate pairs 0 .. M - 1 of
@@ -517,7 +548,7 @@ class ResidentCoherence(_SurrogateTest, _ResidentSlot):
     `release()` or `wct_resident` on the same engine."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence_serial', 'coherence_release'
-    _TRIPLE = False
+    _CLUSTERS = False
     _GONE = ("this coherence is no longer resident: it was released or another wct_resident has "
              "run on the same engine")
 
@@ -693,7 +724,7 @@ class ResidentCoherence(_SurrogateTest, _ResidentSlot):
         the device (`cluster_labels`, 4 bytes per scale-point) until the next `cluster_test`,
         `release()` or `wct_resident`.  ValueError for a `sig` without one entry per scale and for
         the checks of `surrogate_test`; the counts of an earlier `surrogate_test` are kept."""
-        return self._cluster(sig, mc_count, seed, (0, 1), inside_coi, None)
+        return self._cluster(sig, mc_count, seed, inside_coi, (0, 1), None)
 
     @_live
     def cluster_labels(self, rows=slice(None), cols=slice(None)):
@@ -825,7 +856,7 @@ def xwt_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95, wave
 _MEASURES = {'partial': _engine.MEASURE_PARTIAL, 'multiple': _engine.MEASURE_MULTIPLE}
 
 
-class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
+class ResidentCoherence3(_CoherenceTest, _ResidentSlot):
     """RP2, the partial phase and RM2 [S, n0] of one `wct3_resident` call, resident on the device.
 
     The partial phase is the angle of the smoothed partial cross spectrum of y and x1 with x2
@@ -844,7 +875,7 @@ class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
     `ResidentCoherence` (8 bytes per scale-point on the device for the two measures)."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'coherence3_serial', 'coherence3_release'
-    _TRIPLE = True
+    _CLUSTERS = True
     _GONE = ("this partial / multiple coherence is no longer resident: it was released or another "
              "wct3_resident has run on the same engine")
 
@@ -1020,7 +1051,7 @@ class ResidentCoherence3(_SurrogateTest, _ResidentSlot):
         0 .. mc_count - 1 of `surrogate_significance(mc_count=mc_count, seed=seed,
         conditional=conditional)`; `sig` in the units of the measure."""
         m = self._measure(measure)
-        return self._cluster(sig, mc_count, seed, (0, 1, 1) if conditional else (0, 1, 2), inside_coi, m)
+        return self._cluster(sig, mc_count, seed, inside_coi, (0, 1, 1) if conditional else (0, 1, 2), m)
 
     @_live
     def cluster_labels(self, rows=slice(None), cols=slice(None)):
@@ -1042,3 +1073,197 @@ def wct3_resident(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normali
     eng = engine or _engine.default_engine()
     serial = _wct_on_device(eng, p, eng.wct3_resident)
     return ResidentCoherence3(eng, p, normalize, precision, serial)
+
+
+# ---- resident wavelet power and its tests against surrogates --------------------------------------
+# The wavelet power |W|^2 of one series is the map a user draws most; its classic test is the
+# per-scale chi-squared level of `significance()` (TC98 eq. 18), which, applied point by point, paints
+# many spurious patches (Maraun et al. 2007).  `power_resident` keeps W in a device buffer of its own
+# (the handle survives later cwt / xwt / wct / Monte-Carlo calls, until the next `power_resident` or
+# `release()`) and tests it point by point and patch by patch against surrogates drawn on the device:
+#   'ar1'    red noise x = m + sigma z, z[0] = e[0], z[n] = g z[n-1] + sqrt(1 - g^2) e[n], with
+#            g = ar1(series)[0] (the background `significance()` assumes), m = 0 and sigma = 1 for
+#            normalize=True, else the series' mean and standard deviation (ddof 0);
+#   'phase'  the phase-randomised surrogates of the transformed series (the periodogram kept
+#            exactly): is the *local* power larger than a stationary process with the data's own
+#            spectrum would give?
+# Each unit is transformed with the handle's plan, exactly as `cwt` of it would be, and its power is
+# compared with the resident one on every point (`surrogate_test`) or labelled into clusters
+# (`cluster_test`), with the definitions of `ResidentCoherence`.
+
+_NULLS = {'ar1': _engine.NULL_AR1, 'phase': _engine.NULL_PHASE}
+
+
+class ResidentPower(_SurrogateTest, _ResidentSlot):
+    """W[S, n0] of one `power_resident` call, resident on the device, and the tests of its power
+    P = |W|^2.
+
+    `signif` arguments are per-scale thresholds in power units, as `significance()` returns them:
+    with normalize=True, `significance(1.0, dt, scales, 0, g)[0]` (g = ar1(series)[0]); with
+    normalize=False, `significance(series, dt, scales, 0)[0]`.  A point is selected where
+    P > signif[j]; a negative entry raises ValueError, a NaN entry selects no point of its scale.
+
+    Point-wise test: `surrogate_test(mc_count=M, seed=s, null=...)` counts, per point, the units
+    0 .. M - 1 of the null whose power reaches this one, k[s, n] = #{i : P_i[s, n] >= P[s, n]} (a
+    non-finite P_i counts), p = (1 + k) / (1 + M), NaN where P is not finite; the counts take 4 bytes
+    per scale-point on the device.  The readers, FDR control and the cluster test are those of
+    `ResidentCoherence` with P in place of the coherence.  There are no per-scale Monte-Carlo levels:
+    the cluster-forming threshold is the caller's, typically the chi-squared level of
+    `significance()`."""
+
+    _FREQ, _SERIAL, _RELEASE = 'freqs', 'power_serial', 'power_release'
+    _CLUSTERS = _engine.POWER
+    _GONE = ("this power is no longer resident: it was released or another power_resident has run "
+             "on the same engine")
+
+    def __init__(self, engine, wavelet, y, yn, dt, dj, sj, freqs, normalize, precision, serial):
+        super(ResidentPower, self).__init__(engine, wavelet, len(yn), dt, dj, sj, precision, serial)
+        self.freqs = freqs
+        self.normalize = normalize
+        self._y = np.array(y, dtype=np.float64, copy=True)     # raw series: ar1, mean and std
+        self._yn = np.array(yn, dtype=np.float64, copy=True)   # the transformed series: phase null
+        self._padding = bool(_helpers._FFT_NEXT_POW2)
+
+    def _threshold(self, signif):
+        return None if signif is None else _power_threshold(self, signif)
+
+    def _null(self, null):
+        """(engine null, g, m, sigma) of a null's name."""
+        if null not in _NULLS:
+            raise ValueError("null must be 'ar1' or 'phase', got %r" % (null,))
+        g = ar1(self._y)[0] if null == 'ar1' else 0.0
+        m, sigma = (0.0, 1.0) if self.normalize else (float(self._y.mean()), float(self._y.std()))
+        return _NULLS[null], g, m, sigma
+
+    def _on_device(self, call, null, seed, M, *args):
+        kind, g, m, sigma = self._null(null)
+        eng = self.engine
+        _sync_padding(eng, self.n0)
+        return call(self._yn, kind, g, m, sigma, seed, 0, M, self.dt, self.scales,
+                    *self.wavelet._engine_spec(), self._serial, *args)
+
+    def _count_units(self, seed, M, null):
+        self._on_device(self.engine.power_surrogate_counts, null, seed, M)
+
+    def _cluster_units(self, seed, M, thr, lo, hi, q, null):
+        return self._on_device(self.engine.power_cluster_test, null, seed, M, thr, lo, hi, q)
+
+    # -- the products --------------------------------------------------------------------
+    @_live
+    def wave(self):
+        """The coefficients themselves (complex128, S x n0): the expensive fetch."""
+        return self.engine.field_get(_engine.FIELD_POWER)
+
+    @_live
+    def power(self, rows=slice(None), cols=slice(None)):
+        """|W|^2[rows, cols] (float64) for two slices with steps >= 1, formed on the device exactly as
+        the tests form it (re^2 + im^2 in double): 8 bytes per point cross the bus.  The whole map
+        is the expensive fetch."""
+        S, n0 = self.shape
+        r0, nr, rs = _slice_range(rows, S, 'rows')
+        c0, nc, cs = _slice_range(cols, n0, 'cols')
+        out = np.empty((nr, nc))
+        # in blocks of rows, so that the device staging stays below 2^25 points
+        step = max(1, (1 << 25) // max(nc, 1))
+        for b in range(0, nr, step):
+            k = min(step, nr - b)
+            out[b:b + k] = self.engine.power_window(r0 + b * rs, k, rs, c0, nc, cs)
+        return out
+
+    @_live
+    def window(self, rows=slice(None), cols=slice(None)):
+        """W[rows, cols] (complex128) for two slices with steps >= 1, gathered on the device."""
+        return _field_window(self.engine, _engine.FIELD_POWER, self.shape, rows, cols)
+
+    @_live
+    def global_power(self, inside_coi=False, signif=None, alpha=None):
+        """Time mean of |W|^2 per scale over the selected points: inside the cone of influence if
+        `inside_coi`, where |W|^2 > signif[j] if `signif` is given, where the p-value of the last
+        `surrogate_test` is <= alpha if `alpha` is given (all: logical AND).  NaN for a scale
+        without points."""
+        lo, hi = _column_ranges(self, inside_coi)
+        thr = self._threshold(signif)
+        if alpha is not None:
+            st = self._cut_stats(_engine.POWER, lo, hi, thr, alpha)
+        else:
+            st = self.engine.field_row_stats(_engine.FIELD_POWER, lo, hi, thr)
+        return _ratio(st[:, 1], st[:, 0])
+
+    @_live
+    def significant_fraction(self, signif):
+        """Per scale, the fraction of the points inside the cone of influence where
+        |W|^2 > signif[j]; NaN for a scale without such points."""
+        lo, hi = self.coi_ranges()
+        st = self.engine.field_row_stats(_engine.FIELD_POWER, lo, hi, _power_threshold(self, signif))
+        return _ratio(st[:, 0], hi - lo)
+
+    @_live
+    def scale_avg_power(self, period_min, period_max, variance=1.0):
+        """Scale-averaged power over period_min <= period < period_max (TC98 eq. 24), as
+        `ResidentTransform.scale_avg_power`."""
+        _, w = self._band_weights(period_min, period_max, variance)
+        return self.engine.power_scale_avg(w)
+
+    @_live
+    def surrogate_test(self, mc_count=300, seed=None, null='ar1'):
+        """Run the units 0 .. mc_count - 1 of `null` ('ar1' or 'phase') once and count per point the
+        units whose power reaches this one (kept on the device, replacing the counts of an earlier
+        test).  `seed=None` draws the seed from numpy's global RNG; the seed and M are kept as
+        `surrogate_seed` and `surrogate_units`.  ValueError for mc_count outside [1, 2^31 - 1], an
+        unknown null, or when the FFT padding mode differs from the one this power was computed
+        with."""
+        self._null(null)
+        self._count(mc_count, seed, null)
+
+    @_live
+    def pvalues(self, rows=slice(None), cols=slice(None)):
+        """p[rows, cols] = (1 + k) / (1 + M) (float64) of the last `surrogate_test`, with the slicing
+        of `window`; NaN where the power is not finite."""
+        return self._pvalues(_engine.POWER, rows, cols)
+
+    @_live
+    def pvalue_fraction(self, alpha):
+        """Per scale, the fraction of the points inside the cone of influence (with a finite p) whose
+        p <= alpha; NaN for a scale without such points."""
+        return self._pvalue_fraction(_engine.POWER, alpha)
+
+    @_live
+    def fdr_threshold(self, q=0.05, method='bh', inside_coi=True):
+        """`ResidentCoherence.fdr_threshold` over the p-values of the last `surrogate_test`."""
+        return self._fdr_threshold(_engine.POWER, q, method, inside_coi)
+
+    @_live
+    def cluster_test(self, sig, mc_count=300, seed=None, null='ar1', inside_coi=True):
+        """Cluster (areawise) test of this power against the units 0 .. mc_count - 1 of `null`
+        (Maraun et al. 2007): `ResidentCoherence.cluster_test` with a point selected where |W|^2 is
+        finite and > sig[j] (power units, typically the chi-squared level of `significance()`).
+        Returns ClusterResult; the counts of an earlier `surrogate_test` are kept."""
+        self._null(null)
+        return self._cluster(sig, mc_count, seed, inside_coi, null)
+
+    @_live
+    def cluster_labels(self, rows=slice(None), cols=slice(None)):
+        """`ResidentCoherence.cluster_labels` of the last `cluster_test`."""
+        return self._cluster_labels(rows, cols)
+
+
+def power_resident(signal, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', freqs=None, normalize=True,
+                   precision='fp64', engine=None):
+    """The transform of `cwt` of the series (standardised first with `normalize`, as `xwt` and
+    `wct` do), in `precision` ('fp64' or 'fp32'), W kept on the device for the power tests.
+
+    Returns a `ResidentPower`.  Scales, the dropped Paul rows and the un-padded fallback to fp64
+    are resolved by the same code as `cwt_resident` and `wct`; wavelets the engine does not evaluate
+    itself raise TypeError.  No transform stays resident afterwards (handles of `cwt_resident`
+    die); the other resident products survive."""
+    wavelet, spec = _engine_wavelet(wavelet, "power_resident")
+    prec = _coherence_precision(precision)
+    y, yn, _ = _standardise(np.asarray(signal, dtype=np.float64), normalize)
+    n0 = len(yn)
+    sj, freqs = _kept_scales(n0, dt, dj, s0, J, wavelet, freqs)
+    eng = engine or _engine.default_engine()
+    with eng.lock:
+        if _sync_padding(eng, n0):
+            prec = _engine.F64      # un-padded transforms run in fp64
+        serial = eng.power_resident(yn, dt, sj, *spec, precision=prec)
+    return ResidentPower(eng, wavelet, y, yn, dt, dj, sj, freqs, normalize, precision, serial)
