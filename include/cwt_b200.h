@@ -340,6 +340,54 @@ int cwtb_power_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_
 int cwtb_power_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
                               int64_t col_step, int32_t *out);
 
+/* ---- tests of the resident cross spectrum against surrogate pairs -------------------------------
+ * The tests of the power above on W12 of cwtb_xwt_resident, with P = |W12|^2 formed by the same
+ * function.  |W12|^2 is common power: a burst in one series alone can reach it, so these test common
+ * power, not association (the coherence tests do).  The nulls draw two series per unit:
+ *   CWTB_NULL_AR1: series s (0, 1) is the AR(1) unit of cwtb_mc_ar1_surrogates with its own g[s],
+ *     m[s], sigma[s] under the series tag s of the counter (tag 0 is that call's stream, so series 0
+ *     of unit u is its unit u; tag 1 is a stream of its own);
+ *   CWTB_NULL_PHASE: the phase-randomised surrogates of `series` [2][n0] (the two transformed
+ *     series) in phase groups 0 and 1 (cwtb_mc_phase_surrogates): each keeps its periodogram, with
+ *     phases independent of the other's.
+ * A unit [2][n0] is transformed exactly as one cwtb_xwt of its two series in the resident W12's
+ * precision, one unit at a time.  The counts (uint32, 4 bytes per scale-point) and the clusters
+ * live with W12: they die at the next cwtb_xwt_resident, cwtb_cross_release and cwtb_destroy. */
+/* Test hook: the AR(1) pairs first_unit .. first_unit + n_units - 1, out[n_units][2][n0] doubles;
+ * the errors of cwtb_mc_ar1_surrogates for either series. */
+int cwtb_mc_ar1_pair_surrogates(cwtb_ctx *ctx, const double *g, const double *m, const double *sigma,
+                                uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out);
+/* Point-wise test: k[s, n] += 1 where |W12_unit|^2 >= |W12_obs|^2 or is not finite; reset,
+ * accumulation, limits and errors as cwtb_power_surrogate_counts.  g, m, sigma [2] (read by the AR(1)
+ * null only), series [2][n0] (read by the phase null only). */
+int cwtb_cross_surrogate_counts(cwtb_ctx *ctx, const double *series, int null, const double *g, const double *m,
+                                const double *sigma, uint64_t seed, int64_t first_unit, int n_units, int64_t n0,
+                                double dt, const double *scales, int n_scales, int family, double param,
+                                int64_t serial, int reset);
+/* Cluster test of finite |W12|^2 > thr[j] on [lo[j], hi[j]), as cwtb_power_cluster_test. */
+int cwtb_cross_cluster_test(cwtb_ctx *ctx, const double *series, int null, const double *g, const double *m,
+                            const double *sigma, uint64_t seed, int64_t first_unit, int n_units, int64_t n0,
+                            double dt, const double *scales, int n_scales, int family, double param, int64_t serial,
+                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
+                            uint64_t *qmax_out);
+/* Reading the counts and clusters, as the cwtb_power_* calls of the same names: the row stats are
+ * the five sums of cwtb_field_row_stats, the phase sums included. */
+int cwtb_cross_pvalue_window(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                             int64_t col_step, double *p_out);
+int cwtb_cross_pvalue_row_stats(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, const double *thr,
+                                int64_t kmax, double *out);
+int cwtb_cross_count_hist(cwtb_ctx *ctx, const int64_t *lo, const int64_t *hi, int64_t nbins, int64_t *out);
+int cwtb_cross_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points,
+                             int64_t *box);
+int cwtb_cross_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                              int64_t col_step, int32_t *out);
+/* out[n_scales][5]: the five sums of cwtb_field_row_stats over the points that the last
+ * cwtb_cross_cluster_test labelled `cluster` + 1 (row `cluster` of its table), on the columns
+ * [lo[j], hi[j]) of each row (pass the cluster's box: nothing outside it is read).  CWTB_ERR_STATE
+ * before a cluster test, CWTB_ERR_ARG for a cluster outside the table.  Deterministic. */
+int cwtb_cross_cluster_row_stats(cwtb_ctx *ctx, int64_t cluster, const int64_t *lo, const int64_t *hi,
+                                 double *out);
+
 /* ---- partial and multiple wavelet coherence of three series (Mihanovic et al. 2009; Ng & Chan
  * 2012) -------------------------------------------------------------------------------------------
  * y, x1, x2: three signals of n0 samples (standardised by the caller as for cwtb_wct).  With S the

@@ -19,8 +19,11 @@ MEASURE_PARTIAL, MEASURE_MULTIPLE = 0, 1   # the measures of the cwtb_coherence3
 # partial and multiple coherence (cwtb_coherence3_*) and the power (cwtb_power_*)
 PRODUCT_W, PRODUCT_CROSS, PRODUCT_COHERENCE, PRODUCT_COHERENCE3, PRODUCT_POWER = 0, 1, 2, 3, 5   # 4: none
 NULL_AR1, NULL_PHASE = 0, 1      # the nulls of the power tests (cwtb_power_surrogate_counts)
-# the `measure` of the surrogate-test readers below that names the resident power
+# the `measure` of the surrogate-test readers below that names the resident power, and the one that
+# names the resident cross spectrum
 POWER = 'power'
+CROSS = 'cross'
+_COMPLEX = {POWER: PRODUCT_POWER, CROSS: PRODUCT_CROSS}   # their products; each is the prefix of its C calls
 
 _P = ctypes.c_void_p
 _I64 = ctypes.c_int64
@@ -141,6 +144,17 @@ _SIGNATURES = {
     "cwtb_power_count_hist": (_I, [_P, _P, _P, _I64, _P]),
     "cwtb_power_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
     "cwtb_power_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_mc_ar1_pair_surrogates": (_I, [_P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_cross_surrogate_counts": (_I, [_P, _P, _I, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I,
+                                         _D, _I64, _I]),
+    "cwtb_cross_cluster_test": (_I, [_P, _P, _I, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I, _D,
+                                     _I64, _P, _P, _P, _P, _P]),
+    "cwtb_cross_pvalue_window": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_cross_pvalue_row_stats": (_I, [_P, _P, _P, _P, _I64, _P]),
+    "cwtb_cross_count_hist": (_I, [_P, _P, _P, _I64, _P]),
+    "cwtb_cross_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
+    "cwtb_cross_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_cross_cluster_row_stats": (_I, [_P, _I64, _P, _P, _P]),
     "cwtb_cwt_batch": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _I, _D, _I, _P, _P]),
     "cwtb_cwt_batch_dev": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
     "cwtb_comm_unique_id": (_I, [_P]),
@@ -987,9 +1001,9 @@ class Engine(object):
         if measure is None:
             self._shape(PRODUCT_COHERENCE)
             self._check(self.lib.cwtb_coherence_pvalue_window(self.h, *w))
-        elif measure == POWER:
-            self._shape(PRODUCT_POWER)
-            self._check(self.lib.cwtb_power_pvalue_window(self.h, *w))
+        elif measure in _COMPLEX:
+            self._shape(_COMPLEX[measure])
+            self._check(getattr(self.lib, "cwtb_%s_pvalue_window" % measure)(self.h, *w))
         else:
             self._shape(PRODUCT_COHERENCE3)
             self._check(self.lib.cwtb_coherence3_pvalue_window(self.h, int(measure), *w))
@@ -998,14 +1012,14 @@ class Engine(object):
     @_locked
     def pvalue_row_stats(self, measure, lo, hi, kmax, thr=None, want_phase=False):
         """[rows, 4] of `coherence_row_stats` / `coherence3_row_stats` ([rows, 5] of
-        `field_row_stats` for the power) over the points with a finite value and a count k <= kmax."""
-        if measure == POWER:
-            rows, _, _ = self._shape(PRODUCT_POWER)
+        `field_row_stats` for the power and the cross spectrum) over the points with a finite value and
+        a count k <= kmax."""
+        if measure in _COMPLEX:
+            rows, _, _ = self._shape(_COMPLEX[measure])
             lo, hi, thr = _row_args("pvalue_row_stats", rows, lo, hi, thr)
             out = np.empty((rows, 5), dtype=np.float64)
-            self._check(self.lib.cwtb_power_pvalue_row_stats(self.h, _ptr(lo), _ptr(hi),
-                                                             None if thr is None else _ptr(thr), int(kmax),
-                                                             _ptr(out)))
+            fn = getattr(self.lib, "cwtb_%s_pvalue_row_stats" % measure)
+            self._check(fn(self.h, _ptr(lo), _ptr(hi), None if thr is None else _ptr(thr), int(kmax), _ptr(out)))
             return out
         rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else PRODUCT_COHERENCE3)
         lo, hi, thr = _row_args("pvalue_row_stats", rows, lo, hi, thr)
@@ -1022,11 +1036,12 @@ class Engine(object):
         """int64 [nbins]: the number of points with count k over the columns [lo[j], hi[j]) whose
         value is finite; nbins must be M + 1."""
         rows, _, _ = self._shape(PRODUCT_COHERENCE if measure is None else
-                                 PRODUCT_POWER if measure == POWER else PRODUCT_COHERENCE3)
+                                 _COMPLEX[measure] if measure in _COMPLEX else PRODUCT_COHERENCE3)
         lo, hi, _ = _row_args("count_hist", rows, lo, hi, None)
         out = np.empty(int(nbins), dtype=np.int64)
-        if measure == POWER:
-            self._check(self.lib.cwtb_power_count_hist(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
+        if measure in _COMPLEX:
+            fn = getattr(self.lib, "cwtb_%s_count_hist" % measure)
+            self._check(fn(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
         elif measure is None:
             self._check(self.lib.cwtb_coherence_count_hist(self.h, _ptr(lo), _ptr(hi), int(nbins), _ptr(out)))
         else:
@@ -1084,14 +1099,16 @@ class Engine(object):
         return Q, pts, box
 
     def _cluster_call(self, triple, what):
-        """cwtb_{coherence, coherence3, power}_cluster_<what> for `triple` False, True or POWER."""
-        name = "power" if triple == POWER else "coherence3" if triple else "coherence"
+        """cwtb_{coherence, coherence3, power, cross}_cluster_<what> for `triple` False, True, POWER or
+        CROSS."""
+        name = triple if triple in _COMPLEX else "coherence3" if triple else "coherence"
         return getattr(self.lib, "cwtb_%s_cluster_%s" % (name, what))
 
     @_locked
     def cluster_table(self, triple=False):
         """The resident map's clusters of the last cluster test of the coherence (`triple` False),
-        of the partial / multiple coherence (True) or of the power (POWER): (Q, points, box [:, 4] =
+        of the partial / multiple coherence (True), of the power (POWER) or of the cross spectrum
+        (CROSS): (Q, points, box [:, 4] =
         first row, last row + 1, first column, last column + 1), in table order."""
         fn = self._cluster_call(triple, "table")
         return self._table(lambda *a: self._check(fn(self.h, *a)))
@@ -1099,8 +1116,8 @@ class Engine(object):
     @_locked
     def cluster_labels(self, triple, row0, nrows, row_step, col0, ncols, col_step):
         """int32 labels [row0::row_step][:nrows, col0::col_step][:, :ncols] of the last cluster
-        test of the coherence (`triple` False), of the partial / multiple coherence (True) or of the
-        power (POWER): 0 off the clusters, c + 1 on table row c."""
+        test of the coherence (`triple` False), of the partial / multiple coherence (True), of the
+        power (POWER) or of the cross spectrum (CROSS): 0 off the clusters, c + 1 on table row c."""
         out = np.empty((int(nrows), int(ncols)), dtype=np.int32)
         w = (int(row0), int(nrows), int(row_step), int(col0), int(ncols), int(col_step), _ptr(out))
         self._check(self._cluster_call(triple, "labels")(self.h, *w))
@@ -1197,6 +1214,78 @@ class Engine(object):
         self._check(self.lib.cwtb_power_cluster_test(self.h, *a, _ptr(thr), _ptr(lo), _ptr(hi), _ptr(q),
                                                      _ptr(qmax)))
         return qmax
+
+    # ---- tests of the resident cross spectrum against AR(1) or phase-randomised surrogate pairs --
+    @staticmethod
+    def _pair_params(name, g, m, sigma):
+        """The AR(1) parameters of the two series, float64 [2] each."""
+        out = tuple(np.ascontiguousarray(v, dtype=np.float64) for v in (g, m, sigma))
+        if any(v.shape != (2,) for v in out):
+            raise ValueError("%s: g, m and sigma take one entry per series (2)" % name)
+        return out
+
+    @_locked
+    def mc_ar1_pair_surrogates(self, g, m, sigma, seed, first_unit, n_units, n0):
+        """The AR(1) pairs of the cross-spectrum tests, float64 [n_units, 2, n0]: series s with
+        (g[s], m[s], sigma[s]) under the series tag s (series 0 is `mc_ar1_surrogates`' unit)."""
+        g, m, sigma = self._pair_params("mc_ar1_pair_surrogates", g, m, sigma)
+        out = np.empty((int(n_units), 2, int(n0)), dtype=np.float64)
+        self._check(self.lib.cwtb_mc_ar1_pair_surrogates(self.h, _ptr(g), _ptr(m), _ptr(sigma),
+                                                         int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
+                                                         int(n0), _ptr(out)))
+        return out
+
+    def _cross_args(self, name, series, null, g, m, sigma, seed, first_unit, n_units, dt, sj, family, param, serial):
+        """The arguments of a cross-spectrum test up to `serial` (series [2, n0]: the phase null's
+        data), and the arrays the caller keeps alive across the call."""
+        series = np.ascontiguousarray(series, dtype=np.float64)
+        if series.ndim != 2 or series.shape[0] != 2:
+            raise ValueError("%s: the series must be [2, n0]" % name)
+        if null == NULL_PHASE and not np.isfinite(series).all():
+            raise ValueError("%s: non-finite sample" % name)
+        g, m, sigma = self._pair_params(name, g, m, sigma)
+        keep = (series, g, m, sigma)
+        return (_ptr(series), int(null), _ptr(g), _ptr(m), _ptr(sigma), int(seed) & (2 ** 64 - 1), int(first_unit),
+                int(n_units), series.shape[1], float(dt), _ptr(sj), sj.size, int(family), float(param),
+                int(serial)), keep
+
+    @_locked
+    def cross_surrogate_counts(self, series, null, g, m, sigma, seed, first_unit, n_units, dt, scales, family,
+                               param, serial, reset=True):
+        """Count, per point, the pairs of the null whose |W12|^2 reaches the resident cross spectrum's,
+        into its counters (cwtb_cross_surrogate_counts); `serial` is the cross spectrum's serial.
+        `reset` zeroes the counters first, otherwise the units are added."""
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        a, _keep = self._cross_args("cross_surrogate_counts", series, null, g, m, sigma, seed, first_unit, n_units,
+                                    dt, sj, family, param, serial)
+        self._check(self.lib.cwtb_cross_surrogate_counts(self.h, *a, 1 if reset else 0))
+
+    @_locked
+    def cross_cluster_test(self, series, null, g, m, sigma, seed, first_unit, n_units, dt, scales, family, param,
+                           serial, thr, lo, hi, q):
+        """Label the clusters of the resident cross spectrum's |W12|^2 and of every pair's
+        (cwtb_cross_cluster_test): uint64 [n_units], the largest cluster sum Q of each pair."""
+        sj = np.ascontiguousarray(scales, dtype=np.float64)
+        a, _keep = self._cross_args("cross_cluster_test", series, null, g, m, sigma, seed, first_unit, n_units, dt,
+                                    sj, family, param, serial)
+        lo, hi, thr = _row_args("cross_cluster_test", sj.size, lo, hi, thr)
+        q = np.ascontiguousarray(q, dtype=np.uint64)
+        if q.shape != (sj.size,):
+            raise ValueError("cross_cluster_test: q must have one entry per scale")
+        qmax = np.zeros(int(n_units), dtype=np.uint64)
+        self._check(self.lib.cwtb_cross_cluster_test(self.h, *a, _ptr(thr), _ptr(lo), _ptr(hi), _ptr(q),
+                                                     _ptr(qmax)))
+        return qmax
+
+    @_locked
+    def cross_cluster_row_stats(self, cluster, lo, hi):
+        """[rows, 5] of `field_row_stats` over the points of cluster `cluster` (row of the table) of the
+        last cross-spectrum cluster test, on the columns [lo[j], hi[j]) of each row."""
+        rows, _, _ = self._shape(PRODUCT_CROSS)
+        lo, hi, _ = _row_args("cross_cluster_row_stats", rows, lo, hi, None)
+        out = np.empty((rows, 5), dtype=np.float64)
+        self._check(self.lib.cwtb_cross_cluster_row_stats(self.h, int(cluster), _ptr(lo), _ptr(hi), _ptr(out)))
+        return out
 
     @_locked
     def cluster_label_bits(self, bits, n0, q, want_labels=True):

@@ -1691,7 +1691,7 @@ void cwtb_destroy(cwtb_ctx *c) {
   rt_sync(c->stream);
   cwtb_comm_destroy(c);
   for (Buf *b : {&c->osH, &c->osgrp, &c->stage_dev[0], &c->stage_dev[1], &c->batch_power, &c->filt, &c->comm_send, &c->comm_recv, &c->Zx, &c->Cout, &c->wtab, &c->sig, &c->sig2, &c->sig3, &c->spec, &c->Z, &c->Zc[0], &c->Zc[1], &c->Zc[2], &c->Y, &c->B, &c->W, &c->W2, &c->W3, &c->descs, &c->table, &c->scratch,
-                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts, &c->coh.labels, &c->coh3.labels, &c->pw.buf, &c->pw.counts, &c->pw.labels, &c->arc, &c->cl_bits, &c->cl_rows, &c->cl_hdr, &c->cl_runs, &c->cl_qmax})
+                 &c->C, &c->A12, &c->F, &c->aux, &c->rowd, &c->win, &c->mask, &c->hist, &c->noise, &c->wide, &c->blueA, &c->blueX, &c->blueY, &c->pspec, &c->prot, &c->coh.buf, &c->cross.buf, &c->coh3.buf, &c->coh.counts, &c->coh3.counts, &c->coh.labels, &c->coh3.labels, &c->pw.buf, &c->pw.counts, &c->pw.labels, &c->cross.counts, &c->cross.labels, &c->arc, &c->cl_bits, &c->cl_rows, &c->cl_hdr, &c->cl_runs, &c->cl_qmax})
     if (b->p) rt_free(b->p);
   for (auto &kv : c->ntabs) { rt_free(kv.second.hi); rt_free(kv.second.lo); }
   for (auto &kv : c->blue) { rt_free(kv.second.wm); rt_free(kv.second.bf[0]); rt_free(kv.second.bf[1]); }
@@ -2722,6 +2722,10 @@ struct FieldRef {
   const unsigned *cnt = nullptr;
   long long m = 0, kmax = 0;
   bool power = false;   // a complex field's window as its power P (CxPowerView)
+  // a complex field's row stats over the points of one cluster (CxLabelView): the label image of
+  // its last cluster test and the label to select; lab null: every point
+  const int *lab = nullptr;
+  int want = 0;
 };
 
 static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
@@ -2749,10 +2753,12 @@ static int field_ref(cwtb_ctx *c, int field, FieldRef &f) {
   return 0;
 }
 
-// The counts of a tested field f (field_ref of FIELD_COH, FIELD_COH3_P, FIELD_COH3_M or
-// CWTB_FIELD_POWER) added to it, with the row stats' cut kmax
+// The counts of a tested field f (field_ref of FIELD_COH, FIELD_COH3_P, FIELD_COH3_M,
+// CWTB_FIELD_POWER or CWTB_FIELD_CROSS) added to it, with the row stats' cut kmax
 static int count_ref(cwtb_ctx *c, long long kmax, FieldRef &f) {
-  const ResidentSlot &s = f.field == FIELD_COH ? c->coh : f.field == CWTB_FIELD_POWER ? c->pw : c->coh3;
+  const ResidentSlot &s = f.field == FIELD_COH          ? c->coh
+                        : f.field == CWTB_FIELD_POWER   ? c->pw
+                        : f.field == CWTB_FIELD_CROSS   ? c->cross : c->coh3;
   if (s.units < 0 || !s.counts.p) return fail(c, CWTB_ERR_STATE, "no surrogate counts resident for this product");
   f.cnt = (const unsigned *)s.counts.p + (f.field == FIELD_COH3_M ? coh_angle_offset((size_t)s.S * s.n0) : 0);
   f.m = s.units;
@@ -2855,7 +2861,7 @@ static int row_stats_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, cons
       return fail(c, CWTB_ERR_ARG, "row_stats: column range outside [0, n0) or lo > hi");
   }
   if (thr) memcpy(h.data() + 2 * (size_t)S, thr, (size_t)S * sizeof(double));
-  return with_read_view(f, want_phase, [&](auto v) {
+  auto run = [&](auto v) {
     using B = RowStatsBody<decltype(v)>;
     constexpr int K = B::K;
     const int nchunk = (int)((n0 + B::CHUNK - 1) / B::CHUNK);
@@ -2873,7 +2879,10 @@ static int row_stats_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, cons
     RT(rt_d2h(out, dsum, (size_t)S * K * sizeof(double), c->stream));
     RT(rt_sync(c->stream));
     return 0;
-  });
+  };
+  if (!f.lab) return with_read_view(f, want_phase, run);
+  if (f.prec == CWTB_F64) return run(CxLabelView<double>{(const cx<double> *)f.p, f.lab, f.want});
+  return run(CxLabelView<float>{(const cx<float> *)f.p, f.lab, f.want});
 }
 
 // The view's NA weighted sums per column over the rows with a non-zero weight
@@ -3937,10 +3946,11 @@ static int ar1_check(cwtb_ctx *c, const std::string &nm, const Ar1Src &ar) {
 }
 
 extern "C++" {
-// nb AR(1) units from unit0 into out [nb][n0] (nb <= MAX_ROWS); c->arc holds the CTAs' carries
+// nb AR(1) units from unit0 of the series tag `stag` into out [nb][nser][n0] (nb <= MAX_ROWS; out
+// points at the series' first row); c->arc holds the CTAs' carries
 template <typename T>
 static int ar1_units(cwtb_ctx *c, const Ar1Src &ar, unsigned long long seed, long long unit0, int nb, int64_t n0,
-                     T *out) {
+                     T *out, int nser, unsigned stag) {
   const long long per = (long long)NT * AR1_CH;   // samples per CTA
   const int nblk = (int)((n0 + per - 1) / per);
   int e = ensure(c, c->arc, (size_t)nb * nblk * 2 * sizeof(double));
@@ -3948,7 +3958,7 @@ static int ar1_units(cwtb_ctx *c, const Ar1Src &ar, unsigned long long seed, lon
   struct Tag { cwtb_ctx *c; ~Tag() { c->prof_tag = ""; } } tag{c};
   c->prof_tag = "ar1:";
   Ar1Args<T> a{out, (double *)c->arc.p, seed, unit0, (long long)n0, ar.g, std::sqrt((1.0 - ar.g) * (1.0 + ar.g)),
-               ar.m, ar.sigma, nblk, nb};
+               ar.m, ar.sigma, nblk, nb, nser, stag};
   if ((e = launch<Ar1BlockBody<T>>(c, (unsigned)nblk, (unsigned)nb, a))) return e;
   Ar1CarryArgs ca{(double *)c->arc.p, nblk, nb};
   if ((e = launch<Ar1CarryBody>(c, (unsigned)((nb + NT - 1) / NT), 1, ca))) return e;
@@ -3970,37 +3980,42 @@ int cwtb_mc_ar1_surrogates(cwtb_ctx *c, double g, double m, double sigma, uint64
   if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
   for (int i0 = 0; i0 < n_units; i0 += (int)MAX_ROWS) {
     const int nb = std::min((int)MAX_ROWS, n_units - i0);
-    if ((e = ar1_units<double>(c, ar, seed, first_unit + i0, nb, n0, (double *)c->noise.p + (size_t)i0 * n0))) return e;
+    if ((e = ar1_units<double>(c, ar, seed, first_unit + i0, nb, n0, (double *)c->noise.p + (size_t)i0 * n0, 1, 0)))
+      return e;
   }
   RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;
 }
 
-// ---- tests of the resident power against surrogates -------------------------------------------
-// The null of a power test: AR(1) units, or phase-randomised units of the series (its spectrum in
-// c->pspec, phase group 0)
-struct PowerNull { int kind; Ar1Src ar; PhaseSrc ph; };
+// ---- tests of the resident power and cross spectrum against surrogates -----------------------
+// The null of a test of a complex field of nser series (the power: 1, the cross spectrum: 2): AR(1)
+// units, series s with its own parameters ar[s] under the series tag s, or phase-randomised units of
+// the series (their spectra in c->pspec, series s in phase group s: independent phases)
+struct TestNull { int kind, nser; Ar1Src ar[2]; PhaseSrc ph; };
 
-static int power_null(cwtb_ctx *c, const std::string &nm, const double *series, int null, double g, double m,
-                      double sigma, int64_t first_unit, int n_units, int64_t n0, PowerNull &pn) {
-  pn = PowerNull{null, Ar1Src{g, m, sigma}, PhaseSrc{}};
+static int test_null(cwtb_ctx *c, const std::string &nm, const double *series, int nser, int null, const double *g,
+                     const double *m, const double *sigma, int64_t first_unit, int n_units, int64_t n0, TestNull &tn) {
+  tn = TestNull{null, nser, {}, PhaseSrc{}};
   if (null == CWTB_NULL_PHASE) {
-    const int group = 0;
-    return phase_spectra(c, nm.c_str(), series, 1, &group, first_unit, n_units, n0, &pn.ph);
+    const int group[2] = {0, 1};
+    return phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &tn.ph);
   }
   if (null != CWTB_NULL_AR1) return fail(c, CWTB_ERR_ARG, nm + ": unknown null");
-  if (n_units < 0 || first_unit < 0 || first_unit > (1ll << 61) - n_units)
+  if (!g || !m || !sigma || n_units < 0 || first_unit < 0 || first_unit > (1ll << 61) - n_units)
     return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
-  int e = ar1_check(c, nm, pn.ar);
-  if (e) return e;
+  for (int r = 0; r < nser; ++r) {
+    tn.ar[r] = Ar1Src{g[r], m[r], sigma[r]};
+    int e = ar1_check(c, nm, tn.ar[r]);
+    if (e) return e;
+  }
   RT(rt_set_device(c->device));
   return 0;
 }
 
-// the checks of the power tests against the resident power
-static int power_slot(cwtb_ctx *c, const std::string &nm, int64_t serial, int n_scales, int64_t n0, int family) {
-  const ResidentSlot &s = c->pw;
+// the checks of a test against the resident product of slot s
+static int test_slot(cwtb_ctx *c, const ResidentSlot &s, const std::string &nm, int64_t serial, int n_scales,
+                     int64_t n0, int family) {
   if (s.S <= 0 || !s.buf.p || serial != s.serial)
     return fail(c, CWTB_ERR_STATE, nm + ": the serial is not that of the resident product");
   if (n_scales != s.S || n0 != s.n0)
@@ -4021,33 +4036,44 @@ static int power_compare(cwtb_ctx *c, const void *W, const void *obs, unsigned *
              : launch<PowerCountBody<T, false>>(c, gx, (unsigned)S, a);
 }
 
-// The units [unit0, unit0 + n_units) of the null: each drawn, transformed with the resident power's
-// plan (one cwtb_cwt of it: one unit at a time, W in c->W) and compared with the resident W: counts
-// into cnt, or selection bits (sel) labelled right away, the unit's largest cluster into dqmax[i]
+// The units [unit0, unit0 + n_units) of the null, drawn as batches [nb][nser][n0]: each transformed
+// with the resident product's plan, one unit at a time, W in c->W, exactly as one cwtb_cwt of it (one
+// series) or one cwtb_xwt of its two series (W1 stored, W1 conj(W2) in the second transform's
+// epilogue), and compared with the resident field obs: counts into cnt, or selection bits (sel)
+// labelled right away, the unit's largest cluster into dqmax[i]
 template <typename T>
-static int power_units(cwtb_ctx *c, const PowerNull &pn, unsigned long long seed, long long unit0, int n_units,
-                       int64_t n0, double dt, const double *scales, int S, int family, double param, unsigned *cnt,
-                       const SelArgs *sel, const unsigned long long *dq, unsigned long long *dqmax) {
+static int test_units(cwtb_ctx *c, const TestNull &tn, const void *obs, unsigned long long seed, long long unit0,
+                      int n_units, int64_t n0, double dt, const double *scales, int S, int family, double param,
+                      unsigned *cnt, const SelArgs *sel, const unsigned long long *dq, unsigned long long *dqmax) {
   int e = prepare(c, n0, dt, scales, S, family, param, prec_of<T>(), nullptr);
   if (e) return e;
-  const bool phase = pn.kind == CWTB_NULL_PHASE;
+  const bool phase = tn.kind == CWTB_NULL_PHASE;
+  const int nser = tn.nser;
   // the units of one draw: the rotated spectra of phase-randomised units take 16 B per sample
-  const size_t per = (size_t)n0 * (phase ? sizeof(double2) : sizeof(T));
-  const int batch = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_units, ((size_t)256 << 20) / per, (size_t)MAX_ROWS}));
-  if ((e = ensure(c, c->noise, (size_t)batch * n0 * sizeof(T)))) return e;
-  if (phase && (e = ensure(c, c->prot, (size_t)batch * n0 * sizeof(double2)))) return e;
+  const size_t per = (size_t)nser * n0 * (phase ? sizeof(double2) : sizeof(T));
+  const int batch = (int)std::max<size_t>(
+      1, std::min<size_t>({(size_t)n_units, ((size_t)256 << 20) / per, (size_t)MAX_ROWS / nser}));
+  if ((e = ensure(c, c->noise, (size_t)batch * nser * n0 * sizeof(T)))) return e;
+  if (phase && (e = ensure(c, c->prot, (size_t)batch * nser * n0 * sizeof(double2)))) return e;
   c->launches = 0;
   if ((e = time_begin(c))) return e;
   for (int i0 = 0; i0 < n_units; i0 += batch) {
     const int nb = std::min(batch, n_units - i0);
     T *x = (T *)c->noise.p;
-    e = phase ? phase_units<T>(c, pn.ph, 1, seed, unit0 + i0, nb, n0, x) : ar1_units<T>(c, pn.ar, seed, unit0 + i0, nb, n0, x);
-    if (e) return e;
+    if (phase) {
+      if ((e = phase_units<T>(c, tn.ph, nser, seed, unit0 + i0, nb, n0, x))) return e;
+    } else {
+      for (int r = 0; r < nser; ++r)
+        if ((e = ar1_units<T>(c, tn.ar[r], seed, unit0 + i0, nb, n0, x + (size_t)r * n0, nser, (unsigned)r)))
+          return e;
+    }
     for (int i = 0; i < nb; ++i) {
       // run_job joins its streams back into c->stream, where the comparisons of successive units
       // follow each other: the counters and the selection bits have one writer at a time
-      if ((e = run_job<T>(c, c->job, x + (size_t)i * n0, nullptr, EPI_STORE))) return e;
-      if ((e = power_compare<T>(c, c->W.p, c->pw.buf.p, cnt, sel, S, n0))) return e;
+      const T *u = x + (size_t)i * nser * n0;
+      if ((e = run_job<T>(c, c->job, u, nullptr, EPI_STORE))) return e;
+      if (nser == 2 && (e = run_job<T>(c, c->job, u + n0, nullptr, EPI_MULCONJ))) return e;
+      if ((e = power_compare<T>(c, c->W.p, obs, cnt, sel, S, n0))) return e;
       if (sel && (e = label_bits(c, S, n0, dq, dqmax + i0 + i, nullptr, nullptr))) return e;
     }
   }
@@ -4057,49 +4083,49 @@ static int power_units(cwtb_ctx *c, const PowerNull &pn, unsigned long long seed
 }
 }  // extern "C++"
 
-int cwtb_power_surrogate_counts(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
-                                uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
-                                const double *scales, int n_scales, int family, double param, int64_t serial,
-                                int reset) {
+// cwtb_power_surrogate_counts / cwtb_cross_surrogate_counts on slot s, a field of nser series
+static int test_counts(cwtb_ctx *c, const char *name, ResidentSlot &s, int nser, const double *series, int null,
+                       const double *g, const double *m, const double *sigma, uint64_t seed, int64_t first_unit,
+                       int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                       double param, int64_t serial, int reset) {
   if (!c) return CWTB_ERR_ARG;
-  const std::string nm = "power_surrogate_counts";
-  ResidentSlot &s = c->pw;
-  int e = power_slot(c, nm, serial, n_scales, n0, family);
+  const std::string nm = name;
+  int e = test_slot(c, s, nm, serial, n_scales, n0, family);
   if (e) return e;
   const long long base = reset || s.units < 0 ? 0 : s.units;
   if (n_units < 0 || n_units > 0xFFFFFFFFll - base)
     return fail(c, CWTB_ERR_ARG, nm + ": more units than a 32-bit counter holds");
-  PowerNull pn;
-  if ((e = power_null(c, nm, series, null, g, m, sigma, first_unit, n_units, n0, pn))) return e;
+  TestNull tn;
+  if ((e = test_null(c, nm, series, nser, null, g, m, sigma, first_unit, n_units, n0, tn))) return e;
   if ((e = ensure(c, s.counts, (size_t)s.S * s.n0 * sizeof(unsigned)))) return e;
   s.units = -1;   // nothing readable until this call completes
   if (base == 0) RT(rt_memset(s.counts.p, 0, s.counts.bytes, c->stream));
-  e = s.prec == CWTB_F32 ? power_units<float>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                                              (unsigned *)s.counts.p, nullptr, nullptr, nullptr)
-                         : power_units<double>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                                               (unsigned *)s.counts.p, nullptr, nullptr, nullptr);
+  e = s.prec == CWTB_F32 ? test_units<float>(c, tn, s.buf.p, seed, first_unit, n_units, n0, dt, scales, n_scales,
+                                             family, param, (unsigned *)s.counts.p, nullptr, nullptr, nullptr)
+                         : test_units<double>(c, tn, s.buf.p, seed, first_unit, n_units, n0, dt, scales, n_scales,
+                                              family, param, (unsigned *)s.counts.p, nullptr, nullptr, nullptr);
   if (e) return e;
   RT(rt_sync(c->stream));
   s.units = base + n_units;
   return 0;
 }
 
-int cwtb_power_cluster_test(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
-                            uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
-                            const double *scales, int n_scales, int family, double param, int64_t serial,
-                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
-                            uint64_t *qmax_out) {
+// cwtb_power_cluster_test / cwtb_cross_cluster_test on slot s, a field of nser series
+static int test_clusters(cwtb_ctx *c, const char *name, ResidentSlot &s, int nser, const double *series, int null,
+                         const double *g, const double *m, const double *sigma, uint64_t seed, int64_t first_unit,
+                         int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                         double param, int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
+                         const uint64_t *q, uint64_t *qmax_out) {
   if (!c) return CWTB_ERR_ARG;
-  const std::string nm = "power_cluster_test";
-  ResidentSlot &s = c->pw;
+  const std::string nm = name;
   s.clusters = false;   // nothing readable until this call completes
   s.table = ClusterTable{};
-  int e = power_slot(c, nm, serial, n_scales, n0, family);
+  int e = test_slot(c, s, nm, serial, n_scales, n0, family);
   if (e) return e;
   if (!thr || n_units < 0 || (n_units > 0 && !qmax_out)) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
   if ((e = cluster_shape(c, nm, n_scales, n0))) return e;
-  PowerNull pn;
-  if ((e = power_null(c, nm, series, null, g, m, sigma, first_unit, n_units, n0, pn))) return e;
+  TestNull tn;
+  if ((e = test_null(c, nm, series, nser, null, g, m, sigma, first_unit, n_units, n0, tn))) return e;
   SelArgs sel;
   const unsigned long long *dq;
   if ((e = cluster_rows(c, nm, n_scales, n0, thr, lo, hi, q, sel, dq))) return e;
@@ -4107,23 +4133,42 @@ int cwtb_power_cluster_test(cwtb_ctx *c, const double *series, int null, double 
   if ((e = ensure(c, s.labels, (size_t)n_scales * n0 * sizeof(int)))) return e;
   unsigned long long *dqmax = (unsigned long long *)c->cl_qmax.p;
   RT(rt_memset(dqmax, 0, (size_t)(n_units + 1) * sizeof(unsigned long long), c->stream));
-  // the observed map: the comparison kernel's bits of the resident W, labelled as the units' are
+  // the observed map: the comparison kernel's bits of the resident field, labelled as the units' are
   // (every launch writes whole words: no bit past the last column is ever set)
   e = s.prec == CWTB_F32 ? power_compare<float>(c, s.buf.p, nullptr, nullptr, &sel, n_scales, n0)
                          : power_compare<double>(c, s.buf.p, nullptr, nullptr, &sel, n_scales, n0);
   if (e) return e;
   ClusterTable tab;
   if ((e = label_bits(c, n_scales, n0, dq, dqmax + n_units, &tab, (int *)s.labels.p))) return e;
-  e = s.prec == CWTB_F32 ? power_units<float>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                                              nullptr, &sel, dq, dqmax)
-                         : power_units<double>(c, pn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                                               nullptr, &sel, dq, dqmax);
+  e = s.prec == CWTB_F32 ? test_units<float>(c, tn, s.buf.p, seed, first_unit, n_units, n0, dt, scales, n_scales,
+                                             family, param, nullptr, &sel, dq, dqmax)
+                         : test_units<double>(c, tn, s.buf.p, seed, first_unit, n_units, n0, dt, scales, n_scales,
+                                              family, param, nullptr, &sel, dq, dqmax);
   if (e) return e;
   if (n_units > 0) RT(rt_d2h(qmax_out, dqmax, (size_t)n_units * sizeof(unsigned long long), c->stream));
   RT(rt_sync(c->stream));
   s.table = std::move(tab);
   s.clusters = true;
   return 0;
+}
+
+int cwtb_power_surrogate_counts(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
+                                uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                const double *scales, int n_scales, int family, double param, int64_t serial,
+                                int reset) {
+  return c ? test_counts(c, "power_surrogate_counts", c->pw, 1, series, null, &g, &m, &sigma, seed, first_unit,
+                         n_units, n0, dt, scales, n_scales, family, param, serial, reset)
+           : CWTB_ERR_ARG;
+}
+
+int cwtb_power_cluster_test(cwtb_ctx *c, const double *series, int null, double g, double m, double sigma,
+                            uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                            const double *scales, int n_scales, int family, double param, int64_t serial,
+                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
+                            uint64_t *qmax_out) {
+  return c ? test_clusters(c, "power_cluster_test", c->pw, 1, series, null, &g, &m, &sigma, seed, first_unit,
+                           n_units, n0, dt, scales, n_scales, family, param, serial, thr, lo, hi, q, qmax_out)
+           : CWTB_ERR_ARG;
 }
 
 int cwtb_power_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols, int64_t col_step,
@@ -4169,6 +4214,95 @@ int cwtb_power_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, in
                               int64_t col_step, int32_t *out) {
   int e = c ? clusters_of(c, c->pw, "power") : CWTB_ERR_ARG;
   return e ? e : labels_window(c, c->pw, row0, nrows, row_step, col0, ncols, col_step, out);
+}
+
+// ---- tests of the resident cross spectrum against surrogate pairs ---------------------------------
+int cwtb_mc_ar1_pair_surrogates(cwtb_ctx *c, const double *g, const double *m, const double *sigma, uint64_t seed,
+                                int64_t first_unit, int n_units, int64_t n0, double *out) {
+  if (!c) return CWTB_ERR_ARG;
+  const std::string nm = "mc_ar1_pair_surrogates";
+  if (!out || n_units < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  TestNull tn;
+  int e = test_null(c, nm, nullptr, 2, CWTB_NULL_AR1, g, m, sigma, first_unit, n_units, n0, tn);
+  if (e) return e;
+  const size_t cnt = (size_t)n_units * 2 * n0;
+  if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
+  for (int i0 = 0; i0 < n_units; i0 += (int)MAX_ROWS) {
+    const int nb = std::min((int)MAX_ROWS, n_units - i0);
+    double *x = (double *)c->noise.p + (size_t)i0 * 2 * n0;
+    for (int r = 0; r < 2; ++r)
+      if ((e = ar1_units<double>(c, tn.ar[r], seed, first_unit + i0, nb, n0, x + (size_t)r * n0, 2, (unsigned)r)))
+        return e;
+  }
+  RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
+  RT(rt_sync(c->stream));
+  return 0;
+}
+
+int cwtb_cross_surrogate_counts(cwtb_ctx *c, const double *series, int null, const double *g, const double *m,
+                                const double *sigma, uint64_t seed, int64_t first_unit, int n_units, int64_t n0,
+                                double dt, const double *scales, int n_scales, int family, double param,
+                                int64_t serial, int reset) {
+  return c ? test_counts(c, "cross_surrogate_counts", c->cross, 2, series, null, g, m, sigma, seed, first_unit,
+                         n_units, n0, dt, scales, n_scales, family, param, serial, reset)
+           : CWTB_ERR_ARG;
+}
+
+int cwtb_cross_cluster_test(cwtb_ctx *c, const double *series, int null, const double *g, const double *m,
+                            const double *sigma, uint64_t seed, int64_t first_unit, int n_units, int64_t n0,
+                            double dt, const double *scales, int n_scales, int family, double param, int64_t serial,
+                            const double *thr, const int64_t *lo, const int64_t *hi, const uint64_t *q,
+                            uint64_t *qmax_out) {
+  return c ? test_clusters(c, "cross_cluster_test", c->cross, 2, series, null, g, m, sigma, seed, first_unit,
+                           n_units, n0, dt, scales, n_scales, family, param, serial, thr, lo, hi, q, qmax_out)
+           : CWTB_ERR_ARG;
+}
+
+int cwtb_cross_pvalue_window(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                             int64_t col_step, double *p_out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_CROSS, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  if (!p_out && nrows > 0 && ncols > 0) return fail(c, CWTB_ERR_ARG, "null argument");
+  return window_run(c, f, row0, nrows, row_step, col0, ncols, col_step, p_out, nullptr);
+}
+
+int cwtb_cross_pvalue_row_stats(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, const double *thr, int64_t kmax,
+                                double *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_CROSS, f);
+  if (e || (e = count_ref(c, kmax, f))) return e;
+  return row_stats_run(c, f, lo, hi, thr, 0, out);
+}
+
+int cwtb_cross_count_hist(cwtb_ctx *c, const int64_t *lo, const int64_t *hi, int64_t nbins, int64_t *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_CROSS, f);
+  if (e || (e = count_ref(c, 0, f))) return e;
+  return count_hist_run(c, f, lo, hi, nbins, out);
+}
+
+int cwtb_cross_cluster_table(cwtb_ctx *c, int64_t cap, int64_t *count, uint64_t *Q, int64_t *points, int64_t *box) {
+  int e = c ? clusters_of(c, c->cross, "cross spectrum") : CWTB_ERR_ARG;
+  return e ? e : table_out(c, c->cross.table, cap, count, Q, points, box);
+}
+
+int cwtb_cross_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
+                              int64_t col_step, int32_t *out) {
+  int e = c ? clusters_of(c, c->cross, "cross spectrum") : CWTB_ERR_ARG;
+  return e ? e : labels_window(c, c->cross, row0, nrows, row_step, col0, ncols, col_step, out);
+}
+
+int cwtb_cross_cluster_row_stats(cwtb_ctx *c, int64_t cluster, const int64_t *lo, const int64_t *hi, double *out) {
+  int e = c ? clusters_of(c, c->cross, "cross spectrum") : CWTB_ERR_ARG;
+  if (e) return e;
+  if (cluster < 0 || cluster >= (int64_t)c->cross.table.Q.size())
+    return fail(c, CWTB_ERR_ARG, "cross_cluster_row_stats: no such cluster in the last cluster test");
+  FieldRef f;
+  if ((e = field_ref(c, CWTB_FIELD_CROSS, f))) return e;
+  f.lab = (const int *)c->cross.labels.p;
+  f.want = (int)cluster + 1;
+  return row_stats_run(c, f, lo, hi, nullptr, 0, out);
 }
 
 // One pass of the last cwtb_cwt_dev transform with a CUDA event pair around every launch.

@@ -1776,10 +1776,13 @@ struct PhaseRotBody {
 // ---- Bodies: AR(1) red-noise surrogates on the device (the power test's red-noise null) ----------
 // Unit u of length n is x = m + sigma z with z[0] = e[0], z[i] = g z[i-1] + sqrt(1 - g^2) e[i] (the
 // background of Torrence & Compo 1998, section 4), |g| < 1.  e[2j], e[2j+1] are the two normals of
-// one Philox4x32-10 block (philox_normals, NoiseBody's conversion), a pure function of (seed, u, j):
-// counter words (j, 2^31, u lo, 2^31 | (u hi << 2) | 3).  PhaseRotBody's second word is a phase
-// group below 2^31 and NoiseBody's a sample index below 2^26, so bit 31 of the second word keeps this
-// stream apart from both for 0 <= u < 2^61 (j < 2^31).
+// one Philox4x32-10 block (philox_normals, NoiseBody's conversion), a pure function of (seed, s, u,
+// j): counter words (j, 2^31 | s, u lo, 2^31 | (u hi << 2) | 3), s the series tag (0 or 1).  Tag 0
+// is the power test's stream; the cross-wavelet test draws its second series under tag 1, so the two
+// series of one unit are independent even with equal parameters, and its first series is the power
+// test's unit.  PhaseRotBody's second word is a phase group below 2^31 and NoiseBody's a sample
+// index below 2^26, so bit 31 of the second word keeps both tags apart from both for 0 <= u < 2^61
+// (j < 2^31), and the tag's low bit keeps the two tags apart from each other.
 // The recurrence is a linear scan over the whole series: z_end = g^L z_start + b over a stretch of L
 // samples, b its end state from a zero start.  A thread owns AR1_CH consecutive samples (whole
 // normal pairs), a CTA NT of those stretches.  Ar1BlockBody forms every CTA's (g^L, b), Ar1CarryBody
@@ -1789,13 +1792,15 @@ struct PhaseRotBody {
 // rounded).  The stretches depend on NT, the draws (seed, u, j) do not.
 constexpr int AR1_CH = 32;   // samples per thread (even)
 template <typename T> struct Ar1Args {
-  T *out;                   // [n_units][n]
+  T *out;                   // [n_units][nser][n]: unit by's series at out + by nser n
   double *blk;              // [n_units][nblk][2]: (g^L, b) of each CTA, then (., carry-in)
   unsigned long long seed;
   long long unit0;          // global index of the first unit
   long long n;
   double g, s, m, sigma;    // s = sqrt(1 - g^2)
   int nblk, n_units;
+  int nser;                 // series per unit in out (the pairs of the cross test: 2)
+  unsigned tag;             // series tag s of the counter
 };
 // Samples [i0, i1) of unit `unit` from the state z before i0: the state after i1 - 1, and x into dst
 // (null: nothing written)
@@ -1803,7 +1808,7 @@ template <typename T>
 HD double ar1_run(const Ar1Args<T> &a, unsigned long long unit, long long i0, long long i1, double z, T *dst) {
   for (long long i = i0; i < i1; i += 2) {
     unsigned o[4];
-    philox4x32_10((unsigned)(i >> 1), 0x80000000u, (unsigned)unit, 0x80000000u | ((unsigned)(unit >> 32) << 2) | 3u,
+    philox4x32_10((unsigned)(i >> 1), 0x80000000u | a.tag, (unsigned)unit, 0x80000000u | ((unsigned)(unit >> 32) << 2) | 3u,
                   (unsigned)a.seed, (unsigned)(a.seed >> 32), o);
     double e0, e1;
     philox_normals(o, e0, e1);
@@ -1887,7 +1892,7 @@ template <typename T> struct Ar1WriteBody {   // grid (nblk, n_units)
     } else {
       long long i0, i1;
       ar1_span(a, bx, tid, i0, i1);
-      ar1_run<T>(a, (unsigned long long)(a.unit0 + by), i0, i1, sm[NT + tid], a.out + (size_t)by * a.n);
+      ar1_run<T>(a, (unsigned long long)(a.unit0 + by), i0, i1, sm[NT + tid], a.out + (size_t)by * a.n * a.nser);
     }
   }
 };
@@ -2652,6 +2657,31 @@ template <typename T> struct CxCountView {
     o0[dst] = isfinite(P) ? (double)(1 + (long long)cnt[src]) / (double)(1 + m) : P - P;   // inf - inf: NaN
   }
   HD bool finite(size_t o) const { return isfinite(power_of<T>(ld_stream(&F[o]))); }   // CountHistBody
+};
+
+// A complex field over one cluster of its last cluster test (cwtb_cross_cluster_row_stats): CxView's
+// five sums over the points whose label (int32 [rows][n], the field's flat index; 0 off the
+// clusters, c + 1 on cluster c) is `want`.  Row stats only.
+template <typename T> struct CxLabelView {
+  const cx<T> *F;
+  const int *lab;
+  int want;
+  using V16 = CxVec16<T>;
+  static constexpr int K = CxView<T>::K, E = V16::E, VPT = 32;
+  struct Vec { typename V16::V w; int l[E]; };
+  HD Vec load(size_t q) const {
+    Vec v;
+    v.w = ld_stream((const typename V16::V *)F + q);
+#pragma unroll
+    for (int e = 0; e < E; ++e) v.l[e] = ld_stream(&lab[q * E + e]);
+    return v;
+  }
+  HD void add(double (&s)[K], const Vec &v, int e, bool has_thr, double t) const {
+    if (v.l[e] == want) CxView<T>::add1(s, V16::re(v.w, e), V16::im(v.w, e), has_thr, t);
+  }
+  HD void add_at(double (&s)[K], size_t p, bool has_thr, double t) const {
+    if (lab[p] == want) CxView<T>::add1(s, F[p].x, F[p].y, has_thr, t);
+  }
 };
 
 // Per-row sums of a view over the columns [lo_j, hi_j) where thr is null or the view's point

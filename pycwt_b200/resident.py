@@ -416,9 +416,10 @@ class _SurrogateTest(object):
     """The point-wise and cluster tests of a resident product: the counts of its last
     `surrogate_test`, the clusters of its last `cluster_test`, and what is read from them.  A
     subclass names the engine's clusters of its product (`_CLUSTERS`: False for the coherence, True
-    for the partial and multiple coherence, `_engine.POWER` for the power), passes its measure to
-    the readers (None for the coherence, `_engine.POWER` for the power) and runs its units on the
-    device (`_count_units`, `_cluster_units`)."""
+    for the partial and multiple coherence, `_engine.POWER` for the power, `_engine.CROSS` for the
+    cross spectrum), passes its measure to the readers (None for the coherence, `_engine.POWER` /
+    `_engine.CROSS` for the power / the cross spectrum) and runs its units on the device
+    (`_count_units`, `_cluster_units`)."""
 
     _UNTESTED = ("no surrogate test has counted for this product: call surrogate_test first")
     surrogate_seed = None     # seed and M of the last surrogate_test
@@ -754,16 +755,33 @@ def wct_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normalize=T
 # as `xwt` and keeps W12 on the device, in a buffer of its own: the handle stays valid across later
 # cwt / xwt / wct / wct_resident / Monte-Carlo calls, until the next `xwt_resident` on the same
 # engine or `release()`.
+# `xwt`'s `signif` is a per-scale chi-squared level built from two fitted AR(1) spectra; applied point
+# by point it paints spurious patches, as the power's does.  The handle tests |W12|^2 point by point
+# and patch by patch against pairs of surrogates drawn on the device, with the definitions of
+# `ResidentPower`:
+#   'ar1'    two independent AR(1) series per pair, series s with g_s = ar1(y_s)[0] and, with
+#            normalize=True, m = 0 and sigma = 1, else y_s's mean and standard deviation (ddof 0);
+#   'phase'  the phase-randomised surrogates of the two transformed series with independent phases:
+#            each keeps its own periodogram and is independent of the other.
+# Each pair is transformed exactly as `xwt` of it would be.  |W12|^2 is common power: a burst in one
+# series alone reaches it (Maraun & Kurths 2004), so these test common power, not association.
 
-class ResidentCrossWavelet(_ResidentSlot):
+class ResidentCrossWavelet(_SurrogateTest, _ResidentSlot):
     """W12 = W1 conj(W2) [S, n0] of one `xwt_resident` call, resident on the device.
 
     `signif` arguments of the methods are in |W12| units, as `xwt` returns them (`.signif`); a
     point is selected where |W12| > signif[j], i.e. re^2 + im^2 > signif[j]^2.  The sample
     script's `|W12|^2 / signif > 1` convention is `signif=np.sqrt(h.signif)`.  A negative entry
-    raises ValueError, a NaN entry selects no point of its scale."""
+    raises ValueError, a NaN entry selects no point of its scale.
+
+    Tests against surrogate pairs (see the notes above `xwt_resident`): `surrogate_test`, `pvalues`,
+    `pvalue_fraction`, `fdr_threshold`, `cluster_test` and `cluster_labels` are those of
+    `ResidentPower` with |W12|^2 in place of |W|^2; `sig` / `signif` stay in |W12| units.  They test
+    common power, not association: a burst in one series alone can be significant (Maraun & Kurths
+    2004).  The coherence tests are the tests of association."""
 
     _FREQ, _SERIAL, _RELEASE = 'freq', 'cross_serial', 'cross_release'
+    _CLUSTERS = _engine.CROSS
     _GONE = ("this cross spectrum is no longer resident: it was released or another xwt_resident "
              "has run on the same engine")
 
@@ -773,10 +791,62 @@ class ResidentCrossWavelet(_ResidentSlot):
                                                    precision, serial)
         self.freq = p.freq
         self.signif = signif
+        self.normalize = p.normalize
+        # raw series (ar1, mean and std) and the transformed ones (the phase null)
+        self._y = tuple(np.array(y, dtype=np.float64, copy=True) for y in (p.y1, p.y2))
+        self._yn = np.array(np.stack([p.y1n, p.y2n]), dtype=np.float64, copy=True)
+        self._padding = bool(_helpers._FFT_NEXT_POW2)
+
+    def _threshold(self, signif):
+        """A |W12| threshold per scale, squared: the device compares re^2 + im^2."""
+        return None if signif is None else _power_threshold(self, signif) ** 2
 
     def _stats(self, lo, hi, signif):
-        thr = None if signif is None else _power_threshold(self, signif) ** 2
-        return self.engine.field_row_stats(_engine.FIELD_CROSS, lo, hi, thr)
+        return self.engine.field_row_stats(_engine.FIELD_CROSS, lo, hi, self._threshold(signif))
+
+    def _null(self, null):
+        """(engine null, g [2], m [2], sigma [2]) of a null's name."""
+        if null not in _NULLS:
+            raise ValueError("null must be 'ar1' or 'phase', got %r" % (null,))
+        g = [ar1(y)[0] if null == 'ar1' else 0.0 for y in self._y]
+        if self.normalize:
+            m, sigma = [0.0, 0.0], [1.0, 1.0]
+        else:
+            m, sigma = [float(y.mean()) for y in self._y], [float(y.std()) for y in self._y]
+        return _NULLS[null], g, m, sigma
+
+    def _on_device(self, call, null, seed, M, *args):
+        kind, g, m, sigma = self._null(null)
+        _sync_padding(self.engine, self.n0)
+        return call(self._yn, kind, g, m, sigma, seed, 0, M, self.dt, self.scales,
+                    *self.wavelet._engine_spec(), self._serial, *args)
+
+    def _count_units(self, seed, M, null):
+        self._on_device(self.engine.cross_surrogate_counts, null, seed, M)
+
+    def _cluster_units(self, seed, M, thr, lo, hi, q, null):
+        return self._on_device(self.engine.cross_cluster_test, null, seed, M, thr, lo, hi, q)
+
+    def _selected(self, lo, hi, signif, alpha, cluster):
+        """The five row stats of `field_row_stats` over the columns [lo, hi) and the selection of
+        `signif`, `alpha` or `cluster`."""
+        if cluster is None:
+            if alpha is not None:
+                return self._cut_stats(_engine.CROSS, lo, hi, self._threshold(signif), alpha)
+            return self._stats(lo, hi, signif)
+        if signif is not None or alpha is not None:
+            raise ValueError("cluster selects the points of one cluster: it takes no signif or alpha")
+        _, _, box = self.engine.cluster_table(_engine.CROSS)
+        if isinstance(cluster, bool) or not isinstance(cluster, (int, np.integer)) \
+                or not 0 <= cluster < len(box):
+            raise ValueError("cluster must be a row of the last cluster_test's result (0 .. %d), got %r"
+                             % (len(box) - 1, cluster))
+        r0, r1, c0, c1 = (int(v) for v in box[cluster])
+        rows = np.arange(len(self.scales))
+        inside = (rows >= r0) & (rows < r1)
+        lo = np.where(inside, np.maximum(lo, c0), 0)
+        hi = np.where(inside, np.maximum(np.minimum(hi, c1), lo), 0)
+        return self.engine.cross_cluster_row_stats(int(cluster), lo, hi)
 
     # -- the products --------------------------------------------------------------------
     @_live
@@ -791,11 +861,13 @@ class ResidentCrossWavelet(_ResidentSlot):
         return _field_window(self.engine, _engine.FIELD_CROSS, self.shape, rows, cols)
 
     @_live
-    def global_power(self, inside_coi=False, signif=None):
+    def global_power(self, inside_coi=False, signif=None, alpha=None, cluster=None):
         """Mean |W12| per scale over the selected points: inside the cone of influence if
-        `inside_coi`, where |W12| > signif[j] if `signif` is given.  NaN for a scale without
-        points."""
-        st = self._stats(*_column_ranges(self, inside_coi), signif)
+        `inside_coi`, where |W12| > signif[j] if `signif` is given, where the p-value of the last
+        `surrogate_test` is <= alpha if `alpha` is given (all: logical AND), or, with `cluster`, on
+        the points of row `cluster` of the last `cluster_test`'s result (and inside the cone if
+        `inside_coi`; no `signif` or `alpha`).  NaN for a scale without points."""
+        st = self._selected(*_column_ranges(self, inside_coi), signif, alpha, cluster)
         return _ratio(st[:, 2], st[:, 0])
 
     @_live
@@ -808,16 +880,19 @@ class ResidentCrossWavelet(_ResidentSlot):
 
     @_live
     def mean_phase(self, period_min=-np.inf, period_max=np.inf, inside_coi=True, signif=None,
-                   per_scale=False):
+                   per_scale=False, alpha=None, cluster=None):
         """Circular mean of angle(W12) over the points of the scales with period_min <= period <
-        period_max, inside the cone of influence if `inside_coi`, where |W12| > signif if given
-        (Grinsted et al. 2004): MeanPhase(angle = atan2(sum sin, sum cos), strength =
-        |sum e^{i angle}| / count, count), for the whole band or, with `per_scale`, per scale
-        (NaN angle and strength where the count is 0).  A zero coefficient has phase 0."""
+        period_max, inside the cone of influence if `inside_coi`, where |W12| > signif if given and
+        where the p-value of the last `surrogate_test` is <= alpha if given (Grinsted et al. 2004),
+        or, with `cluster`, on the points of row `cluster` of the last `cluster_test`'s result (the
+        lead or lag inside one significant patch; no `signif` or `alpha`): MeanPhase(angle =
+        atan2(sum sin, sum cos), strength = |sum e^{i angle}| / count, count), for the whole band
+        or, with `per_scale`, per scale (NaN angle and strength where the count is 0).  A zero
+        coefficient has phase 0."""
         sel = self._band(period_min, period_max)
         lo, hi = _column_ranges(self, inside_coi)
         lo, hi = np.where(sel, lo, 0), np.where(sel, hi, 0)
-        st = self._stats(lo, hi, signif)
+        st = self._selected(lo, hi, signif, alpha, cluster)
         return _mean_phase(st[:, 0], st[:, 3], st[:, 4], per_scale)
 
     @_live
@@ -829,6 +904,45 @@ class ResidentCrossWavelet(_ResidentSlot):
         if not sel.any():
             raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
         return self.engine.cross_scale_avg(w)
+
+    @_live
+    def surrogate_test(self, mc_count=300, seed=None, null='ar1'):
+        """Run the pairs 0 .. mc_count - 1 of `null` ('ar1' or 'phase') once and count per point the
+        pairs whose |W12|^2 reaches this one (kept on the device, replacing the counts of an earlier
+        test).  Seed, records and errors as `ResidentPower.surrogate_test`."""
+        self._null(null)
+        self._count(mc_count, seed, null)
+
+    @_live
+    def pvalues(self, rows=slice(None), cols=slice(None)):
+        """p[rows, cols] = (1 + k) / (1 + M) (float64) of the last `surrogate_test`, with the slicing
+        of `window`; NaN where |W12| is not finite."""
+        return self._pvalues(_engine.CROSS, rows, cols)
+
+    @_live
+    def pvalue_fraction(self, alpha):
+        """Per scale, the fraction of the points inside the cone of influence (with a finite p) whose
+        p <= alpha; NaN for a scale without such points."""
+        return self._pvalue_fraction(_engine.CROSS, alpha)
+
+    @_live
+    def fdr_threshold(self, q=0.05, method='bh', inside_coi=True):
+        """`ResidentCoherence.fdr_threshold` over the p-values of the last `surrogate_test`."""
+        return self._fdr_threshold(_engine.CROSS, q, method, inside_coi)
+
+    @_live
+    def cluster_test(self, sig, mc_count=300, seed=None, null='ar1', inside_coi=True):
+        """Cluster (areawise) test of this cross spectrum against the pairs 0 .. mc_count - 1 of
+        `null`: `ResidentCoherence.cluster_test` with a point selected where |W12| is finite and
+        > sig[j] (|W12| units: `h.cluster_test(h.signif, ...)` is the natural call).  Returns
+        ClusterResult; the counts of an earlier `surrogate_test` are kept."""
+        self._null(null)
+        return self._cluster(sig, mc_count, seed, inside_coi, null)
+
+    @_live
+    def cluster_labels(self, rows=slice(None), cols=slice(None)):
+        """`ResidentCoherence.cluster_labels` of the last `cluster_test`."""
+        return self._cluster_labels(rows, cols)
 
 
 def xwt_resident(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95, wavelet='morlet',
