@@ -339,6 +339,17 @@ int cwtb_power_cluster_table(cwtb_ctx *ctx, int64_t cap, int64_t *count, uint64_
                              int64_t *box);
 int cwtb_power_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_step, int64_t col0, int64_t ncols,
                               int64_t col_step, int32_t *out);
+/* cwtb_field_reconstruct of the kept W over the points with a finite P and k <= kmax of the last
+ * cwtb_power_surrogate_counts (and P > thr[j] where thr is not NULL).  CWTB_ERR_STATE without a
+ * power or without counts. */
+int cwtb_power_pvalue_reconstruct(cwtb_ctx *ctx, const double *weights, const int64_t *lo, const int64_t *hi,
+                                  const double *thr, int64_t kmax, double *out);
+/* cwtb_field_reconstruct of the kept W over the points that the last cwtb_power_cluster_test labelled
+ * c + 1 for some c in clusters[0 .. n_clusters) (rows of its table; a repeated row counts once,
+ * n_clusters == 0 gives zeros).  CWTB_ERR_STATE before a cluster test, CWTB_ERR_ARG for a row outside
+ * the table, n_clusters < 0 or a NULL clusters with n_clusters > 0. */
+int cwtb_power_cluster_reconstruct(cwtb_ctx *ctx, const double *weights, const int64_t *lo, const int64_t *hi,
+                                   const int64_t *clusters, int64_t n_clusters, double *out);
 
 /* ---- tests of the resident cross spectrum against surrogate pairs -------------------------------
  * The tests of the power above on W12 of cwtb_xwt_resident, with P = |W12|^2 formed by the same
@@ -468,6 +479,18 @@ int cwtb_field_window(cwtb_ctx *ctx, int field, int row0, int nrows, int row_ste
  * sin phi = im/|F|; a zero coefficient has phase 0 (adds (1, 0)). */
 int cwtb_field_row_stats(cwtb_ctx *ctx, int field, const int64_t *lo, const int64_t *hi,
                          const double *thr, double *out);
+/* Reconstruction over a selection (Torrence & Compo 1998, eq. 29 restricted to selected points), the
+ * column-wise counterpart of cwtb_field_row_stats: out[n] = sum_j weights[j] * Re F[j,n] (n0 doubles)
+ * over the points with lo[j] <= n < hi[j] and, where thr is not NULL, re^2 + im^2 > thr[j] (in double,
+ * false for a NaN threshold).  The inverse transform's factor dj sqrt(dt) / (Cdelta psi(0)) is the
+ * caller's; pass weights[j] = 1 / sqrt(s_j) on the rows to sum and 0 elsewhere: rows with weight 0
+ * or an empty range are not read, and a column without a selected point is 0.  For CWTB_FIELD_W and
+ * CWTB_FIELD_POWER only: CWTB_ERR_ARG for CWTB_FIELD_CROSS (no inverse is defined for it), an unknown
+ * field, a NULL weights / lo / hi / out, lo[j] < 0, lo[j] > hi[j] or hi[j] > n0.  Each column adds
+ * its rows in ascending order, each step weights[j] * Re F rounded and then added rounded (no fused
+ * multiply-add, no atomics): repeated calls are bit-identical. */
+int cwtb_field_reconstruct(cwtb_ctx *ctx, int field, const double *weights, const int64_t *lo,
+                           const int64_t *hi, const double *thr, double *out);
 /* out[n] = sum_j weights[j] * W12[j,n] (n0 complex128) over the cross spectrum.  Rows with weight
  * 0 are not read. */
 int cwtb_cross_scale_avg(cwtb_ctx *ctx, const double *weights, void *out);

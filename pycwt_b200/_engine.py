@@ -98,6 +98,7 @@ _SIGNATURES = {
     "cwtb_field_get": (_I, [_P, _I, _I, _I, _P]),
     "cwtb_field_window": (_I, [_P, _I, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_field_row_stats": (_I, [_P, _I, _P, _P, _P, _P]),
+    "cwtb_field_reconstruct": (_I, [_P, _I, _P, _P, _P, _P, _P]),
     "cwtb_cross_scale_avg": (_I, [_P, _P, _P]),
     "cwtb_smooth": (_I, [_P, _P, _I, _I, _I64, _D, _P, _I, _P]),
     "cwtb_wct_mc": (_I, [_P, _P, _I, _I64, _D, _D, _P, _I, _I, _D, _I, _P, _I, _I, _P]),
@@ -144,6 +145,8 @@ _SIGNATURES = {
     "cwtb_power_count_hist": (_I, [_P, _P, _P, _I64, _P]),
     "cwtb_power_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
     "cwtb_power_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
+    "cwtb_power_pvalue_reconstruct": (_I, [_P, _P, _P, _P, _P, _I64, _P]),
+    "cwtb_power_cluster_reconstruct": (_I, [_P, _P, _P, _P, _P, _I64, _P]),
     "cwtb_mc_ar1_pair_surrogates": (_I, [_P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _P]),
     "cwtb_cross_surrogate_counts": (_I, [_P, _P, _I, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I,
                                          _D, _I64, _I]),
@@ -794,6 +797,22 @@ class Engine(object):
                                                   None if thr is None else _ptr(thr), _ptr(out)))
         return out
 
+    def _reconstruct(self, name, product, weights, lo, hi, thr, call):
+        """float64 [n0] of a cwtb_*_reconstruct `call(w, lo, hi, thr, out)` on the resident product."""
+        rows, n0, _ = self._shape(product)
+        w = _weights(name, rows, weights)
+        lo, hi, thr = _row_args(name, rows, lo, hi, thr)
+        out = self.result_array((n0,), np.float64)
+        self._check(call(_ptr(w), _ptr(lo), _ptr(hi), None if thr is None else _ptr(thr), _ptr(out)))
+        return out
+
+    @_locked
+    def field_reconstruct(self, field, weights, lo, hi, thr=None):
+        """sum_j weights[j] Re F[j, n] (float64, n0) over the columns [lo[j], hi[j]) where thr is None
+        or |F|^2 > thr[j] (cwtb_field_reconstruct: W or the power's W)."""
+        return self._reconstruct("field_reconstruct", field, weights, lo, hi, thr,
+                                 lambda *a: self.lib.cwtb_field_reconstruct(self.h, int(field), *a))
+
     @_locked
     def cross_scale_avg(self, weights):
         """sum_j w_j W12[j, :] (complex128, n0)."""
@@ -1163,6 +1182,23 @@ class Engine(object):
         out = self.result_array((n0,), np.float64)
         self._check(self.lib.cwtb_power_scale_avg(self.h, _ptr(w), _ptr(out)))
         return out
+
+    @_locked
+    def power_pvalue_reconstruct(self, weights, lo, hi, kmax, thr=None):
+        """`field_reconstruct` of the resident power over the points with a finite |W|^2 and k <= kmax
+        of its counts (cwtb_power_pvalue_reconstruct)."""
+        return self._reconstruct("power_pvalue_reconstruct", PRODUCT_POWER, weights, lo, hi, thr,
+                                 lambda w, lo, hi, thr, out: self.lib.cwtb_power_pvalue_reconstruct(
+                                     self.h, w, lo, hi, thr, int(kmax), out))
+
+    @_locked
+    def power_cluster_reconstruct(self, weights, lo, hi, clusters):
+        """`field_reconstruct` of the resident power over the points of the clusters `clusters` (rows of
+        the table) of its last cluster test (cwtb_power_cluster_reconstruct)."""
+        cl = np.ascontiguousarray(clusters, dtype=np.int64).reshape(-1)
+        return self._reconstruct("power_cluster_reconstruct", PRODUCT_POWER, weights, lo, hi, None,
+                                 lambda w, lo, hi, thr, out: self.lib.cwtb_power_cluster_reconstruct(
+                                     self.h, w, lo, hi, _ptr(cl), cl.size, out))
 
     @_locked
     def mc_ar1_surrogates(self, g, m, sigma, seed, first_unit, n_units, n0):

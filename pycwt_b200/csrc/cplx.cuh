@@ -72,6 +72,16 @@ HD double norm2_rn(double re, double im) {
 #endif
 }
 
+// s + w x with each operation rounded (no fused multiply-add): a sum of such steps in a fixed order
+// is one fixed sequence of correctly rounded operations, on the device and on the host alike
+HD double add_mul_rn(double s, double w, double x) {
+#if defined(__CUDA_ARCH__) && !defined(CWTB_HOST_EMU)
+  return __dadd_rn(s, __dmul_rn(w, x));
+#else
+  return s + w * x;
+#endif
+}
+
 // ---- DFT_R in registers: x[c] <- sum_i x[i] e^{SIGN 2 pi i * i*c/R}, natural order ----
 template <int SIGN, typename V> HD void dft2(V &a, V &b) {
   V t = csub(a, b);

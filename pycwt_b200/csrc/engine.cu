@@ -2915,6 +2915,62 @@ static int scale_avg_run(cwtb_ctx *c, const FieldRef &f, const double *weights, 
   });
 }
 
+// The reconstruction's sum out[n] = sum_j weights[j] Re F[j, n] of a complex field (cwtb_*_reconstruct)
+// over the columns [lo_j, hi_j), where thr is null or P > thr[j], and, for a field with counts
+// (count_ref), where P is finite and k <= kmax, or, with `mark` (n_mark bytes over the labels of
+// f.lab), where mark[label] != 0.  Rows with a zero weight or an empty range are not read; a
+// column without a selected point is 0.
+static int reconstruct_run(cwtb_ctx *c, const FieldRef &f, const double *weights, const int64_t *lo,
+                           const int64_t *hi, const double *thr, const unsigned char *mark, size_t n_mark,
+                           double *out) {
+  if (!weights || !lo || !hi || !out) return fail(c, CWTB_ERR_ARG, "null argument");
+  const int S = f.S;
+  const long long n0 = f.n0;
+  std::vector<int> sel;
+  for (int j = 0; j < S; ++j) {
+    if (lo[j] < 0 || hi[j] > n0 || lo[j] > hi[j])
+      return fail(c, CWTB_ERR_ARG, "reconstruct: column range outside [0, n0) or lo > hi");
+    if (weights[j] != 0.0 && lo[j] < hi[j]) sel.push_back(j);
+  }
+  const int nsel = (int)sel.size();
+  // aux, 8-byte words: [weights S][lo S][hi S][thr S][selected rows, S ints][mark bytes][out n0]
+  const size_t wsel = ((size_t)S + 1) / 2, wmark = (n_mark + 7) / 8;
+  const size_t head = 4 * (size_t)S + wsel + wmark;
+  std::vector<double> h(head, 0.0);
+  memcpy(h.data(), weights, (size_t)S * sizeof(double));
+  memcpy(h.data() + S, lo, (size_t)S * sizeof(int64_t));
+  memcpy(h.data() + 2 * (size_t)S, hi, (size_t)S * sizeof(int64_t));
+  if (thr) memcpy(h.data() + 3 * (size_t)S, thr, (size_t)S * sizeof(double));
+  if (nsel) memcpy(h.data() + 4 * (size_t)S, sel.data(), (size_t)nsel * sizeof(int));
+  if (n_mark) memcpy(h.data() + 4 * (size_t)S + wsel, mark, n_mark);
+  int e = ensure(c, c->aux, (head + (size_t)n0) * sizeof(double));
+  if (e) return e;
+  double *dh = (double *)c->aux.p, *dout = dh + head;
+  RT(rt_h2d(dh, h.data(), head * sizeof(double), c->stream));
+  const long long *dlo = (const long long *)(dh + S), *dhi = dlo + S;
+  const int *dsel = (const int *)(dh + 4 * (size_t)S);
+  const unsigned char *dmark = (const unsigned char *)(dh + 4 * (size_t)S + wsel);
+  auto run = [&](auto v) {
+    using B = SelScaleAvgBody<decltype(v)>;
+    typename B::Args a{v, dh, dsel, nsel, dout, n0, dlo, dhi, thr ? dh + 3 * (size_t)S : nullptr};
+    int e2 = launch<B>(c, (unsigned)((n0 + NT - 1) / NT), 1, a);
+    if (e2) return e2;
+    RT(rt_d2h(out, dout, (size_t)n0 * sizeof(double), c->stream));
+    RT(rt_sync(c->stream));
+    return 0;
+  };
+  if (f.prec == CWTB_F64) {
+    const cx<double> *F = (const cx<double> *)f.p;
+    if (mark) return run(CxReView<double, RE_LABEL>{F, nullptr, 0, f.lab, dmark});
+    if (f.cnt) return run(CxReView<double, RE_COUNT>{F, f.cnt, f.kmax});
+    return run(CxReView<double, RE_ALL>{F});
+  }
+  const cx<float> *F = (const cx<float> *)f.p;
+  if (mark) return run(CxReView<float, RE_LABEL>{F, nullptr, 0, f.lab, dmark});
+  if (f.cnt) return run(CxReView<float, RE_COUNT>{F, f.cnt, f.kmax});
+  return run(CxReView<float, RE_ALL>{F});
+}
+
 // Histogram [M + 1] of the counts of a field with counts over the columns [lo_j, hi_j) of every
 // row, of the points whose value is finite
 static int count_hist_run(cwtb_ctx *c, const FieldRef &f, const int64_t *lo, const int64_t *hi, int64_t nbins,
@@ -2976,6 +3032,15 @@ int cwtb_field_row_stats(cwtb_ctx *c, int field, const int64_t *lo, const int64_
   FieldRef f;
   int e = cx_field_ref(c, field, f);
   return e ? e : row_stats_run(c, f, lo, hi, thr, 0, out);
+}
+
+int cwtb_field_reconstruct(cwtb_ctx *c, int field, const double *weights, const int64_t *lo, const int64_t *hi,
+                           const double *thr, double *out) {
+  if (c && field == CWTB_FIELD_CROSS)
+    return fail(c, CWTB_ERR_ARG, "reconstruct: the cross spectrum has no inverse transform");
+  FieldRef f;
+  int e = cx_field_ref(c, field, f);
+  return e ? e : reconstruct_run(c, f, weights, lo, hi, thr, nullptr, 0, out);
 }
 
 int cwtb_cross_scale_avg(cwtb_ctx *c, const double *weights, void *out) {
@@ -4214,6 +4279,33 @@ int cwtb_power_cluster_labels(cwtb_ctx *c, int row0, int nrows, int row_step, in
                               int64_t col_step, int32_t *out) {
   int e = c ? clusters_of(c, c->pw, "power") : CWTB_ERR_ARG;
   return e ? e : labels_window(c, c->pw, row0, nrows, row_step, col0, ncols, col_step, out);
+}
+
+int cwtb_power_pvalue_reconstruct(cwtb_ctx *c, const double *weights, const int64_t *lo, const int64_t *hi,
+                                  const double *thr, int64_t kmax, double *out) {
+  FieldRef f;
+  int e = field_ref(c, CWTB_FIELD_POWER, f);
+  if (e || (e = count_ref(c, kmax, f))) return e;
+  return reconstruct_run(c, f, weights, lo, hi, thr, nullptr, 0, out);
+}
+
+int cwtb_power_cluster_reconstruct(cwtb_ctx *c, const double *weights, const int64_t *lo, const int64_t *hi,
+                                   const int64_t *clusters, int64_t n_clusters, double *out) {
+  int e = c ? clusters_of(c, c->pw, "power") : CWTB_ERR_ARG;
+  if (e) return e;
+  if (n_clusters < 0 || (n_clusters > 0 && !clusters)) return fail(c, CWTB_ERR_ARG, "null argument");
+  // mark[label]: label c + 1 is row c of the table, label 0 is off the clusters
+  const size_t nt = c->pw.table.Q.size();
+  std::vector<unsigned char> mark(nt + 1, 0);
+  for (int64_t i = 0; i < n_clusters; ++i) {
+    if (clusters[i] < 0 || clusters[i] >= (int64_t)nt)
+      return fail(c, CWTB_ERR_ARG, "power_cluster_reconstruct: no such cluster in the last cluster test");
+    mark[(size_t)clusters[i] + 1] = 1;
+  }
+  FieldRef f;
+  if ((e = field_ref(c, CWTB_FIELD_POWER, f))) return e;
+  f.lab = (const int *)c->pw.labels.p;
+  return reconstruct_run(c, f, weights, lo, hi, nullptr, mark.data(), mark.size(), out);
 }
 
 // ---- tests of the resident cross spectrum against surrogate pairs ---------------------------------

@@ -2447,7 +2447,8 @@ template <typename T> struct ScaleAvgBody {
 //               in double, after widening
 // A view supplies, for RowStatsBody: K sums per row, E elements per 16-byte vector, VPT 16-byte
 // vectors per thread per chunk, load (vector q), add (element e of a vector) and add_at (element
-// p, at a chunk's odd edge); for SelScaleAvgBody: NA sums per column, Pt, point, acc and put; for
+// p, at a chunk's odd edge); for SelScaleAvgBody: NA sums per column, SEL, Pt, point, acc and put
+// (and keep with SEL); for
 // WindowBody: copy.
 
 // Row stats [count, sum WCT, sum cos aWCT, sum sin aWCT] of the points with WCT > thr_j; aWCT is
@@ -2460,6 +2461,7 @@ template <bool PHASE> struct CohViewT {
   const double *WCT, *aWCT;   // aWCT: unused (may be null) without PHASE
   int want_phase;
   static constexpr int K = 4, E = 2, VPT = 16, NA = 3;   // VPT: two loads each, one per field
+  static constexpr bool SEL = false;                     // SelScaleAvgBody: every column of a row
   struct Vec { double2 w, g; };
   HD Vec load(size_t q) const {
     Vec v{ld_stream((const double2 *)WCT + q), make_double2(0, 0)};
@@ -2582,6 +2584,7 @@ template <typename T> struct CxView {
   using V16 = CxVec16<T>;
   using Vec = typename V16::V;
   static constexpr int K = 5, E = V16::E, VPT = 32, NA = 2;
+  static constexpr bool SEL = false;
   HD Vec load(size_t q) const { return ld_stream((const Vec *)F + q); }
   HD static void add1(double (&s)[K], double re, double im, bool has_thr, double t) {
     const double p = norm2_rn(re, im);
@@ -2772,8 +2775,48 @@ template <int K> struct RowSumBody {
   }
 };
 
+// The real part of a complex field for the reconstruction (cwtb_*_reconstruct): NA = 1 sum
+// w_j Re F[j, n], each step rounded on its own (add_mul_rn), over the points that SelScaleAvgBody's
+// column range and threshold on P = power_of(F) pass and that the form's predicate keeps:
+//   RE_ALL    every point
+//   RE_COUNT  P finite and k <= kmax (CxCountView's cut; cnt: the power's counts)
+//   RE_LABEL  mark[label] != 0 (lab: the label image of the last cluster test, mark: a byte table
+//             over the labels [0, n_clusters])
+enum ReForm { RE_ALL, RE_COUNT, RE_LABEL };
+template <typename T, int FORM> struct CxReView {
+  const cx<T> *F;
+  const unsigned *cnt = nullptr;
+  long long kmax = 0;
+  const int *lab = nullptr;
+  const unsigned char *mark = nullptr;
+  static constexpr int NA = 1;
+  static constexpr bool SEL = true;
+  struct Pt { cx<T> v; unsigned k; };   // k: the count (RE_COUNT) or the label (RE_LABEL)
+  HD Pt point(size_t p) const {
+    Pt r{ld_stream(&F[p]), 0u};
+    if constexpr (FORM == RE_COUNT) r.k = ld_stream(&cnt[p]);
+    if constexpr (FORM == RE_LABEL) r.k = (unsigned)ld_stream(&lab[p]);
+    return r;
+  }
+  HD bool keep(const Pt &v, bool has_thr, double t) const {
+    if constexpr (FORM == RE_LABEL) {
+      if (!mark[v.k]) return false;
+    }
+    if (FORM == RE_COUNT || has_thr) {
+      const double P = power_of<T>(v.v);
+      if (has_thr && !(P > t)) return false;
+      if constexpr (FORM == RE_COUNT) return isfinite(P) && (long long)v.k <= kmax;
+    }
+    return true;
+  }
+  HD static void acc(double (&s)[NA], double wj, const Pt &v) { s[0] = add_mul_rn(s[0], wj, (double)v.v.x); }
+  HD static void put(double *out, long long n, long long, const double (&s)[NA]) { st_stream(&out[n], s[0]); }
+};
+
 // The view's NA weighted sums over the selected rows (the selected-rows pattern of ScaleAvgBody),
-// four rows at a time: one thread per column adds the rows in order, no atomics.
+// four rows at a time: one thread per column adds the rows in order, no atomics.  A view with SEL
+// (CxReView) also takes a per-row column range [lo_j, hi_j), an optional per-row threshold and its
+// own predicate (keep): a point outside them adds nothing.  Views without SEL read none of them.
 template <typename View> struct SelScaleAvgArgs {
   View f;
   const double *w;     // per row
@@ -2781,6 +2824,8 @@ template <typename View> struct SelScaleAvgArgs {
   int nsel;
   double *out;         // NA doubles per column, laid out by View::put
   long long n;
+  const long long *lo = nullptr, *hi = nullptr;   // per row (SEL)
+  const double *thr = nullptr;                    // per row, or null (SEL)
 };
 template <typename View> struct SelScaleAvgBody {
   using Args = SelScaleAvgArgs<View>;
@@ -2790,6 +2835,33 @@ template <typename View> struct SelScaleAvgBody {
     const long long n = (long long)bx * NT + tid;
     if (n >= a.n) return;
     double s[View::NA] = {};
+    if constexpr (View::SEL) {
+      const bool has_thr = a.thr != nullptr;
+      auto in = [&](int j) { return n >= a.lo[j] && n < a.hi[j]; };
+      auto add = [&](int j, const typename View::Pt &v) {
+        if (a.f.keep(v, has_thr, has_thr ? a.thr[j] : 0.0)) View::acc(s, a.w[j], v);
+      };
+      int i = 0;
+      for (; i + 4 <= a.nsel; i += 4) {
+        typename View::Pt v[4] = {};
+        bool on[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int j = a.sel[i + u];
+          on[u] = in(j);
+          if (on[u]) v[u] = a.f.point((size_t)j * a.n + n);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (on[u]) add(a.sel[i + u], v[u]);
+      }
+      for (; i < a.nsel; ++i) {
+        const int j = a.sel[i];
+        if (in(j)) add(j, a.f.point((size_t)j * a.n + n));
+      }
+      View::put(a.out, n, a.n, s);
+      return;
+    }
     int i = 0;
     for (; i + 4 <= a.nsel; i += 4) {
       typename View::Pt v[4];

@@ -214,16 +214,47 @@ class ResidentTransform(_Resident):
     @_live
     def icwt(self):
         """Inverse transform of the resident coefficients (wavelet.py:169-170)."""
-        red = self.engine.icwt_sum()
-        fac = self.dj * np.sqrt(self.dt) / (self.wavelet.cdelta * self.wavelet.psi(0))
-        if not np.iscomplexobj(fac):
-            return fac * red
-        # complex factor (Morlet / Paul: psi(0) is complex in the reference, so is its icwt): one pass per
-        # component instead of NumPy's promote-then-multiply over N points
-        out = self.engine.result_array(red.shape, np.complex128)   # pooled: no first-touch page faults per call
-        np.multiply(red, np.real(fac), out=out.real)
-        np.multiply(red, np.imag(fac), out=out.imag)
-        return out
+        return _inverse(self, self.engine.icwt_sum())
+
+    @_live
+    def reconstruct(self, period_min=-np.inf, period_max=np.inf, inside_coi=False, signif=None):
+        """The inverse transform summed over the selected points only (wavelet filtering, TC98 §5
+        eq. 29): x[n] = dj sqrt(dt) / (Cdelta psi(0)) * sum over the selected (j, n) of
+        Re W[j, n] / sqrt(s_j), length n0, with the factor and the dtype of `icwt()`.  A point is
+        selected where every condition given holds: period_min <= period_j < period_max (ValueError
+        when no scale is in the band), inside the cone of influence if `inside_coi`, |W|^2 > signif[j]
+        if `signif` is given (power units; a NaN entry selects none of its scale).  A column without a
+        selected point is 0.  With everything selected it equals `icwt()` to rounding: the sums run in
+        another order.  W is read on the device; n0 numbers cross the bus."""
+        thr = None if signif is None else _power_threshold(self, signif)
+        w, lo, hi = _reconstruct_rows(self, period_min, period_max, inside_coi)
+        return _inverse(self, self.engine.field_reconstruct(_engine.FIELD_W, w, lo, hi, thr))
+
+
+def _inverse(h, red):
+    """dj sqrt(dt) / (Cdelta psi(0)) * red: the inverse transform of a sum of Re W / sqrt(s_j)."""
+    fac = h.dj * np.sqrt(h.dt) / (h.wavelet.cdelta * h.wavelet.psi(0))
+    if not np.iscomplexobj(fac):
+        return fac * red
+    # complex factor (Morlet / Paul: psi(0) is complex in the reference, so is its icwt): one pass per
+    # component instead of NumPy's promote-then-multiply over N points
+    out = h.engine.result_array(red.shape, np.complex128)   # pooled: no first-touch page faults per call
+    np.multiply(red, np.real(fac), out=out.real)
+    np.multiply(red, np.imag(fac), out=out.imag)
+    return out
+
+
+def _reconstruct_rows(h, period_min, period_max, inside_coi):
+    """(weights, lo, hi) of a reconstruction: 1 / sqrt(s_j) on the band and 0 elsewhere, and the
+    columns of each row."""
+    if h.wavelet.cdelta == -1:
+        raise ValueError('Cdelta not defined for this wavelet')
+    sel = h._band(period_min, period_max)
+    if not sel.any():
+        raise ValueError("no scale with %r <= period < %r" % (period_min, period_max))
+    w = np.where(sel, 1.0 / np.sqrt(np.asarray(h.scales, dtype=float)), 0.0)
+    lo, hi = _column_ranges(h, inside_coi)
+    return w, lo, hi
 
 
 def _engine_wavelet(wavelet, name):
@@ -1317,6 +1348,45 @@ class ResidentPower(_SurrogateTest, _ResidentSlot):
         `ResidentTransform.scale_avg_power`."""
         _, w = self._band_weights(period_min, period_max, variance)
         return self.engine.power_scale_avg(w)
+
+    @_live
+    def reconstruct(self, period_min=-np.inf, period_max=np.inf, inside_coi=False, signif=None, alpha=None,
+                    cluster=None):
+        """The series behind a band, the significant points or the significant clusters of this power:
+        `ResidentTransform.reconstruct` on this handle's W, x[n] = dj sqrt(dt) / (Cdelta psi(0)) * sum
+        over the selected (j, n) of Re W[j, n] / sqrt(s_j).  A point is selected where every condition
+        given holds: the band and `inside_coi` as there; P > signif[j] if `signif` is given; a finite P
+        whose p-value of the last `surrogate_test` is <= alpha if `alpha` is given (EngineError without
+        a test); or, with `cluster` (an int or a sequence of ints, rows of the last `cluster_test`'s
+        ClusterResult, e.g. `np.flatnonzero(res.pvalue <= 0.05)`; a repeated row counts once, an empty
+        one gives zeros), on the points of those clusters, with no `signif` or `alpha`.
+
+        W is the W of the transformed series: with normalize=True the result is in standardised units;
+        multiply it by the series' standard deviation (`y.std()`) for data units."""
+        thr = self._threshold(signif)
+        w, lo, hi = _reconstruct_rows(self, period_min, period_max, inside_coi)
+        if cluster is not None:
+            if signif is not None or alpha is not None:
+                raise ValueError("cluster selects the points of clusters: it takes no signif or alpha")
+            rows = self._cluster_rows(cluster)
+            red = self.engine.power_cluster_reconstruct(w, lo, hi, rows)
+        elif alpha is not None:
+            red = self.engine.power_pvalue_reconstruct(w, lo, hi, _kmax(alpha, self._units()), thr)
+        else:
+            red = self.engine.field_reconstruct(_engine.FIELD_POWER, w, lo, hi, thr)
+        return _inverse(self, red)
+
+    def _cluster_rows(self, cluster):
+        """int64 rows of the last cluster_test's table: an int or a sequence of ints."""
+        Q, _, _ = self.engine.cluster_table(_engine.POWER)
+        rows = np.asarray(cluster)
+        if rows.ndim > 1 or rows.dtype == bool or (rows.size and not np.issubdtype(rows.dtype, np.integer)):
+            raise ValueError("cluster must be an int or a sequence of ints, got %r" % (cluster,))
+        rows = rows.astype(np.int64).reshape(-1)
+        if ((rows < 0) | (rows >= len(Q))).any():
+            raise ValueError("cluster must hold rows of the last cluster_test's result (0 .. %d), got %r"
+                             % (len(Q) - 1, cluster))
+        return rows
 
     @_live
     def surrogate_test(self, mc_count=300, seed=None, null='ar1'):
