@@ -290,7 +290,7 @@ int64_t cwtb_power_serial(cwtb_ctx *ctx);
 int cwtb_power_release(cwtb_ctx *ctx);
 /* cwtb_scale_avg_power on the kept W */
 int cwtb_power_scale_avg(cwtb_ctx *ctx, const double *weights, double *out);
-/* The nulls of the power tests.  CWTB_NULL_AR1: unit u is x = m + sigma z, z[0] = e[0],
+/* The nulls of the tests against surrogates (power, cross spectrum, coherence).  CWTB_NULL_AR1: unit u is x = m + sigma z, z[0] = e[0],
  * z[i] = g z[i-1] + sqrt(1 - g^2) e[i], e standard normals that are a pure function of (seed, u, i)
  * (the Philox4x32-10 stream of cwtb_wct_mc_seeded under a counter tag of its own: no counter of
  * the white-noise pairs or triples or of the phase-randomised surrogates recurs for
@@ -575,6 +575,28 @@ int cwtb_wct_mc_phase(cwtb_ctx *ctx, const double *series, int nser, const int *
 /* Test hook: the surrogates themselves, out[n_units][nser][n0]. */
 int cwtb_mc_phase_surrogates(cwtb_ctx *ctx, const double *series, int nser, const int *group,
                              uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out);
+/* cwtb_wct_mc_phase with the null of choice (cwtb_wct_mc_phase is this call with CWTB_NULL_PHASE):
+ *   CWTB_NULL_PHASE: the phase-randomised surrogates of `series` in the phase groups `group`, as
+ *     cwtb_wct_mc_phase (g, m, sigma and held are not read);
+ *   CWTB_NULL_AR1: series s of unit u is the AR(1) series of cwtb_mc_ar1_surrogates with its own
+ *     g[s], m[s], sigma[s] under the series tag s of the counter (tag 0 is that call's stream, tag 1
+ *     the second series of cwtb_mc_ar1_pair_surrogates, tag 2 a stream of its own), at the data's
+ *     length n0, in double (fp32: rounded).  held[s] = 1 (held may be NULL: none) keeps row s of
+ *     `series` [nser][n0] in every unit instead, uploaded once per call in the coherence precision
+ *     as cwtb_wct3 uploads its inputs; only x1 and x2 of three series can be held.  `group` is not
+ *     read; `series` only for the held rows.
+ * CWTB_ERR_ARG also for an unknown null, AR(1) parameters that cwtb_mc_ar1_surrogates refuses (of
+ * the drawn series), a held flag other than 0 / 1, on y or on a series of a pair, and held rows
+ * without `series`. */
+int cwtb_wct_mc_null(cwtb_ctx *ctx, const double *series, int nser, int null, const int *group, const double *g,
+                     const double *m, const double *sigma, const int *held, uint64_t seed, int64_t first_unit,
+                     int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                     double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist_a,
+                     int64_t *hist_b);
+/* Test hook: the AR(1) units of nser = 1, 2 or 3 series (tags 0 .. nser - 1),
+ * out[n_units][nser][n0]; nser = 2 is cwtb_mc_ar1_pair_surrogates, nser = 1 cwtb_mc_ar1_surrogates. */
+int cwtb_mc_ar1_series_surrogates(cwtb_ctx *ctx, int nser, const double *g, const double *m, const double *sigma,
+                                  uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out);
 
 /* ---- point-wise tests of the resident coherence against phase-randomised surrogates ----------
  * cwtb_coherence_surrogate_counts (two series: the resident coherence of cwtb_wct_resident) and
@@ -604,6 +626,21 @@ int cwtb_coherence3_surrogate_counts(cwtb_ctx *ctx, const double *series, const 
                                      int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                                      int64_t *hist_partial, int64_t *hist_multiple, int64_t serial,
                                      int reset);
+/* The same with the null of choice, as cwtb_wct_mc_null (the calls above are these with
+ * CWTB_NULL_PHASE).  The counts remember the null of their units: reset == 0 on counts of another
+ * null is CWTB_ERR_STATE. */
+int cwtb_coherence_surrogate_counts_null(cwtb_ctx *ctx, const double *series, int null, const int *group,
+                                         const double *g, const double *m, const double *sigma, const int *held,
+                                         uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                         const double *scales, int n_scales, int family, double param,
+                                         int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist,
+                                         int64_t serial, int reset);
+int cwtb_coherence3_surrogate_counts_null(cwtb_ctx *ctx, const double *series, int null, const int *group,
+                                          const double *g, const double *m, const double *sigma, const int *held,
+                                          uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                          const double *scales, int n_scales, int family, double param,
+                                          int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                                          int64_t *hist_partial, int64_t *hist_multiple, int64_t serial, int reset);
 /* Reading the counts of M units.  They return CWTB_ERR_STATE when the product or its counts are not
  * resident, and the errors of the corresponding cwtb_coherence*_window / _row_stats calls.
  * p-value window: p = (1 + k) / (1 + M) in double, NaN where the observed value is not finite, with
@@ -655,6 +692,21 @@ int cwtb_coherence3_cluster_test(cwtb_ctx *ctx, const double *series, const int 
                                  int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
                                  int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
                                  const uint64_t *q, int measure, uint64_t *qmax_out);
+/* The same with the null of choice, as cwtb_wct_mc_null (the calls above are these with
+ * CWTB_NULL_PHASE). */
+int cwtb_coherence_cluster_test_null(cwtb_ctx *ctx, const double *series, int null, const int *group, const double *g,
+                                     const double *m, const double *sigma, const int *held, uint64_t seed,
+                                     int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                     int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                     int maxscale, int nbins, int64_t *hist, int64_t serial, const double *thr,
+                                     const int64_t *lo, const int64_t *hi, const uint64_t *q, uint64_t *qmax_out);
+int cwtb_coherence3_cluster_test_null(cwtb_ctx *ctx, const double *series, int null, const int *group, const double *g,
+                                      const double *m, const double *sigma, const int *held, uint64_t seed,
+                                      int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                      int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                      int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
+                                      int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
+                                      const uint64_t *q, int measure, uint64_t *qmax_out);
 /* The clusters of the resident map of the last cluster test, ordered by Q descending, ties by the
  * row-major index of the cluster's first point: *count = their number, and the first
  * min(cap, count) rows into Q[cap], points[cap] (point count) and box[cap][4] = first row, last

@@ -1,5 +1,6 @@
 """ctypes binding of the C-ABI engine (include/cwt_b200.h).  No PyTorch, no CPU
 fallback: if the CUDA library or a device is missing, calls raise EngineError."""
+import collections
 import ctypes
 import os
 import threading
@@ -18,7 +19,17 @@ MEASURE_PARTIAL, MEASURE_MULTIPLE = 0, 1   # the measures of the cwtb_coherence3
 # the resident products of cwtb_resident_shape: the two fields, the coherence (cwtb_coherence_*), the
 # partial and multiple coherence (cwtb_coherence3_*) and the power (cwtb_power_*)
 PRODUCT_W, PRODUCT_CROSS, PRODUCT_COHERENCE, PRODUCT_COHERENCE3, PRODUCT_POWER = 0, 1, 2, 3, 5   # 4: none
-NULL_AR1, NULL_PHASE = 0, 1      # the nulls of the power tests (cwtb_power_surrogate_counts)
+NULL_AR1, NULL_PHASE = 0, 1      # the nulls of the tests against surrogates (enum cwtb_null)
+
+
+class CoherenceNull(collections.namedtuple('CoherenceNull', 'kind groups g m sigma held')):
+    """The null of a coherence Monte-Carlo call (cwtb_wct_mc_null): NULL_PHASE with the phase group of
+    each series (`groups`), or NULL_AR1 with each series' AR(1) parameters g, m, sigma and held flag
+    (1: the data's row in every unit, None: every series drawn)."""
+    __slots__ = ()
+
+    def __new__(cls, kind, groups=None, g=None, m=None, sigma=None, held=None):
+        return super(CoherenceNull, cls).__new__(cls, kind, groups, g, m, sigma, held)
 # the `measure` of the surrogate-test readers below that names the resident power, and the one that
 # names the resident cross spectrum
 POWER = 'power'
@@ -127,6 +138,19 @@ _SIGNATURES = {
                                           _P, _I, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P]),
     "cwtb_coherence_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
     "cwtb_coherence3_cluster_table": (_I, [_P, _I64, _P, _P, _P, _P]),
+    # the coherence Monte-Carlo calls with the null of choice: (series, nser,) null, group, g, m, sigma,
+    # held in place of group
+    "cwtb_wct_mc_null": (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D, _P, _I, _I,
+                              _D, _I, _P, _I, _I, _P, _P]),
+    "cwtb_mc_ar1_series_surrogates": (_I, [_P, _I, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _P]),
+    "cwtb_coherence_surrogate_counts_null": (_I, [_P, _P, _I, _P, _P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64,
+                                                  _D, _P, _I, _I, _D, _I, _P, _I, _I, _P, _I64, _I]),
+    "cwtb_coherence3_surrogate_counts_null": (_I, [_P, _P, _I, _P, _P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64,
+                                                   _D, _P, _I, _I, _D, _I, _P, _I, _I, _P, _P, _I64, _I]),
+    "cwtb_coherence_cluster_test_null": (_I, [_P, _P, _I, _P, _P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D,
+                                              _P, _I, _I, _D, _I, _P, _I, _I, _P, _I64, _P, _P, _P, _P, _P]),
+    "cwtb_coherence3_cluster_test_null": (_I, [_P, _P, _I, _P, _P, _P, _P, _P, ctypes.c_uint64, _I64, _I, _I64, _D,
+                                               _P, _I, _I, _D, _I, _P, _I, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P]),
     "cwtb_coherence_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_coherence3_cluster_labels": (_I, [_P, _I, _I, _I, _I64, _I64, _I64, _P]),
     "cwtb_cluster_label_bits": (_I, [_P, _P, _I, _I64, _P, _I64, _P, _P, _P, _P, _P, _P]),
@@ -948,15 +972,38 @@ class Engine(object):
             raise ValueError("%s: non-finite sample" % name)
         return series, groups
 
+    @classmethod
+    def _null_inputs(cls, name, series, null):
+        """The data [nser, n0], the C arguments null, group, g, m, sigma, held of a coherence
+        Monte-Carlo call (cwtb_wct_mc_null) and the arrays behind them, which the caller keeps alive
+        across the call.  `null` is a CoherenceNull, or the phase groups of the phase null."""
+        if not isinstance(null, CoherenceNull):
+            null = CoherenceNull(NULL_PHASE, null)
+        if null.kind != NULL_AR1:   # the phase null, or an unknown one for the engine to refuse
+            series, groups = cls._phase_inputs(name, series, null.groups)
+            return series, (int(null.kind), _ptr(groups), None, None, None, None), groups
+        series = np.ascontiguousarray(series, dtype=np.float64)
+        if series.ndim != 2 or series.shape[0] not in (2, 3):
+            raise ValueError("%s: series must be [2 or 3, n0]" % name)
+        nser = series.shape[0]
+        held = np.zeros(nser) if null.held is None else null.held
+        arrays = tuple(np.ascontiguousarray(v, dtype=t) for v, t in ((null.g, np.float64), (null.m, np.float64),
+                                                                     (null.sigma, np.float64), (held, np.int32)))
+        if any(v.shape != (nser,) for v in arrays):
+            raise ValueError("%s: g, m, sigma and held take one entry per series (%d)" % (name, nser))
+        if not np.isfinite(series[arrays[3] != 0]).all():
+            raise ValueError("%s: non-finite sample in a held series" % name)
+        return series, (NULL_AR1, None) + tuple(_ptr(v) for v in arrays), arrays
+
     @_locked
-    def wct_mc_phase(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+    def wct_mc_phase(self, series, null, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
                      mask, maxscale, nbins, hist_a, hist_b=None, precision=F64):
-        """Monte-Carlo histograms of `n_units` phase-randomised surrogate units of `series`
-        [nser, n0] (cwtb_wct_mc_phase): series of equal `groups` number share the random phases and
-        keep their coherence.  Two series: `hist_a` the coherence histogram.  Three (y, x1, x2):
-        `hist_a` the partial, `hist_b` the multiple coherence, either may be None.  Accumulated
-        into the histograms [S, nbins]."""
-        series, groups = self._phase_inputs("wct_mc_phase", series, groups)
+        """Monte-Carlo histograms of `n_units` surrogate units of `series` [nser, n0]
+        (cwtb_wct_mc_null): `null` the phase groups of phase-randomised units (series of equal group
+        number share the random phases and keep their coherence) or a CoherenceNull.  Two series:
+        `hist_a` the coherence histogram.  Three (y, x1, x2): `hist_a` the partial, `hist_b` the
+        multiple coherence, either may be None.  Accumulated into the histograms [S, nbins]."""
+        series, nargs, _keep = self._null_inputs("wct_mc_phase", series, null)
         nser, n0 = series.shape
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
@@ -966,10 +1013,10 @@ class Engine(object):
             raise ValueError("wct_mc_phase: two series have one histogram")
         ha, hb = self._mc_hists("wct_mc_phase", sj.size, nbins, hist_a, hist_b)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
-        self._check(self.lib.cwtb_wct_mc_phase(self.h, _ptr(series), nser, _ptr(groups), int(seed) & (2 ** 64 - 1),
-                                               int(first_unit), int(n_units), n0, float(dt), _ptr(sj), sj.size,
-                                               int(family), float(param), int(boxcar_len), _ptr(mask),
-                                               int(maxscale), int(nbins), ha, hb))
+        self._check(self.lib.cwtb_wct_mc_null(self.h, _ptr(series), nser, *nargs, int(seed) & (2 ** 64 - 1),
+                                              int(first_unit), int(n_units), n0, float(dt), _ptr(sj), sj.size,
+                                              int(family), float(param), int(boxcar_len), _ptr(mask),
+                                              int(maxscale), int(nbins), ha, hb))
         return hist_a, hist_b
 
     @_locked
@@ -986,13 +1033,13 @@ class Engine(object):
     # `measure` None: the resident coherence (cwtb_coherence_*); MEASURE_PARTIAL / _MULTIPLE: the
     # resident partial / multiple coherence (cwtb_coherence3_*).
     @_locked
-    def surrogate_counts(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+    def surrogate_counts(self, series, null, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
                          mask, maxscale, nbins, hist_a, hist_b=None, serial=None, reset=True, precision=F64):
         """`wct_mc_phase` that also counts, per point, the units whose coherence (two series) or
         partial and multiple coherence (three) reach the resident product's, into that product's
-        counters (cwtb_coherence*_surrogate_counts); `serial` is the product's serial.  `reset`
-        zeroes the counters first, otherwise the units are added."""
-        series, groups = self._phase_inputs("surrogate_counts", series, groups)
+        counters (cwtb_coherence*_surrogate_counts_null); `serial` is the product's serial.  `reset`
+        zeroes the counters first, otherwise the units are added (to counts of the same null)."""
+        series, nargs, _keep = self._null_inputs("surrogate_counts", series, null)
         nser, n0 = series.shape
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
@@ -1002,13 +1049,13 @@ class Engine(object):
             raise ValueError("surrogate_counts: two series have one histogram")
         ha, hb = self._mc_hists("surrogate_counts", sj.size, nbins, hist_a, hist_b)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
-        args = (self.h, _ptr(series), _ptr(groups), int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
+        args = (self.h, _ptr(series), *nargs, int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
                 float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
                 int(nbins))
         if nser == 2:
-            self._check(self.lib.cwtb_coherence_surrogate_counts(*args, ha, int(serial), 1 if reset else 0))
+            self._check(self.lib.cwtb_coherence_surrogate_counts_null(*args, ha, int(serial), 1 if reset else 0))
         else:
-            self._check(self.lib.cwtb_coherence3_surrogate_counts(*args, ha, hb, int(serial), 1 if reset else 0))
+            self._check(self.lib.cwtb_coherence3_surrogate_counts_null(*args, ha, hb, int(serial), 1 if reset else 0))
         return hist_a, hist_b
 
     @_locked
@@ -1072,14 +1119,14 @@ class Engine(object):
     # `measure` None: the resident coherence; MEASURE_PARTIAL / _MULTIPLE: the resident partial /
     # multiple coherence.
     @_locked
-    def cluster_test(self, series, groups, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
+    def cluster_test(self, series, null, seed, first_unit, n_units, dt, scales, family, param, boxcar_len,
                      mask, maxscale, nbins, hist_a, hist_b=None, serial=None, thr=None, lo=None, hi=None, q=None,
                      measure=None, precision=F64):
         """`wct_mc_phase` that also labels the clusters of the resident product's map and of every
-        unit's (cwtb_coherence*_cluster_test): uint64 [n_units], the largest cluster sum Q of each
-        unit.  The resident map's clusters stay with the product (`cluster_table`,
+        unit's (cwtb_coherence*_cluster_test_null): uint64 [n_units], the largest cluster sum Q of
+        each unit.  The resident map's clusters stay with the product (`cluster_table`,
         `cluster_labels`)."""
-        series, groups = self._phase_inputs("cluster_test", series, groups)
+        series, nargs, _keep = self._null_inputs("cluster_test", series, null)
         nser, n0 = series.shape
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         mask = np.ascontiguousarray(mask, dtype=np.uint8)
@@ -1094,15 +1141,15 @@ class Engine(object):
             raise ValueError("cluster_test: q must have one entry per scale")
         qmax = np.zeros(int(n_units), dtype=np.uint64)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
-        args = (self.h, _ptr(series), _ptr(groups), int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
+        args = (self.h, _ptr(series), *nargs, int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
                 float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
                 int(nbins))
         rows = (_ptr(thr), _ptr(lo), _ptr(hi), _ptr(q))
         if nser == 2:
-            self._check(self.lib.cwtb_coherence_cluster_test(*args, ha, int(serial), *rows, _ptr(qmax)))
+            self._check(self.lib.cwtb_coherence_cluster_test_null(*args, ha, int(serial), *rows, _ptr(qmax)))
         else:
-            self._check(self.lib.cwtb_coherence3_cluster_test(*args, ha, hb, int(serial), *rows, int(measure),
-                                                              _ptr(qmax)))
+            self._check(self.lib.cwtb_coherence3_cluster_test_null(*args, ha, hb, int(serial), *rows, int(measure),
+                                                                   _ptr(qmax)))
         return qmax
 
     @staticmethod
@@ -1269,6 +1316,19 @@ class Engine(object):
         self._check(self.lib.cwtb_mc_ar1_pair_surrogates(self.h, _ptr(g), _ptr(m), _ptr(sigma),
                                                          int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
                                                          int(n0), _ptr(out)))
+        return out
+
+    @_locked
+    def mc_ar1_series_surrogates(self, g, m, sigma, seed, first_unit, n_units, n0):
+        """The AR(1) units of len(g) = 1, 2 or 3 series, float64 [n_units, nser, n0]: series s with
+        (g[s], m[s], sigma[s]) under the series tag s (two series: `mc_ar1_pair_surrogates`)."""
+        g, m, sigma = (np.ascontiguousarray(v, dtype=np.float64).reshape(-1) for v in (g, m, sigma))
+        if not g.shape == m.shape == sigma.shape:
+            raise ValueError("mc_ar1_series_surrogates: g, m and sigma take one entry per series")
+        out = np.empty((int(n_units), g.size, int(n0)), dtype=np.float64)
+        self._check(self.lib.cwtb_mc_ar1_series_surrogates(self.h, g.size, _ptr(g), _ptr(m), _ptr(sigma),
+                                                           int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units),
+                                                           int(n0), _ptr(out)))
         return out
 
     def _cross_args(self, name, series, null, g, m, sigma, seed, first_unit, n_units, dt, sj, family, param, serial):

@@ -175,6 +175,7 @@ struct ResidentSlot {
   // measure (cwtb_coherence*_surrogate_counts), and the units they hold (-1: none readable)
   Buf counts;
   long long units = -1;
+  int null = CWTB_NULL_PHASE;    // the coherence slots: the null of the units counted (cwtb_null)
   // the coherence slots: the observed clusters of the last cwtb_coherence*_cluster_test, the label
   // image int32 [S][n0] (0: no cluster, c + 1: row c of the table) and the table, valid with
   // `clusters`
@@ -3471,10 +3472,29 @@ static int label_bits(cwtb_ctx *c, int S, long long n0, const unsigned long long
 
 // common part of the Monte-Carlo entry points, for surrogate units of nser = 2 series (coherence,
 // one histogram) or 3 (partial and multiple coherence, hist[0] and hist[1], either may be null):
-// `noise` host surrogates [n_units][nser][n0]; or `phase` groups -> phase-randomised surrogates of
-// the data whose spectra are in c->pspec, drawn on the device from (seed, unit0 + i); or neither ->
-// white noise drawn on the device from (seed, unit0 + i); coherence in the engine type T
+// `noise` host surrogates [n_units][nser][n0]; or a null `tn` drawn on the device from (seed,
+// unit0 + i) (test_null: phase-randomised surrogates of the data whose spectra are in c->pspec, or
+// AR(1) series with held rows); or neither -> white noise drawn on the device from (seed,
+// unit0 + i); coherence in the engine type T
 struct PhaseSrc { int group[3]; };
+struct Ar1Src { double g, m, sigma; };
+// The null of a test of nser series: AR(1) units, series s with its own parameters ar[s] under the
+// series tag s, or phase-randomised units of the series (their spectra in c->pspec, series s in
+// phase group ph.group[s]).  An AR(1) series with held[s] is not drawn: every unit has the data's
+// row s of `series` there (host doubles, read once per call; the coherence tests only).
+struct TestNull {
+  int kind, nser;
+  Ar1Src ar[3];
+  PhaseSrc ph;
+  int held[3];
+  const double *series;
+};
+
+extern "C++" {
+template <typename T>
+static int ar1_units(cwtb_ctx *c, const Ar1Src &ar, unsigned long long seed, long long unit0, int nb, int64_t n0,
+                     T *out, int nser, unsigned stag);
+}  // extern "C++"
 // the exceedance counters of a counting run (cwtb_coherence*_surrogate_counts) and the observed
 // fields they compare against, per measure: the coherence in [0]; the partial and the multiple
 // coherence in [0] and [1] (either counter may be null)
@@ -3512,7 +3532,7 @@ static int phase_units(cwtb_ctx *c, const PhaseSrc &ph, int nser, unsigned long 
 }
 
 template <typename T>
-static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed, long long unit0,
+static int mc_run(cwtb_ctx *c, int nser, const double *noise, const TestNull *tn, unsigned long long seed, long long unit0,
                   int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                   double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                   int64_t *const hist[2], const CountDst *cd = nullptr) {
@@ -3520,6 +3540,19 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
   if (e) return e;
   if ((e = upload_window(c, boxcar_len))) return e;
   if ((e = upload_row_tables(c, c->job))) return e;
+  const bool phase = tn && tn->kind == CWTB_NULL_PHASE, ar1 = tn && tn->kind == CWTB_NULL_AR1;
+  // AR(1): the held rows in the engine type, where wct3_run keeps x1 and x2 (row 0 is always
+  // drawn); the drawn rows of a unit are consecutive, row r at slot[r]
+  Buf *const held_buf[3] = {&c->sig, &c->sig2, &c->sig3};
+  int ndraw = nser, slot[3] = {0, 1, 2};
+  if (ar1) {
+    ndraw = 0;
+    for (int r = 0; r < nser; ++r) {
+      slot[r] = ndraw;
+      if (!tn->held[r]) ++ndraw;
+      else if ((e = upload_series<T>(c, *held_buf[r], tn->series + (size_t)r * n0, n0))) return e;
+    }
+  }
   const size_t cnt = (size_t)n_scales * n0;
   if ((e = ensure(c, c->mask, cnt))) return e;
   RT(rt_h2d(c->mask.p, mask, cnt, c->stream));
@@ -3532,13 +3565,13 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
     if (hist[k]) dh[k] = (unsigned long long *)c->hist.p + (size_t)k * n_scales * nbins;
   // surrogates of at most `batch` units are resident at a time
   // (host surrogates stay double on the device; an fp32 run rounds one unit at a time into sig)
-  const size_t usz = (size_t)nser * n0;             // samples per unit
-  // (the rotated spectra of a batch of phase-randomised units take 16 B per sample; a batch drawn on
-  // the device is one launch of nser rows per unit)
-  const size_t resident = phase ? sizeof(double2) : sizeof(double);
+  const size_t usz = (size_t)ndraw * n0;            // samples drawn per unit
+  // (the rotated spectra of a batch of phase-randomised units take 16 B per sample, AR(1) units
+  // sizeof(T); a batch drawn on the device is one launch of ndraw rows per unit)
+  const size_t resident = phase ? sizeof(double2) : ar1 ? sizeof(T) : sizeof(double);
   const int batch = noise ? n_units
                           : (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_units, ((size_t)256 << 20) / (usz * resident),
-                                                                       (size_t)(MAX_ROWS / nser)}));
+                                                                       (size_t)(MAX_ROWS / ndraw)}));
   const size_t nsz = noise ? sizeof(double) : sizeof(T);
   if ((e = ensure(c, c->noise, (size_t)std::max(batch, 1) * usz * nsz))) return e;
   if (phase && (e = ensure(c, c->prot, (size_t)std::max(batch, 1) * usz * sizeof(double2)))) return e;
@@ -3550,7 +3583,12 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
   for (int i0 = 0; i0 < n_units; i0 += batch) {
     const int nb = std::min(batch, n_units - i0);
     if (phase) {
-      if ((e = phase_units<T>(c, *phase, nser, seed, unit0 + i0, nb, n0, (T *)c->noise.p))) return e;
+      if ((e = phase_units<T>(c, tn->ph, nser, seed, unit0 + i0, nb, n0, (T *)c->noise.p))) return e;
+    } else if (ar1) {
+      for (int r = 0; r < nser; ++r)
+        if (!tn->held[r] && (e = ar1_units<T>(c, tn->ar[r], seed, unit0 + i0, nb, n0, (T *)c->noise.p + (size_t)slot[r] * n0,
+                                              ndraw, (unsigned)r)))
+          return e;
     } else if (!noise) {
       NoiseArgs<T> na{(T *)c->noise.p, seed, unit0 + i0, (long long)n0, nb, nser};
       if ((e = launch<NoiseBody<T>>(c, (unsigned)(((n0 + 1) / 2 + NT - 1) / NT), (unsigned)(nser * nb), na))) return e;
@@ -3565,6 +3603,8 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
       } else {
         a = (const T *)c->noise.p + (size_t)i * usz;
       }
+      const T *u[3];
+      for (int r = 0; r < nser; ++r) u[r] = ar1 && tn->held[r] ? (const T *)held_buf[r]->p : a + (size_t)slot[r] * n0;
       const unsigned char *dmask = (const unsigned char *)c->mask.p;
       // The counters are read and written without atomics by the final kernel of every unit.  That
       // kernel runs on c->stream (run_job forks its transforms onto other streams but joins them
@@ -3574,9 +3614,9 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
       // unit's final launch writes them again.
       const CountDst k = cd ? *cd : CountDst{};
       const SelArgs *sel = k.sel.bits ? &k.sel : nullptr;
-      e = nser == 2 ? wct_core<T>(c, c->job, a, a + n0, boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0],
+      e = nser == 2 ? wct_core<T>(c, c->job, u[0], u[1], boxcar_len, nullptr, nullptr, dmask, maxscale, nbins, dh[0],
                                   k.obs[0], k.cnt[0], sel)
-                    : wct3_core<T>(c, c->job, a, a + n0, a + 2 * n0, boxcar_len, nullptr, nullptr, dmask, maxscale,
+                    : wct3_core<T>(c, c->job, u[0], u[1], u[2], boxcar_len, nullptr, nullptr, dmask, maxscale,
                                    nbins, dh[0], dh[1], nullptr, k.obs[0], k.obs[1], k.cnt[0], k.cnt[1], sel);
       if (e) return e;
       if (sel && (e = label_bits(c, n_scales, n0, k.q, k.qmax + i0 + i, nullptr, nullptr))) return e;
@@ -3595,7 +3635,7 @@ static int mc_run(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *ph
 }
 }  // extern "C++"
 
-static int mc_core(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *phase, unsigned long long seed,
+static int mc_core(cwtb_ctx *c, int nser, const double *noise, const TestNull *tn, unsigned long long seed,
                    long long unit0, int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
                    double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                    int64_t *const hist[2], const CountDst *cd = nullptr) {
@@ -3605,9 +3645,9 @@ static int mc_core(cwtb_ctx *c, int nser, const double *noise, const PhaseSrc *p
     return fail(c, CWTB_ERR_UNSUPPORTED, nser == 2 ? "wct_mc needs an analytic wavelet family"
                                                    : "wct3_mc needs an analytic wavelet family");
   return c->coh_precision == CWTB_F32
-             ? mc_run<float>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+             ? mc_run<float>(c, nser, noise, tn, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
                              boxcar_len, mask, maxscale, nbins, hist, cd)
-             : mc_run<double>(c, nser, noise, phase, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
+             : mc_run<double>(c, nser, noise, tn, seed, unit0, n_units, n0, dt, scales, n_scales, family, param,
                               boxcar_len, mask, maxscale, nbins, hist, cd);
 }
 
@@ -3704,19 +3744,42 @@ static int phase_spectra(cwtb_ctx *c, const char *name, const double *series, in
   return 0;
 }
 
+static int test_null(cwtb_ctx *c, const std::string &nm, const double *series, int nser, int null, const int *group,
+                     const double *g, const double *m, const double *sigma, const int *held, int64_t first_unit,
+                     int n_units, int64_t n0, TestNull &tn);
+
+static int wct_mc_null(cwtb_ctx *c, const std::string &nm, const double *series, int nser, int null,
+                       const int *group, const double *g, const double *m, const double *sigma, const int *held,
+                       uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                       int n_scales, int family, double param, int boxcar_len, const uint8_t *mask, int maxscale,
+                       int nbins, int64_t *hist_a, int64_t *hist_b) {
+  if (nser == 2 && hist_b) return fail(c, CWTB_ERR_ARG, nm + ": two series have one histogram");
+  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, nm + " needs an analytic wavelet family");
+  if (!mask || !(hist_a || hist_b) || (nser != 2 && nser != 3)) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
+  TestNull tn;
+  int e = test_null(c, nm, series, nser, null, group, g, m, sigma, held, first_unit, n_units, n0, tn);
+  if (e) return e;
+  int64_t *const h[2] = {hist_a, hist_b};
+  return mc_core(c, nser, nullptr, &tn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+                 boxcar_len, mask, maxscale, nbins, h);
+}
+
 int cwtb_wct_mc_phase(cwtb_ctx *c, const double *series, int nser, const int *group, uint64_t seed,
                       int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
                       int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
                       int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b) {
-  if (nser == 2 && hist_b) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: two series have one histogram");
-  if (family == CWTB_TABLE) return fail(c, CWTB_ERR_UNSUPPORTED, "wct_mc_phase needs an analytic wavelet family");
-  if (!mask || !(hist_a || hist_b) || (nser != 2 && nser != 3)) return fail(c, CWTB_ERR_ARG, "wct_mc_phase: bad argument");
-  PhaseSrc ph{};
-  int e = phase_spectra(c, "wct_mc_phase", series, nser, group, first_unit, n_units, n0, &ph);
-  if (e) return e;
-  int64_t *const h[2] = {hist_a, hist_b};
-  return mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                 boxcar_len, mask, maxscale, nbins, h);
+  return wct_mc_null(c, "wct_mc_phase", series, nser, CWTB_NULL_PHASE, group, nullptr, nullptr, nullptr, nullptr,
+                     seed, first_unit, n_units, n0, dt, scales, n_scales, family, param, boxcar_len, mask, maxscale,
+                     nbins, hist_a, hist_b);
+}
+
+int cwtb_wct_mc_null(cwtb_ctx *c, const double *series, int nser, int null, const int *group, const double *g,
+                     const double *m, const double *sigma, const int *held, uint64_t seed, int64_t first_unit,
+                     int n_units, int64_t n0, double dt, const double *scales, int n_scales, int family,
+                     double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist_a,
+                     int64_t *hist_b) {
+  return wct_mc_null(c, "wct_mc_null", series, nser, null, group, g, m, sigma, held, seed, first_unit, n_units, n0,
+                     dt, scales, n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist_a, hist_b);
 }
 
 int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const int *group, uint64_t seed,
@@ -3742,7 +3805,8 @@ int cwtb_mc_phase_surrogates(cwtb_ctx *c, const double *series, int nser, const 
 // ---- point-wise tests against surrogates: counting -------------------------------------------
 // The units' exceedance counts of the resident coherence (nser 2) or partial and multiple
 // coherence (nser 3) added to the slot's counters, with the histograms of cwtb_wct_mc_phase
-static int surrogate_counts(cwtb_ctx *c, int nser, const double *series, const int *group, uint64_t seed,
+static int surrogate_counts(cwtb_ctx *c, int nser, const double *series, int null, const int *group,
+                            const double *g, const double *m, const double *sigma, const int *held, uint64_t seed,
                             int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
                             int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
                             int maxscale, int nbins, int64_t *hist_a, int64_t *hist_b, int64_t serial, int reset) {
@@ -3758,9 +3822,11 @@ static int surrogate_counts(cwtb_ctx *c, int nser, const double *series, const i
   const long long base = reset || s.units < 0 ? 0 : s.units;
   if (n_units < 0 || n_units > 0xFFFFFFFFll - base)
     return fail(c, CWTB_ERR_ARG, nm + ": more units than a 32-bit counter holds");
-  PhaseSrc ph{};
-  int e = phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &ph);
+  TestNull tn;
+  int e = test_null(c, nm, series, nser, null, group, g, m, sigma, held, first_unit, n_units, n0, tn);
   if (e) return e;
+  if (base > 0 && null != s.null)
+    return fail(c, CWTB_ERR_STATE, nm + ": the counts hold the units of another null: reset them first");
   const size_t cnt = (size_t)s.S * s.n0, off = coh_angle_offset(cnt);
   if ((e = ensure(c, s.counts, (nser == 2 ? cnt : off + cnt) * sizeof(unsigned)))) return e;
   s.units = -1;   // nothing readable until this call completes
@@ -3769,10 +3835,11 @@ static int surrogate_counts(cwtb_ctx *c, int nser, const double *series, const i
   unsigned *k = (unsigned *)s.counts.p;           // one field; RP2's at 0 and RM2's at off
   const CountDst cd = nser == 2 ? CountDst{{obs, nullptr}, {k, nullptr}} : CountDst{{obs, obs + 2 * off}, {k, k + off}};
   int64_t *const h[2] = {hist_a, hist_b};
-  if ((e = mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+  if ((e = mc_core(c, nser, nullptr, &tn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
                    boxcar_len, mask, maxscale, nbins, h, &cd)))
     return e;
   s.units = base + n_units;
+  s.null = null;
   return 0;
 }
 
@@ -3780,8 +3847,9 @@ int cwtb_coherence_surrogate_counts(cwtb_ctx *c, const double *series, const int
                                     int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
                                     int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
                                     int maxscale, int nbins, int64_t *hist, int64_t serial, int reset) {
-  return surrogate_counts(c, 2, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                          boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, reset);
+  return surrogate_counts(c, 2, series, CWTB_NULL_PHASE, group, nullptr, nullptr, nullptr, nullptr, seed, first_unit,
+                          n_units, n0, dt, scales, n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist,
+                          nullptr, serial, reset);
 }
 
 int cwtb_coherence3_surrogate_counts(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
@@ -3789,8 +3857,30 @@ int cwtb_coherence3_surrogate_counts(cwtb_ctx *c, const double *series, const in
                                      int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
                                      int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
                                      int64_t serial, int reset) {
-  return surrogate_counts(c, 3, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                          boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial, reset);
+  return surrogate_counts(c, 3, series, CWTB_NULL_PHASE, group, nullptr, nullptr, nullptr, nullptr, seed, first_unit,
+                          n_units, n0, dt, scales, n_scales, family, param, boxcar_len, mask, maxscale, nbins,
+                          hist_partial, hist_multiple, serial, reset);
+}
+
+int cwtb_coherence_surrogate_counts_null(cwtb_ctx *c, const double *series, int null, const int *group,
+                                         const double *g, const double *m, const double *sigma, const int *held,
+                                         uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                         const double *scales, int n_scales, int family, double param,
+                                         int boxcar_len, const uint8_t *mask, int maxscale, int nbins, int64_t *hist,
+                                         int64_t serial, int reset) {
+  return surrogate_counts(c, 2, series, null, group, g, m, sigma, held, seed, first_unit, n_units, n0, dt, scales,
+                          n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, reset);
+}
+
+int cwtb_coherence3_surrogate_counts_null(cwtb_ctx *c, const double *series, int null, const int *group,
+                                          const double *g, const double *m, const double *sigma, const int *held,
+                                          uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double dt,
+                                          const double *scales, int n_scales, int family, double param,
+                                          int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
+                                          int64_t *hist_partial, int64_t *hist_multiple, int64_t serial, int reset) {
+  return surrogate_counts(c, 3, series, null, group, g, m, sigma, held, seed, first_unit, n_units, n0, dt, scales,
+                          n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple,
+                          serial, reset);
 }
 
 // ---- cluster tests against surrogates ----------------------------------------------------------
@@ -3830,7 +3920,8 @@ static int cluster_shape(cwtb_ctx *c, const std::string &nm, long long S, long l
   return 0;
 }
 
-static int cluster_test(cwtb_ctx *c, int nser, const double *series, const int *group, uint64_t seed,
+static int cluster_test(cwtb_ctx *c, int nser, const double *series, int null, const int *group, const double *g,
+                        const double *m, const double *sigma, const int *held, uint64_t seed,
                         int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales, int n_scales,
                         int family, double param, int boxcar_len, const uint8_t *mask, int maxscale, int nbins,
                         int64_t *hist_a, int64_t *hist_b, int64_t serial, const double *thr, const int64_t *lo,
@@ -3851,8 +3942,8 @@ static int cluster_test(cwtb_ctx *c, int nser, const double *series, const int *
   if (e) return e;
   FieldRef f;
   if ((e = nser == 2 ? field_ref(c, FIELD_COH, f) : coh3_ref(c, measure, false, f))) return e;
-  PhaseSrc ph{};
-  if ((e = phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &ph))) return e;
+  TestNull tn;
+  if ((e = test_null(c, nm, series, nser, null, group, g, m, sigma, held, first_unit, n_units, n0, tn))) return e;
   SelArgs sel;
   const unsigned long long *dq;
   if ((e = cluster_rows(c, nm, n_scales, n0, thr, lo, hi, q, sel, dq))) return e;
@@ -3874,7 +3965,7 @@ static int cluster_test(cwtb_ctx *c, int nser, const double *series, const int *
   cd.q = dq;
   cd.qmax = dqmax;
   int64_t *const h[2] = {hist_a, hist_b};
-  if ((e = mc_core(c, nser, nullptr, &ph, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
+  if ((e = mc_core(c, nser, nullptr, &tn, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
                    boxcar_len, mask, maxscale, nbins, h, &cd)))
     return e;
   if (n_units > 0) RT(rt_d2h(qmax_out, dqmax, (size_t)n_units * sizeof(unsigned long long), c->stream));
@@ -3889,8 +3980,9 @@ int cwtb_coherence_cluster_test(cwtb_ctx *c, const double *series, const int *gr
                                 int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
                                 int maxscale, int nbins, int64_t *hist, int64_t serial, const double *thr,
                                 const int64_t *lo, const int64_t *hi, const uint64_t *q, uint64_t *qmax_out) {
-  return cluster_test(c, 2, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                      boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, thr, lo, hi, q, 0, qmax_out);
+  return cluster_test(c, 2, series, CWTB_NULL_PHASE, group, nullptr, nullptr, nullptr, nullptr, seed, first_unit,
+                      n_units, n0, dt, scales, n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist,
+                      nullptr, serial, thr, lo, hi, q, 0, qmax_out);
 }
 
 int cwtb_coherence3_cluster_test(cwtb_ctx *c, const double *series, const int *group, uint64_t seed,
@@ -3899,9 +3991,32 @@ int cwtb_coherence3_cluster_test(cwtb_ctx *c, const double *series, const int *g
                                  int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
                                  int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
                                  const uint64_t *q, int measure, uint64_t *qmax_out) {
-  return cluster_test(c, 3, series, group, seed, first_unit, n_units, n0, dt, scales, n_scales, family, param,
-                      boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial, thr, lo, hi, q,
-                      measure, qmax_out);
+  return cluster_test(c, 3, series, CWTB_NULL_PHASE, group, nullptr, nullptr, nullptr, nullptr, seed, first_unit,
+                      n_units, n0, dt, scales, n_scales, family, param, boxcar_len, mask, maxscale, nbins,
+                      hist_partial, hist_multiple, serial, thr, lo, hi, q, measure, qmax_out);
+}
+
+int cwtb_coherence_cluster_test_null(cwtb_ctx *c, const double *series, int null, const int *group, const double *g,
+                                     const double *m, const double *sigma, const int *held, uint64_t seed,
+                                     int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                     int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                     int maxscale, int nbins, int64_t *hist, int64_t serial, const double *thr,
+                                     const int64_t *lo, const int64_t *hi, const uint64_t *q, uint64_t *qmax_out) {
+  return cluster_test(c, 2, series, null, group, g, m, sigma, held, seed, first_unit, n_units, n0, dt, scales,
+                      n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist, nullptr, serial, thr, lo, hi,
+                      q, 0, qmax_out);
+}
+
+int cwtb_coherence3_cluster_test_null(cwtb_ctx *c, const double *series, int null, const int *group, const double *g,
+                                      const double *m, const double *sigma, const int *held, uint64_t seed,
+                                      int64_t first_unit, int n_units, int64_t n0, double dt, const double *scales,
+                                      int n_scales, int family, double param, int boxcar_len, const uint8_t *mask,
+                                      int maxscale, int nbins, int64_t *hist_partial, int64_t *hist_multiple,
+                                      int64_t serial, const double *thr, const int64_t *lo, const int64_t *hi,
+                                      const uint64_t *q, int measure, uint64_t *qmax_out) {
+  return cluster_test(c, 3, series, null, group, g, m, sigma, held, seed, first_unit, n_units, n0, dt, scales,
+                      n_scales, family, param, boxcar_len, mask, maxscale, nbins, hist_partial, hist_multiple, serial,
+                      thr, lo, hi, q, measure, qmax_out);
 }
 
 // the first min(cap, count) rows of a table
@@ -4002,8 +4117,6 @@ int cwtb_cluster_label_bits(cwtb_ctx *c, const uint32_t *bits, int n_scales, int
 }
 
 // ---- AR(1) red-noise surrogates (Ar1BlockBody, Ar1CarryBody, Ar1WriteBody) ------------------------
-struct Ar1Src { double g, m, sigma; };
-
 static int ar1_check(cwtb_ctx *c, const std::string &nm, const Ar1Src &ar) {
   if (!std::isfinite(ar.g) || !(std::fabs(ar.g) < 1.0) || !std::isfinite(ar.m) || !std::isfinite(ar.sigma))
     return fail(c, CWTB_ERR_ARG, nm + ": the AR(1) parameters must be finite, with |g| < 1");
@@ -4053,30 +4166,41 @@ int cwtb_mc_ar1_surrogates(cwtb_ctx *c, double g, double m, double sigma, uint64
   return 0;
 }
 
-// ---- tests of the resident power and cross spectrum against surrogates -----------------------
-// The null of a test of a complex field of nser series (the power: 1, the cross spectrum: 2): AR(1)
-// units, series s with its own parameters ar[s] under the series tag s, or phase-randomised units of
-// the series (their spectra in c->pspec, series s in phase group s: independent phases)
-struct TestNull { int kind, nser; Ar1Src ar[2]; PhaseSrc ph; };
-
-static int test_null(cwtb_ctx *c, const std::string &nm, const double *series, int nser, int null, const double *g,
-                     const double *m, const double *sigma, int64_t first_unit, int n_units, int64_t n0, TestNull &tn) {
-  tn = TestNull{null, nser, {}, PhaseSrc{}};
-  if (null == CWTB_NULL_PHASE) {
-    const int group[2] = {0, 1};
-    return phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &tn.ph);
-  }
+// ---- the nulls of the tests against surrogates ---------------------------------------------------
+// The null of a test of nser series (TestNull): phase-randomised units in the phase groups `group`,
+// or AR(1) units with the parameters g, m, sigma [nser] and, where held (may be null: none) is 1, the
+// data's row of `series` in every unit.  Only the coherence tests hold rows: x1 and x2 of the
+// partial and multiple coherence (y, and the series of a pair, are always drawn).
+static int test_null(cwtb_ctx *c, const std::string &nm, const double *series, int nser, int null, const int *group,
+                     const double *g, const double *m, const double *sigma, const int *held, int64_t first_unit,
+                     int n_units, int64_t n0, TestNull &tn) {
+  tn = TestNull{null, nser, {}, PhaseSrc{}, {0, 0, 0}, nullptr};
+  if (null == CWTB_NULL_PHASE) return phase_spectra(c, nm.c_str(), series, nser, group, first_unit, n_units, n0, &tn.ph);
   if (null != CWTB_NULL_AR1) return fail(c, CWTB_ERR_ARG, nm + ": unknown null");
-  if (!g || !m || !sigma || n_units < 0 || first_unit < 0 || first_unit > (1ll << 61) - n_units)
+  if (!g || !m || !sigma || nser < 1 || nser > 3 || n_units < 0 || first_unit < 0 ||
+      first_unit > (1ll << 61) - n_units)
     return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
   for (int r = 0; r < nser; ++r) {
+    tn.held[r] = held ? held[r] : 0;
+    if (tn.held[r] != 0 && (tn.held[r] != 1 || r == 0 || nser != 3))
+      return fail(c, CWTB_ERR_ARG, nm + ": only x1 and x2 of three series can be held at the data");
+    if (tn.held[r]) {
+      if (!series) return fail(c, CWTB_ERR_ARG, nm + ": held series without data");
+      continue;
+    }
     tn.ar[r] = Ar1Src{g[r], m[r], sigma[r]};
     int e = ar1_check(c, nm, tn.ar[r]);
     if (e) return e;
   }
+  tn.series = series;
   RT(rt_set_device(c->device));
   return 0;
 }
+
+// ---- tests of the resident power and cross spectrum against surrogates -----------------------
+// Their nulls draw every series (the power: 1, the cross spectrum: 2): AR(1) units, or phase-
+// randomised units of the series in phase group s: independent phases
+static const int PHASE_GROUPS[2] = {0, 1};
 
 // the checks of a test against the resident product of slot s
 static int test_slot(cwtb_ctx *c, const ResidentSlot &s, const std::string &nm, int64_t serial, int n_scales,
@@ -4161,7 +4285,7 @@ static int test_counts(cwtb_ctx *c, const char *name, ResidentSlot &s, int nser,
   if (n_units < 0 || n_units > 0xFFFFFFFFll - base)
     return fail(c, CWTB_ERR_ARG, nm + ": more units than a 32-bit counter holds");
   TestNull tn;
-  if ((e = test_null(c, nm, series, nser, null, g, m, sigma, first_unit, n_units, n0, tn))) return e;
+  if ((e = test_null(c, nm, series, nser, null, PHASE_GROUPS, g, m, sigma, nullptr, first_unit, n_units, n0, tn))) return e;
   if ((e = ensure(c, s.counts, (size_t)s.S * s.n0 * sizeof(unsigned)))) return e;
   s.units = -1;   // nothing readable until this call completes
   if (base == 0) RT(rt_memset(s.counts.p, 0, s.counts.bytes, c->stream));
@@ -4190,7 +4314,7 @@ static int test_clusters(cwtb_ctx *c, const char *name, ResidentSlot &s, int nse
   if (!thr || n_units < 0 || (n_units > 0 && !qmax_out)) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
   if ((e = cluster_shape(c, nm, n_scales, n0))) return e;
   TestNull tn;
-  if ((e = test_null(c, nm, series, nser, null, g, m, sigma, first_unit, n_units, n0, tn))) return e;
+  if ((e = test_null(c, nm, series, nser, null, PHASE_GROUPS, g, m, sigma, nullptr, first_unit, n_units, n0, tn))) return e;
   SelArgs sel;
   const unsigned long long *dq;
   if ((e = cluster_rows(c, nm, n_scales, n0, thr, lo, hi, q, sel, dq))) return e;
@@ -4309,26 +4433,37 @@ int cwtb_power_cluster_reconstruct(cwtb_ctx *c, const double *weights, const int
 }
 
 // ---- tests of the resident cross spectrum against surrogate pairs ---------------------------------
-int cwtb_mc_ar1_pair_surrogates(cwtb_ctx *c, const double *g, const double *m, const double *sigma, uint64_t seed,
-                                int64_t first_unit, int n_units, int64_t n0, double *out) {
+// the AR(1) units of nser series, series s under the tag s, out [n_units][nser][n0]
+static int mc_ar1_units(cwtb_ctx *c, const std::string &nm, int nser, const double *g, const double *m,
+                        const double *sigma, uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out) {
   if (!c) return CWTB_ERR_ARG;
-  const std::string nm = "mc_ar1_pair_surrogates";
   if (!out || n_units < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, nm + ": bad argument");
   TestNull tn;
-  int e = test_null(c, nm, nullptr, 2, CWTB_NULL_AR1, g, m, sigma, first_unit, n_units, n0, tn);
+  int e = test_null(c, nm, nullptr, nser, CWTB_NULL_AR1, nullptr, g, m, sigma, nullptr, first_unit, n_units, n0, tn);
   if (e) return e;
-  const size_t cnt = (size_t)n_units * 2 * n0;
+  const size_t cnt = (size_t)n_units * nser * n0;
   if ((e = ensure(c, c->noise, cnt * sizeof(double)))) return e;
   for (int i0 = 0; i0 < n_units; i0 += (int)MAX_ROWS) {
     const int nb = std::min((int)MAX_ROWS, n_units - i0);
-    double *x = (double *)c->noise.p + (size_t)i0 * 2 * n0;
-    for (int r = 0; r < 2; ++r)
-      if ((e = ar1_units<double>(c, tn.ar[r], seed, first_unit + i0, nb, n0, x + (size_t)r * n0, 2, (unsigned)r)))
+    double *x = (double *)c->noise.p + (size_t)i0 * nser * n0;
+    for (int r = 0; r < nser; ++r)
+      if ((e = ar1_units<double>(c, tn.ar[r], seed, first_unit + i0, nb, n0, x + (size_t)r * n0, nser, (unsigned)r)))
         return e;
   }
   RT(rt_d2h(out, c->noise.p, cnt * sizeof(double), c->stream));
   RT(rt_sync(c->stream));
   return 0;
+}
+
+int cwtb_mc_ar1_pair_surrogates(cwtb_ctx *c, const double *g, const double *m, const double *sigma, uint64_t seed,
+                                int64_t first_unit, int n_units, int64_t n0, double *out) {
+  return mc_ar1_units(c, "mc_ar1_pair_surrogates", 2, g, m, sigma, seed, first_unit, n_units, n0, out);
+}
+
+int cwtb_mc_ar1_series_surrogates(cwtb_ctx *c, int nser, const double *g, const double *m, const double *sigma,
+                                  uint64_t seed, int64_t first_unit, int n_units, int64_t n0, double *out) {
+  if (c && (nser < 1 || nser > 3)) return fail(c, CWTB_ERR_ARG, "mc_ar1_series_surrogates: nser must be 1, 2 or 3");
+  return mc_ar1_units(c, "mc_ar1_series_surrogates", nser, g, m, sigma, seed, first_unit, n_units, n0, out);
 }
 
 int cwtb_cross_surrogate_counts(cwtb_ctx *c, const double *series, int null, const double *g, const double *m,

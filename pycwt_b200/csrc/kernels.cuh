@@ -1777,12 +1777,13 @@ struct PhaseRotBody {
 // Unit u of length n is x = m + sigma z with z[0] = e[0], z[i] = g z[i-1] + sqrt(1 - g^2) e[i] (the
 // background of Torrence & Compo 1998, section 4), |g| < 1.  e[2j], e[2j+1] are the two normals of
 // one Philox4x32-10 block (philox_normals, NoiseBody's conversion), a pure function of (seed, s, u,
-// j): counter words (j, 2^31 | s, u lo, 2^31 | (u hi << 2) | 3), s the series tag (0 or 1).  Tag 0
-// is the power test's stream; the cross-wavelet test draws its second series under tag 1, so the two
-// series of one unit are independent even with equal parameters, and its first series is the power
-// test's unit.  PhaseRotBody's second word is a phase group below 2^31 and NoiseBody's a sample
-// index below 2^26, so bit 31 of the second word keeps both tags apart from both for 0 <= u < 2^61
-// (j < 2^31), and the tag's low bit keeps the two tags apart from each other.
+// j): counter words (j, 2^31 | s, u lo, 2^31 | (u hi << 2) | 3), s the series tag (0, 1 or 2).  Tag 0
+// is the power test's stream; the cross-wavelet and coherence tests draw their second series under
+// tag 1 and the third series of the partial and multiple coherence under tag 2, so the series of one
+// unit are independent even with equal parameters, and the first series is the power test's unit.
+// PhaseRotBody's second word is a phase group below 2^31 and NoiseBody's a sample index below 2^26,
+// so bit 31 of the second word keeps every tag apart from both for 0 <= u < 2^61 (j < 2^31), and the
+// tag's two low bits keep the tags apart from each other.
 // The recurrence is a linear scan over the whole series: z_end = g^L z_start + b over a stretch of L
 // samples, b its end state from a zero start.  A thread owns AR1_CH consecutive samples (whole
 // normal pairs), a CTA NT of those stretches.  Ar1BlockBody forms every CTA's (g^L, b), Ar1CarryBody

@@ -26,8 +26,9 @@ import numpy as np
 from . import _engine
 from . import helpers as _helpers
 from .helpers import ar1, fft, fft_kwargs
-from .wavelet import (_check_parameter_wavelet, _coherence_precision, _coi, _mc_levels, _nan_rows,
-                      _precision, _resolve_scales, _standardise, _surrogate_histogram, _surrogate_problem, _surrogate_seed,
+from .wavelet import (_ar1_params, _check_parameter_wavelet, _coherence_null, _coherence_precision, _coi,
+                      _mc_levels, _nan_rows, _null_kind, _precision, _resolve_scales, _standardise,
+                      _surrogate_histogram, _surrogate_problem, _surrogate_seed,
                       _sync_padding, _wct_on_device, _wct_problem, _wct_significance,
                       _xwt_on_device, _xwt_problem, _xwt_signif, wct3_significance,
                       wct3_surrogate_significance, wct_surrogate_significance)
@@ -453,8 +454,9 @@ class _SurrogateTest(object):
     (`_count_units`, `_cluster_units`)."""
 
     _UNTESTED = ("no surrogate test has counted for this product: call surrogate_test first")
-    surrogate_seed = None     # seed and M of the last surrogate_test
+    surrogate_seed = None     # seed, M and null of the last surrogate_test
     surrogate_units = None
+    surrogate_null = None
 
     def _seed_of_run(self, mc_count, seed):
         """The checks of a surrogate run of units 0 .. mc_count - 1, and its seed."""
@@ -490,13 +492,13 @@ class _SurrogateTest(object):
             return np.empty((nr, nc), dtype=np.int32)
         return self.engine.cluster_labels(self._CLUSTERS, r0, nr, rs, c0, nc, cs)
 
-    def _count(self, mc_count, seed, *args):
-        """What `_count_units` returns for a counting run of units 0 .. mc_count - 1 (the caller
-        holds the lock)."""
+    def _count(self, mc_count, seed, null, *args):
+        """What `_count_units` returns for a counting run of units 0 .. mc_count - 1 of `null` (the
+        caller holds the lock)."""
         seed = self._seed_of_run(mc_count, seed)
-        self.surrogate_seed = self.surrogate_units = None
-        out = self._count_units(seed, int(mc_count), *args)
-        self.surrogate_seed, self.surrogate_units = seed, int(mc_count)
+        self.surrogate_seed = self.surrogate_units = self.surrogate_null = None
+        out = self._count_units(seed, int(mc_count), null, *args)
+        self.surrogate_seed, self.surrogate_units, self.surrogate_null = seed, int(mc_count), null
         return out
 
     def _units(self):
@@ -536,28 +538,34 @@ class _SurrogateTest(object):
 
 
 class _CoherenceTest(_SurrogateTest):
-    """The units of the coherence products' tests: the phase-randomised surrogates of their series
-    through the whole coherence pipeline, with the Monte-Carlo histograms of `_surrogate_problem`."""
+    """The units of the coherence products' tests: the surrogates of `_coherence_null` ('phase' or
+    'ar1', conditional or not for three series) through the whole coherence pipeline, with the
+    Monte-Carlo histograms of `_surrogate_problem`."""
 
-    def _count_units(self, seed, M, groups):
-        """(prob, hist) of a counting run."""
+    def _problem(self, null, conditional):
+        """(p, prob, the engine's null) of a run."""
+        _null_kind(null)
         p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
                                      self.normalize, self.precision)
-        hist = _surrogate_histogram(p, prob, groups, seed, 0, M, engine=self.engine,
+        return p, prob, _coherence_null(null, p, self.normalize, conditional)
+
+    def _count_units(self, seed, M, null, conditional=True):
+        """(prob, hist) of a counting run."""
+        p, prob, cnull = self._problem(null, conditional)
+        hist = _surrogate_histogram(p, prob, cnull, seed, 0, M, engine=self.engine,
                                     serial=self._serial)
         return prob, hist
 
-    def _cluster_units(self, seed, M, thr, lo, hi, q, groups, measure):
+    def _cluster_units(self, seed, M, thr, lo, hi, q, null, conditional, measure):
         """The units' largest cluster sums, uint64 [M]."""
-        p, prob = _surrogate_problem(self._y, self.dt, self.dj, self.s0, self.J, self.wavelet,
-                                     self.normalize, self.precision)
+        p, prob, cnull = self._problem(null, conditional)
         nser = len(p.yns)
         hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
         eng = self.engine
 
         def call(*a, boxcar_len, precision):
             dt, _, sj, family, param = a[nser:]
-            return eng.cluster_test(np.stack(a[:nser]), groups, seed, 0, M, dt, sj, family,
+            return eng.cluster_test(np.stack(a[:nser]), cnull, seed, 0, M, dt, sj, family,
                                     param, boxcar_len, prob['mask'], prob['maxscale'], prob['nbins'],
                                     *hist, serial=self._serial, thr=thr, lo=lo, hi=hi, q=q,
                                     measure=measure, precision=precision)
@@ -691,23 +699,29 @@ class ResidentCoherence(_CoherenceTest, _ResidentSlot):
         return out[0] / float(sel.sum()), np.arctan2(out[2], out[1])
 
     @_live
-    def surrogate_significance(self, significance_level=0.95, mc_count=300, seed=None):
-        """`wct_surrogate_significance` on this handle's series and arguments.  The coherence stays
-        resident."""
+    def surrogate_significance(self, significance_level=0.95, mc_count=300, seed=None, null='phase'):
+        """`wct_surrogate_significance` on this handle's series and arguments, against `null`
+        ('phase' or 'ar1').  The coherence stays resident."""
         return wct_surrogate_significance(*self._y, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
                                           significance_level=significance_level,
                                           wavelet=self.wavelet, normalize=self.normalize,
-                                          mc_count=mc_count, seed=seed, precision=self.precision)
+                                          mc_count=mc_count, seed=seed, precision=self.precision,
+                                          null=null)
 
     @_live
-    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95):
-        """Run the surrogate pairs 0 .. mc_count - 1 once: count per point the pairs whose coherence
-        reaches this one (kept on the device, replacing the counts of an earlier test) and return
-        the per-scale levels, bit-identical to `surrogate_significance` with the same `seed` and
-        `mc_count`.  `seed=None` draws the seed from numpy's global RNG; the seed and M are kept as
-        `surrogate_seed` and `surrogate_units`.  ValueError for mc_count outside [1, 2^31 - 1] or
-        when the FFT padding mode differs from the one this coherence was computed with."""
-        prob, hist = self._count(mc_count, seed, (0, 1))
+    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95, null='phase'):
+        """Run the surrogate pairs 0 .. mc_count - 1 of `null` once ('phase': phase-randomised
+        surrogates of the two series, 'ar1': two independent red-noise series with the data's lag-1
+        autocorrelations; see `wct_surrogate_significance`): count per point the pairs whose
+        coherence reaches this one (kept on the device, replacing the counts of an earlier test) and
+        return the per-scale levels, bit-identical to `surrogate_significance` with the same `seed`,
+        `mc_count` and `null`.  `seed=None` draws the seed from numpy's global RNG; the seed, M and
+        null are kept as `surrogate_seed`, `surrogate_units` and `surrogate_null`.  ValueError for
+        mc_count outside [1, 2^31 - 1], an unknown null, an AR(1) null whose g is not finite or has
+        |g| >= 1, or when the FFT padding mode differs from the one this coherence was computed
+        with."""
+        _null_kind(null)
+        prob, hist = self._count(mc_count, seed, null)
         return _mc_levels(prob, hist[0], significance_level)
 
     @_live
@@ -737,9 +751,9 @@ class ResidentCoherence(_CoherenceTest, _ResidentSlot):
         return self._fdr_threshold(None, q, method, inside_coi)
 
     @_live
-    def cluster_test(self, sig, mc_count=300, seed=None, inside_coi=True):
+    def cluster_test(self, sig, mc_count=300, seed=None, inside_coi=True, null='phase'):
         """Cluster (areawise) test of this coherence against the surrogate pairs 0 .. mc_count - 1 of
-        `surrogate_significance(mc_count=mc_count, seed=seed)` (Maraun et al. 2007; Schulte et
+        `surrogate_significance(mc_count=mc_count, seed=seed, null=null)` (Maraun et al. 2007; Schulte et
         al. 2015).  A point is selected where WCT is finite and > sig[j] (a NaN selects nothing),
         inside the cone of influence if `inside_coi`; clusters are the 8-connected patches of the
         selection, in this map and in every surrogate pair's, labelled on the device.  A cluster's
@@ -756,7 +770,8 @@ class ResidentCoherence(_CoherenceTest, _ResidentSlot):
         the device (`cluster_labels`, 4 bytes per scale-point) until the next `cluster_test`,
         `release()` or `wct_resident`.  ValueError for a `sig` without one entry per scale and for
         the checks of `surrogate_test`; the counts of an earlier `surrogate_test` are kept."""
-        return self._cluster(sig, mc_count, seed, inside_coi, (0, 1), None)
+        _null_kind(null)
+        return self._cluster(sig, mc_count, seed, inside_coi, null, True, None)
 
     @_live
     def cluster_labels(self, rows=slice(None), cols=slice(None)):
@@ -837,14 +852,8 @@ class ResidentCrossWavelet(_SurrogateTest, _ResidentSlot):
 
     def _null(self, null):
         """(engine null, g [2], m [2], sigma [2]) of a null's name."""
-        if null not in _NULLS:
-            raise ValueError("null must be 'ar1' or 'phase', got %r" % (null,))
-        g = [ar1(y)[0] if null == 'ar1' else 0.0 for y in self._y]
-        if self.normalize:
-            m, sigma = [0.0, 0.0], [1.0, 1.0]
-        else:
-            m, sigma = [float(y.mean()) for y in self._y], [float(y.std()) for y in self._y]
-        return _NULLS[null], g, m, sigma
+        kind = _null_kind(null)
+        return (kind,) + _ar1_params(self._y, self.normalize, [null == 'ar1'] * 2)
 
     def _on_device(self, call, null, seed, M, *args):
         kind, g, m, sigma = self._null(null)
@@ -1153,23 +1162,27 @@ class ResidentCoherence3(_CoherenceTest, _ResidentSlot):
 
     @_live
     def surrogate_significance(self, significance_level=0.95, mc_count=300, seed=None,
-                               conditional=True):
+                               conditional=True, null='phase'):
         """(sig_partial, sig_multiple) of `wct3_surrogate_significance` on this handle's series and
-        arguments.  The fields stay resident."""
+        arguments, against `null` ('phase' or 'ar1').  The fields stay resident."""
         return wct3_surrogate_significance(*self._y, dt=self.dt, dj=self.dj, s0=self.s0, J=self.J,
                                            significance_level=significance_level,
                                            wavelet=self.wavelet, normalize=self.normalize,
                                            mc_count=mc_count, seed=seed, precision=self.precision,
-                                           conditional=conditional)
+                                           conditional=conditional, null=null)
 
     @_live
-    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95, conditional=True):
-        """Run the surrogate triples 0 .. mc_count - 1 once: count per point the triples whose RP2
-        and RM2 reach this handle's (one count field per measure, kept on the device, replacing the
-        counts of an earlier test) and return (sig_partial, sig_multiple), bit-identical to
-        `surrogate_significance` with the same `seed`, `mc_count` and `conditional`.  Seed, errors
-        and records as `ResidentCoherence.surrogate_test`."""
-        prob, hist = self._count(mc_count, seed, (0, 1, 1) if conditional else (0, 1, 2))
+    def surrogate_test(self, mc_count=300, seed=None, significance_level=0.95, conditional=True,
+                       null='phase'):
+        """Run the surrogate triples 0 .. mc_count - 1 of `null` once ('phase' or 'ar1'; with
+        `conditional=True` and 'ar1', y is red noise and x1, x2 are held at the data in every triple,
+        see `wct3_surrogate_significance`): count per point the triples whose RP2 and RM2 reach this
+        handle's (one count field per measure, kept on the device, replacing the counts of an
+        earlier test) and return (sig_partial, sig_multiple), bit-identical to
+        `surrogate_significance` with the same `seed`, `mc_count`, `conditional` and `null`.  Seed,
+        errors and records as `ResidentCoherence.surrogate_test`."""
+        _null_kind(null)
+        prob, hist = self._count(mc_count, seed, null, conditional)
         return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
 
     @_live
@@ -1191,12 +1204,13 @@ class ResidentCoherence3(_CoherenceTest, _ResidentSlot):
 
     @_live
     def cluster_test(self, sig, mc_count=300, seed=None, inside_coi=True, measure='partial',
-                     conditional=True):
+                     conditional=True, null='phase'):
         """`ResidentCoherence.cluster_test` of the measure against the surrogate triples
         0 .. mc_count - 1 of `surrogate_significance(mc_count=mc_count, seed=seed,
-        conditional=conditional)`; `sig` in the units of the measure."""
+        conditional=conditional, null=null)`; `sig` in the units of the measure."""
         m = self._measure(measure)
-        return self._cluster(sig, mc_count, seed, inside_coi, (0, 1, 1) if conditional else (0, 1, 2), m)
+        _null_kind(null)
+        return self._cluster(sig, mc_count, seed, inside_coi, null, conditional, m)
 
     @_live
     def cluster_labels(self, rows=slice(None), cols=slice(None)):
@@ -1236,9 +1250,6 @@ def wct3_resident(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, wavelet='morlet', normali
 # compared with the resident one on every point (`surrogate_test`) or labelled into clusters
 # (`cluster_test`), with the definitions of `ResidentCoherence`.
 
-_NULLS = {'ar1': _engine.NULL_AR1, 'phase': _engine.NULL_PHASE}
-
-
 class ResidentPower(_SurrogateTest, _ResidentSlot):
     """W[S, n0] of one `power_resident` call, resident on the device, and the tests of its power
     P = |W|^2.
@@ -1274,11 +1285,9 @@ class ResidentPower(_SurrogateTest, _ResidentSlot):
 
     def _null(self, null):
         """(engine null, g, m, sigma) of a null's name."""
-        if null not in _NULLS:
-            raise ValueError("null must be 'ar1' or 'phase', got %r" % (null,))
-        g = ar1(self._y)[0] if null == 'ar1' else 0.0
-        m, sigma = (0.0, 1.0) if self.normalize else (float(self._y.mean()), float(self._y.std()))
-        return _NULLS[null], g, m, sigma
+        kind = _null_kind(null)
+        g, m, sigma = _ar1_params([self._y], self.normalize, [null == 'ar1'])
+        return kind, g[0], m[0], sigma[0]
 
     def _on_device(self, call, null, seed, M, *args):
         kind, g, m, sigma = self._null(null)

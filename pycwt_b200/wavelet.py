@@ -728,19 +728,62 @@ def _surrogate_problem(series, dt, dj, s0, J, wavelet, normalize, precision):
     return p, _mc_problem(dt, dj, p.s0, p.J, p.wavelet, N=p.n0)
 
 
-def _surrogate_histogram(p, prob, groups, seed, first, count, engine=None, serial=None):
+_NULLS = {'ar1': _engine.NULL_AR1, 'phase': _engine.NULL_PHASE}
+
+
+def _null_kind(null):
+    """The engine's null of a null's name."""
+    if null not in _NULLS:
+        raise ValueError("null must be 'ar1' or 'phase', got %r" % (null,))
+    return _NULLS[null]
+
+
+def _ar1_params(ys, normalize, fit):
+    """Lists g, m, sigma of the AR(1) null of the raw series `ys`: g = ar1(y)[0] where `fit` (a flag
+    per series) is set, else 0; m = 0 and sigma = 1 with `normalize` (the units are standardised as
+    the data are), else y's mean and standard deviation (ddof 0)."""
+    g = [ar1(y)[0] if f else 0.0 for y, f in zip(ys, fit)]
+    if normalize:
+        return g, [0.0] * len(ys), [1.0] * len(ys)
+    return g, [float(y.mean()) for y in ys], [float(y.std()) for y in ys]
+
+
+def _coherence_null(null, p, normalize, conditional=True):
+    """The engine's null (`_engine.CoherenceNull`) of a coherence test of the series of `p` (a
+    `_wct_problem`): 'phase' puts the series in the phase groups (0, 1), or (0, 1, 1) for a
+    conditional triple and (0, 1, 2) otherwise; 'ar1' draws every series, except x1 and x2 of a
+    conditional triple, which are held at the data as transformed (`p.yns`).  With normalize=False
+    the AR(1) m and sigma are the mean and standard deviation of `p.yns`.  ValueError for an
+    unknown name and for a drawn series whose g is not finite or has |g| >= 1."""
+    kind = _null_kind(null)
+    nser = len(p.ys)
+    if kind == _engine.NULL_PHASE:
+        return _engine.CoherenceNull(kind, (0, 1) if nser == 2 else (0, 1, 1) if conditional else (0, 1, 2))
+    held = (0, 1, 1) if nser == 3 and conditional else (0,) * nser
+    # normalize=False: the series as transformed, in the binade `_unit_binade` gives them, so that the
+    # drawn series share the binade of the held ones (g, and the coherence, are the same either way)
+    g, m, sigma = _ar1_params(p.ys if normalize else p.yns, normalize, [not h for h in held])
+    for s, (gs, h) in enumerate(zip(g, held)):
+        if not h and not (np.isfinite(gs) and abs(gs) < 1):
+            raise ValueError("the AR(1) null needs a finite lag-1 autocorrelation with |g| < 1; series %d "
+                             "has g = %r" % (s, gs))
+    return _engine.CoherenceNull(kind, None, g, m, sigma, held)
+
+
+def _surrogate_histogram(p, prob, null, seed, first, count, engine=None, serial=None):
     """Histograms int64 [nser - 1, S, nbins] of the coherence (two series) or of the partial and
-    multiple coherence (three) of the surrogate units first .. first + count - 1 of the
-    standardised data `p.yns`, drawn and accumulated on the device in one transaction.  With the
-    `serial` of the resident product of the same data, the same run also counts, per point, the
-    units that reach the product's value (`Engine.surrogate_counts`, counters reset first)."""
+    multiple coherence (three) of the surrogate units first .. first + count - 1 of `null` (a
+    `_coherence_null` of `p`) for the standardised data `p.yns`, drawn and accumulated on the device
+    in one transaction.  With the `serial` of the resident product of the same data, the same run
+    also counts, per point, the units that reach the product's value (`Engine.surrogate_counts`,
+    counters reset first)."""
     nser = len(p.yns)
     hist = np.zeros((nser - 1, p.sj.size, prob['nbins']), dtype=np.int64)
     eng = engine or _engine.default_engine()
 
     def call(*a, boxcar_len, precision):
         dt, _, sj, family, param = a[nser:]
-        args = (np.stack(a[:nser]), groups, seed, first, count, dt, sj, family, param, boxcar_len,
+        args = (np.stack(a[:nser]), null, seed, first, count, dt, sj, family, param, boxcar_len,
                 prob['mask'], prob['maxscale'], prob['nbins'], *hist)
         if serial is None:
             eng.wct_mc_phase(*args, precision=precision)
@@ -758,16 +801,26 @@ def _surrogate_seed(seed):
 
 def wct_surrogate_significance(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
                                wavelet='morlet', normalize=True, mc_count=300, seed=None,
-                               precision='fp64'):
+                               precision='fp64', null='phase'):
     """Monte-Carlo significance level of the wavelet coherence of `y1` and `y2` per scale, against
-    phase-randomised surrogates of the data themselves.  An extension: the reference tests against
+    surrogates of the data's length drawn on the device.  An extension: the reference tests against
     white noise only (`wct_significance`).
 
-    Null: each surrogate pair is the two standardised series with the Fourier phases of each
-    replaced by independent uniform random phases (Theiler et al. 1992), at the series' own length
-    n0: X'_k = X_k e^{i phi_k} for 1 <= k < n0/2, Hermitian completion, mean and Nyquist bin kept.
-    Every surrogate keeps the power spectrum, mean and variance of its series exactly; the two are
-    independent of each other.  Each pair goes through the whole pipeline of `wct`.
+    Null `null='phase'` (default): each surrogate pair is the two standardised series with the
+    Fourier phases of each replaced by independent uniform random phases (Theiler et al. 1992), at
+    the series' own length n0: X'_k = X_k e^{i phi_k} for 1 <= k < n0/2, Hermitian completion, mean
+    and Nyquist bin kept.  Every surrogate keeps the power spectrum, mean and variance of its series
+    exactly; the two are independent of each other.
+
+    `null='ar1'`: red noise (Grinsted et al. 2004), two independent AR(1) series per pair, series s
+    x = m + sigma z, z[0] = e[0], z[n] = g z[n-1] + sqrt(1 - g^2) e[n], with g = ar1(y_s)[0] of the
+    raw series, m = 0 and sigma = 1 with normalize=True, else the mean and standard deviation (ddof
+    0) of y_s as the coherence transforms it (scaled by the power of two that brings max|y_s| into
+    [1/2, 1)): the pairs of `ResidentCrossWavelet.surrogate_test(null='ar1')` for the same seed and
+    parameters.  It makes no assumption of a circular record.  ValueError where a g is not finite or
+    |g| >= 1.
+
+    Each pair goes through the whole pipeline of `wct` at the data's length.
 
     The arguments are those of `wct`, resolved the same way (scales, boxcar, standardisation,
     `precision`, errors), so the result, float64 [J + 1], lines up row for row with the WCT of the
@@ -787,16 +840,17 @@ def wct_surrogate_significance(y1, y2, dt, dj=1/12, s0=-1, J=-1, significance_le
     level, so detrend the series first (as the samples do).  The surrogates are Gaussian-like
     whatever the data's amplitude distribution (no amplitude adjustment)."""
     p, prob = _surrogate_problem((y1, y2), dt, dj, s0, J, wavelet, normalize, precision)
-    hist = _surrogate_histogram(p, prob, (0, 1), _surrogate_seed(seed), 0, mc_count)
+    hist = _surrogate_histogram(p, prob, _coherence_null(null, p, normalize), _surrogate_seed(seed), 0, mc_count)
     return _mc_levels(prob, hist[0], significance_level)
 
 
 def wct3_surrogate_significance(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, significance_level=0.95,
                                 wavelet='morlet', normalize=True, mc_count=300, seed=None,
-                                precision='fp64', conditional=True):
+                                precision='fp64', conditional=True, null='phase'):
     """Monte-Carlo significance levels of `partial_wct` and `multiple_wct` per scale, against
-    phase-randomised surrogates of the data themselves.  Returns (sig_partial, sig_multiple),
-    float64 [J + 1] each, row for row with the RP2 / RM2 of the same arguments.
+    phase-randomised surrogates of the data themselves (`null='phase'`, the default) or red noise
+    (`null='ar1'`).  Returns (sig_partial, sig_multiple), float64 [J + 1] each, row for row with the
+    RP2 / RM2 of the same arguments.
 
     Null, `conditional=True` (default): in every surrogate triple x1 and x2 are rotated by the SAME
     random phases and y by phases of its own (Prichard & Theiler 1994).  x1 and x2 keep their power
@@ -805,6 +859,15 @@ def wct3_surrogate_significance(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, significanc
     x2, which are related to each other as in the data", the one RP2 and RM2 need where x1 and x2
     share a driver.  `conditional=False`: three independent sets of phases, the data-coloured
     counterpart of `wct3_significance`'s null (no coherence between x1 and x2 is kept).
+
+    Null `null='ar1'`, `conditional=True`: y is red noise, the AR(1) series of
+    `wct_surrogate_significance(null='ar1')` with y's own g, m and sigma, and x1 and x2 are held at
+    the data in every triple: the standardised series exactly as `partial_wct` transforms them.  The
+    null is "y is red noise unrelated to x1 and x2, and x1 and x2 are as observed": the relation
+    between x1 and x2 is kept exactly, not just their cross spectrum, and no model of the drivers is
+    needed (which is why it is preferred here to a fitted VAR(1) pair).  `conditional=False`: three
+    independent AR(1) series, each with its own g, m and sigma (x2 under a counter stream of its
+    own).  ValueError where a drawn series' g is not finite or |g| >= 1.
 
     Everything else as `wct_surrogate_significance`: arguments and errors of `partial_wct`, the
     data's length and cone of influence, the conventions of `wct_significance` for the levels, a
@@ -816,7 +879,7 @@ def wct3_surrogate_significance(y, x1, x2, dt, dj=1/12, s0=-1, J=-1, significanc
     level, so detrend the series first (as the samples do).  The surrogates are Gaussian-like
     whatever the data's amplitude distribution (no amplitude adjustment)."""
     p, prob = _surrogate_problem((y, x1, x2), dt, dj, s0, J, wavelet, normalize, precision)
-    hist = _surrogate_histogram(p, prob, (0, 1, 1) if conditional else (0, 1, 2), _surrogate_seed(seed),
+    hist = _surrogate_histogram(p, prob, _coherence_null(null, p, normalize, conditional), _surrogate_seed(seed),
                                 0, mc_count)
     return _mc_levels(prob, hist[0], significance_level), _mc_levels(prob, hist[1], significance_level)
 
