@@ -496,7 +496,8 @@ int cwtb_field_reconstruct(cwtb_ctx *ctx, int field, const double *weights, cons
 int cwtb_cross_scale_avg(cwtb_ctx *ctx, const double *weights, void *out);
 
 /* Morlet.smooth on a caller-supplied host array (mothers.py:61-104).
- * in: n_scales x n (complex128 if is_complex else float64); out same type. */
+ * in: n_scales x n (complex128 if is_complex else float64); out same type.  At most 65535 scales
+ * (one launch row each): more are refused with CWTB_ERR_ARG. */
 int cwtb_smooth(cwtb_ctx *ctx, const void *in, int is_complex, int n_scales,
                 int64_t n, double dt, const double *scales, int boxcar_len,
                 void *out);
@@ -726,7 +727,8 @@ int cwtb_coherence3_cluster_labels(cwtb_ctx *ctx, int row0, int nrows, int row_s
  * n / 32; no bit set past column n0 - 1) with the weights q[n_scales] through the cluster tests'
  * labeller: the table as cwtb_coherence_cluster_table returns it, the label image labels
  * [n_scales][n0] (may be NULL) and the largest Q into *qmax.  The shape is checked before anything
- * is read or allocated: CWTB_ERR_UNSUPPORTED for n_scales * n0 >= 2^32. */
+ * is read or allocated: CWTB_ERR_UNSUPPORTED for n_scales * n0 >= 2^32, CWTB_ERR_ARG for more than
+ * 65535 scales (one launch row each). */
 int cwtb_cluster_label_bits(cwtb_ctx *ctx, const uint32_t *bits, int n_scales, int64_t n0, const uint64_t *q,
                             int64_t cap, int64_t *count, uint64_t *Q, int64_t *points, int64_t *box,
                             int32_t *labels, uint64_t *qmax);
@@ -787,7 +789,8 @@ int cwtb_memcpy_d2h(cwtb_ctx *ctx, void *dst, const void *src, size_t bytes);
 int cwtb_sync(cwtb_ctx *ctx);
 
 /* Test hook: plain batched complex DFT of `batch` rows of length n through the engine's own
- * kernels (any n >= 2; lengths other than 2^k go through Bluestein's algorithm, fp64 only);
+ * kernels (any n >= 2; lengths other than 2^k go through Bluestein's algorithm, fp64 only; any
+ * batch, run in chunks of at most 65535 rows);
  * sign = -1 forward, +1 inverse (unnormalised).
  * in/out: host complex128 (precision selects the arithmetic). */
 int cwtb_fft_c2c(cwtb_ctx *ctx, const void *in, void *out, int64_t n, int batch,

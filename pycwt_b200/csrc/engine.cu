@@ -1045,10 +1045,11 @@ static int get_blue(cwtb_ctx *c, unsigned n, const BluePlan **out) {
   return 0;
 }
 
-// rows of the convolution buffers a chunk may use (two buffers of L complex per row)
+// rows of the convolution buffers a chunk may use (two buffers of L complex per row), and at most
+// MAX_ROWS: every launch of a chunk has one row per chunk row
 static int blue_chunk_rows(unsigned L, int nrows) {
   const size_t per_row = (size_t)L * sizeof(double2);
-  return (int)std::max<size_t>(1, std::min<size_t>((size_t)nrows, ((size_t)1 << 30) / per_row));
+  return (int)std::max<size_t>(1, std::min<size_t>({(size_t)nrows, ((size_t)1 << 30) / per_row, (size_t)MAX_ROWS}));
 }
 
 // convolution core: blueA rows (pitch n) already hold a = x * w_s; result rows y in blueY
@@ -1938,7 +1939,8 @@ static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, i
   if (precision != CWTB_F64 && precision != CWTB_F32) return fail(c, CWTB_ERR_ARG, "bad precision");
   if (!scales) return fail(c, CWTB_ERR_ARG, "null scales");
   RT(rt_set_device(c->device));
-  if (nbatch < 1 || (long long)nbatch * S > 60000) return fail(c, CWTB_ERR_ARG, "batch too large for one launch");
+  if (nbatch < 1 || (long long)nbatch * S > 60000)
+    return fail(c, CWTB_ERR_ARG, "batch too large for one launch: n_chan * n_scales must be at most 60000");
   // whatever transform was resident is about to be replaced, and the re-runs of cwtb_bench_last /
   // cwtb_profile_last wait for a signal of the new plan
   slot_begin(c->wt);
@@ -3347,6 +3349,7 @@ int cwtb_smooth(cwtb_ctx *c, const void *in, int is_complex, int n_scales, int64
   if (!c || !in || !out || !scales || n_scales < 1 || n < 1 || !(dt > 0))
     return fail(c, CWTB_ERR_ARG, "smooth: bad argument");
   if (n > (1ll << 26)) return fail(c, CWTB_ERR_UNSUPPORTED, "smooth: rows longer than 2^26");
+  if (n_scales > (int)MAX_ROWS) return fail(c, CWTB_ERR_ARG, "smooth: more than 65535 scales in one call");
   RT(rt_set_device(c->device));
   const int S = n_scales;
   const size_t cnt = (size_t)S * n;
@@ -3917,6 +3920,7 @@ static int cluster_shape(cwtb_ctx *c, const std::string &nm, long long S, long l
   if (S < 1 || n0 < 1) return fail(c, CWTB_ERR_ARG, nm + ": bad n_scales / n0");
   if ((unsigned long long)S * (unsigned long long)n0 >= (1ull << 32))
     return fail(c, CWTB_ERR_UNSUPPORTED, nm + ": n_scales * n0 must stay below 2^32");
+  if (S > (long long)MAX_ROWS) return fail(c, CWTB_ERR_ARG, nm + ": more than 65535 scales");
   return 0;
 }
 
