@@ -41,12 +41,17 @@ enum cwtb_status {
   CWTB_ERR_COMM = -6       /* NCCL error / libnccl not loadable           */
 };
 
-/* Mother-wavelet families, pycwt/mothers.py:13-233.  MexicanHat == DOG m=2. */
+/* Mother-wavelet families, pycwt/mothers.py:13-233.  MexicanHat == DOG m=2.
+ * CWTB_MORSE is the generalized Morse wavelet of Olhede & Walden (2002), unit energy:
+ *   psi_ft(w) = A w^be exp(-w^ga) for w > 0, else 0,  A = sqrt(ga 2^((2be+1)/ga) / Gamma((2be+1)/ga)),
+ * with 1 <= be <= 256 passed as `param` and 1 <= ga <= 12 taken from the context
+ * (cwtb_set_morse_ga, default 3); ga = 1, be = m is Paul(m)'s response. */
 enum cwtb_family {
   CWTB_MORLET = 0,  /* param = f0 (mothers.py:26-28)  */
   CWTB_PAUL = 1,    /* param = m  (mothers.py:118-122) */
   CWTB_DOG = 2,     /* param = m  (mothers.py:170-173) */
-  CWTB_TABLE = 3    /* caller supplies psi_ft on the [S, Np] grid (duck-typed wavelets) */
+  CWTB_TABLE = 3,   /* caller supplies psi_ft on the [S, Np] grid (duck-typed wavelets) */
+  CWTB_MORSE = 4    /* param = be; ga from cwtb_set_morse_ga */
 };
 
 enum cwtb_precision { CWTB_F64 = 0, CWTB_F32 = 1 };
@@ -100,6 +105,11 @@ int cwtb_set_coherence_precision(cwtb_ctx *ctx, int precision);
  * (Paul, DOG: SURVEY 8f rank 4; pycwt_b200.mothers.enable_generic_smoothing).  The table stays in
  * force until replaced or cleared; calls whose rows / length differ fail with CWTB_ERR_STATE. */
 int cwtb_set_smooth_filter(cwtb_ctx *ctx, const double *table, int n_rows, int64_t n);
+/* Shape parameter ga of CWTB_MORSE (default 3) for the following calls with that family, the second
+ * parameter of the family kept on the context like the smoothing filter above, so that every entry
+ * point keeps its (family, param) pair.  A resident plan built for one ga is never reused for another.
+ * Returns CWTB_ERR_ARG for ga outside [1, 12]. */
+int cwtb_set_morse_ga(cwtb_ctx *ctx, double ga);
 
 /* Pinned host memory (so D2H of multi-GiB results runs at PCIe speed and can
  * overlap with compute).  numpy wraps the returned pointer. */

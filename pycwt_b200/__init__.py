@@ -17,6 +17,7 @@ from .resident import xwt_resident, ResidentCrossWavelet  # noqa: F401  (extensi
 from .resident import wct3_resident, ResidentCoherence3  # noqa: F401  (extension)
 from .resident import power_resident, ResidentPower  # noqa: F401  (extension)
 from .resident import ClusterResult  # noqa: F401  (extension)
+from .mothers import Morse  # noqa: F401  (extension: generalized Morse wavelets)
 
 __all__ = ['cwt', 'icwt', 'significance', 'xwt', 'wct', 'wct_significance',
            'mothers', 'Morlet', 'Paul', 'DOG', 'MexicanHat']

@@ -11,7 +11,9 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcwtb200.so")
 
-MORLET, PAUL, DOG, TABLE = 0, 1, 2, 3
+MORLET, PAUL, DOG, TABLE, MORSE = 0, 1, 2, 3, 4
+#: Morse's shape parameter ga when `param` gives be alone
+MORSE_GA = 3.0
 F64, F32 = 0, 1
 # complex fields of the cwtb_field_* calls, each with the id of its product below
 FIELD_W, FIELD_CROSS, FIELD_POWER = 0, 1, 5
@@ -57,6 +59,7 @@ _SIGNATURES = {
     "cwtb_set_padding": (_I, [_P, _I]),
     "cwtb_set_coherence_precision": (_I, [_P, _I]),
     "cwtb_set_smooth_filter": (_I, [_P, _P, _I, _I64]),
+    "cwtb_set_morse_ga": (_I, [_P, _D]),
     "cwtb_host_alloc": (_I, [_P, ctypes.c_size_t, ctypes.POINTER(_P)]),
     "cwtb_host_free": (_I, [_P, _P]),
     "cwtb_cwt": (_I, [_P, _P, _I, _I64, _D, _P, _I, _I, _D, _I, _P]),
@@ -342,6 +345,17 @@ class Engine(object):
                              % (r, n, "?" if rows is None else rows, "?" if n0 is None else n0))
         return r, n, prec
 
+    def _fam(self, family, param):
+        """(family, param) of the C calls.  Morse's `param` is be or (be, ga) (ga = MORSE_GA with be
+        alone); its ga goes to the context here, so every call sets it inside the same locked call as
+        the transform that reads it."""
+        family = int(family)
+        if family != MORSE:
+            return family, float(param)
+        be, ga = (param, MORSE_GA) if np.ndim(param) == 0 else param
+        self._check(self.lib.cwtb_set_morse_ga(self.h, float(ga)))
+        return family, float(be)
+
     @_locked
     def set_band_eps(self, eps):
         self._check(self.lib.cwtb_set_band_eps(self.h, float(eps)))
@@ -474,11 +488,11 @@ class Engine(object):
                 dtype = np.complex128 if (precision == F64 or out_f64) else np.complex64
                 W = self.result_array((sj.size, sig.size), dtype)
                 self._check(self.lib.cwtb_cwt_to_host(self.h, _ptr(sig), is32, sig.size, float(dt),
-                                                      _ptr(sj), sj.size, int(family), float(param),
+                                                      _ptr(sj), sj.size, *self._fam(family, param),
                                                       int(precision), _ptr(W), 1 if out_f64 else 0))
                 return W
             self._check(self.lib.cwtb_cwt(self.h, _ptr(sig), is32, sig.size, float(dt),
-                                          _ptr(sj), sj.size, int(family), float(param),
+                                          _ptr(sj), sj.size, *self._fam(family, param),
                                           int(precision), tptr))
             if not fetch:
                 return None
@@ -613,7 +627,7 @@ class Engine(object):
         with self.lock:
             self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_xwt(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), _ptr(sj),
-                                          sj.size, int(family), float(param), _ptr(out)))
+                                          sj.size, *self._fam(family, param), _ptr(out)))
         return out
 
     @_locked
@@ -628,7 +642,7 @@ class Engine(object):
         with self.lock:
             self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_wct(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
-                                          _ptr(sj), sj.size, int(family), float(param),
+                                          _ptr(sj), sj.size, *self._fam(family, param),
                                           int(boxcar_len), _ptr(WCT),
                                           _ptr(aWCT) if want_angle else None))
         return WCT, aWCT
@@ -647,8 +661,8 @@ class Engine(object):
         RM2 = self.result_array((sj.size, ys[0].size), np.float64) if want_multiple else None
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]), ys[0].size,
-                                       float(dt), float(dj), _ptr(sj), sj.size, int(family),
-                                       float(param), int(boxcar_len),
+                                       float(dt), float(dj), _ptr(sj), sj.size,
+                                       *self._fam(family, param), int(boxcar_len),
                                        _ptr(RP2) if want_partial else None,
                                        _ptr(RM2) if want_multiple else None))
         return RP2, RM2
@@ -667,7 +681,7 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt), float(dj),
-                                               _ptr(sj), sj.size, int(family), float(param),
+                                               _ptr(sj), sj.size, *self._fam(family, param),
                                                int(boxcar_len)))
         return self.coherence_serial()
 
@@ -724,7 +738,7 @@ class Engine(object):
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_resident(self.h, _ptr(ys[0]), _ptr(ys[1]), _ptr(ys[2]),
                                                 ys[0].size, float(dt), float(dj), _ptr(sj), sj.size,
-                                                int(family), float(param), int(boxcar_len)))
+                                                *self._fam(family, param), int(boxcar_len)))
         return self.coherence3_serial()
 
     @_locked
@@ -782,7 +796,7 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_xwt_resident(self.h, _ptr(y1), _ptr(y2), y1.size, float(dt),
-                                               _ptr(sj), sj.size, int(family), float(param)))
+                                               _ptr(sj), sj.size, *self._fam(family, param)))
         return self.cross_serial()
 
     @_locked
@@ -876,8 +890,8 @@ class Engine(object):
         with self.lock:
             self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
             self._check(self.lib.cwtb_wct_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2],
-                                             float(dt), float(dj), _ptr(sj), sj.size, int(family),
-                                             float(param), int(boxcar_len), _ptr(mask),
+                                             float(dt), float(dj), _ptr(sj), sj.size,
+                                             *self._fam(family, param), int(boxcar_len), _ptr(mask),
                                              int(maxscale), int(nbins), h))
         return hist
 
@@ -893,8 +907,8 @@ class Engine(object):
         h, _ = self._mc_hists("wct_mc_seeded", sj.size, nbins, hist, None)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_pair), int(n_pairs),
-                                                int(n0), float(dt), _ptr(sj), sj.size, int(family),
-                                                float(param), int(boxcar_len), _ptr(mask), int(maxscale),
+                                                int(n0), float(dt), _ptr(sj), sj.size,
+                                                *self._fam(family, param), int(boxcar_len), _ptr(mask), int(maxscale),
                                                 int(nbins), h))
         return hist
 
@@ -932,7 +946,7 @@ class Engine(object):
         hp, hm = self._mc_hists("wct3_mc", sj.size, nbins, hist_partial, hist_multiple)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_mc(self.h, _ptr(noise), noise.shape[0], noise.shape[2], float(dt),
-                                          _ptr(sj), sj.size, int(family), float(param), int(boxcar_len),
+                                          _ptr(sj), sj.size, *self._fam(family, param), int(boxcar_len),
                                           _ptr(mask), int(maxscale), int(nbins), hp, hm))
         return hist_partial, hist_multiple
 
@@ -949,7 +963,7 @@ class Engine(object):
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct3_mc_seeded(self.h, int(seed) & (2 ** 64 - 1), int(first_triple),
                                                  int(n_triples), int(n0), float(dt), _ptr(sj), sj.size,
-                                                 int(family), float(param), int(boxcar_len), _ptr(mask),
+                                                 *self._fam(family, param), int(boxcar_len), _ptr(mask),
                                                  int(maxscale), int(nbins), hp, hm))
         return hist_partial, hist_multiple
 
@@ -1015,7 +1029,7 @@ class Engine(object):
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_wct_mc_null(self.h, _ptr(series), nser, *nargs, int(seed) & (2 ** 64 - 1),
                                               int(first_unit), int(n_units), n0, float(dt), _ptr(sj), sj.size,
-                                              int(family), float(param), int(boxcar_len), _ptr(mask),
+                                              *self._fam(family, param), int(boxcar_len), _ptr(mask),
                                               int(maxscale), int(nbins), ha, hb))
         return hist_a, hist_b
 
@@ -1050,7 +1064,7 @@ class Engine(object):
         ha, hb = self._mc_hists("surrogate_counts", sj.size, nbins, hist_a, hist_b)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         args = (self.h, _ptr(series), *nargs, int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
-                float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
+                float(dt), _ptr(sj), sj.size, *self._fam(family, param), int(boxcar_len), _ptr(mask), int(maxscale),
                 int(nbins))
         if nser == 2:
             self._check(self.lib.cwtb_coherence_surrogate_counts_null(*args, ha, int(serial), 1 if reset else 0))
@@ -1142,7 +1156,7 @@ class Engine(object):
         qmax = np.zeros(int(n_units), dtype=np.uint64)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         args = (self.h, _ptr(series), *nargs, int(seed) & (2 ** 64 - 1), int(first_unit), int(n_units), n0,
-                float(dt), _ptr(sj), sj.size, int(family), float(param), int(boxcar_len), _ptr(mask), int(maxscale),
+                float(dt), _ptr(sj), sj.size, *self._fam(family, param), int(boxcar_len), _ptr(mask), int(maxscale),
                 int(nbins))
         rows = (_ptr(thr), _ptr(lo), _ptr(hi), _ptr(q))
         if nser == 2:
@@ -1200,7 +1214,7 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         self._check(self.lib.cwtb_set_coherence_precision(self.h, int(precision)))
         self._check(self.lib.cwtb_power_resident(self.h, _ptr(y), y.size, float(dt), _ptr(sj), sj.size,
-                                                 int(family), float(param)))
+                                                 *self._fam(family, param)))
         return self.power_serial()
 
     @_locked
@@ -1256,8 +1270,7 @@ class Engine(object):
                                                     int(n0), _ptr(out)))
         return out
 
-    @staticmethod
-    def _power_args(name, series, null, g, m, sigma, seed, first_unit, n_units, dt, sj, family, param, serial):
+    def _power_args(self, name, series, null, g, m, sigma, seed, first_unit, n_units, dt, sj, family, param, serial):
         """The arguments of a power test up to `serial` (the series: the phase null's data, 1-D).  The
         caller keeps `series` and `sj` alive across the call."""
         if series.ndim != 1:
@@ -1265,8 +1278,8 @@ class Engine(object):
         if null == NULL_PHASE and not np.isfinite(series).all():
             raise ValueError("%s: non-finite sample" % name)
         return (_ptr(series), int(null), float(g), float(m), float(sigma), int(seed) & (2 ** 64 - 1),
-                int(first_unit), int(n_units), series.size, float(dt), _ptr(sj), sj.size, int(family),
-                float(param), int(serial))
+                int(first_unit), int(n_units), series.size, float(dt), _ptr(sj), sj.size,
+                *self._fam(family, param), int(serial))
 
     @_locked
     def power_surrogate_counts(self, series, null, g, m, sigma, seed, first_unit, n_units, dt, scales, family,
@@ -1342,7 +1355,7 @@ class Engine(object):
         g, m, sigma = self._pair_params(name, g, m, sigma)
         keep = (series, g, m, sigma)
         return (_ptr(series), int(null), _ptr(g), _ptr(m), _ptr(sigma), int(seed) & (2 ** 64 - 1), int(first_unit),
-                int(n_units), series.shape[1], float(dt), _ptr(sj), sj.size, int(family), float(param),
+                int(n_units), series.shape[1], float(dt), _ptr(sj), sj.size, *self._fam(family, param),
                 int(serial)), keep
 
     @_locked
@@ -1418,8 +1431,8 @@ class Engine(object):
             W = np.empty((nch, sj.size, n0), dtype=np.complex128 if precision == F64 else np.complex64)
         with self.lock:
             self._check(self.lib.cwtb_cwt_batch(self.h, _ptr(X), int(X.dtype == np.float32), nch, n0,
-                                                float(dt), _ptr(sj), sj.size, int(family),
-                                                float(param), int(precision),
+                                                float(dt), _ptr(sj), sj.size,
+                                                *self._fam(family, param), int(precision),
                                                 _ptr(power) if want_power else None,
                                                 _ptr(W) if want_w else None))
         return power, W
@@ -1444,7 +1457,7 @@ class Engine(object):
     def cwt_dev(self, dptr, is_f32, n0, dt, scales, family, param, precision=F64):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         self._check(self.lib.cwtb_cwt_dev(self.h, dptr, int(is_f32), int(n0), float(dt),
-                                          _ptr(sj), sj.size, int(family), float(param),
+                                          _ptr(sj), sj.size, *self._fam(family, param),
                                           int(precision)))
 
     @_locked
@@ -1453,7 +1466,7 @@ class Engine(object):
         sj = np.ascontiguousarray(scales, dtype=np.float64)
         power = np.empty((n_chan, sj.size), dtype=np.float64) if want_power else None
         self._check(self.lib.cwtb_cwt_batch_dev(self.h, dptr, int(n_chan), int(n0), float(dt),
-                                                _ptr(sj), sj.size, int(family), float(param),
+                                                _ptr(sj), sj.size, *self._fam(family, param),
                                                 int(precision), _ptr(power) if want_power else None))
         return power
 

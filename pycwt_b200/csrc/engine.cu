@@ -281,6 +281,7 @@ struct cwtb_ctx {
   Buf filt;                      // caller-supplied time-smoothing responses [S][N] (cwtb_set_smooth_filter)
   int filt_rows = 0;
   long long filt_n = 0;
+  double morse_ga = 3.0;         // shape parameter of CWTB_MORSE (cwtb_set_morse_ga)
   Buf Zx, Cout, wtab;            // expansion path: intermediate of the coarse transforms, coarse samples,
                                  // interpolation weight tables
   std::map<std::array<long long, 3>, long long> wtab_index;   // (log2R, taps, round(beta*1e6)) -> offset
@@ -299,10 +300,11 @@ struct cwtb_ctx {
   struct PlanKey {
     long long n0 = -1;
     double dt = 0, param = 0, band_eps = 0, band_eps32 = 0, expand_eps = 0, expand_eps32 = 0;
+    double ga = 0;                 // Morse's shape parameter (0 for the other families)
     int S = 0, family = 0, precision = 0, nbatch = 0, pad = 0;
     std::vector<double> scales;
     bool operator==(const PlanKey &o) const {
-      return n0 == o.n0 && dt == o.dt && param == o.param && band_eps == o.band_eps && band_eps32 == o.band_eps32 &&
+      return n0 == o.n0 && dt == o.dt && param == o.param && ga == o.ga && band_eps == o.band_eps && band_eps32 == o.band_eps32 &&
              expand_eps == o.expand_eps && expand_eps32 == o.expand_eps32 && S == o.S && family == o.family &&
              precision == o.precision && nbatch == o.nbatch && pad == o.pad && scales == o.scales;
     }
@@ -512,11 +514,35 @@ static double solve_upper(double m, bool gaussian, double target, double fstart)
 }
 
 // frequency-domain support [flo, fhi] (in f = s*w) where |psi_ft| >= eps * max|psi_ft|
-static void family_band(int family, double param, double eps, double *flo, double *fhi, bool *pos_only) {
+// (ga: Morse's shape parameter, unused by the other families)
+static void family_band(int family, double param, double ga, double eps, double *flo, double *fhi, bool *pos_only) {
   const double LN_MIN = -745.2;  // exp() underflows to exactly 0 below this
   const double lneps = eps > 0 ? std::log(eps) : 0;
   *pos_only = false;
-  if (family == CWTB_MORLET) {
+  if (family == CWTB_MORSE) {
+    // the peak-relative exponent g(u) = be u - (be/ga) expm1(ga u), u = ln(f / f_p), rises to 0 at
+    // u = 0 and falls on both sides; its two roots of g = target by bisection in u.  (The value
+    // itself carries the constant psi_ft(f_p) = O(1), so the exact-mode floor applies to g as is.)
+    const double be = param, bg = be / ga;
+    const double target = eps > 0 ? lneps : LN_MIN;
+    auto g = [&](double u) { return be * u - bg * std::expm1(ga * u); };
+    double lo = (target - bg) / be, hi = 0;    // g(u) <= be u + be/ga: g(lo) <= target
+    for (int it = 0; it < 200; ++it) {
+      const double mid = 0.5 * (lo + hi);
+      if (g(mid) < target) lo = mid; else hi = mid;
+    }
+    const double ulo = lo;
+    lo = 0; hi = 1;
+    while (g(hi) > target) hi *= 2;               // expm1 overflows to inf: g = -inf ends it
+    for (int it = 0; it < 200; ++it) {
+      const double mid = 0.5 * (lo + hi);
+      if (g(mid) > target) lo = mid; else hi = mid;
+    }
+    const double lnfp = std::log(bg) / ga;
+    *flo = std::exp(ulo + lnfp);
+    *fhi = std::exp(hi + lnfp);
+    *pos_only = true;
+  } else if (family == CWTB_MORLET) {
     double xc = std::sqrt(-2.0 * (eps > 0 ? lneps : LN_MIN));
     *flo = param - xc;
     *fhi = param + xc;
@@ -647,10 +673,13 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
                      int family, double param, int precision, bool have_table, int nbatch = 1,
                      const std::vector<OsRow> *os = nullptr) {
   if (n0 < 1 || S < 1 || !(dt > 0)) return fail(c, CWTB_ERR_ARG, "bad n0 / n_scales / dt");
-  if (family < 0 || family > 3) return fail(c, CWTB_ERR_ARG, "unknown wavelet family");
+  if (family < 0 || family > 4) return fail(c, CWTB_ERR_ARG, "unknown wavelet family");
   if (family == CWTB_TABLE && !have_table) return fail(c, CWTB_ERR_ARG, "CWTB_TABLE needs a table");
   if ((family == CWTB_PAUL || family == CWTB_DOG) && (param != std::floor(param) || param < 1 || param > 64))
     return fail(c, CWTB_ERR_ARG, "Paul/DOG order must be an integer in [1, 64]");
+  const double ga = c->morse_ga;
+  if (family == CWTB_MORSE && !(param >= 1 && param <= 256 && ga >= 1 && ga <= 12))
+    return fail(c, CWTB_ERR_ARG, "Morse needs 1 <= be <= 256 and 1 <= ga <= 12");
   if (n0 > (1ll << 28)) return fail(c, CWTB_ERR_UNSUPPORTED, "signal longer than 2^28");
   job = Job();
   job.precision = precision;
@@ -678,6 +707,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
   fam.dw = 1.0 / ((double)N * dt);
   fam.table = nullptr;
   fam.tpitch = N;
+  fam.be = fam.ga = fam.lnfp = fam.bg = 0;
   double fconst = 1.0;
   if (family == CWTB_MORLET) fconst = std::pow(M_PI, -0.25);
   else if (family == CWTB_PAUL) {
@@ -691,6 +721,16 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
     // conj(-(1j**m)):  m%4: 0 -> -1, 1 -> +i, 2 -> +1, 3 -> -i
     static const int unit_of[4] = {2, 1, 0, 3};
     fam.unit = unit_of[m & 3];
+  } else if (family == CWTB_MORSE) {
+    const double be = param;
+    fam.be = be;
+    fam.ga = ga;
+    fam.bg = be / ga;
+    fam.lnfp = std::log(fam.bg) / ga;
+    // psi_ft(f_p) = A f_p^be exp(-f_p^ga), A = sqrt(ga 2^r / Gamma(r)), r = (2be+1)/ga, in logs (both
+    // factors overflow for large be, their product is O(1))
+    const double r = (2 * be + 1) / ga;
+    fconst = std::exp(0.5 * (std::log(ga) + r * std::log(2.0) - std::lgamma(r)) + be * fam.lnfp - fam.bg);
   }
   // ftfreqs[1]; for Np == 2 numpy's fftfreq(2)[1] is -0.5/dt, so the reference's
   // normalisation sqrt(s*w1*Np) is NaN there -- reproduced.
@@ -699,7 +739,7 @@ static int build_job(cwtb_ctx *c, Job &job, long long n0, double dt, const doubl
   bool pos_only = false;
   // eps = 0 (exact mode) applies to both engines
   const double beps = (precision == CWTB_F32 && c->band_eps > 0) ? std::max(c->band_eps, c->band_eps32) : c->band_eps;
-  if (family != CWTB_TABLE) family_band(family, param, beps, &flo, &fhi, &pos_only);
+  if (family != CWTB_TABLE) family_band(family, param, ga, beps, &flo, &fhi, &pos_only);
 
   std::vector<ScaleDesc> ds(S);
   job.plan_log2K.assign(S, 0);
@@ -1311,7 +1351,8 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
     if (first >= 0) {
       BandArgs<T> ba{ddesc, spec, Bbuf, fam, N, first};
       const unsigned Kmax = 1u << maxlk;
-      if ((e = launch<BandBody<T>>(c, (Kmax + NT * BandBody<T>::PER - 1) / (NT * BandBody<T>::PER), nrows, ba)))
+      const unsigned gx = (Kmax + NT * BandBody<T>::PER - 1) / (NT * BandBody<T>::PER);
+      if ((e = fam.family == CWTB_MORSE ? launch<BandBodyMorse<T>>(c, gx, nrows, ba) : launch<BandBody<T>>(c, gx, nrows, ba)))
         return e;
     }
   }
@@ -1488,7 +1529,8 @@ static int run_job(cwtb_ctx *c, const Job &job, const T *dsig, cx<T> *Wout = nul
       b.pf_dist = c->pf_dist; b.ny = ng;
       if (!dense) {
         BandArgs<T> ba{ddesc, spec, Bbuf, fam, N, cl.first + g0};
-        if ((e = launch<BandBody<T>>(c, (K + NT * BandBody<T>::PER - 1) / (NT * BandBody<T>::PER), ng, ba)))
+        const unsigned gx = (K + NT * BandBody<T>::PER - 1) / (NT * BandBody<T>::PER);
+        if ((e = fam.family == CWTB_MORSE ? launch<BandBodyMorse<T>>(c, gx, ng, ba) : launch<BandBody<T>>(c, gx, ng, ba)))
           return e;
       }
       e = dense ? dispatch_passA<T, +1, MODE_DENSE>(c, cl.log2K - l2k, a, ng)
@@ -1948,6 +1990,7 @@ static int prepare(cwtb_ctx *c, long long n0, double dt, const double *scales, i
   cwtb_ctx::PlanKey key;
   key.n0 = n0; key.dt = dt; key.param = param; key.band_eps = c->band_eps; key.band_eps32 = c->band_eps32;
   key.expand_eps = c->expand_eps; key.expand_eps32 = c->expand_eps32; key.S = S; key.family = family;
+  key.ga = family == CWTB_MORSE ? c->morse_ga : 0;
   key.precision = precision; key.nbatch = nbatch; key.pad = c->pad_pow2;
   key.scales.assign(scales, scales + std::max(S, 0));
   if (c->plan_reuse && family != CWTB_TABLE && c->job.valid && key == c->plan_key) return 0;
@@ -3317,6 +3360,13 @@ int cwtb_set_coherence_precision(cwtb_ctx *c, int precision) {
   if (!c) return CWTB_ERR_ARG;
   if (precision != CWTB_F64 && precision != CWTB_F32) return fail(c, CWTB_ERR_ARG, "bad precision");
   c->coh_precision = precision;
+  return 0;
+}
+
+int cwtb_set_morse_ga(cwtb_ctx *c, double ga) {
+  if (!c) return CWTB_ERR_ARG;
+  if (!(ga >= 1 && ga <= 12)) return fail(c, CWTB_ERR_ARG, "Morse ga must be in [1, 12]");
+  c->morse_ga = ga;
   return 0;
 }
 

@@ -32,7 +32,7 @@ struct ScaleDesc {
 };
 
 struct Fam {
-  int family;      // 0 Morlet, 1 Paul, 2 DOG, 3 table
+  int family;      // 0 Morlet, 1 Paul, 2 DOG, 3 table, 4 Morse
   int m;           // order (Paul, DOG)
   int unit;        // multiply by i^unit  (conj(-(1j**m)) for DOG)
   int pad_;
@@ -40,6 +40,11 @@ struct Fam {
   double dw;       // 1 / (Np * dt)   (numpy fftfreq's `val`)
   const double2 *table;  // [S][Np] complex128: sqrt(s*w1*Np)*conj(psi_ft)  (family 3)
   long long tpitch;
+  // Morse (family 4): psi_ft(f) / psi_ft(f_p) = exp(be u - (be/ga) expm1(ga u)), u = ln(f / f_p),
+  // f_p = (be/ga)^(1/ga) the peak; the family constant psi_ft(f_p) is folded into ScaleDesc::amp
+  double be, ga;
+  double lnfp;     // ln f_p
+  double bg;       // be / ga  (= f_p^ga)
 };
 
 HD double ipow(double f, int m) {
@@ -51,7 +56,8 @@ HD double ipow(double f, int m) {
 
 // |conj(psi_ft(s*w_k))| without the family constant; pycwt/mothers.py:26-28,118-122,170-173.
 // w_k is formed as numpy does: 2*pi * (k * (1/(Np*dt))).
-HD double amp_eval(const Fam &fp, double s, int k) {
+// (MORSE = false: the Morse branch is compiled out, for kernels that never see a Morse row; see BandBody)
+template <bool MORSE = true> HD double amp_eval(const Fam &fp, double s, int k) {
   const double w = 6.283185307179586 * ((double)k * fp.dw);
   const double f = s * w;
   if (fp.family == 0) {
@@ -59,6 +65,11 @@ HD double amp_eval(const Fam &fp, double s, int k) {
     return exp(-0.5 * d * d);
   } else if (fp.family == 1) {
     return f > 0.0 ? ipow(f, fp.m) * exp(-f) : 0.0;
+  } else if (MORSE && fp.family == 4) {
+    // peak-relative log form: no power of f is formed, so a large be never gives inf * 0
+    if (!(f > 0.0)) return 0.0;
+    const double u = log(f) - fp.lnfp;
+    return exp(fp.be * u - fp.bg * expm1(fp.ga * u));
   } else {
     return ipow(f, fp.m) * exp(-0.5 * f * f);
   }
@@ -68,9 +79,9 @@ HD double amp_eval(const Fam &fp, double s, int k) {
 // and evaluates the power and the exponential in float (the caller keeps orders above 8 in double:
 // their powers overflow float).  fp64 instructions run at half the fp32 rate on H100: one double exp per band product
 // would make the band-product launches and the generating first kernel fp64-pipe bound in the fp32 engine.
-template <typename T> HD T amp_eval_t(const Fam &fp, double s, int k) {
+template <typename T, bool MORSE = true> HD T amp_eval_t(const Fam &fp, double s, int k) {
   if constexpr (sizeof(T) == 8) {
-    return amp_eval(fp, s, k);
+    return amp_eval<MORSE>(fp, s, k);
   } else {
     const double w = 6.283185307179586 * ((double)k * fp.dw);
     const double f = s * w;
@@ -96,7 +107,7 @@ template <typename T> HD cx<T> rot_unit(cx<T> v, int unit) {
 }
 
 // value of x^[bin] * conj(psi_ft)(s, k) * norm / Np  for one scale
-template <typename T>
+template <typename T, bool MORSE = true>
 HD cx<T> band_value(const Fam &fp, const ScaleDesc &d, const cx<T> *spec, unsigned bin, int k, unsigned N) {
   cx<T> v = ldg(&spec[(size_t)d.chan * N + bin]);
   if (fp.family == 3) {
@@ -104,9 +115,14 @@ HD cx<T> band_value(const Fam &fp, const ScaleDesc &d, const cx<T> *spec, unsign
     cx<T> tt = mk<T>((T)(t.x * d.amp), (T)(t.y * d.amp));
     return cmul(v, tt);
   }
-  // (orders above 8: value and normalisation only combine to a float-range number in double)
-  const T a = (sizeof(T) == 8 || (fp.family != 0 && fp.m > 8)) ? (T)(amp_eval(fp, d.s, k) * d.amp)
-                                                               : (T)(amp_eval_t<T>(fp, d.s, k) * (T)d.amp);
+  // (Paul / DOG orders above 8: value and normalisation only combine to a float-range number in
+  // double.  Morse too is evaluated in double in the fp32 engine: a float evaluation of its exponent
+  // (logf, expm1f, expf) inlined here raised the fp32 dense first kernel PassABody<float, 16> from 78 to
+  // 88 registers and made config 3 measurably slower for Paul and DOG; the double one reuses the code
+  // the orders above 8 already take.)
+  const T a = (sizeof(T) == 8 || (MORSE && fp.family == 4) || (fp.family != 0 && fp.m > 8))
+                  ? (T)(amp_eval<MORSE>(fp, d.s, k) * d.amp)
+                  : (T)(amp_eval_t<T, MORSE>(fp, d.s, k) * (T)d.amp);
   return rot_unit<T>(cscale(v, a), fp.unit);
 }
 
@@ -1416,7 +1432,7 @@ template <typename T> struct BandBody {
   static constexpr int NPHASE = 1;
   static constexpr size_t SMEM = 0;
   static constexpr int PER = 4;
-  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+  template <bool MORSE> HD static void fill(const Args &a, int bx, int by, int tid) {
     const ScaleDesc d = a.descs[a.first + by];
     const int K = 1 << d.log2K;
 #pragma unroll
@@ -1425,9 +1441,18 @@ template <typename T> struct BandBody {
       if (r >= K) return;
       const int k = r - (r >= d.rsplit ? K : 0);
       V v = mk<T>(0, 0);
-      if (k >= d.k_lo && k <= d.k_hi) v = band_value<T>(a.fam, d, a.spec, (unsigned)k & (a.N - 1), k, a.N);
+      if (k >= d.k_lo && k <= d.k_hi) v = band_value<T, MORSE>(a.fam, d, a.spec, (unsigned)k & (a.N - 1), k, a.N);
       a.Bbuf[d.boff + r] = v;
     }
+  }
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) { fill<false>(a, bx, by, tid); }
+};
+// the band products of Morse rows: BandBody with the Morse response compiled in (inlined into BandBody
+// itself, its log and expm1 take the kernel from 32 to 36 registers in fp32 and from 34 to 38 in fp64)
+template <typename T> struct BandBodyMorse : BandBody<T> {
+  using Args = typename BandBody<T>::Args;
+  template <int PH> HD static void phase(const Args &a, int bx, int by, int tid, void *) {
+    BandBody<T>::template fill<true>(a, bx, by, tid);
   }
 };
 

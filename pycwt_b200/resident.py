@@ -266,8 +266,8 @@ def _engine_wavelet(wavelet, name):
     if spec is None:
         # duck-typed objects, subclasses that override psi_ft, non-integer or out-of-range orders
         raise TypeError("%s needs one of the analytic families the engine evaluates "
-                        "itself: Morlet(f0), Paul(m) or DOG(m) with an integer order in [1, 64] "
-                        "and the stock psi_ft" % name)
+                        "itself: Morlet(f0), Paul(m) or DOG(m) with an integer order in [1, 64], "
+                        "or Morse(ga, be), with the stock psi_ft" % name)
     return wavelet, spec
 
 

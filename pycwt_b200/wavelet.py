@@ -21,7 +21,7 @@ from . import _engine
 from . import helpers as _helpers
 from .helpers import (ar1, ar1_spectrum, fft, fft_kwargs, find, get_cache_dir,
                       rednoise)
-from .mothers import Morlet, Paul, DOG, MexicanHat
+from .mothers import Morlet, Paul, DOG, MexicanHat, Morse
 
 _PRECISIONS = {'fp64': _engine.F64, 'f64': _engine.F64, 'float64': _engine.F64,
                'fp32': _engine.F32, 'f32': _engine.F32, 'float32': _engine.F32}
@@ -362,7 +362,7 @@ def _family_of(wavelet):
     spec = _engine_family(wavelet)
     if spec is None:
         raise NotImplementedError(
-            'xwt/wct on the GPU need a Morlet, Paul or DOG mother wavelet')
+            'xwt/wct on the GPU need a Morlet, Paul, DOG or Morse mother wavelet')
     return spec
 
 
@@ -905,7 +905,7 @@ def _smooth_device(W, dt, dj, scales, deltaj0, wavelet=None):
 def _check_parameter_wavelet(wavelet):
     """Strings map to default-constructed mother wavelets, anything else is returned as
     is (reference wavelet.py:650-663); unknown names raise KeyError."""
-    mothers = {'morlet': Morlet, 'paul': Paul, 'dog': DOG, 'mexicanhat': MexicanHat}
+    mothers = {'morlet': Morlet, 'paul': Paul, 'dog': DOG, 'mexicanhat': MexicanHat, 'morse': Morse}
     if isinstance(wavelet, str):
         return mothers[wavelet]()
     return wavelet
